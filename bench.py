@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py - self-play throughput (BASELINE.json metric: env-steps/s and MCTS simulations/s) on N B200s.
+"""bench.py - self-play throughput (BASELINE.json metric: env-steps/s and MCTS simulations/s) on N H100s.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl ours|reference]
-                  [--extras a,b,c | --no-extras] [--no-cpu-baseline] [--no-loop]
+                  [--extras a,b,c | --no-extras] [--no-cpu-baseline] [--no-loop] [--dump-outputs DIR]
 
 What is timed
 -------------
@@ -15,6 +15,9 @@ search would otherwise give a 12 ms sample); the L2 is flushed (256 MiB write, u
 `loop`  = env-steps/s of the WHOLE self-play loop through the public `SelfPlay` API (SURVEY.md 8d's full definition:
           search + environment step + action sampling + GameHistory hand-over), timed >= 1 s;
 `workloads` = the same sub-lines for the other BASELINE configs at this --gpus N.
+--dump-outputs DIR writes the arrays the last timed search of the headline workload returned (SearchOutput fields,
+float32 / float64 .npy).  The inputs are seeded and the last timed search always runs on the same input batch, so two
+builds can be compared output for output.
 
 N=1 headline workload: BASELINE.json configs[1] - CartPole, fully-connected net, num_simulations=50, 4096 parallel
 games per GPU (weak scaling: every rank owns its own games; no data-path collective - one all-gather of per-rank
@@ -52,21 +55,12 @@ NET_FLOPS = {"cartpole": (1312.0, 2752.0), "tictactoe": (1.880e5, 2.315e5), "con
 
 
 def load_peaks():
-    """(HBM GB/s, dense bf16 TFLOP/s, which) from the driver-written MEASURED_PEAKS.json, else the fallback."""
+    """(HBM GB/s, dense bf16 TFLOP/s, which) from an optional MEASURED_PEAKS.json, else the H100 SXM data sheet."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "measured"
-    return 6650.0, 1400.0, "fallback"
-
-
-def load_traffic():
-    """Measured DRAM bytes per launch of the dominant kernels, from the committed ncu captures (profiles/traffic.json)."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        return json.load(open(p))
-    except (OSError, ValueError):
-        return {}
+    return 3350.0, 989.0, "data sheet"
 
 
 def conv3x3_flops(spec, N):
@@ -317,8 +311,8 @@ def run_workload(name, args, D, rank, local_rank, world, with_loop, headline):
         est = D.max([est])[0]
         inner = max(1, int(math.ceil(MIN_TIMED_SECONDS / max(est * steps, 1e-9))))
         D.barrier()
-        per_search, per_step, kern, visits = [], [], 0.0, None
-        i = 0
+        per_search, per_step, kern, last = [], [], 0.0, None
+        i = -(steps * inner) % n_batches           # the last timed search always runs on batch n_batches - 1
         for _ in range(steps):
             acc = 0.0
             for _ in range(inner):
@@ -327,11 +321,11 @@ def run_workload(name, args, D, rank, local_rank, world, with_loop, headline):
                 acc += dt
                 per_search.append(1000.0 * dt)
                 kern += out.device_ms
-                visits = out.visit_counts
+                last = out
             per_step.append(1000.0 * acc)
         D.barrier()
         return dict(wall=sum(per_step) / 1000.0, kern_ms=kern, searches=steps * inner, inner=inner,
-                    per_search=per_search, per_step=per_step, visits=visits)
+                    per_search=per_search, per_step=per_step, last=last)
 
     clocks = ClockSampler(local_rank) if headline else None
     if clocks:
@@ -343,8 +337,10 @@ def run_workload(name, args, D, rank, local_rank, world, with_loop, headline):
     launches = eng.launch_count - launches0
     graph_parts = eng.graph_partitions
     clk = clocks.stop() if clocks else None
+    if headline and args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dv["last"])
     hv = timed(search_host, args.steps, args.warmup)
-    assert int(numpy.asarray(hv["visits"]).sum()) == B * N
+    assert int(numpy.asarray(hv["last"].visit_counts).sum()) == B * N
     kernel_split = {}
     if game != "cartpole":
         eng.kernel_timing(True)
@@ -360,19 +356,16 @@ def run_workload(name, args, D, rank, local_rank, world, with_loop, headline):
     table, totals = parallel.gather_counters(D.dist, 0, B * dv["searches"], B * dv["searches"] * N, device=dev)
     total_steps = totals[1]
     hbm_peak, bf16_peak, peak_kind = load_peaks()
-    traffic = load_traffic()
     value = total_steps / wall
     kern_s = kern_ms / 1000.0 / dv["searches"]
     if game == "cartpole":
         # dominant kernel: the fused search kernel, one launch per search (SURVEY 8d: HBM roofline)
         alg_bytes = B * (N * bytes_per_sim + eng.obs_elems * 4 + A * 8 + A * 4 + 8)
         achieved = alg_bytes / kern_s / 1e9
-        tr = traffic.get("fc_search_kernel", {})
-        roofline = {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s",
-                    "frac": achieved / hbm_peak, "traffic": tr.get("dram_bytes_per_launch"), "traffic_source": tr.get("source"),
+        roofline = {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
                     "peak_kind": peak_kind, "kernel": "fc_search_kernel", "algorithmic_bytes_per_launch": alg_bytes,
                     "avg_launch_us": 1e6 * kern_s,
-                    "note": "tree + hidden states live in shared memory for FC nets: measured DRAM traffic is a fraction "
+                    "note": "tree + hidden states live in shared memory for FC nets: DRAM traffic is a fraction "
                             "of the algorithmic bytes, the kernel is issue/latency-bound, not HBM-bound"}
     else:
         # residual nets: tensor roofline (SURVEY 8d) for the dominant kernel, timed live with CUDA event pairs around every
@@ -393,10 +386,7 @@ def run_workload(name, args, D, rank, local_rank, world, with_loop, headline):
         # the dominant class's share of the conv FLOPs ~ its share of the conv time is NOT assumed: classes other than the
         # dominant one only run the stem / DownSample convs, a few % of the FLOPs; achieved uses ALL conv FLOPs over ALL conv time
         achieved = conv_flops / (conv_ms / 1000.0) / 1e12
-        tr = traffic.get(f"{dominant}:{game}@{mode}" if mode else f"{dominant}:{game}") or \
-            traffic.get(f"{dominant}:{game}" if not mode else "", {}) or {}
-        roofline = {"bound": "tensor", "achieved": achieved, "peak": bf16_peak, "unit": "TFLOP/s",
-                    "frac": achieved / bf16_peak, "traffic": tr.get("dram_bytes_per_launch"), "traffic_source": tr.get("source"),
+        roofline = {"bound": "tensor", "achieved": achieved, "peak": bf16_peak, "unit": "TFLOP/s", "frac": achieved / bf16_peak,
                     "peak_kind": peak_kind + " dense bf16 (sustained)",
                     "kernel": dominant, "launches_per_search": dom["launches"],
                     "avg_launch_us": 1000.0 * dom["ms"] / max(dom["launches"], 1),
@@ -436,6 +426,16 @@ def run_workload(name, args, D, rank, local_rank, world, with_loop, headline):
         else:
             os.environ["MZ_TC_MODE"] = prev_mode
     return sub
+
+
+def dump_outputs(out_dir, out):
+    """The arrays of one SearchOutput as out_dir/<field>.npy: floats keep their precision, integers become float32."""
+    os.makedirs(out_dir, exist_ok=True)
+    for field in ("visit_counts", "root_value", "root_predicted_value", "max_tree_depth", "tie_count", "root_priors",
+                  "value_range"):
+        a = getattr(out, field)
+        a = a.cpu().numpy() if hasattr(a, "cpu") else numpy.asarray(a)
+        numpy.save(os.path.join(out_dir, field + ".npy"), a if a.dtype in (numpy.float32, numpy.float64) else a.astype(numpy.float32))
 
 
 def saturation_curve(cfg, spec, N, device, dev):
@@ -514,7 +514,11 @@ def main():
     ap.add_argument("--no-saturation", action="store_true")
     ap.add_argument("--cpu-seconds", type=float, default=12.0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed search of the headline workload returned as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        raise SystemExit("--steps must be at least 1")
     if args.impl == "ours":
         args.warmup = max(args.warmup, 3)
     base = args.workload.partition("@")[0]

@@ -1,5 +1,5 @@
 /*
- * mzb200 - C ABI of the B200-native self-play search library (libmzb200.so).
+ * mzb200 - C ABI of the H100-native self-play search library (libmzb200.so).
  *
  * The reference (werner-duvaud/muzero-general) is pure Python and has no FFI; the drop-in
  * boundary is therefore the set of Python call sites listed next to each entry point below
@@ -215,7 +215,7 @@ double mz_last_search_ms(const MzHandle* h);
 /* Per-kernel-class device timing for the roofline line of bench.py.  While enabled (process-wide), the step-wise
  * pipeline runs launch by launch with a CUDA event pair around every kernel instead of replaying its CUDA graph.
  * mz_kernel_times synchronises and returns the accumulated milliseconds / launch counts since the last call:
- * [0] tree_step_kernel, [1] conv_tower_tc_kernel (tcgen05 towers, resident or streaming), [2] heads_kernel,
+ * [0] tree_step_kernel, [1] conv_tower_tc_kernel (wgmma towers, resident or streaming), [2] heads_kernel,
  * [3] conv3x3_kernel (CUDA cores, one conv per launch), [4] other, [5] small_tower_kernel (fused CUDA-core towers),
  * [6] small_search_kernel (small residual networks: all simulations of a search in one launch). */
 #define MZ_KERNEL_CLASSES 7
@@ -231,7 +231,7 @@ int mz_debug_small_search_plan(int32_t H, int32_t W, int32_t C, int32_t A, int32
                                int32_t heads_floats, int32_t scratch_floats, int32_t cap_channels, int64_t* plan);
 
 /* Debug / parity: one conv3x3 (C -> C, stride 1, pad 1; models.py:206-209) with optional bias, residual and
- * ReLU on host NCHW fp32 data, through the CUDA-core kernel (use_tensor_cores = 0) or the tcgen05 implicit
+ * ReLU on host NCHW fp32 data, through the CUDA-core kernel (use_tensor_cores = 0) or the wgmma implicit
  * GEMM (C = 64, H <= 6, W <= 7): 1 = fp16 operands, 2 = split fp16+bf16 operands with three partial products
  * (fp32-grade, the default of the search path).  w is [C][C][3][3] as in the reference state_dict. */
 int mz_debug_conv3x3(int device, int32_t n, int32_t C, int32_t H, int32_t W, const float* x, const float* w,

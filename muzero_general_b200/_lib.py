@@ -154,7 +154,7 @@ def load_library():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing. Build it with `python -m muzero_general_b200.build` "
-            "(nvcc, sm_100a). There is no CPU fallback.")
+            "(nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, restype, argtypes in SYMBOLS:
         fn = getattr(lib, name)          # AttributeError if the ABI and the binary disagree

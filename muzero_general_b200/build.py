@@ -1,4 +1,4 @@
-"""Builds libmzb200.so in-tree with nvcc for sm_100a (no torch involved)."""
+"""Builds libmzb200.so in-tree with nvcc for sm_90a (no torch involved)."""
 import os
 import subprocess
 import sys
@@ -9,7 +9,7 @@ LIB = os.path.join(HERE, "libmzb200.so")
 SOURCES = ["abi.cu", "ktimer.cu", "fc_search.cu", "fc_infer.cu", "tree_kernels.cu", "tree_wide.cu", "pipeline.cu", "resnet.cu", "conv_tc.cu", "conv_x3.cu", "small_tower.cu", "small_search.cu", "selfplay.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-fmad=false", "-diag-suppress", "177",                     # tree arithmetic must never be contracted; FMAs are explicit fmaf()
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O2", "--expt-relaxed-constexpr",
 ] + os.environ.get("MZ_NVCC_EXTRA", "").split()        # e.g. -DMZ_DUAL_ISSUER for the experiment in conv_tc.cu
@@ -42,7 +42,7 @@ def build(force=False, verbose=False):
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed")
-    subprocess.check_call([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+    subprocess.check_call([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB
 
 

@@ -397,7 +397,7 @@ static int search_partitions(MzHandle* h, int n, int continue_from) {
     const int forced = penv ? atoi(penv) : 0;
     if (forced == 1 || continue_from > 0 || h->net.kind != MZ_NET_RESNET || h->net.action_space > 32 || !h->res) return 1;
     if (!resnet_can_partition(h->res)) return 1;
-    // default: two branches, four from 1024 games on (Connect4 1024 games, N = 200: 43.3 / 39.4 / 38.8 ms per search with 1 / 2 / 4)
+    // default: two branches, four from 1024 games on
     int parts = forced > 1 ? std::min(forced, (int)MzHandle::kMaxParts) : (n >= 1024 ? 4 : 2);
     if (forced <= 1 && !resnet_uses_tensor_cores(h->res)) return 1;          // default: the tensor-core towers only
     while (parts > 1 && n < parts * 64) --parts;

@@ -1,34 +1,31 @@
-// conv3x3 (C -> C, stride 1, pad 1) as an implicit GEMM on the 5th-generation tensor cores.
+// conv3x3 (C -> C, stride 1, pad 1) as an implicit GEMM on the Hopper tensor cores (wgmma).
 //
 // Used for the residual towers of board-sized states (H <= 6, W <= 7, C = 64: Connect4,
 // models.py:213-229 inside representation / dynamics / prediction).  Two kernels share the MMA loop:
 //
-//   conv_tower_resident_kernel   up to 4 tiles per CTA (1184 boards on 148 SMs): the activations of a CTA's tiles stay
+//   conv_tower_resident_kernel   up to 4 tiles per CTA (1056 boards on 132 SMs): the activations of a CTA's tiles stay
 //                                in shared memory through all layers of a tower (see the comment above the kernel)
 //   conv_tower_tc_kernel         larger batches / single convs: activations stream through L2, per CTA
 //
-//     weights  [tap 9][cout C][cin C] fp16, BN folded, 128B-swizzled   shared memory (bulk copy), two slot sets
-//     A tile   two boards = 128 rows of the "P64S" layout    2-stage ring, one 8 KB cp.async.bulk per board
-//     D        128 x 64 fp32 accumulator                     TMEM, double buffered
-//     out      two output tiles staged in shared memory      one 8 KB bulk store per board (dedicated warp)
+//     weights  [tap 9][cout C][cin C] fp16, BN folded, 128B-swizzled   shared memory (bulk copy)
+//     A tile   two boards = 128 rows of the "P64S" layout               one 8 KB cp.async.bulk per board
+//     D        64 x 64 fp32 accumulator per board                       registers of the board's warpgroup
 //
-// Operands are fp16 (10-bit mantissa - the same as tf32 - with fp32 accumulation): one tcgen05.mma
-// consumes K = 16 channels per 32-byte operand row, so a tile needs 36 MMAs instead of the 72 a tf32
-// formulation needs, and every activation / weight byte moved through L2 and shared memory is halved.
-// Measured motivation: profiles/r01_conv_tc_bottleneck.md (the M128 x N64 MMA is operand-fetch bound).
+// Operands are fp16 (10-bit mantissa - the same as tf32 - with fp32 accumulation): one wgmma consumes K = 16
+// channels per 32-byte operand row, so a board needs 36 m64n64k16 MMAs per layer, and every activation / weight byte
+// moved through L2 and shared memory is half of what a tf32 formulation moves.
 //
 // P64S activation layout (HBM and shared): a board is 64 positions p = (y+1)*8 + x (row 0, rows H+1.. and columns
 // W..7 are zero padding), every position one 128-byte row of 64 fp16 channels whose eight 16-byte chunks are stored
-// XOR-ed with p % 8 - i.e. the boards sit in HBM already in the UMMA K-major SWIZZLE_128B shared-memory image, so a
-// plain 1-D bulk copy lands them ready for the tensor core.  Filter tap (dy,dx) is the SAME shared-memory tile with
-// its start address moved by (dy*8+dx) rows (the hardware swizzles on absolute address bits, so base_offset stays 0):
-// the implicit GEMM needs no im2col copy.  Epilogue warps read the accumulator with tcgen05.ld, add the folded-BN
-// bias, the optional residual and the optional action-plane term (models.py:557-572 folded into a per-position
-// table), apply ReLU, zero the padding positions, convert to fp16 (round to nearest, saturating) and store P64S again.
+// XOR-ed with p % 8 - i.e. the boards sit in HBM already in the K-major SWIZZLE_128B shared-memory image of a wgmma
+// operand, so a plain 1-D bulk copy lands them ready for the tensor core.  Filter tap (dy,dx) is the SAME shared-memory
+// tile with its start address moved by (dy*8+dx) rows (the hardware swizzles on absolute address bits): the implicit
+// GEMM needs no im2col copy.  The epilogue works on the accumulator registers: folded-BN bias, the optional residual
+// and the optional action-plane term (models.py:557-572 folded into a per-position table), ReLU, zero padding
+// positions, convert to fp16 (round to nearest, saturating) and store P64S again.
 //
-// Warp roles (384 threads): 0 = bulk-copy producer, 1 = MMA issuer (one elected thread issues every tcgen05.mma of
-// the CTA), 2 = TMEM allocator, 3 = output store (bulk copies shared -> global), 4..11 = epilogue (TMEM lane quarter
-// = warp % 4; streaming kernel: accumulator column half = (warp - 4) / 4, resident kernel: tile parity = (warp - 4) / 4).
+// Warp roles: warpgroup b (warps 4b..4b+3) multiplies and finishes board b of every tile (M = 64 = one board), one
+// more warp is the bulk-copy producer; the streaming kernel has a further warp for the output bulk stores.
 #include <cuda_fp16.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -46,20 +43,19 @@ using namespace tc;
 
 constexpr int kC = 64;                 // channels in = out
 constexpr int kPos = 64;               // positions per board (8 x 8 padded grid)
-constexpr int kBoards = 2;             // boards per tile -> M = 128
+constexpr int kBoards = 2;             // boards per tile, one per consumer warpgroup
 constexpr int kHalo = 16;              // zero rows above / below the tile (|shift| <= 9; multiple of 8 keeps the swizzle phase)
 constexpr int kRows = kBoards * kPos + 2 * kHalo;      // 160 rows
 constexpr int kRowBytes = kC * 2;                      // 128 B: one position, 64 fp16 channels = one 128B-swizzle row
-constexpr int kPlanes = kC / 8;                        // 8 sixteen-byte chunks per row
 constexpr int kStageBytes = kRows * kRowBytes;         // 20480
 constexpr int kStages = 2;
 constexpr int kTapBytes = kC * kRowBytes;               // 8192: [cout 64][128 B]
 constexpr int kWBytes = 9 * kTapBytes;                 // 73728
 constexpr int kOutBytes = kBoards * kPos * kRowBytes;  // 16384: one output tile in the global board layout
 constexpr int kBoardHalves = kC * kPos;                // 4096 fp16 per board
-constexpr int kAccCols = 64;
-constexpr int kThreads = 384;             // 4 control warps + 8 epilogue warps
-constexpr int kEpiWarps = 8;
+constexpr int kConsumerWarps = 4 * kBoards;            // two warpgroups
+constexpr int kThreads = 32 * kConsumerWarps + 64;     // + producer warp + store warp
+constexpr int kThreadsR = 32 * kConsumerWarps + 32;    // resident kernel: + producer warp
 
 struct Smem {
     // offsets
@@ -68,33 +64,36 @@ struct Smem {
     static constexpr int out = a + kStages * kStageBytes;                  // 2 output tiles (2 boards x 8 KB) staged for the bulk store
     static constexpr int bias = out + 2 * kOutBytes;                       // [kTowerMaxLayers][64] floats
     static constexpr int bars = bias + kTowerMaxLayers * kC * 4;           // 8-byte aligned
-    static constexpr int tmem_ptr = bars + 64 * 8;
-    static constexpr int total = tmem_ptr + 16;
+    static constexpr int total = bars + 64 * 8;
 };
 static_assert(Smem::total <= 232448, "shared memory budget");
 
-// kind::f16 with fp16 operands (format 0), fp32 accumulate, A and B K-major, M = 128, N = 64
-// (cute::UMMA::InstrDescriptor)
-constexpr uint32_t kIdesc = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(kAccCols >> 3) << 17) | ((128u >> 4) << 24);
-
-MZ_DEVINL void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(kIdesc), "r"(accumulate) : "memory");
+// The 36 MMAs of one board and one layer: D = sum over taps and 16-channel K steps of the shifted board window times
+// the tap's weights.  a16 / w16: descriptor low words of the board's row 0 and of tap 0 of the weight set.
+MZ_DEVINL void board_conv(float* d, uint32_t a16, uint32_t w16, uint32_t bar_w_full0, int wait_weights, uint32_t w_parity) {
+    wgmma_fence();
+#pragma unroll
+    for (int tap = 0; tap < 9; ++tap) {
+        if (wait_weights) mbar_wait(bar_w_full0 + 8u * tap, w_parity);
+        constexpr int kRow16 = kRowBytes / 16;                       // 8 sixteen-byte units per row
+        const int shift = (tap / 3 - 1) * 8 + (tap % 3 - 1);         // compile-time after unrolling
+#pragma unroll
+        for (int ks = 0; ks < kC / 16; ++ks)                         // K = 16 channels = 32 bytes of the row
+            wgmma_m64n64k16(d, a16 + (uint32_t)(shift * kRow16 + ks * 2), w16 + (uint32_t)(tap * (kTapBytes / 16) + ks * 2),
+                            (tap | ks) != 0);                        // start addresses < 2^14 units: no carry into the flags
+    }
+    wgmma_commit();
+    wgmma_wait_all();
 }
-MZ_DEVINL void umma_f16_words(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "mov.b64 da, {%1, %5};\n\t"
-        "mov.b64 db, {%2, %5};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t"
-        "}" ::"r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(kIdesc), "r"(accumulate), "r"(kDescHi) : "memory");
+
+// bias + residual + action term + ReLU of one accumulator pair, packed to fp16x2 (the inputs of a padding position are
+// irrelevant: callers store zero there)
+MZ_DEVINL uint32_t finish_pair(float d0, float d1, const float* bias, uint32_t res, const float* atab, float act_scale, int relu) {
+    const float2 rf = unpack_f16x2(res);
+    float r0 = d0 + bias[0] + rf.x, r1 = d1 + bias[1] + rf.y;
+    if (atab) { r0 = fmaf(act_scale, atab[0], r0); r1 = fmaf(act_scale, atab[1], r1); }
+    if (relu) { r0 = fmaxf(r0, 0.0f); r1 = fmaxf(r1, 0.0f); }
+    return pack_f16x2(r0, r1);
 }
 }  // namespace
 
@@ -118,12 +117,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tower_tc_kernel(const __grid
     auto bar_w_empty = [&](int set, int tap) { return bars + 8u * (18 + set * 9 + tap); };    // last MMA of the layer on this tap done
     auto bar_a_full = [&](int s) { return bars + 8u * (36 + s); };
     auto bar_a_empty = [&](int s) { return bars + 8u * (38 + s); };
-    auto bar_acc_full = [&](int s) { return bars + 8u * (40 + s); };
-    auto bar_acc_empty = [&](int s) { return bars + 8u * (42 + s); };
     auto bar_tile_done = [&](int k) { return bars + 8u * (44 + k); };      // layer output of my k-th tile stored
     auto bar_out_full = [&](int st) { return bars + 8u * (52 + st); };     // output tile staged in shared memory
     auto bar_out_empty = [&](int st) { return bars + 8u * (54 + st); };    // ... and drained by the bulk store
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + Smem::tmem_ptr);
 
     const int n_tiles = (a.n + kBoards - 1) / kBoards;
     const int my_tiles = ((int)blockIdx.x < n_tiles) ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
@@ -141,31 +137,21 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tower_tc_kernel(const __grid
         s_bias[i] = b ? b[i % kC] : 0.0f;
     }
     if (threadIdx.x == 0) {
-        for (int t = 0; t < 18; ++t) { mbar_init(bar_w_full(t / 9, t % 9), 1); mbar_init(bar_w_empty(t / 9, t % 9), 1); }
+        for (int t = 0; t < 18; ++t) { mbar_init(bar_w_full(t / 9, t % 9), 1); mbar_init(bar_w_empty(t / 9, t % 9), kConsumerWarps); }
         for (int s = 0; s < kStages; ++s) {
             mbar_init(bar_a_full(s), 1);
-            mbar_init(bar_a_empty(s), 1);
-            mbar_init(bar_acc_full(s), 1);
-            mbar_init(bar_acc_empty(s), kEpiWarps);   // one arrival per epilogue warp
+            mbar_init(bar_a_empty(s), kConsumerWarps);   // one arrival per consumer warp
         }
         for (int k = 0; k < kTowerMaxTiles; ++k) mbar_init(bar_tile_done(k), 1);
-        for (int st = 0; st < 2; ++st) { mbar_init(bar_out_full(st), kEpiWarps); mbar_init(bar_out_empty(st), 1); }
+        for (int st = 0; st < 2; ++st) { mbar_init(bar_out_full(st), kConsumerWarps); mbar_init(bar_out_empty(st), 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic zero-fill -> async proxy readers
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(s_base + Smem::tmem_ptr), "r"(2 * kAccCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_launch_dependents();
     pdl_wait();
 
-    if (warp == 0) {
+    if (warp == kConsumerWarps) {
         // ================= producer =================
         int it = 0;
         // weights: two sets of nine tap slots; layer l uses set l & 1 and is loaded one layer ahead, as soon as the
@@ -205,127 +191,75 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tower_tc_kernel(const __grid
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        int it = 0;
-        for (int l = 0; l < L; ++l) {
-            for (int k = 0; k < my_tiles; ++k, ++it) {
-                const int s = it % kStages;
-                const uint32_t ph = (it / kStages) & 1;
-                mbar_wait(bar_acc_empty(s), ph ^ 1);
-                mbar_wait(bar_a_full(s), ph);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint32_t d = tmem_base + (uint32_t)(s * kAccCols);
-                    // Descriptors differ only in the 14-bit start-address field: build the constant words once and
-                    // derive every MMA's descriptor with one add (the single issuing thread is latency-bound, so the
-                    // instruction count per MMA is what sets the tensor-pipe duty cycle).
-                    const uint32_t a16 = ((s_a + s * kStageBytes + kHalo * kRowBytes) >> 4) | kDescLoFlags;     // tile row 0, in 16-byte units
-                    const uint32_t w16 = ((s_w + (uint32_t)((l & 1) * kWBytes)) >> 4) | kDescLoFlags;
-                    uint32_t acc = 0;
-#pragma unroll
-                    for (int tap = 0; tap < 9; ++tap) {
-                        if (a.debug_skip & 1) break;
-                        if (k == 0) { mbar_wait(bar_w_full(l & 1, tap), (uint32_t)((l >> 1) & 1)); tc_fence_after(); }
-                        constexpr int kRow16 = kRowBytes / 16;                       // 8 sixteen-byte units per row
-                        const int shift = (tap / 3 - 1) * 8 + (tap % 3 - 1);         // compile-time after unrolling
-#pragma unroll
-                        for (int ks = 0; ks < kC / 16; ++ks) {                       // K = 16 channels = 32 bytes of the row
-                            const uint32_t alo = a16 + (uint32_t)(shift * kRow16 + ks * 2);      // < 2^14: never carries into the flag bits
-                            const uint32_t blo = w16 + (uint32_t)(tap * (kTapBytes / 16) + ks * 2);
-                            umma_f16_words(d, alo, blo, acc);
-                            acc = 1;
-                        }
-                        if (k == my_tiles - 1) umma_commit(bar_w_empty(l & 1, tap));   // slot reusable by layer l + 2
-                    }
-                    if (a.debug_skip & 1) { if (k == my_tiles - 1) for (int tap = 0; tap < 9; ++tap) umma_commit(bar_w_empty(l & 1, tap)); }
-                    umma_commit(bar_a_empty(s));          // smem stage reusable once the MMAs have read it
-                    umma_commit(bar_acc_full(s));         // accumulator complete
-                }
-                __syncwarp();
-            }
-        }
-    } else if (warp >= 4) {
-        // ================= epilogue =================
-        const int q = warp & 3;                       // TMEM lane quarter
-        const int half = (warp - 4) >> 2;             // accumulator columns [32*half, 32*half+32)
-        const int row = q * 32 + lane;                // tile row = TMEM lane
-        const int b = row / kPos, p = row % kPos;
-        const int y = p / 8 - 1, x = p % 8;
-        const bool inside = (y >= 0 && y < a.H && x < a.W);
-        constexpr int kJ = kPlanes / 2;               // 16-byte chunks (8 channels) handled by this warp: 32 channels
-        const size_t row_off = (size_t)p * kC;        // this position's 128-byte row, in fp16 elements
-        const int sw = p & 7;                         // chunk c of the row is stored at chunk c ^ sw
+    } else if (warp < kConsumerWarps) {
+        // ================= MMA + epilogue: warpgroup wg owns board wg of every tile =================
+        const int wg = warp >> 2;
+        const int r0 = 16 * (warp & 3) + (lane >> 2);  // this thread's accumulator rows (board positions): r0, r0 + 8
+        const int cq = 2 * (lane & 3);                 // ... and channels 8 j + cq, 8 j + cq + 1
+        const int sw = lane >> 2;                      // r0 % 8 = (r0 + 8) % 8: chunk c of the row is stored at chunk c ^ sw
         int it = 0;
         for (int l = 0; l < L; ++l) {
             const TowerLayer& ly = a.layer[l];
-            const float* bias = s_bias + l * kC + half * 32;
+            const float* bias = s_bias + l * kC;
             for (int k = 0; k < my_tiles; ++k, ++it) {
                 const int tile = blockIdx.x + k * gridDim.x;
                 const int s = it % kStages;
                 const uint32_t ph = (it / kStages) & 1;
-                const int g = tile * kBoards + b;
-                const bool live = inside && g < a.n;
+                const int g = tile * kBoards + wg;
                 // ---- prefetch everything that does not depend on the accumulator
-                uint4 res[kJ];                          // residual, 8 fp16 per channel group
+                uint32_t res[2][8];                     // residual, fp16x2 per (row, channel group)
                 float act_scale = 0.0f;
 #pragma unroll
-                for (int j = 0; j < kJ; ++j) res[j] = make_uint4(0, 0, 0, 0);
-                if (live) {
-                    if (ly.res_buf >= 0 && !(a.debug_skip & 8)) {
-                        const __half* rp = tower_board(a, ly.res_buf, g) + row_off;
+                for (int h = 0; h < 2; ++h)
 #pragma unroll
-                        for (int j = 0; j < kJ; ++j) res[j] = __ldcg(reinterpret_cast<const uint4*>(rp + (((half * kJ + j) ^ sw) << 3)));   // written by bulk stores: not through L1
+                    for (int j = 0; j < 8; ++j) res[h][j] = 0u;
+                if (g < a.n) {
+                    if (ly.res_buf >= 0 && !(a.debug_skip & 8)) {
+                        const __half* rp = tower_board(a, ly.res_buf, g);
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+#pragma unroll
+                            for (int j = 0; j < 8; ++j)        // written by bulk stores: not through L1
+                                res[h][j] = __ldcg(reinterpret_cast<const unsigned int*>(rp + (size_t)(r0 + 8 * h) * kC + ((j ^ sw) << 3) + cq));
                     }
                     if (ly.action_table) act_scale = __fdiv_rn((float)a.action[g], (float)a.A);
                 }
-                mbar_wait(bar_acc_full(s), ph);
-                tc_fence_after();
-                uint32_t v[32];
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(s * kAccCols + half * 32);
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                      "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                      "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                      "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                tc_fence_before();
+                mbar_wait(bar_a_full(s), ph);
+                float d[32];
+                if (a.debug_skip & 1) {
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) d[i] = 0.0f;
+                    if (k == 0) for (int tap = 0; tap < 9; ++tap) mbar_wait(bar_w_full(l & 1, tap), (uint32_t)((l >> 1) & 1));
+                } else {
+                    const uint32_t a16 = ((s_a + s * kStageBytes + (kHalo + wg * kPos) * kRowBytes) >> 4) | kDescLoFlags;
+                    const uint32_t w16 = ((s_w + (uint32_t)((l & 1) * kWBytes)) >> 4) | kDescLoFlags;
+                    board_conv(d, a16, w16, bar_w_full(l & 1, 0), k == 0, (uint32_t)((l >> 1) & 1));
+                }
                 __syncwarp();
-                if (lane == 0) mbar_arrive(bar_acc_empty(s));        // accumulator half read: may be overwritten
+                if (lane == 0) {
+                    mbar_arrive(bar_a_empty(s));                   // smem stage reusable: this warp's MMAs have read it
+                    if (k == my_tiles - 1)
+                        for (int tap = 0; tap < 9; ++tap) mbar_arrive(bar_w_empty(l & 1, tap));   // slot reusable by layer l + 2
+                }
                 // the output tile is staged in shared memory in the global board layout and leaves with one bulk store
-                // per board (warp 3): the epilogue never waits for global memory
+                // per board (store warp): the epilogue never waits for global memory
                 const int st = it & 1;
                 mbar_wait(bar_out_empty(st), ((uint32_t)(it >> 1) & 1u) ^ 1u);
                 if (g < a.n) {
-                    unsigned char* dst = smem + Smem::out + st * kOutBytes + (b * kPos + p) * kRowBytes;
-                    const float* atab = ly.action_table ? ly.action_table + (size_t)p * kC + half * 32 : nullptr;
+                    unsigned char* dst = smem + Smem::out + st * kOutBytes + wg * kPos * kRowBytes;
 #pragma unroll
-                    for (int j = 0; j < kJ; ++j) {
-                        uint4 o = make_uint4(0, 0, 0, 0);
-                        if (inside) {
-                            float r[8];
-                            const uint32_t rw[4] = {res[j].x, res[j].y, res[j].z, res[j].w};
+                    for (int h = 0; h < 2; ++h) {
+                        const int p = r0 + 8 * h;
+                        const int y = p / 8 - 1, x = p % 8;
+                        const bool inside = (y >= 0 && y < a.H && x < a.W);
+                        const float* atab = ly.action_table ? ly.action_table + (size_t)p * kC + cq : nullptr;
 #pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const float2 rf = unpack_f16x2(rw[e]);
-                                r[2 * e + 0] = __uint_as_float(v[8 * j + 2 * e + 0]) + bias[8 * j + 2 * e + 0] + rf.x;
-                                r[2 * e + 1] = __uint_as_float(v[8 * j + 2 * e + 1]) + bias[8 * j + 2 * e + 1] + rf.y;
-                            }
-                            if (atab) {
-#pragma unroll
-                                for (int e = 0; e < 8; ++e) r[e] = fmaf(act_scale, atab[8 * j + e], r[e]);
-                            }
-                            if (ly.relu) {
-#pragma unroll
-                                for (int e = 0; e < 8; ++e) r[e] = fmaxf(r[e], 0.0f);
-                            }
-                            o = make_uint4(pack_f16x2(r[0], r[1]), pack_f16x2(r[2], r[3]), pack_f16x2(r[4], r[5]), pack_f16x2(r[6], r[7]));
+                        for (int j = 0; j < 8; ++j) {
+                            const uint32_t o = inside ? finish_pair(d[4 * j + 2 * h], d[4 * j + 2 * h + 1], bias + 8 * j + cq, res[h][j],
+                                                                    atab ? atab + 8 * j : nullptr, act_scale, ly.relu)
+                                                      : 0u;
+                            *reinterpret_cast<uint32_t*>(dst + p * kRowBytes + ((j ^ sw) << 4) + 2 * cq) = o;
                         }
-                        *reinterpret_cast<uint4*>(dst + (((half * kJ + j) ^ sw) << 4)) = o;
                     }
                 }
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic smem writes -> bulk-copy reader
@@ -333,7 +267,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tower_tc_kernel(const __grid
                 if (lane == 0) mbar_arrive(bar_out_full(st));
             }
         }
-    } else if (warp == 3) {
+    } else {
         // ================= output store =================
         if (lane == 0) {
             int it = 0;
@@ -367,24 +301,19 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tower_tc_kernel(const __grid
             }
         }
     }
-    // ---- teardown
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2 * kAccCols) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // Resident tower: the same convolutions, but the activations of a CTA's tiles never leave shared memory between the
 // layers.  Two activation buffers B0 / B1 hold the CTA's (up to kResTiles) tiles back to back in the board layout
-// (consecutive boards are separated by their own zero padding rows, so a tap window that leaves a board only reads
-// zeros); layer l reads B[l & 1] and writes B[(l & 1) ^ 1]; the second conv of a block adds the residual IN PLACE (the
-// block input is what the output buffer still holds, and a row is read and overwritten by the same thread).  Global
-// memory is touched three times per tower: bulk loads of the input boards, the weight taps (one slot set, refilled
-// for layer l+1 while the last tile of layer l multiplies), bulk stores of the last layer's tiles.  There is no
-// activation ring, no per-tile store fence and no "tile stored" handshake: MMA(l+1, k) only waits for the epilogue
-// of (l, k); write-after-read hazards are excluded by the in-order completion of the MMAs (the epilogue of layer
-// l+2 starts after a tcgen05.commit that follows every MMA of layer l+1).
+// (consecutive boards are separated by their own zero padding rows, so a tap window of a real position never leaves
+// its board); layer l reads B[l & 1] and writes B[(l & 1) ^ 1]; the second conv of a block adds the residual IN PLACE
+// (the block input is what the output buffer still holds, and a row is read and overwritten by the same thread).
+// Global memory is touched three times per tower: bulk loads of the input boards, the weight taps (one slot set,
+// refilled for layer l+1 while the last tile of layer l multiplies), bulk stores of the last layer's boards.  A
+// warpgroup only ever reads the rows of its own boards for the positions it keeps (other boards' rows only enter
+// padding outputs, which are stored as zeros), so the two warpgroups never wait for each other: a warpgroup's own
+// MMA -> epilogue -> next MMA order covers every hazard.
 // ------------------------------------------------------------------------------------------------------------------
 constexpr int kResTiles = 4;
 constexpr int kResRows = kResTiles * kBoards * kPos + 2 * kHalo;      // 544
@@ -395,13 +324,12 @@ struct SmemR {
     static constexpr int act = kWBytes;                                    // B0 | B1
     static constexpr int bias = act + 2 * kResBufBytes;
     static constexpr int bars = bias + kTowerMaxLayers * kC * 4;
-    static constexpr int tmem_ptr = bars + 48 * 8;
-    static constexpr int total = tmem_ptr + 16;
+    static constexpr int total = bars + 32 * 8;
 };
 static_assert(SmemR::total <= 232448, "shared memory budget");
 static_assert(SmemR::act % 1024 == 0 && kResBufBytes % 1024 == 0, "activation buffers must keep the 1024-byte swizzle phase");
 
-__global__ void __launch_bounds__(kThreads, 1) conv_tower_resident_kernel(const __grid_constant__ TowerArgs a) {
+__global__ void __launch_bounds__(kThreadsR, 1) conv_tower_resident_kernel(const __grid_constant__ TowerArgs a) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t s_base = smem_u32(smem);
@@ -411,48 +339,30 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tower_resident_kernel(const 
     auto bar_w_full = [&](int tap) { return bars + 8u * tap; };
     auto bar_w_empty = [&](int tap) { return bars + 8u * (9 + tap); };
     auto bar_in_full = [&](int k) { return bars + 8u * (18 + k); };         // input boards of my k-th tile landed
-    auto bar_tile_ready = [&](int k) { return bars + 8u * (22 + k); };      // epilogue of (layer, k) wrote its rows (one phase per layer)
-    auto bar_out_ready = [&](int k) { return bars + 8u * (26 + k); };       // last layer's rows of tile k written
-    auto bar_acc_full = [&](int s) { return bars + 8u * (30 + s); };
-    auto bar_acc_empty = [&](int s) { return bars + 8u * (32 + s); };
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + SmemR::tmem_ptr);
 
     const int n_tiles = (a.n + kBoards - 1) / kBoards;
     const int my_tiles = ((int)blockIdx.x < n_tiles) ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
     const int L = a.n_layers;
 
-    // ---- one-time setup: zero halos of both buffers, biases, barriers, TMEM
-    for (int i = threadIdx.x; i < 2 * 2 * kHalo * (kRowBytes / 16); i += kThreads) {
+    // ---- one-time setup: zero halos of both buffers, biases, barriers
+    for (int i = threadIdx.x; i < 2 * 2 * kHalo * (kRowBytes / 16); i += kThreadsR) {
         const int chunk = i % (kRowBytes / 16), r = (i / (kRowBytes / 16)) % (2 * kHalo), bf = i / ((kRowBytes / 16) * 2 * kHalo);
         const int row = r < kHalo ? r : kResRows - 2 * kHalo + r;
         reinterpret_cast<uint4*>(smem + SmemR::act + bf * kResBufBytes + row * kRowBytes)[chunk] = make_uint4(0, 0, 0, 0);
     }
-    for (int i = threadIdx.x; i < L * kC; i += kThreads) {
+    for (int i = threadIdx.x; i < L * kC; i += kThreadsR) {
         const float* b = a.layer[i / kC].bias;
         s_bias[i] = b ? b[i % kC] : 0.0f;
     }
     if (threadIdx.x == 0) {
-        for (int t = 0; t < 9; ++t) { mbar_init(bar_w_full(t), 1); mbar_init(bar_w_empty(t), 1); }
-        for (int k = 0; k < kResTiles; ++k) {
-            mbar_init(bar_in_full(k), 1);
-            mbar_init(bar_tile_ready(k), kEpiWarps / 2);
-            mbar_init(bar_out_ready(k), kEpiWarps / 2);
-        }
-        for (int s = 0; s < 2; ++s) { mbar_init(bar_acc_full(s), 1); mbar_init(bar_acc_empty(s), kEpiWarps / 2); }
+        for (int t = 0; t < 9; ++t) { mbar_init(bar_w_full(t), 1); mbar_init(bar_w_empty(t), kConsumerWarps); }
+        for (int k = 0; k < kResTiles; ++k) mbar_init(bar_in_full(k), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(s_base + SmemR::tmem_ptr), "r"(2 * kAccCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == kConsumerWarps) {
         // ================= producer: weights of every layer, input boards once =================
         pdl_launch_dependents();
         if (my_tiles > 0 && lane < 9) {
@@ -481,148 +391,64 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tower_resident_kernel(const 
             }
             __syncwarp();
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        int it = 0;
-        for (int l = 0; l < L; ++l) {
-            for (int k = 0; k < my_tiles; ++k, ++it) {
-                const int s = it & 1;
-                const uint32_t ph = (uint32_t)(it >> 1) & 1u;
-                if (l == 0) mbar_wait(bar_in_full(k), 0);
-                else mbar_wait(bar_tile_ready(k), (uint32_t)((l - 1) & 1));
-                mbar_wait(bar_acc_empty(s), ph ^ 1);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint32_t d = tmem_base + (uint32_t)(s * kAccCols);
-                    const uint32_t a16 = ((s_act + (uint32_t)((l & 1) * kResBufBytes + (kHalo + k * kBoards * kPos) * kRowBytes)) >> 4) | kDescLoFlags;
-                    const uint32_t w16 = (s_w >> 4) | kDescLoFlags;
-                    uint32_t acc = 0;
-#pragma unroll
-                    for (int tap = 0; tap < 9; ++tap) {
-                        if (a.debug_skip & 1) break;
-                        if (k == 0) { mbar_wait(bar_w_full(tap), (uint32_t)(l & 1)); tc_fence_after(); }
-                        constexpr int kRow16 = kRowBytes / 16;
-                        const int shift = (tap / 3 - 1) * 8 + (tap % 3 - 1);
-#pragma unroll
-                        for (int ks = 0; ks < kC / 16; ++ks) {
-                            const uint32_t alo = a16 + (uint32_t)(shift * kRow16 + ks * 2);      // < 2^14: never carries into the flag bits
-                            const uint32_t blo = w16 + (uint32_t)(tap * (kTapBytes / 16) + ks * 2);
-                            umma_f16_words(d, alo, blo, acc);
-                            acc = 1;
-                        }
-                        if (k == my_tiles - 1) umma_commit(bar_w_empty(tap));
-                    }
-                    if (a.debug_skip & 1) { if (k == my_tiles - 1) for (int tap = 0; tap < 9; ++tap) umma_commit(bar_w_empty(tap)); }
-                    umma_commit(bar_acc_full(s));
-                }
-                __syncwarp();
-            }
-        }
-    } else if (warp == 3) {
-        // ================= output store: the last layer's tiles leave as bulk copies =================
-        if (lane == 0) {
-            __half* out = reinterpret_cast<__half*>(a.buf[a.layer[L - 1].out_buf]);
-            const uint32_t src = s_act + (uint32_t)((((L - 1) & 1) ^ 1) * kResBufBytes + kHalo * kRowBytes);
-            for (int k = 0; k < my_tiles; ++k) {
-                const int tile = blockIdx.x + k * gridDim.x;
-                const int nb = min(kBoards, a.n - tile * kBoards);
-                mbar_wait(bar_out_ready(k), 0);
-                if (!(a.debug_skip & 4))
-                    for (int b = 0; b < nb; ++b)
-                        bulk_s2g(out + (size_t)(tile * kBoards + b) * kBoardHalves, src + (uint32_t)((k * kBoards + b) * kPos * kRowBytes),
-                                 kPos * kRowBytes);
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            }
-            asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-        }
-    } else if (warp >= 4) {
-        // ================= epilogue: two groups of four warps, group s owns accumulator stage s =================
+    } else {
+        // ================= MMA + epilogue: warpgroup wg owns board wg of every tile =================
         pdl_wait();                                    // reads a.action (written by the tree kernel)
-        // (consecutive tiles are drained by different groups, so the wait -> tcgen05.ld -> store -> fence -> arrive
-        // chain of one tile overlaps the next tile's)
-        const int q = warp & 3;                       // TMEM lane quarter
-        const int grp = (warp - 4) >> 2;              // tiles with (it & 1) == grp
-        const int row = q * 32 + lane;                // tile row = TMEM lane
-        const int b = row / kPos, p = row % kPos;
-        const int y = p / 8 - 1, x = p % 8;
-        const bool inside = (y >= 0 && y < a.H && x < a.W);
-        const int sw = p & 7;                         // chunk c of the row is stored at chunk c ^ sw
-        int it = 0;
+        const int wg = warp >> 2;
+        const int r0 = 16 * (warp & 3) + (lane >> 2);  // accumulator rows r0, r0 + 8; channels 8 j + cq (+1)
+        const int cq = 2 * (lane & 3);
+        const int sw = lane >> 2;                      // chunk c of the row is stored at chunk c ^ sw
+        const bool store_lead = (threadIdx.x & 127) == 0;
         for (int l = 0; l < L; ++l) {
             const TowerLayer& ly = a.layer[l];
             const float* bias = s_bias + l * kC;
             const bool last = l == L - 1;
-            for (int k = 0; k < my_tiles; ++k, ++it) {
-                if ((it & 1) != grp) continue;
+            for (int k = 0; k < my_tiles; ++k) {
                 const int tile = blockIdx.x + k * gridDim.x;
-                const int s = grp;
-                const uint32_t ph = (uint32_t)(it >> 1) & 1u;
-                const int g = tile * kBoards + b;
-                const bool live = inside && g < a.n;
-                // this thread's row in the output buffer (residual source and destination)
-                unsigned char* orow = smem + SmemR::act + ((l & 1) ^ 1) * kResBufBytes + (kHalo + k * kBoards * kPos + row) * kRowBytes;
+                const int g = tile * kBoards + wg;
+                const int brow = kHalo + (k * kBoards + wg) * kPos;               // row 0 of my board in a buffer
                 float act_scale = 0.0f;
-                if (live && ly.action_table) act_scale = __fdiv_rn((float)a.action[g], (float)a.A);
-                mbar_wait(bar_acc_full(s), ph);
-                tc_fence_after();
-                uint32_t v[64];
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(s * kAccCols);
+                if (g < a.n && ly.action_table) act_scale = __fdiv_rn((float)a.action[g], (float)a.A);
+                if (l == 0) mbar_wait(bar_in_full(k), 0);
+                float d[32];
+                if (a.debug_skip & 1) {
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) d[i] = 0.0f;
+                    if (k == 0) for (int tap = 0; tap < 9; ++tap) mbar_wait(bar_w_full(tap), (uint32_t)(l & 1));
+                } else {
+                    const uint32_t a16 = ((s_act + (uint32_t)((l & 1) * kResBufBytes + brow * kRowBytes)) >> 4) | kDescLoFlags;
+                    board_conv(d, a16, (s_w >> 4) | kDescLoFlags, bar_w_full(0), k == 0, (uint32_t)(l & 1));
+                }
+                __syncwarp();
+                if (lane == 0 && k == my_tiles - 1)
+                    for (int tap = 0; tap < 9; ++tap) mbar_arrive(bar_w_empty(tap));
+                unsigned char* ob = smem + SmemR::act + ((l & 1) ^ 1) * kResBufBytes + brow * kRowBytes;   // output board
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
-                    uint32_t* w = v + 32 * h;
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                        : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]),
-                          "=r"(w[8]), "=r"(w[9]), "=r"(w[10]), "=r"(w[11]), "=r"(w[12]), "=r"(w[13]), "=r"(w[14]), "=r"(w[15]),
-                          "=r"(w[16]), "=r"(w[17]), "=r"(w[18]), "=r"(w[19]), "=r"(w[20]), "=r"(w[21]), "=r"(w[22]), "=r"(w[23]),
-                          "=r"(w[24]), "=r"(w[25]), "=r"(w[26]), "=r"(w[27]), "=r"(w[28]), "=r"(w[29]), "=r"(w[30]), "=r"(w[31])
-                        : "r"(taddr + (uint32_t)(32 * h)));
-                }
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_acc_empty(s));        // accumulator rows read: may be overwritten
-                const float* atab = ly.action_table ? ly.action_table + (size_t)p * kC : nullptr;
+                    const int p = r0 + 8 * h;
+                    const int y = p / 8 - 1, x = p % 8;
+                    const bool live = (y >= 0 && y < a.H && x < a.W) && g < a.n;
+                    const float* atab = ly.action_table ? ly.action_table + (size_t)p * kC + cq : nullptr;
 #pragma unroll
-                for (int j = 0; j < kPlanes; ++j) {
-                    uint4* slot = reinterpret_cast<uint4*>(orow + ((j ^ sw) << 4));
-                    uint4 o = make_uint4(0, 0, 0, 0);
-                    if (live) {
-                        uint4 res = make_uint4(0, 0, 0, 0);
-                        if (ly.res_buf >= 0) res = *slot;               // block input, added in place
-                        float r[8];
-                        const uint32_t rw[4] = {res.x, res.y, res.z, res.w};
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const float2 rf = unpack_f16x2(rw[e]);
-                            r[2 * e + 0] = __uint_as_float(v[8 * j + 2 * e + 0]) + bias[8 * j + 2 * e + 0] + rf.x;
-                            r[2 * e + 1] = __uint_as_float(v[8 * j + 2 * e + 1]) + bias[8 * j + 2 * e + 1] + rf.y;
-                        }
-                        if (atab) {
-#pragma unroll
-                            for (int e = 0; e < 8; ++e) r[e] = fmaf(act_scale, atab[8 * j + e], r[e]);
-                        }
-                        if (ly.relu) {
-#pragma unroll
-                            for (int e = 0; e < 8; ++e) r[e] = fmaxf(r[e], 0.0f);
-                        }
-                        o = make_uint4(pack_f16x2(r[0], r[1]), pack_f16x2(r[2], r[3]), pack_f16x2(r[4], r[5]), pack_f16x2(r[6], r[7]));
+                    for (int j = 0; j < 8; ++j) {
+                        uint32_t* slot = reinterpret_cast<uint32_t*>(ob + p * kRowBytes + ((j ^ sw) << 4) + 2 * cq);
+                        uint32_t o = 0u;                                   // zeros on padding rows and missing boards
+                        if (live)
+                            o = finish_pair(d[4 * j + 2 * h], d[4 * j + 2 * h + 1], bias + 8 * j + cq, ly.res_buf >= 0 ? *slot : 0u,
+                                            atab ? atab + 8 * j : nullptr, act_scale, ly.relu);   // residual: the block input, in place
+                        *slot = o;
                     }
-                    *slot = o;                                         // zeros on padding rows and missing boards
                 }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic smem writes -> tcgen05 / bulk-copy readers
-                __syncwarp();
-                if (lane == 0) mbar_arrive(last ? bar_out_ready(k) : bar_tile_ready(k));
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic smem writes -> wgmma / bulk-copy readers
+                warpgroup_sync(wg);
+                if (last && store_lead && g < a.n && !(a.debug_skip & 4)) {
+                    bulk_s2g(reinterpret_cast<__half*>(a.buf[ly.out_buf]) + (size_t)g * kBoardHalves, smem_u32(ob), kPos * kRowBytes);
+                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                }
             }
         }
+        if (store_lead) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
     }
-    // ---- teardown
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2 * kAccCols) : "memory");
 }
 
 // the resident kernel needs the block structure: every residual is the input of the layer before, buffers alternate
@@ -661,7 +487,7 @@ cudaError_t launch_conv_tower_tc(const TowerArgs& a, int sm_count, cudaStream_t 
     }
     if (a.n_layers < 1 || a.n_layers > kTowerMaxLayers) return cudaErrorInvalidValue;
     const int n_tiles = (a.n + kBoards - 1) / kBoards;
-    // two co-resident CTAs per SM (fp16 operands leave room): their MMA streams interleave on the tensor core
+    // up to two co-resident CTAs per SM where shared memory allows (the occupancy query decides)
     const int slots = sm_count * tower_ctas_per_sm();
     const int grid = n_tiles < slots ? n_tiles : slots;
     if (a.n_layers > 1 && (n_tiles + grid - 1) / grid > kTowerMaxTiles) return cudaErrorInvalidConfiguration;
@@ -675,7 +501,7 @@ cudaError_t launch_conv_tower_tc(const TowerArgs& a, int sm_count, cudaStream_t 
             attr_r = true;
         }
         const int grid_r = n_tiles < sm_count ? n_tiles : sm_count;
-        cudaError_t e = launch_chained(conv_tower_resident_kernel, dim3(grid_r), dim3(kThreads), SmemR::total, stream, a);
+        cudaError_t e = launch_chained(conv_tower_resident_kernel, dim3(grid_r), dim3(kThreadsR), SmemR::total, stream, a);
         return e != cudaSuccess ? e : cudaGetLastError();
     }
     cudaError_t e = launch_chained(conv_tower_tc_kernel, dim3(grid), dim3(kThreads), Smem::total, stream, a);

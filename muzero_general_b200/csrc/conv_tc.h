@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM conv3x3 on the P64C8 fp16 board layout (conv_tc.cu).
+// wgmma implicit-GEMM conv3x3 on the P64C8 fp16 board layout (conv_tc.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

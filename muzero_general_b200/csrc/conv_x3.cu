@@ -1,7 +1,7 @@
 // Residual towers on the tensor cores at fp32-grade accuracy ("x3" mode, the default for 64-channel board nets).
 //
-// The reference evaluates its networks in fp32 (models.py:206-231).  A tcgen05 kind::f16 MMA only takes 16-bit
-// operands, so every fp32 operand is split in two 16-bit terms and three of the four partial products are kept:
+// The reference evaluates its networks in fp32 (models.py:206-231).  An f16 wgmma only takes 16-bit operands, so
+// every fp32 operand is split in two 16-bit terms and three of the four partial products are kept:
 //
 //     x = x_h + x_l/2^11   x_h = fp16(x) (11 significant bits),  x_l = fp16((x - x_h) 2^11) (11 more bits; the scale keeps
 //                          the remainder a NORMAL fp16 number wherever x_h is one, so small activations keep 22 bits too)
@@ -9,29 +9,30 @@
 //                          w_h = fp16(w s), w_l = fp16(w s - w_h): 22 significant bits relative to the row maximum
 //     conv = sum x_h w_h + x_h w_l + x_l w_h                    (the dropped x_l w_l term is 2^-22 of |x||w|)
 //
-// Products of 16-bit operands are exact in fp32 and the accumulation in TMEM is fp32, so the result carries ~2^-20
-// relative error per term: the class of an fp32 FMA loop in a different summation order, and two to three orders of
-// magnitude inside the 2e-4 network tolerance of the test-suite.  (kind::f16 takes fp16 or bf16 operands but not one of
-// each - an x_l in bf16 against an fp16 w_h raises an illegal-instruction fault - hence the scaled fp16 remainder.)
-// Activations beyond the fp16 range (|x| > 65504) saturate x_h (and possibly x_l): they leave the accuracy contract,
-// so the epilogue tracks the largest |x| it stores and bumps a counter the host checks after every search
-// (ResNetDevice falls back to the fp32 CUDA-core towers, resnet.cu).
+// Products of 16-bit operands are exact in fp32 and the accumulation is fp32, so the result carries ~2^-20 relative
+// error per term: the class of an fp32 FMA loop in a different summation order, and two to three orders of magnitude
+// inside the 2e-4 network tolerance of the test-suite.  (An f16 MMA takes fp16 or bf16 operands but not one of each,
+// hence the scaled fp16 remainder.)  Activations beyond the fp16 range (|x| > 65504) saturate x_h (and possibly x_l):
+// they leave the accuracy contract, so the epilogue tracks the largest |x| it stores and bumps a counter the host
+// checks after every search (ResNetDevice falls back to the fp32 CUDA-core towers, resnet.cu).
 //
-// Cost: 2 MMAs per 16-channel K-step instead of 1 - the two products that share x_h are ONE M128 x N128 x K16 MMA
-// against [w_h ; w_l] stacked along N (the A tile is fetched from shared memory once), x_l w_h is an M128 x N64 x K16
-// MMA into a third group of 64 accumulator columns; the epilogue forms col[c] + col[64 + c] + col[128 + c] / 2^11.
+// Cost: 3 MMAs per 16-channel K-step instead of 1.  x_h w_h and x_h w_l accumulate into the same registers (both are
+// on the scale of w); x_l w_h goes to a second accumulator, and the epilogue forms acc + acc_l / 2^11.
 //
 // Kernel structure (one CTA per SM, up to two tiles = four boards per CTA, all layers of a tower in one launch):
 //   weights   [9 taps][128 rows: w_h couts | w_l couts][64 cin fp16], 128B-swizzled, 144 KB, ONE slot set refilled
 //             tap by tap for layer l+1 while the last tile of layer l still multiplies
 //   X         the CTA's boards as two swizzled fp16 planes (x_h, x_l), 2 x 36 KB, updated IN PLACE: a layer's
-//             output may overwrite its input because (a) the epilogue of a tile starts after the last MMA that reads
-//             the tile's rows, (b) neighbouring tiles only ever read each other's padding rows, which hold zeros before
-//             and after, and (c) the residual stream lives in the epilogue threads' REGISTERS in fp32 (each thread owns
-//             one board position of one tile through the whole tower), so a block input never has to stay in memory
-//   D         TMEM, 192 columns per tile (tile k starts at column 256 k)
-// Warp roles as in conv_tc.cu: 0 = bulk-copy producer, 1 = MMA issuer (one elected thread), 2 = TMEM allocator,
-// 3 = output store, 4..7 = epilogue of tile 0, 8..11 = epilogue of tile 1.
+//             output may overwrite its input because (a) the warpgroup that owns a board rewrites it only after its own
+//             MMAs on the board have completed, (b) other boards' MMAs only read this board's rows for their padding
+//             outputs, which are stored as zeros, and (c) the residual stream lives in the epilogue threads' REGISTERS
+//             in fp32 (each thread owns two board positions x 16 channels through the whole tower), so a block input
+//             never has to stay in memory
+//   D         registers: 2 x 32 fp32 per thread (m64n64 accumulators of the board's warpgroup)
+// Warp roles: warpgroup 2k + b (warps 4(2k+b)..+3) multiplies and finishes board b of tile k and bulk-stores it after
+// the last layer.  Warp 0 also issues the bulk loads: the inputs and layer 0's weights up front, and layer l+1's weights
+// after its own epilogue of layer l, once every warpgroup has finished its MMAs of layer l (which it has to wait for
+// anyway before it can multiply layer l+1).  A separate producer warp would cap the 128 MMA threads below 128 registers.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <stdio.h>
@@ -50,7 +51,7 @@ using namespace tc;
 
 constexpr int kC = 64;
 constexpr int kPos = 64;
-constexpr int kBoards = 2;                                   // boards per tile -> M = 128
+constexpr int kBoards = 2;                                   // boards per tile
 constexpr int kHalo = 16;
 constexpr int kRowBytes = 128;
 constexpr int kTiles = 2;                                    // tiles per CTA
@@ -60,9 +61,9 @@ constexpr int kTapBytes = 128 * kRowBytes;                   // 16384
 constexpr int kWBytes = 9 * kTapBytes;                       // 147456
 constexpr int kBoardPlane = kPos * kRowBytes;                // 8192: one plane of one board
 constexpr int kBoardBytes = 2 * kBoardPlane;                 // 16384: x_h plane | x_l plane
-constexpr int kAccCols = 256;                                // columns reserved per tile (192 used: x_h w_h | x_h w_l | x_l w_h)
 constexpr float kLoScale = 2048.0f, kLoUnscale = 1.0f / 2048.0f;
-constexpr int kThreads = 384;
+constexpr int kConsumerWarps = 4 * kTiles * kBoards;         // one warpgroup per board
+constexpr int kThreads = 32 * kConsumerWarps;
 
 struct SmemX {
     static constexpr int w = 0;
@@ -71,44 +72,15 @@ struct SmemX {
     static constexpr int bias = lo + kPlaneBytes;                          // [kTowerMaxLayers][64]
     static constexpr int scale = bias + kTowerMaxLayers * kC * 4;          // [kTowerMaxLayers][64]
     static constexpr int bars = scale + kTowerMaxLayers * kC * 4;
-    static constexpr int tmem_ptr = bars + 32 * 8;
-    static constexpr int total = tmem_ptr + 16;
+    static constexpr int total = bars + 32 * 8;
 };
 static_assert(SmemX::total <= 232448, "shared memory budget");
 static_assert(SmemX::hi % 1024 == 0 && SmemX::lo % 1024 == 0, "activation planes must keep the 1024-byte swizzle phase");
-
-// kind::f16, fp32 accumulate, K-major A and B, M = 128.  a_format / b_format: 0 = fp16, 1 = bf16.
-constexpr uint32_t idesc(uint32_t a_fmt, uint32_t b_fmt, uint32_t n) {
-    return (1u << 4) | (a_fmt << 7) | (b_fmt << 10) | ((n >> 3) << 17) | ((128u >> 4) << 24);
-}
-constexpr uint32_t kIdescMain = idesc(0, 0, 128);      // x_h x [w_h ; w_l]
-constexpr uint32_t kIdescLo = idesc(0, 0, 64);         // x_l x w_h
-
-MZ_DEVINL void umma_words(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t idesc_word, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "mov.b64 da, {%1, %5};\n\t"
-        "mov.b64 db, {%2, %5};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t"
-        "}" ::"r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(idesc_word), "r"(accumulate), "r"(kDescHi) : "memory");
-}
 
 // x = x_h + x_l / 2^11 from the two packed planes
 MZ_DEVINL float2 join_split(uint32_t h, uint32_t l) {
     const float2 hf = unpack_f16x2(h), lf = unpack_f16x2(l);
     return make_float2(fmaf(lf.x, kLoUnscale, hf.x), fmaf(lf.y, kLoUnscale, hf.y));
-}
-
-MZ_DEVINL void tmem_ld16(uint32_t taddr, uint32_t* v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
 }
 
 // boards hold two 8 KB planes (x_h | x_l); the host side types the buffers float*: 4096 float slots per board
@@ -134,17 +106,13 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tower_x3_kernel(const __grid
     auto bar_w_full = [&](int tap) { return bars + 8u * tap; };
     auto bar_w_empty = [&](int tap) { return bars + 8u * (9 + tap); };
     auto bar_in_full = [&](int k) { return bars + 8u * (18 + k); };         // input boards of my k-th tile landed
-    auto bar_tile_ready = [&](int k) { return bars + 8u * (20 + k); };      // epilogue of (layer, k) rewrote the tile (one phase per layer)
-    auto bar_out_ready = [&](int k) { return bars + 8u * (22 + k); };       // last layer's rows of tile k written
-    auto bar_acc_full = [&](int k) { return bars + 8u * (24 + k); };
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + SmemX::tmem_ptr);
 
     const int n_tiles = (a.n + kBoards - 1) / kBoards;
     const int tile0 = (int)blockIdx.x * kTiles;
     const int my_tiles = min(kTiles, n_tiles - tile0);
     const int L = a.n_layers;
 
-    // ---- one-time setup: zero halos of both planes, biases / scales, barriers, TMEM
+    // ---- one-time setup: zero halos of both planes, biases / scales, barriers
     for (int i = threadIdx.x; i < 2 * 2 * kHalo * (kRowBytes / 16); i += kThreads) {
         const int chunk = i % (kRowBytes / 16), r = (i / (kRowBytes / 16)) % (2 * kHalo), pl = i / ((kRowBytes / 16) * 2 * kHalo);
         const int row = r < kHalo ? r : kRowsX - 2 * kHalo + r;
@@ -164,37 +132,24 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tower_x3_kernel(const __grid
         s_scale[i] = sc ? sc[i % kC] : 1.0f;
     }
     if (threadIdx.x == 0) {
-        for (int t = 0; t < 9; ++t) { mbar_init(bar_w_full(t), 1); mbar_init(bar_w_empty(t), 1); }
-        for (int k = 0; k < kTiles; ++k) {
-            mbar_init(bar_in_full(k), 1);
-            mbar_init(bar_tile_ready(k), 4);
-            mbar_init(bar_out_ready(k), 4);
-            mbar_init(bar_acc_full(k), 1);
-        }
+        // every warp of the warpgroups with a tile arrives once per layer
+        for (int t = 0; t < 9; ++t) { mbar_init(bar_w_full(t), 1); mbar_init(bar_w_empty(t), 4 * kBoards * my_tiles); }
+        for (int k = 0; k < kTiles; ++k) mbar_init(bar_in_full(k), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(s_base + SmemX::tmem_ptr), "r"(kTiles * kAccCols) : "memory");       // 512 columns: one CTA per SM
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (a.timeline && blockIdx.x == 0 && threadIdx.x == 0) a.timeline[kStampBase + 1] = clock64();
 
+    auto load_weights = [&](int l) {                  // warp 0, lane = tap
+        mbar_expect_tx(bar_w_full(lane), kTapBytes);
+        bulk_g2s(s_w + lane * kTapBytes, reinterpret_cast<const unsigned char*>(a.layer[l].w) + (size_t)lane * kTapBytes, kTapBytes,
+                 bar_w_full(lane));
+    };
     if (warp == 0) {
-        // ================= producer: weights of every layer, input boards once =================
         pdl_launch_dependents();
-        if (my_tiles > 0 && lane < 9) {
-            mbar_expect_tx(bar_w_full(lane), kTapBytes);
-            bulk_g2s(s_w + lane * kTapBytes, reinterpret_cast<const unsigned char*>(a.layer[0].w) + (size_t)lane * kTapBytes, kTapBytes,
-                     bar_w_full(lane));
-        }
+        if (lane < 9) load_weights(0);
         pdl_wait();                                    // weights are constants; the boards come from the previous kernel
-        __syncwarp();
         const int in_buf = a.layer[0].in_buf;
         for (int k = 0; k < my_tiles; ++k) {
             const int b0 = (tile0 + k) * kBoards;
@@ -207,198 +162,147 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tower_x3_kernel(const __grid
                          x3_board(a, in_buf, a.g0 + b0 + b) + pl * kBoardPlane, kBoardPlane, bar_in_full(k));
             }
         }
-        for (int l = 1; l < L; ++l) {
-            if (my_tiles > 0 && lane < 9) {
-                mbar_wait(bar_w_empty(lane), (uint32_t)((l - 1) & 1));        // last tile of layer l-1 is done with this tap
-                mbar_expect_tx(bar_w_full(lane), kTapBytes);
-                bulk_g2s(s_w + lane * kTapBytes, reinterpret_cast<const unsigned char*>(a.layer[l].w) + (size_t)lane * kTapBytes,
-                         kTapBytes, bar_w_full(lane));
+        __syncwarp();
+    }
+    // ================= MMA + epilogue: warpgroup wg owns board wg & 1 of tile wg >> 1, for the whole tower =================
+    const int wg = warp >> 2;
+    const int k = wg >> 1, b = wg & 1;
+    if (k >= my_tiles) return;
+    pdl_wait();                                        // reads a.action (written by the tree kernel)
+    const int r0 = 16 * (warp & 3) + (lane >> 2);      // accumulator rows (board positions) r0, r0 + 8; channels 8 j + cq (+1)
+    const int cq = 2 * (lane & 3);
+    const int sw = lane >> 2;                          // chunk c of the row is stored at chunk c ^ sw
+    const int gl = (tile0 + k) * kBoards + b;          // board inside this launch
+    const int g = a.g0 + gl;
+    const bool stamp = a.timeline && blockIdx.x == 0 && b == 0 && (threadIdx.x & 127) == 0;
+    const int brow = kHalo + (k * kBoards + b) * kPos;
+    bool live[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int p = r0 + 8 * h, y = p / 8 - 1, x = p % 8;
+        live[h] = (y >= 0 && y < a.H && x < a.W) && gl < a.n;
+    }
+    // this thread's 4-byte slot (row r0 + 8 h, channels 8 j + cq, +1) in a plane; i = 4 j + 2 h + e indexes the accumulators
+    auto slot_off = [&](int h, int j) { return (brow + r0 + 8 * h) * kRowBytes + ((j ^ sw) << 4) + 2 * cq; };
+    float res[32];                                     // residual stream of this thread's positions / channels, fp32
+#pragma unroll
+    for (int i = 0; i < 32; ++i) res[i] = 0.0f;
+    float peak = 0.0f;                                 // largest |activation| this thread read or stored
+    const bool res_from_input = L >= 2 && a.layer[1].res_buf >= 0;      // the tower starts with a block
+    const bool res_external = a.layer[0].res_buf >= 0;                  // single conv with a residual (debug entry)
+    mbar_wait(bar_in_full(k), 0);
+    if (res_from_input && gl < a.n) {                  // a missing board's rows were never loaded
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const float2 xf = join_split(*reinterpret_cast<const uint32_t*>(smem + SmemX::hi + slot_off(h, j)),
+                                             *reinterpret_cast<const uint32_t*>(smem + SmemX::lo + slot_off(h, j)));
+                res[4 * j + 2 * h] = xf.x;
+                res[4 * j + 2 * h + 1] = xf.y;
+                peak = fmaxf(peak, fmaxf(fabsf(xf.x), fabsf(xf.y)));
+            }
+    } else if (res_external && gl < a.n) {
+        const unsigned char* rb = x3_board(a, a.layer[0].res_buf, g);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int off = (r0 + 8 * h) * kRowBytes + ((j ^ sw) << 4) + 2 * cq;
+                const float2 xf = join_split(__ldg(reinterpret_cast<const unsigned int*>(rb + off)),
+                                             __ldg(reinterpret_cast<const unsigned int*>(rb + kBoardPlane + off)));
+                res[4 * j + 2 * h] = xf.x;
+                res[4 * j + 2 * h + 1] = xf.y;
+                peak = fmaxf(peak, fmaxf(fabsf(xf.x), fabsf(xf.y)));
+            }
+    }
+    const uint32_t ah16 = ((s_hi + (uint32_t)(brow * kRowBytes)) >> 4) | kDescLoFlags;
+    const uint32_t al16 = ((s_lo + (uint32_t)(brow * kRowBytes)) >> 4) | kDescLoFlags;
+    const uint32_t w16 = (s_w >> 4) | kDescLoFlags;
+    for (int l = 0; l < L; ++l) {
+        const TowerLayer& ly = a.layer[l];
+        const float* bias = s_bias + l * kC;
+        const float* scale = s_scale + l * kC;
+        const bool last = l == L - 1;
+        const bool add_res = ly.res_buf >= 0;
+        const bool keep = l + 2 < L && a.layer[l + 2].res_buf >= 0;     // this output is the input of a block
+        float act_scale = 0.0f;
+        if (gl < a.n && ly.action_table) act_scale = __fdiv_rn((float)a.action[g], (float)a.A);
+        // the action table entries of this thread (dynamics stem) go to the idle residual registers before the MMAs, so
+        // the loads overlap them.  The table sits on the stem, before the first block: the registers are free (the
+        // launcher rejects a table anywhere else)
+        const bool table = ly.action_table != nullptr;
+        if (table) {
+#pragma unroll
+            for (int i = 0; i < 32; ++i)
+                res[i] = __ldg(ly.action_table + (size_t)(r0 + 8 * ((i >> 1) & 1)) * kC + 8 * (i >> 2) + cq + (i & 1));
+        }
+        if (stamp) a.timeline[(l * kTiles + k) * 4 + 0] = clock64();
+        float dm[32], dl[32];                          // x_h (w_h + w_l) | x_l w_h
+        wgmma_fence();
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap) {
+            mbar_wait(bar_w_full(tap), (uint32_t)(l & 1));
+            constexpr int kRow16 = kRowBytes / 16;
+            const int shift = (tap / 3 - 1) * 8 + (tap % 3 - 1);
+#pragma unroll
+            for (int ks = 0; ks < kC / 16; ++ks) {
+                const uint32_t off = (uint32_t)(shift * kRow16 + ks * 2);
+                const uint32_t bh = w16 + (uint32_t)(tap * (kTapBytes / 16) + ks * 2);     // w_h rows; w_l rows 64 further
+                wgmma_m64n64k16(dm, ah16 + off, bh, (tap | ks) != 0);
+                wgmma_m64n64k16(dm, ah16 + off, bh + (uint32_t)(kC * kRowBytes / 16), 1);
+                wgmma_m64n64k16(dl, al16 + off, bh, (tap | ks) != 0);
+            }
+        }
+        wgmma_commit();
+        if (stamp) a.timeline[(l * kTiles + k) * 4 + 1] = clock64();
+        wgmma_wait_all();
+        if (stamp) a.timeline[(l * kTiles + k) * 4 + 2] = clock64();
+        __syncwarp();
+        if (lane == 0)
+            for (int tap = 0; tap < 9; ++tap) mbar_arrive(bar_w_empty(tap));
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+            const int c = 8 * (i >> 2) + cq + (i & 1);
+            float v = fmaf(dl[i], kLoUnscale, dm[i]) * scale[c] + bias[c];
+            if (add_res) v += res[i];
+            if (table) v = fmaf(act_scale, res[i], v);
+            if (ly.relu) v = fmaxf(v, 0.0f);
+            if (!live[(i >> 1) & 1]) v = 0.0f;        // padding rows and missing boards stay zero
+            if (keep) res[i] = v;
+            peak = fmaxf(peak, fabsf(v));
+            dm[i] = v;
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const float v0 = dm[4 * j + 2 * h], v1 = dm[4 * j + 2 * h + 1];
+                const uint32_t hw = pack_f16x2(v0, v1);
+                const float2 hf = unpack_f16x2(hw);
+                *reinterpret_cast<uint32_t*>(smem + SmemX::hi + slot_off(h, j)) = hw;
+                *reinterpret_cast<uint32_t*>(smem + SmemX::lo + slot_off(h, j)) = pack_f16x2((v0 - hf.x) * kLoScale, (v1 - hf.y) * kLoScale);
+            }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic smem writes -> wgmma / bulk-copy readers
+        warpgroup_sync(wg);
+        if (stamp) a.timeline[(l * kTiles + k) * 4 + 3] = clock64();
+        if (warp == 0 && l + 1 < L) {
+            if (lane < 9) {
+                mbar_wait(bar_w_empty(lane), (uint32_t)(l & 1));             // every warpgroup is done with this tap
+                load_weights(l + 1);
             }
             __syncwarp();
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        for (int l = 0; l < L; ++l) {
-            for (int k = 0; k < my_tiles; ++k) {
-                if (l == 0) mbar_wait(bar_in_full(k), 0);
-                else mbar_wait(bar_tile_ready(k), (uint32_t)((l - 1) & 1));
-                tc_fence_after();
-                if (elect_one()) {
-                    if (a.timeline && blockIdx.x == 0) a.timeline[(l * kTiles + k) * 4 + 0] = clock64();
-                    const uint32_t d = tmem_base + (uint32_t)(k * kAccCols);
-                    const uint32_t row0 = (uint32_t)((kHalo + k * kBoards * kPos) * kRowBytes);
-                    const uint32_t ah16 = ((s_hi + row0) >> 4) | kDescLoFlags;
-                    const uint32_t al16 = ((s_lo + row0) >> 4) | kDescLoFlags;
-                    const uint32_t w16 = (s_w >> 4) | kDescLoFlags;
-                    uint32_t acc = 0;
-#pragma unroll
-                    for (int tap = 0; tap < 9; ++tap) {
-                        if (k == 0) { mbar_wait(bar_w_full(tap), (uint32_t)(l & 1)); tc_fence_after(); }
-                        constexpr int kRow16 = kRowBytes / 16;
-                        const int shift = (tap / 3 - 1) * 8 + (tap % 3 - 1);
-#pragma unroll
-                        for (int ks = 0; ks < kC / 16; ++ks) {
-                            const uint32_t off = (uint32_t)(shift * kRow16 + ks * 2);
-                            const uint32_t blo = w16 + (uint32_t)(tap * (kTapBytes / 16) + ks * 2);
-                            umma_words(d, ah16 + off, blo, kIdescMain, acc);        // [x_h w_h | x_h w_l] -> columns 0..127
-                            umma_words(d + 128u, al16 + off, blo, kIdescLo, acc);   // x_l w_h -> columns 128..191
-                            acc = 1;
-                        }
-                        if (k == my_tiles - 1) umma_commit(bar_w_empty(tap));
-                    }
-                    umma_commit(bar_acc_full(k));
-                    if (a.timeline && blockIdx.x == 0) a.timeline[(l * kTiles + k) * 4 + 1] = clock64();
-                }
-                __syncwarp();
-            }
-        }
-    } else if (warp == 3) {
-        // ================= output store: the last layer's tiles leave as bulk copies =================
-        if (lane == 0) {
-            unsigned char* out = reinterpret_cast<unsigned char*>(a.buf[a.layer[L - 1].out_buf]);
-            for (int k = 0; k < my_tiles; ++k) {
-                const int b0 = (tile0 + k) * kBoards;
-                const int nb = min(kBoards, a.n - b0);
-                mbar_wait(bar_out_ready(k), 0);
-                for (int b = 0; b < nb; ++b) {
-                    const uint32_t rows = (uint32_t)((kHalo + (k * kBoards + b) * kPos) * kRowBytes);
-                    unsigned char* dst = out + (size_t)(a.g0 + b0 + b) * kBoardBytes;
-                    bulk_s2g(dst, s_hi + rows, kBoardPlane);
-                    bulk_s2g(dst + kBoardPlane, s_lo + rows, kBoardPlane);
-                }
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            }
+        if (last && (threadIdx.x & 127) == 0 && gl < a.n) {
+            unsigned char* dst = reinterpret_cast<unsigned char*>(a.buf[ly.out_buf]) + (size_t)g * kBoardBytes;
+            bulk_s2g(dst, s_hi + (uint32_t)(brow * kRowBytes), kBoardPlane);
+            bulk_s2g(dst + kBoardPlane, s_lo + (uint32_t)(brow * kRowBytes), kBoardPlane);
+            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-            if (a.timeline && blockIdx.x == 0) a.timeline[kStampBase + 2] = clock64();
-        }
-    } else if (warp >= 4) {
-        // ================= epilogue: warps 4..7 own tile 0, warps 8..11 tile 1, for the whole tower =================
-        pdl_wait();                                    // reads a.action (written by the tree kernel)
-        const int k = (warp - 4) >> 2;                 // my tile
-        if (k < my_tiles) {
-            const int q = warp & 3;                       // TMEM lane quarter
-            const int row = q * 32 + lane;                // tile row = TMEM lane
-            const int b = row / kPos, p = row % kPos;
-            const int y = p / 8 - 1, x = p % 8;
-            const int gl = (tile0 + k) * kBoards + b;     // board inside this launch
-            const int g = a.g0 + gl;
-            const bool live = (y >= 0 && y < a.H && x < a.W) && gl < a.n;
-            const int sw = p & 7;
-            const size_t row_off = (size_t)(kHalo + k * kBoards * kPos + row) * kRowBytes;
-            unsigned char* hi_row = smem + SmemX::hi + row_off;
-            unsigned char* lo_row = smem + SmemX::lo + row_off;
-            float res[kC];                                 // residual stream of this board position, fp32, in registers
-#pragma unroll
-            for (int c = 0; c < kC; ++c) res[c] = 0.0f;
-            float peak = 0.0f;                             // largest |activation| this thread read or stored
-            const bool res_from_input = L >= 2 && a.layer[1].res_buf >= 0;      // the tower starts with a block
-            const bool res_external = a.layer[0].res_buf >= 0;                  // single conv with a residual (debug entry)
-            if (res_from_input) {
-                mbar_wait(bar_in_full(k), 0);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const uint4 h = *reinterpret_cast<const uint4*>(hi_row + ((j ^ sw) << 4));
-                    const uint4 lw = *reinterpret_cast<const uint4*>(lo_row + ((j ^ sw) << 4));
-                    const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lv[4] = {lw.x, lw.y, lw.z, lw.w};
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const float2 xf = join_split(hw[e], lv[e]);
-                        res[8 * j + 2 * e] = xf.x;
-                        res[8 * j + 2 * e + 1] = xf.y;
-                        peak = fmaxf(peak, fmaxf(fabsf(xf.x), fabsf(xf.y)));
-                    }
-                }
-            } else if (res_external && live) {
-                const unsigned char* rb = x3_board(a, a.layer[0].res_buf, g) + (size_t)p * kRowBytes;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const uint4 h = __ldg(reinterpret_cast<const uint4*>(rb + ((j ^ sw) << 4)));
-                    const uint4 lw = __ldg(reinterpret_cast<const uint4*>(rb + kBoardPlane + ((j ^ sw) << 4)));
-                    const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lv[4] = {lw.x, lw.y, lw.z, lw.w};
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const float2 xf = join_split(hw[e], lv[e]);
-                        res[8 * j + 2 * e] = xf.x;
-                        res[8 * j + 2 * e + 1] = xf.y;
-                        peak = fmaxf(peak, fmaxf(fabsf(xf.x), fabsf(xf.y)));
-                    }
-                }
-            }
-            for (int l = 0; l < L; ++l) {
-                const TowerLayer& ly = a.layer[l];
-                const float* bias = s_bias + l * kC;
-                const float* scale = s_scale + l * kC;
-                const bool last = l == L - 1;
-                const bool add_res = ly.res_buf >= 0;
-                const bool keep = l + 2 < L && a.layer[l + 2].res_buf >= 0;     // this output is the input of a block
-                float act_scale = 0.0f;
-                if (live && ly.action_table) act_scale = __fdiv_rn((float)a.action[g], (float)a.A);
-                // the action table row of this position (dynamics stem): fetched into the idle residual registers while the
-                // MMAs of the layer run - 64 dependent L2 loads after the accumulator wait cost 20 k cycles per launch
-                // (profiles/r02_x3_timeline.md).  The table sits on the stem, before the first block: the registers are free.
-                // (the launcher rejects a table anywhere else)
-                const bool table = ly.action_table != nullptr;
-                if (table) {
-                    const float4* atab4 = reinterpret_cast<const float4*>(ly.action_table + (size_t)p * kC);
-#pragma unroll
-                    for (int j = 0; j < kC / 4; ++j) {
-                        const float4 t4 = __ldg(atab4 + j);
-                        res[4 * j] = t4.x; res[4 * j + 1] = t4.y; res[4 * j + 2] = t4.z; res[4 * j + 3] = t4.w;
-                    }
-                }
-                mbar_wait(bar_acc_full(k), (uint32_t)(l & 1));
-                tc_fence_after();
-                if (a.timeline && blockIdx.x == 0 && q == 0 && lane == 0) a.timeline[(l * kTiles + k) * 4 + 2] = clock64();
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(k * kAccCols);
-#pragma unroll
-                for (int c4 = 0; c4 < 4; ++c4) {
-                    uint32_t vm[16], vc[16], vl[16];
-                    tmem_ld16(taddr + (uint32_t)(16 * c4), vm);
-                    tmem_ld16(taddr + (uint32_t)(64 + 16 * c4), vc);
-                    tmem_ld16(taddr + (uint32_t)(128 + 16 * c4), vl);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    float r[16];
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) {
-                        const int c = 16 * c4 + e;
-                        float v = fmaf(__uint_as_float(vl[e]), kLoUnscale, __uint_as_float(vm[e]) + __uint_as_float(vc[e])) * scale[c] + bias[c];
-                        if (add_res) v += res[c];
-                        if (table) v = fmaf(act_scale, res[c], v);
-                        if (ly.relu) v = fmaxf(v, 0.0f);
-                        if (!live) v = 0.0f;               // padding rows and missing boards stay zero
-                        if (keep) res[c] = v;
-                        peak = fmaxf(peak, fabsf(v));
-                        r[e] = v;
-                    }
-#pragma unroll
-                    for (int j2 = 0; j2 < 2; ++j2) {
-                        uint32_t hw[4], lw[4];
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const float v0 = r[8 * j2 + 2 * e], v1 = r[8 * j2 + 2 * e + 1];
-                            hw[e] = pack_f16x2(v0, v1);
-                            const float2 hf = unpack_f16x2(hw[e]);
-                            lw[e] = pack_f16x2((v0 - hf.x) * kLoScale, (v1 - hf.y) * kLoScale);
-                        }
-                        const int j = 2 * c4 + j2;
-                        *reinterpret_cast<uint4*>(hi_row + ((j ^ sw) << 4)) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                        *reinterpret_cast<uint4*>(lo_row + ((j ^ sw) << 4)) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                    }
-                }
-                tc_fence_before();
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic smem writes -> tcgen05 / bulk-copy readers
-                __syncwarp();
-                if (lane == 0) mbar_arrive(last ? bar_out_ready(k) : bar_tile_ready(k));
-                if (a.timeline && blockIdx.x == 0 && q == 0 && lane == 0) a.timeline[(l * kTiles + k) * 4 + 3] = clock64();
-            }
-            if (peak > 65504.0f && a.sat_count) atomicAdd(a.sat_count, 1);
+            if (stamp) a.timeline[kStampBase + 2] = clock64();
         }
     }
-    // ---- teardown
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTiles * kAccCols) : "memory");
+    if (peak > 65504.0f && a.sat_count) atomicAdd(a.sat_count, 1);
 }
 
 // Any batch: chunks of at most sm_count * 4 boards, one launch each (balanced, multiples of one CTA's four boards).

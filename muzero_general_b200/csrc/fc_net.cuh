@@ -224,8 +224,7 @@ MZ_DEVINL void support_to_scalar_group2(const float* la, const float* lb, int S,
 // Fixed-shape recurrent inference (the fused search kernel's per-simulation network call).
 //
 // The generic code above walks run-time layer descriptors: for CartPole's 8 -> 16 -> {8, 21, 2, 21} networks seven of eight
-// instructions it executes are loop control, predicates and address arithmetic (profiles/r02_fc_search_ncu.md: FMAs are 13 %
-// of the network code).  When the five MLPs have the common shape
+// instructions it executes are loop control, predicates and address arithmetic.  When the five MLPs have the common shape
 //     dynamics  [E | one_hot(A)] -> H -> E          reward / value  E -> H -> F = 2S+1          policy  E -> H -> A
 // with compile-time E, H, F, A, everything unrolls: per four inputs one broadcast 128-bit load of x, one 128-bit load of
 // the packed weights and four FMAs; the next state, the 2 x F value / reward logits and the policy logit never leave

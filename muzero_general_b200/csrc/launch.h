@@ -2,7 +2,7 @@
 //
 // A search step is a chain of small dependent kernels (tower -> heads -> tower -> heads -> tree step) replayed from
 // a CUDA graph.  With the programmatic-stream-serialization attribute a kernel's CTAs may start while the previous
-// kernel is still draining: everything up to `pdl_wait()` (barrier / TMEM set-up, staging of weights - data no
+// kernel is still draining: everything up to `pdl_wait()` (barrier set-up, staging of weights - data no
 // kernel of the chain writes) overlaps the predecessor's tail, `pdl_wait()` then blocks until the predecessor has
 // completed and its writes are visible.  Every kernel calls `pdl_launch_dependents()` first thing, so its successor
 // is released as early as the hardware has room for it.  MZ_NO_PDL=1 launches without the attribute (the device-side

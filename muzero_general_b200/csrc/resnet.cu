@@ -372,7 +372,7 @@ struct ResNetDevice {
     float* scratch_hidden = nullptr;   // [B, C*hh*hw] rescaled state when no pool is given (dense NCHW)
     float* scratch_state = nullptr;    // [B, 4096 fp16] same state in P64C8 (tensor-core path)
     bool loaded = false;
-    bool use_tc = false;               // residual towers on tcgen05 (conv_tc.cu / conv_x3.cu)
+    bool use_tc = false;               // residual towers on the tensor cores (conv_tc.cu / conv_x3.cu)
     bool split = false;                // x3 mode: split operands, fp32-grade accuracy (conv_x3.cu); false = plain fp16 operands
     bool tc_capable = false;           // the shape allows the tensor-core towers at all
     float* big_scratch = nullptr;      // activations of the generic heads route (heads_big)
@@ -412,7 +412,7 @@ ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, s
         max_elems = std::max(max_elems, (size_t)net.channels * H * W);
     }
     max_elems = std::max(max_elems, (size_t)(net.channels + 1) * r->hh * r->hw);
-    // MZ_TC_MODE = "off": fp32 CUDA-core towers everywhere; anything else: tcgen05 towers where the shape allows
+    // MZ_TC_MODE = "off": fp32 CUDA-core towers everywhere; anything else: tensor-core towers where the shape allows
     // (conv_tc.cu).  MZ_NO_TC=1 is the older spelling of "off".
     const char* no_tc = getenv("MZ_NO_TC");
     const char* tc_mode = getenv("MZ_TC_MODE");
@@ -540,7 +540,7 @@ bool pack_conv(Loader& L, const std::string& conv, const std::string& bn, int ci
     if (tc == kLayoutSplit) {
         // x3 image [tap][128 rows][cin 64]: rows 0..63 = w_h of cout 0..63, rows 64..127 = w_l; w' = w * 2^k with k per
         // output channel such that the row's largest |w'| lies in [1, 2); w_h = fp16(w'), w_l = fp16(w' - w_h).
-        // The 16-byte chunks of a row are XOR-ed with row % 8 (UMMA K-major SWIZZLE_128B).
+        // The 16-byte chunks of a row are XOR-ed with row % 8 (wgmma K-major SWIZZLE_128B).
         const int C = cout;
         l.tc_off = (long)blob.size();
         blob.resize(blob.size() + (size_t)9 * 128 * C / 2);
@@ -587,7 +587,7 @@ bool pack_conv(Loader& L, const std::string& conv, const std::string& bn, int ci
         }
     } else if (tc) {
         // fp16 image [tap][cout][cin] over the first 64 input channels, the 16-byte chunks of a cout row XOR-ed with
-        // cout % 8 (UMMA K-major SWIZZLE_128B; two halves per float slot of the blob); an extra (65th) input channel
+        // cout % 8 (wgmma K-major SWIZZLE_128B; two halves per float slot of the blob); an extra (65th) input channel
         // is the constant action plane and becomes a per-position fp32 table (sum of the taps that stay inside the board)
         const int C = cout;
         l.tc_off = (long)blob.size();
@@ -1206,7 +1206,7 @@ int resnet_debug_conv(int n, int C, int H, int W, const float* x, const float* w
         cudaEventElapsedTime(&ms, e0, e1);
         const double flops = 2.0 * n * H * W * (double)C * C * 9;
         fprintf(stderr, "[mz_debug_conv3x3] %s n=%d C=%d %dx%d residual=%d: %.2f us per launch, %.1f TFLOP/s useful\n",
-                use_tc ? "tcgen05" : "cuda-core", n, C, H, W, residual ? 1 : 0, 1000.0 * ms / reps, flops / (ms / reps * 1e-3) / 1e12);
+                use_tc ? "wgmma" : "cuda-core", n, C, H, W, residual ? 1 : 0, 1000.0 * ms / reps, flops / (ms / reps * 1e-3) / 1e12);
         cudaEventDestroy(e0); cudaEventDestroy(e1);
     }
     if (good) cudaMemcpy(out, d_out, dense * 4, cudaMemcpyDeviceToHost);

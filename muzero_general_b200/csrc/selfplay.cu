@@ -325,7 +325,7 @@ MZ_DEVINL float initial_priority(const SpDev& s, int g, int T, int i) {
 // unless the slot is parked; then, whatever `act`, a finished game is copied into the staging area by the whole warp and
 // the slot starts its next game (act == 0 is the drain-only pass that re-packs games parked by an earlier call).
 // Staging space is reserved with ONE atomicAdd per finished game (a compare-and-swap loop serialises hundreds of
-// finishing warps per move: 89 us per launch at 4096 CartPole games, profiles/r02_selfplay_loop.md): the cursor may run
+// finishing warps per move): the cursor may run
 // past the capacity, reservations that end beyond it are void (the game stays parked), and since the cursor only grows
 // the valid reservations are a contiguous prefix whose end is tracked in counters[5].
 constexpr int kStepThreads = 1024;

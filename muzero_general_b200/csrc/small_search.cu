@@ -1,7 +1,7 @@
 // Fused search kernel for small residual networks: every simulation of MCTS.run (self_play.py:302-353) in ONE launch.
 //
 // The step-wise pipeline runs a simulation as five dependent kernels (dynamics tower -> reward head + rescale ->
-// prediction tower -> value / policy heads -> tree step).  For a small board each of them is a 30-50 us latency-bound
+// prediction tower -> value / policy heads -> tree step).  For a small board each of them is a latency-bound
 // launch that re-stages its weights and round-trips its activations through L2, and a search is 5 N of them.  But
 // nothing in a simulation couples two games: the tree step of game g needs the network outputs of game g only, the next
 // dynamics call the leaf that tree step selected.  So a CTA takes a tile of games through ALL N simulations by itself:

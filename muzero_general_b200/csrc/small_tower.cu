@@ -114,7 +114,7 @@ cudaError_t launch(const SmallTowerArgs& a, const Plan& pl, cudaStream_t stream)
 
 bool small_tower_supported(const SmallTowerArgs& a) {
     SmallTowerArgs copy = a;
-    return make_plan(copy, 148).ok;
+    return make_plan(copy, 132).ok;
 }
 
 cudaError_t launch_small_tower(SmallTowerArgs a, int sm_count, cudaStream_t stream) {

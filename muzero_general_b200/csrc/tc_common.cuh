@@ -1,5 +1,5 @@
-// Device helpers shared by the tcgen05 tower kernels (conv_tc.cu, conv_x3.cu): mbarriers, bulk copies (TMA unit),
-// leader election, tcgen05 fences / commit, shared-memory matrix descriptor words.
+// Device helpers shared by the tensor-core tower kernels (conv_tc.cu, conv_x3.cu): mbarriers, bulk copies (TMA unit),
+// warpgroup MMAs (wgmma) with shared-memory matrix descriptors, fp16 packing.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
@@ -36,34 +36,48 @@ MZ_DEVINL void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t 
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
-// exactly one lane of a converged warp (ptxas then knows the tcgen05 operands come from a single thread and
-// moves them to uniform registers without a broadcast loop)
-MZ_DEVINL bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P;\n\t"
-        "elect.sync _|P, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, P;\n\t"
-        "}" : "=r"(pred));
-    return pred != 0;
-}
-MZ_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-MZ_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// descriptor words shared by every A / B descriptor of this kernel (K-major SWIZZLE_128B, SBO = 1024 B, version 1);
-// the hardware applies the 128B swizzle on absolute shared-memory address bits, so row-shifted tap windows need
-// no base_offset (checked: tests/test_conv_gpu.py is exact with base_offset = 0 and wrong with the row phase)
-constexpr uint32_t kDescLoFlags = 1u << 16;                                           // LBO field = 1 (unused)
-constexpr uint32_t kDescHi = ((1024u >> 4) & 0x3FFFu) | (1u << 14) | (2u << 29);      // SBO | version | SWIZZLE_128B
+// wgmma matrix descriptor words shared by every A / B operand (K-major SWIZZLE_128B, SBO = 1024 B between 8-row groups):
+// lo = start address / 16 | LBO field 1 (unused for K-major swizzled operands), hi = SBO / 16 | layout type 1 (128B
+// swizzle, bits 62-63).  The 128B swizzle is applied on absolute shared-memory address bits, so row-shifted tap windows
+// need no base_offset (tests/test_conv_gpu.py is exact only if that holds).
+constexpr uint32_t kDescLoFlags = 1u << 16;
+constexpr uint32_t kDescHi = ((1024u >> 4) & 0x3FFFu) | (1u << 30);
 
 // shared -> global bulk copy (TMA unit), tracked by the thread's bulk async-group
 MZ_DEVINL void bulk_s2g(void* gdst, uint32_t ssrc, uint32_t bytes) {
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(ssrc), "r"(bytes) : "memory");
 }
-MZ_DEVINL void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+
+MZ_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+MZ_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+MZ_DEVINL void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T on one warpgroup: fp16 operands from shared memory (descriptor low words,
+// K-major), fp32 accumulators in registers.  Thread t of the warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and
+// columns 8 j + 2 (t % 4) (+ 1): d[4 j + 2 h + e] = D[row + 8 h][8 j + 2 (t % 4) + e].
+MZ_DEVINL void wgmma_m64n64k16(float* d, uint32_t a_lo, uint32_t b_lo, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        ".reg .b64 da, db;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "mov.b64 da, {%32, %35};\n\t"
+        "mov.b64 db, {%33, %35};\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, da, db, p, 1, 1, 0, 0;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a_lo), "r"(b_lo), "r"(accumulate), "r"(kDescHi)
+        : "memory");
 }
+
+// barrier over the 128 threads of warpgroup wg (named barrier 1 + wg; 0 is __syncthreads)
+MZ_DEVINL void warpgroup_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+
 // two fp32 -> packed fp16x2, round to nearest even, saturating to the finite range
 MZ_DEVINL uint32_t pack_f16x2(float lo, float hi) {
     uint32_t r;

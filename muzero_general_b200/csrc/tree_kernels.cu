@@ -87,7 +87,7 @@ cudaError_t launch_tree_step(const TreeStepArgs& a, cudaStream_t stream) {
     const int grid = (a.n + games_per_cta - 1) / games_per_cta;
     // below ~4 resident warps per scheduler the kernel is latency-bound (MZ_TREE_LATENCY = 0 / 1 forces a variant: A/B switch)
     static const int forced = getenv("MZ_TREE_LATENCY") ? atoi(getenv("MZ_TREE_LATENCY")) : -1;
-    const bool latency = forced >= 0 ? forced != 0 : (long)a.n * G <= 148L * 512;
+    const bool latency = forced >= 0 ? forced != 0 : (long)a.n * G <= 132L * 512;
     cudaError_t e = cudaSuccess;
 #define MZ_TREE(GG)                                                                                 \
     case GG:                                                                                        \

@@ -473,7 +473,7 @@ def parse_staged_games(buf: bytes, index):
 
 def debug_conv3x3(x, w, bias=None, residual=None, relu=False, tensor_cores=False, device=0):
     """One conv3x3 (pad 1, stride 1) on the device through mz_debug_conv3x3; numpy NCHW in and out.
-    ``tensor_cores``: False / "off" = CUDA cores, "fp16" = tcgen05 with fp16 operands, True / "x3" = tcgen05 split operands."""
+    ``tensor_cores``: False / "off" = CUDA cores, "fp16" = wgmma with fp16 operands, True / "x3" = wgmma on split operands."""
     lib = _lib.load_library()
     x = numpy.ascontiguousarray(x, numpy.float32)
     w = numpy.ascontiguousarray(w, numpy.float32)

@@ -596,8 +596,29 @@ def main_round2():
     print("network fixtures (batch 64, stress weights) written")
 
 
+def main_priorities():
+    """PER priorities of the reference's ReplayBuffer.save_game on the seeded random histories of
+    tests/test_reanalyse_cpu.py (per_priorities.npz: <case key> -> float32 priorities, <case key>_top -> game priority)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_reanalyse_cpu import PRIORITY_CASES, PRIORITY_LENGTHS, priority_histories
+    _, _, ref_rb, _ = load_reference()
+    out = {}
+    for name, td, discount, alpha, reanalysed in PRIORITY_CASES:
+        ref_cfg = load_reference_game(name).MuZeroConfig()
+        ref_cfg.td_steps, ref_cfg.discount, ref_cfg.PER_alpha, ref_cfg.PER = td, discount, alpha, True
+        for key, gh in priority_histories(name, td, reanalysed, ref_cfg):
+            buf = ref_rb.ReplayBuffer({"num_played_games": 0, "num_played_steps": 0}, {}, ref_cfg)
+            buf.save_game(gh)
+            out[key] = gh.priorities
+            out[key + "_top"] = numpy.float32(gh.game_priority)
+    numpy.savez_compressed(os.path.join(OUT, "per_priorities.npz"), **out)
+    print("per_priorities.npz:", len(out) // 2, "histories over", len(PRIORITY_LENGTHS), "lengths")
+
+
 if __name__ == "__main__":
     if "--round2" in sys.argv:
         main_round2()
+    elif "--priorities" in sys.argv:
+        main_priorities()
     else:
         main()

@@ -141,16 +141,17 @@ def test_small_search_launch_plan():
     from muzero_general_b200 import _lib
     lib = _lib.load_library()
 
-    def plan(H, W, Cc, A, n, tower=11664, heads=5000, scratch=868, cap=17, sms=148):
+    def plan(H, W, Cc, A, n, tower=11664, heads=5000, scratch=868, cap=17, sms=132):
         out = (C.c_int64 * 8)()
         ok = lib.mz_debug_small_search_plan(H, W, Cc, A, n, sms, tower, heads, scratch, cap, out)
         return dict(zip(("P", "CO", "G", "tile", "threads", "smem", "row_stride", "board_stride"), out)) if ok else None
 
-    # TicTacToe, BASELINE batch: 8192 games -> two even waves of CTAs, one lane group per game, four output channels per thread
+    # TicTacToe, BASELINE batch: 8192 games on 132 SMs -> three even waves of CTAs, one lane group per game, four output channels
+    # per thread
     p = plan(3, 3, 16, 9, 8192)
     assert (p["P"], p["CO"], p["G"]) == (3, 4, 16)
     ctas = -(-8192 // p["tile"])
-    assert 1.9 < ctas / 148 <= 2.0 and p["tile"] * 16 <= p["threads"] <= 512 and p["threads"] % 32 == 0
+    assert 2.9 < ctas / 132 <= 3.0 and p["tile"] * 16 <= p["threads"] <= 512 and p["threads"] % 32 == 0
     assert p["smem"] <= 227 * 1024
     # bank spreading of the uniform-weight mapping: odd row stride, 32 consecutive rows (board, y) hit 32 different banks
     assert p["row_stride"] % 2 == 1 and p["board_stride"] >= 17 * 5 * p["row_stride"]
@@ -159,7 +160,7 @@ def test_small_search_launch_plan():
     # a handful of games: one channel per thread (more threads per board), still one CTA per tile
     q = plan(3, 3, 16, 9, 5)
     assert q["CO"] == 1 and q["tile"] == 1
-    # the Breakout configuration's hidden board: 6 x 6 x 16, 4 actions, 128 games on 148 SMs -> one game per CTA
+    # the Breakout configuration's hidden board: 6 x 6 x 16, 4 actions, 128 games on 132 SMs -> one game per CTA
     b = plan(6, 6, 16, 4, 128, tower=21024, heads=8600, scratch=1408)
     assert b["G"] == 4 and b["tile"] == 1 and b["smem"] <= 227 * 1024
     # same board, a large batch: uniform weights with P = W = 6

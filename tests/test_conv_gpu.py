@@ -1,8 +1,8 @@
 """conv3x3 kernels against torch's fp32 conv2d (a floating-point kernel: torch fp32 is the reference).
 
-Tolerances stated here: the CUDA-core path accumulates in fp32 (rtol 1e-4); the tcgen05 "fp16" mode multiplies
+Tolerances stated here: the CUDA-core path accumulates in fp32 (rtol 1e-4); the wgmma "fp16" mode multiplies
 fp16 operands (10-bit mantissa, like tf32) with fp32 accumulation and stores fp16:
-|err| <= 2e-3 * (|w| . |x|) + 1e-3 * |out| per output; the tcgen05 "x3" mode (split fp16 operands (x = x_h + x_l/2^11), three partial
+|err| <= 2e-3 * (|w| . |x|) + 1e-3 * |out| per output; the wgmma "x3" mode (split fp16 operands (x = x_h + x_l/2^11), three partial
 products, csrc/conv_x3.cu) is fp32-grade: |err| <= 4e-6 * (|w| . |x|) + 2e-6 * |out| + 1e-6 - two orders of magnitude
 inside the CUDA-core path's own tolerance."""
 import numpy

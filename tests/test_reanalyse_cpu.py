@@ -1,18 +1,17 @@
 """Bulk callers either side of the self-play path (muzero_general_b200/reanalyse.py) on the CPU: PER priorities against
-the unmodified reference ReplayBuffer, batched Reanalyse against the oracle network."""
+those of the unmodified reference ReplayBuffer, batched Reanalyse against the oracle network."""
 import copy
 
 import numpy
 import pytest
 import torch
 
-from conftest import weights_for
+from conftest import golden_npz, weights_for
 from fake_engine import FakeSearchEngine
 from muzero_general_b200 import reanalyse as ra
 from muzero_general_b200 import self_play as sp
 from muzero_general_b200.games import load_game_module
 from muzero_general_b200.netspec import netspec_from_config
-from oracle.refload import reference_available
 
 torch.set_num_threads(1)
 
@@ -29,34 +28,45 @@ def _random_history(rs, cfg, T, players):
     return gh
 
 
-@pytest.mark.skipif(not reference_available(), reason="needs /root/reference (not present on the GPU box)")
-@pytest.mark.parametrize("name,td,discount,alpha,reanalysed", [("tictactoe", 20, 1, 0.5, False), ("cartpole", 50, 0.997, 0.5, False),
-                                                               ("cartpole", 7, 0.9, 1.0, True), ("connect4", 3, 1, 0.7, True)])
-def test_bulk_priorities_equal_the_reference_save_game(name, td, discount, alpha, reanalysed):
-    """initial_priorities == what the unmodified ReplayBuffer.save_game computes, bit for bit (float32 priorities, game
-    priority), for one- and two-player games, with and without reanalysed values, short and long td horizons."""
-    from oracle.refload import load_reference, load_reference_game
-    _, _, ref_rb, _ = load_reference()
-    ref_cfg = load_reference_game(name).MuZeroConfig()
-    ref_cfg.td_steps, ref_cfg.discount, ref_cfg.PER_alpha, ref_cfg.PER = td, discount, alpha, True
-    ck = {"num_played_games": 0, "num_played_steps": 0}
+PRIORITY_CASES = [("tictactoe", 20, 1, 0.5, False), ("cartpole", 50, 0.997, 0.5, False), ("cartpole", 7, 0.9, 1.0, True),
+                  ("connect4", 3, 1, 0.7, True)]
+PRIORITY_LENGTHS = (1, 2, 9, 42, 130)
+
+
+def priority_histories(name, td, reanalysed, cfg):
+    """(fixture key, GameHistory) of the seeded histories the priority fixtures were computed on."""
     rs = numpy.random.RandomState(4)
-    for T in (1, 2, 9, 42, 130):
-        gh = _random_history(rs, ref_cfg, T, len(ref_cfg.players))
+    for T in PRIORITY_LENGTHS:
+        gh = _random_history(rs, cfg, T, len(cfg.players))
         if reanalysed:
             gh.reanalysed_predicted_root_values = rs.standard_normal(T).astype(numpy.float32)
-        mine, top = ra.initial_priorities(copy.deepcopy(gh), ref_cfg)
-        buf = ref_rb.ReplayBuffer(copy.deepcopy(ck), {}, ref_cfg)
-        theirs = copy.deepcopy(gh)
-        buf.save_game(theirs)
-        assert mine.dtype == theirs.priorities.dtype == numpy.float32
-        assert numpy.array_equal(mine, theirs.priorities), (name, T)
-        assert top == theirs.game_priority
-        # and save_games attaches them so that the reference keeps them as they are
-        buf2 = ref_rb.ReplayBuffer(copy.deepcopy(ck), {}, ref_cfg)
-        g2 = copy.deepcopy(gh)
-        ra.save_games(buf2, [g2], ref_cfg)
-        assert numpy.array_equal(buf2.buffer[0].priorities, theirs.priorities) and buf2.num_played_steps == T
+        yield f"{name}_td{td}_T{T}", gh
+
+
+class _Recorder:
+    def __init__(self):
+        self.buffer = []
+
+    def save_game(self, game_history, shared_storage=None):
+        self.buffer.append(game_history)
+
+
+@pytest.mark.parametrize("name,td,discount,alpha,reanalysed", PRIORITY_CASES)
+def test_bulk_priorities_equal_the_reference_save_game(name, td, discount, alpha, reanalysed):
+    """initial_priorities == what the unmodified ReplayBuffer.save_game computed (tests/golden/per_priorities.npz, from
+    oracle/gen_golden.py --priorities), bit for bit (float32 priorities, game priority), for one- and two-player games,
+    with and without reanalysed values, short and long td horizons; save_games hands them to the buffer as they are."""
+    cfg = load_game_module(name).MuZeroConfig()
+    cfg.td_steps, cfg.discount, cfg.PER_alpha, cfg.PER = td, discount, alpha, True
+    gold = golden_npz("per_priorities.npz")
+    for key, gh in priority_histories(name, td, reanalysed, cfg):
+        mine, top = ra.initial_priorities(copy.deepcopy(gh), cfg)
+        assert mine.dtype == gold[key].dtype == numpy.float32
+        assert numpy.array_equal(mine, gold[key]), key
+        assert top == gold[key + "_top"]
+        buf = _Recorder()
+        ra.save_games(buf, [copy.deepcopy(gh)], cfg)
+        assert numpy.array_equal(buf.buffer[0].priorities, gold[key]) and buf.buffer[0].game_priority == top
 
 
 def test_batched_reanalyse_matches_per_game_inference(monkeypatch):

@@ -1,7 +1,7 @@
 """GPU parity of the residual-network kernels and the step-wise search, in the three tower modes (MZ_TC_MODE):
 
   "off"   fp32 CUDA-core convs everywhere (reference arithmetic, different summation order)
-  "x3"    DEFAULT for 64-channel board nets: tcgen05 towers on split fp16 operands (x = x_h + x_l/2^11), three partial products, fp32
+  "x3"    DEFAULT for 64-channel board nets: wgmma towers on split fp16 operands (x = x_h + x_l/2^11), three partial products, fp32
           accumulation (csrc/conv_x3.cu) - fp32-grade, held to the SAME tolerance as "off"
   "fp16"  opt-in fast mode: plain fp16 operands (csrc/conv_tc.cu), 3x fewer MMAs; per-quantity bounds below
 
