@@ -379,11 +379,37 @@ struct ResNetDevice {
     size_t big_elems = 0;
     int* d_sat = nullptr;              // x3 mode: number of epilogue threads that stored an activation beyond the fp16 range
     int fell_back = 0;                 // set when the range guard switched this net to the fp32 CUDA-core towers
+    bool heads_off_tc = false;         // a 64-channel board net kept off the tensor cores because its heads exceed shared memory
     bool fuse_small = true;            // CUDA-core towers as one fused launch where they fit (small_tower.cu); MZ_NO_FUSE=1: per layer
     int state_elems = 0;               // float slots per stored hidden state (dense C*H*W, or 2048 = 4096 fp16 for P64C8)
 };
 
 static int conv_out(int h, int stride) { return (h - 1) / stride + 1; }
+
+// Offsets of one head in the head blob, which holds *size floats so far: conv1x1 weight [rc][C] and bias [rc], then per
+// FC layer the weights packed [in/4][out][4] (zero rows pad `in`) and the bias; every part that is read as float4 starts
+// 16-byte aligned.  *size grows by the head.
+static void layout_head(int C, int rc, int HW, const int32_t* hidden, int n_hidden, int n_out, size_t* size, HeadDesc& d) {
+    size_t o = (*size + 3) & ~(size_t)3;
+    d.rc = rc; d.n_out = n_out;
+    d.w1_off = (int)o; o += (size_t)rc * C;
+    d.b1_off = (int)o; o += rc;
+    int sz[MZ_MAX_LAYERS + 2];
+    sz[0] = rc * HW;
+    for (int i = 0; i < n_hidden; ++i) sz[i + 1] = hidden[i];
+    sz[n_hidden + 1] = n_out;
+    d.mlp.n = n_hidden + 1;
+    for (int l = 0; l < d.mlp.n; ++l) {
+        const int in = sz[l], out = sz[l + 1];
+        d.mlp.in[l] = in; d.mlp.out[l] = out;
+        o = (o + 3) & ~(size_t)3;
+        d.mlp.w_off[l] = (int)o; o += (size_t)((in + 3) / 4) * out * 4;
+        d.mlp.b_off[l] = (int)o; o += out;
+    }
+    *size = (o + 3) & ~(size_t)3;
+}
+
+static bool tc_heads_fit(ResNetDevice* r);
 
 ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, std::string* err) {
     ResNetDevice* r = new ResNetDevice();
@@ -422,6 +448,22 @@ ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, s
     // default "x3": split 16-bit operands, three partial products, fp32-grade accuracy; "fp16": plain fp16 operands
     // (3x fewer MMAs, ~1e-2 hidden-state error: opt-in)
     r->split = r->use_tc && !(tc_mode && strcmp(tc_mode, "fp16") == 0);
+    // The heads of the tensor-core route read the board layout and have no generic (global-memory) variant.  A net whose
+    // head weights do not fit in shared memory next to one sample's tile (e.g. support 300, or a 128-wide value layer
+    // over 16 reduced channels) runs on the fp32 CUDA-core towers and the generic heads route instead.  The head shapes
+    // are known here, so the hidden-state pool and the workspaces are sized for the route that will run.
+    if (r->use_tc) {
+        const int HW = r->hh * r->hw, F = 2 * net.support_size + 1;
+        size_t size = 0;
+        layout_head(net.channels, net.reduced_reward, HW, net.res_fc_reward, net.n_res_fc_reward, F, &size, r->reward_head);
+        layout_head(net.channels, net.reduced_value, HW, net.res_fc_value, net.n_res_fc_value, F, &size, r->value_head);
+        layout_head(net.channels, net.reduced_policy, HW, net.res_fc_policy, net.n_res_fc_policy, net.action_space, &size,
+                    r->policy_head);
+        if (!tc_heads_fit(r)) {
+            r->tc_capable = r->use_tc = r->split = false;
+            r->heads_off_tc = true;
+        }
+    }
     const char* no_fuse = getenv("MZ_NO_FUSE");
     r->fuse_small = !(no_fuse && no_fuse[0] == '1');
     r->state_elems = r->use_tc ? conv_tc_board_elems(r->split) : r->C * r->hh * r->hw;
@@ -629,32 +671,21 @@ bool pack_head(Loader& L, const std::string& conv, const std::string& fc, int C,
     const MzTensor* w = L.get(conv + ".weight", (int64_t)rc * C);
     const MzTensor* b = L.get(conv + ".bias", rc);
     if (!w || !b) return false;
-    d.rc = rc; d.n_out = n_out;
-    while (blob.size() % 4) blob.push_back(0.0f);          // every head starts 16-byte aligned (float4 staging)
-    d.w1_off = (int)blob.size(); blob.insert(blob.end(), w->data, w->data + (size_t)rc * C);
-    d.b1_off = (int)blob.size(); blob.insert(blob.end(), b->data, b->data + rc);
-    std::vector<int> sz;
-    sz.push_back(rc * HW);
-    for (int i = 0; i < n_hidden; ++i) sz.push_back(hidden[i]);
-    sz.push_back(n_out);
-    d.mlp.n = (int)sz.size() - 1;
+    size_t size = blob.size();
+    layout_head(C, rc, HW, hidden, n_hidden, n_out, &size, d);
+    blob.resize(size, 0.0f);
+    std::copy(w->data, w->data + (size_t)rc * C, blob.begin() + d.w1_off);
+    std::copy(b->data, b->data + rc, blob.begin() + d.b1_off);
     for (int l = 0; l < d.mlp.n; ++l) {
-        const int in = sz[l], out = sz[l + 1];
+        const int in = d.mlp.in[l], out = d.mlp.out[l];
         const MzTensor* lw = L.get(fc + "." + std::to_string(2 * l) + ".weight", (int64_t)in * out);
         const MzTensor* lb = L.get(fc + "." + std::to_string(2 * l) + ".bias", out);
         if (!lw || !lb) return false;
-        d.mlp.in[l] = in; d.mlp.out[l] = out;
-        while (blob.size() % 4) blob.push_back(0.0f);
-        d.mlp.w_off[l] = (int)blob.size();
-        const int in4 = (in + 3) / 4;
-        blob.resize(blob.size() + (size_t)in4 * out * 4, 0.0f);        // packed [in/4][out][4], zero rows pad `in`
         float* dst = blob.data() + d.mlp.w_off[l];
         for (int o = 0; o < out; ++o)
             for (int i = 0; i < in; ++i) dst[((size_t)(i / 4) * out + o) * 4 + (i % 4)] = lw->data[(size_t)o * in + i];
-        d.mlp.b_off[l] = (int)blob.size();
-        blob.insert(blob.end(), lb->data, lb->data + out);
+        std::copy(lb->data, lb->data + out, blob.begin() + d.mlp.b_off[l]);
     }
-    while (blob.size() % 4) blob.push_back(0.0f);
     return true;
 }
 }  // namespace
@@ -767,16 +798,18 @@ struct Runner {
             if (nf < 3) free_ws[nf++] = const_cast<float*>(ext);      // ext is itself a workspace: reusable as the third
             float *cur = free_ws[0], *tmp = free_ws[1], *spare = free_ws[2];
             size_t first = first_layer;
-            const float* x = ext;
-            if (stem) { if (!conv_tc(layers[first], ext, cur, nullptr, true, gather_parent, pool_stride, action)) return nullptr; first += 1; x = cur; }
+            // (the result buffer may be ext itself when ext is one of the workspaces: whether any layer ran decides
+            // what is returned, not a comparison with ext)
+            const bool any = stem || count > 0;
+            if (stem) { if (!conv_tc(layers[first], ext, cur, nullptr, true, gather_parent, pool_stride, action)) return nullptr; first += 1; }
             if (count > 0 && !stem) {
                 if (!conv_tc(layers[first], ext, tmp, nullptr, true, gather_parent, pool_stride)) return nullptr;
                 if (!conv_tc(layers[first + 1], tmp, spare, ext, true)) return nullptr;      // residual = ext (plain addressing only)
                 { float* t = cur; cur = spare; spare = t; }
-                first += 2; count -= 1; x = cur;
+                first += 2; count -= 1;
             }
             if (!blocks_tc(layers, first, count, &cur, &tmp, &spare)) return nullptr;
-            return x == ext ? x : cur;
+            return any ? cur : ext;
         }
         size_t li = first_layer, blocks_left = count;
         bool stem_left = stem;
@@ -1042,6 +1075,20 @@ struct Runner {
 };
 }  // namespace
 
+// every heads launch of resnet_inference_tc (rescale only, reward head, value + policy heads) fits in shared memory with
+// one sample per CTA
+static bool tc_heads_fit(ResNetDevice* r) {
+    std::string err; int64_t launches = 0;
+    Runner R{r, nullptr, &launches, &err, 1, 0};
+    const HeadsArgs calls[3] = {
+        R.heads_args(nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, true),
+        R.heads_args(nullptr, 1, &r->reward_head, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, true),
+        R.heads_args(nullptr, 2, &r->value_head, &r->policy_head, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, true)};
+    for (const HeadsArgs& a : calls)
+        if (((size_t)a.w_floats + a.warp_floats) * 4 > 227 * 1024) return false;
+    return true;
+}
+
 // Tensor-core variant: every C->C conv of the three towers runs in conv_tc.cu on the P64C4 layout; the
 // stem conv (obs -> C) and the heads stay on the CUDA-core kernels above, reading / writing that layout.
 static int resnet_inference_tc(ResNetDevice* r, const InferCall& c, cudaStream_t stream, int64_t* launches, std::string* err) {
@@ -1119,7 +1166,8 @@ bool resnet_can_partition(const ResNetDevice* r0) {
     return ((size_t)(hi - lo) + warp_floats) * 4 <= 227 * 1024;
 }
 const char* resnet_numerics(const ResNetDevice* r) {
-    if (!r->use_tc) return r->fell_back ? "f32 nets + f64 tree statistics (tensor-core towers left after an activation exceeded the fp16 range)"
+    if (!r->use_tc) return r->heads_off_tc ? "f32 nets + f64 tree statistics (no tensor-core towers: the head weights exceed shared memory)"
+                         : r->fell_back ? "f32 nets + f64 tree statistics (tensor-core towers left after an activation exceeded the fp16 range)"
                                         : "f32 nets + f64 tree statistics";
     return r->split ? "f32-grade nets (tensor-core towers on split fp16 operands x = x_h + x_l/2^11, 3 partial products, f32 accumulate; f32 heads) + f64 tree statistics"
                     : "fp16 operands / f32 accumulate (tensor-core towers), f32 heads, f64 tree statistics";
