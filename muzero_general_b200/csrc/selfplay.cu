@@ -229,7 +229,9 @@ MZ_DEVINL int sample_action(const SpDev& s, int g, double temperature, double u)
         for (int k = 0; k < A; ++k) if (lg[k] && idx-- == 0) return k;
         return last;
     }
-    // p = visit_counts ** (1 / T) / sum, then the first action whose cumulative probability exceeds u.
+    // numpy.random.choice(actions, p=p) with p = visit_counts ** (1 / T) / sum(...): cdf = p.cumsum(), cdf /= cdf[-1],
+    // then the number of cdf entries <= u.  Illegal actions carry p = 0 and repeat the previous entry, so counting
+    // over the whole action space lands on the same legal action; after the division the last entry is exactly 1 > u.
     // 1/T is 1, 2 or 4 for every reference schedule (games/*.py visit_softmax_temperature_fn): integer powers are exact
     const double inv = 1.0 / temperature;
     double total = 0.0;
@@ -243,12 +245,13 @@ MZ_DEVINL int sample_action(const SpDev& s, int g, double temperature, double u)
         total += x;
     }
     double cdf = 0.0;
-    int pick = 0;
     for (int k = 0; k < A; ++k) {
         cdf = __dadd_rn(cdf, __ddiv_rn(p[k], total));
-        if (u >= cdf) pick = k + 1;
+        p[k] = cdf;
     }
-    return pick > last ? last : pick;                          // rounding can leave u >= cdf[-1]
+    int pick = 0;
+    for (int k = 0; k < A; ++k) pick += __ddiv_rn(p[k], cdf) <= u;
+    return pick;
 }
 
 // select_action + Game.step + record for slot g (one thread)
@@ -569,6 +572,10 @@ static int sp_enqueue(MzHandle* h, int32_t n_moves, double temperature, const Mz
         return fail(h, MZ_EINVAL, std::string(who) + ": per-move overrides need n_moves == 1");
     if (!(temperature >= 0.0)) return fail(h, MZ_EINVAL, std::string(who) + ": temperature must be >= 0");
     MzSelfPlay* sp = h->sp;
+    if (inj && inj->uniform)
+        for (int g = 0; g < sp->dev.B; ++g)
+            if (!(inj->uniform[g] >= 0.0 && inj->uniform[g] < 1.0))
+                return fail(h, MZ_EINVAL, std::string(who) + ": injected uniforms must lie in [0, 1)");
     if (sp->in_flight) return fail(h, MZ_ESTATE, std::string(who) + ": moves already enqueued, call mz_selfplay_wait first");
     MZ_CUDA(h, cudaSetDevice(h->device));
     SpDev s = sp->dev;

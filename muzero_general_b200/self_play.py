@@ -869,10 +869,13 @@ class BatchedSelfPlay:
         with numpy.errstate(divide="ignore"):
             p = visit_counts.astype(numpy.float64) ** (1.0 / numpy.where(greedy, 1.0, t))[:, None]
         p = numpy.where(legal > 0, p, 0.0)           # 0 ** 0 = 1 at T = inf must not give illegal actions any mass
-        cdf = numpy.cumsum(p / p.sum(1, keepdims=True), axis=1)
+        # numpy.random.choice(p=p / sum(p)) for a given uniform: the sum left to right like select_action's builtin
+        # sum (cumsum; ndarray.sum is pairwise), then cdf = p.cumsum(), cdf /= cdf[-1], count the entries <= u
+        # (oracle/mcts.py::numpy_choice_index)
+        cdf = numpy.cumsum(p / numpy.cumsum(p, axis=1)[:, -1:], axis=1)
+        cdf /= cdf[:, -1:]
         u = self.fast.random_sample(B)
-        last_legal = self.A - 1 - numpy.argmax(legal[:, ::-1] > 0, axis=1)
-        sampled = numpy.minimum((u[:, None] >= cdf).sum(1), last_legal)    # cdf rounding can leave u >= cdf[-1]
+        sampled = (cdf <= u[:, None]).sum(1)
         return numpy.where(greedy, numpy.where(legal > 0, visit_counts, -1).argmax(1), sampled).astype(numpy.int64)
 
     def _begin(self):

@@ -87,13 +87,24 @@ class InjectedDraws:
     ``noise``        Dirichlet sample for this search (length = number of legal actions)
     ``first_index``  index into the root's child list picked at the first simulation
     ``tie_fn``       called for any later exact tie: tie_fn(n_tied, ctx) -> index
+    ``uniform``      the uniform in [0, 1) behind the action choice: ``numpy_choice_index`` at a finite temperature,
+                     ``floor(uniform * n)`` at T = inf (the device's documented rule)
     """
 
-    def __init__(self, noise=None, first_index=None, tie_fn=None):
+    def __init__(self, noise=None, first_index=None, tie_fn=None, uniform=None):
         self.noise = noise
         self.first_index = first_index
         self.tie_fn = tie_fn
+        self.uniform = uniform
         self.later_ties = 0
+
+    def sample_index(self, probabilities, ctx=None):
+        assert self.uniform is not None, "no uniform supplied for the action choice"
+        return numpy_choice_index(probabilities, self.uniform)
+
+    def uniform_index(self, n, ctx=None):
+        assert self.uniform is not None, "no uniform supplied for the action choice"
+        return min(int(self.uniform * n), n - 1)
 
     def dirichlet(self, alpha, n, ctx=None):
         assert self.noise is not None and len(self.noise) == n
@@ -353,6 +364,18 @@ class TableEvaluator:
 
 
 # ----------------------------------------------------------------------------- action choice
+def numpy_choice_index(p, u):
+    """The index ``numpy.random.RandomState.choice(len(p), p=p)`` returns when its one uniform draw is ``u``.
+
+    Legacy ``choice`` with ``p`` consumes exactly one ``random_sample()`` double and computes
+    ``cdf = p.cumsum(); cdf /= cdf[-1]; cdf.searchsorted(u, side="right")``.  The division by ``cdf[-1]`` matters:
+    the sequential cumulative sum of ``dist / sum(dist)`` often ends one ulp away from 1, which moves interior
+    boundaries by an ulp."""
+    cdf = numpy.cumsum(numpy.asarray(p, dtype=numpy.float64))
+    cdf /= cdf[-1]
+    return int(cdf.searchsorted(u, side="right"))
+
+
 def select_action(actions, visit_counts, temperature, draws, ctx=None):
     """self_play.py:222-245 on the root's (actions, visit counts) in child order."""
     counts = numpy.array(visit_counts, dtype="int32")

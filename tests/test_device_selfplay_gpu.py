@@ -8,6 +8,7 @@ import pytest
 from conftest import golden_json, weights_for
 from muzero_general_b200.games import load_game_module
 from muzero_general_b200.netspec import netspec_from_config
+from oracle import mcts as om
 
 pytestmark = pytest.mark.gpu
 
@@ -121,7 +122,8 @@ def test_cartpole_physics_one_step_at_a_time():
 @pytest.mark.parametrize("name,B,N,moves", [("cartpole", 48, 20, 14), ("tictactoe", 40, 16, 12), ("connect4", 24, 12, 30)])
 def test_device_loop_equals_host_composition_with_injected_draws(name, B, N, moves, monkeypatch):
     """One move at a time with the host's draws injected (root noise, action uniforms): the action the device plays and
-    the record it keeps equal [mz_search on the peeked observation] + [the host's visit-count sampling rule]."""
+    the record it keeps equal [mz_search on the peeked observation] + [select_action with numpy's choice rule for the
+    injected uniform (oracle/mcts.py::numpy_choice_index)]."""
     monkeypatch.setenv("MZ_TC_MODE", "off")
     from muzero_general_b200.engine import SearchEngine
     mod, cfg, spec, eng, loop = _loop(name, B, N, seed=5)
@@ -139,10 +141,9 @@ def test_device_loop_equals_host_composition_with_injected_draws(name, B, N, mov
         u = rs.random_sample(B)
         out = ref.search(obs=pk["obs"], legal_mask=legal, to_play=pk["to_play"], add_exploration_noise=True, noise=noise,
                          game_id=pk["game_id"], move_index=pk["move_index"])
-        p = numpy.where(legal > 0, out.visit_counts.astype(numpy.float64), 0.0)
-        cdf = numpy.cumsum(p / p.sum(1, keepdims=True), axis=1)
-        last_legal = A - 1 - numpy.argmax(legal[:, ::-1] > 0, axis=1)
-        want = numpy.minimum((u[:, None] >= cdf).sum(1), last_legal)
+        want = numpy.array([om.select_action([int(a) for a in numpy.nonzero(legal[g])[0]],
+                                             out.visit_counts[g][legal[g] > 0], 1.0, om.InjectedDraws(uniform=u[g]))
+                            for g in range(B)])
         for g in range(B):
             expected.setdefault(int(pk["game_id"][g]), []).append((out.visit_counts[g].copy(), out.root_value[g], int(want[g])))
         loop.moves(1, 1.0, uniform=u, noise=noise)

@@ -230,3 +230,46 @@ def test_search_rejects_a_row_without_legal_actions():
     eng.A, eng.N, eng.obs_elems = 3, 2, 4
     with pytest.raises(AssertionError, match="Legal actions should not be an empty array"):
         eng.search(obs=numpy.zeros((2, 4), numpy.float32), legal_mask=numpy.array([[1, 0, 0], [0, 0, 0]], numpy.uint8))
+
+
+def test_fast_mode_action_sampling_is_numpy_choice():
+    """BatchedSelfPlay._actions (rng_mode="fast") for a given uniform per game equals select_action with numpy's
+    choice rule (oracle/mcts.py::numpy_choice_index), on uniforms placed on numpy's boundaries cdf_k / cdf[-1], one
+    ulp either side, and on the unnormalised boundaries; T = 0 and moves past the threshold take the first maximum."""
+    from oracle import mcts as om
+    rs = numpy.random.RandomState(3)
+    B, A = 64, 9
+    checked = 0
+    for T, thr in ((1.0, None), (0.5, None), (0.25, None), (0.7, None), (0.0, None), (1.0, 3)):
+        for _ in range(6):
+            visits = rs.randint(0, 4, (B, A)).astype(numpy.int32)
+            legal = (rs.random_sample((B, A)) < 0.7).astype(numpy.uint8)
+            legal[numpy.arange(B), rs.randint(0, A, B)] = 1
+            visits[legal == 0] = 0
+            visits[numpy.arange(B), numpy.argmax(legal, 1)] += 1
+            moves = rs.randint(0, 5, B)
+            u = rs.random_sample(B)
+            for g in range(B):                        # a boundary of game g's own distribution, or a plain draw
+                idx = numpy.nonzero(legal[g])[0]
+                if T > 0 and len(idx) > 1:
+                    d = visits[g, idx] ** (1 / T)
+                    raw = numpy.cumsum(d / sum(d))
+                    k = rs.randint(len(idx) - 1)
+                    u[g] = float(rs.choice([raw[k] / raw[-1], numpy.nextafter(raw[k] / raw[-1], 0),
+                                            numpy.nextafter(raw[k] / raw[-1], 2), raw[k], u[g]]))
+                    u[g] = min(u[g], numpy.nextafter(1.0, 0))
+
+            class Fixed(numpy.random.RandomState):
+                def random_sample(self, size=None):
+                    return u.copy()
+            bsp = object.__new__(sp.BatchedSelfPlay)
+            bsp.B, bsp.A, bsp.temperature, bsp.temperature_threshold = B, A, T, thr
+            bsp.numpy_mode, bsp.fast = False, Fixed(0)
+            got = bsp._actions(visits, legal, moves)
+            for g in range(B):
+                idx = [int(a) for a in numpy.nonzero(legal[g])[0]]
+                t = T if not thr or moves[g] + 1 < thr else 0
+                want = om.select_action(idx, visits[g, idx], t, om.InjectedDraws(uniform=float(u[g])))
+                assert got[g] == want, (T, thr, g, visits[g], legal[g], u[g])
+                checked += 1
+    assert checked == 6 * 6 * B
