@@ -12,6 +12,7 @@
 #include "kernels.h"
 
 #include <stdlib.h>
+#include <vector>
 
 namespace mz {
 
@@ -40,6 +41,43 @@ __host__ __device__ inline GameSmem game_smem_layout(int N, int A, int E, int ma
     off += 16;          // odd multiple of 16 B between games: spreads games over banks
     L.bytes = off;
     return L;
+}
+
+// Phase split (scripts/fc_phase_split.py builds a copy of the library with -DMZ_FC_PHASES): every group times its game's
+// root, select, network, expand and backup phases with clock() and adds them, with the levels and selection rounds it
+// walked, to device counters that mz_fc_phase_counters reads.  The library built without the macro is unchanged.
+enum { kPhRoot, kPhSelect, kPhNet, kPhExpand, kPhBackup, kPhLevels, kPhRounds, kPhSims, kPhCount };
+// The counters are per game and added to in memory as the game goes (fire-and-forget reductions to distinct addresses):
+// accumulators held in registers would push the kernel past 128 registers and change its occupancy.
+#ifdef MZ_FC_PHASES
+constexpr int kPhMaxGames = 1 << 16;
+__device__ unsigned long long g_fc_phase[kPhMaxGames][kPhCount];
+struct PhaseClock {
+    int row = -1;                     // game of this group's lane 0, -1 on the other lanes
+    unsigned last = 0;
+    MZ_DEVINL void start(int g, bool leader) {
+        row = (leader && g < kPhMaxGames) ? g : -1;
+        last = (unsigned)clock();
+    }
+    MZ_DEVINL void mark(int p) {
+        const unsigned now = (unsigned)clock();
+        if (row >= 0) atomicAdd(&g_fc_phase[row][p], (unsigned long long)(now - last));
+        last = now;
+    }
+    MZ_DEVINL void count(int p, int n) { if (row >= 0) atomicAdd(&g_fc_phase[row][p], (unsigned long long)n); }
+};
+#else
+struct PhaseClock {
+    MZ_DEVINL void start(int, bool) {}
+    MZ_DEVINL void mark(int) {}
+    MZ_DEVINL void count(int, int) {}
+};
+#endif
+
+template <typename SH>
+constexpr int fixed_actions() {
+    if constexpr (SH::kEnabled) return SH::A;
+    else return 0;
 }
 
 // SH: FcFixedShape<E, H, S, A> runs the per-simulation network call through the fully unrolled fixed-shape code
@@ -88,8 +126,14 @@ __global__ void __launch_bounds__(kFcMaxThreads) fc_search_kernel(const __grid_c
     float* const hb[3][2] = {{s_act + 3 * maxw, s_act + 4 * maxw}, {s_act + 5 * maxw, s_act + 6 * maxw},
                              {s_act + 7 * maxw, s_act + 8 * maxw}};
     const bool fused_heads = (a.net.rew.n == a.net.pol.n) && (a.net.pol.n == a.net.val.n);
+    // multi-level selection: A fixed at compile time for the fixed network shapes
+    constexpr int kA = fixed_actions<SH>();
+    constexpr int kMaxD = select_levels_for(kA ? kA : 2, G);
+    const SelectLanes sl = select_lanes<G, kA>(A, min(a.select_levels, kMaxD));
+    PhaseClock ph;
 
     for (int g = blockIdx.x * groups_per_cta + gi; g < a.n_games; g += gridDim.x * groups_per_cta) {
+        ph.start(g, lane == 0);
         const int64_t game_id = a.game_id ? a.game_id[g] : (int64_t)g;
         const int move = a.move_index ? a.move_index[g] : 0;
         const int to_play0 = a.to_play ? a.to_play[g] : 0;
@@ -126,11 +170,16 @@ __global__ void __launch_bounds__(kFcMaxThreads) fc_search_kernel(const __grid_c
         tree_init_root<G>(c, t, prior, root_reward,
                           (a.add_noise && a.noise) ? a.noise + (size_t)g * A : nullptr, a.add_noise && !a.noise,
                           game_id, move, a.trace.noise ? a.trace.noise + (size_t)g * A : nullptr);
+        ph.mark(kPhRoot);
 
         // ------------------------------------------------------------------ simulations
         int max_depth = 0;
         for (int sim = 0; sim < N; ++sim) {
-            const Leaf leaf = tree_select<G>(c, t, sim, game_id, move, first_index);
+            int rounds;
+            const Leaf leaf = tree_select_lookahead<G, kMaxD, kA>(c, t, sl, sim, game_id, move, first_index, rounds);
+            ph.mark(kPhSelect);
+            ph.count(kPhLevels, leaf.depth);
+            ph.count(kPhRounds, rounds);
             float value, reward;
             if (kTeacher) {
                 value = a.teacher.value[(size_t)g * N + sim];
@@ -171,6 +220,7 @@ __global__ void __launch_bounds__(kFcMaxThreads) fc_search_kernel(const __grid_c
                 if constexpr (SH::kEnabled) prior = group_softmax_masked_w<G, pow2_ceil_c(SH::A)>(logit, lane < A);
                 else prior = group_softmax_masked<G>(logit, lane < A);
             }
+            ph.mark(kPhNet);
             if (a.trace.depth) {
                 const size_t ti = (size_t)g * N + sim;
                 if (lane == 0) { a.trace.depth[ti] = leaf.depth; a.trace.value[ti] = value; a.trace.reward[ti] = reward; }
@@ -179,9 +229,12 @@ __global__ void __launch_bounds__(kFcMaxThreads) fc_search_kernel(const __grid_c
                     a.trace.actions[ti * a.trace.max_depth + j] = (uint8_t)(t.path[j + 1] % A);
             }
             tree_expand<G>(c, t, leaf, reward, prior);
+            ph.mark(kPhExpand);
             tree_backup<G>(c, t, leaf, value);
+            ph.mark(kPhBackup);
             max_depth = max(max_depth, leaf.depth);
         }
+        ph.count(kPhSims, N);
 
         // ------------------------------------------------------------------ results
         if (lane < A) {
@@ -225,7 +278,10 @@ __global__ void __launch_bounds__(kFcMaxThreads) fc_search_kernel(const __grid_c
 // host launcher
 // ------------------------------------------------------------------------------------------
 template <int G, bool T, typename SH>
-static cudaError_t launch_one(const FcSearchArgs& a, int sm_count, size_t smem_cap, cudaStream_t stream, FcLaunchInfo* info) {
+static cudaError_t launch_one(const FcSearchArgs& a_in, int sm_count, size_t smem_cap, cudaStream_t stream, FcLaunchInfo* info) {
+    FcSearchArgs a = a_in;
+    const char* one_level = getenv("MZ_FC_SELECT_LEVELS");    // A/B switch: "1" = one tree level per selection round
+    a.select_levels = (one_level && one_level[0] == '1' && one_level[1] == 0) ? 1 : select_levels_for(a.A, G);
     const GameSmem L = game_smem_layout(a.N, a.A, a.net.E, a.net.maxw, !T);
     const size_t shared_bytes = ((2 * (size_t)(a.N + 2) * 8 + (T ? 0 : (size_t)a.net.blob_floats) * 4) + 15) & ~(size_t)15;
     const int threads = a.threads;
@@ -270,6 +326,25 @@ cudaError_t launch_fc_search(const FcSearchArgs& a, int group, bool teacher, int
 #undef MZ_CASE
     return cudaErrorInvalidValue;
 }
+
+#ifdef MZ_FC_PHASES
+// counters of the phase-split build: out[kPhCount] = root, select, network, expand, backup cycles, levels, rounds,
+// simulations, each summed over games; reset != 0 zeroes them afterwards
+extern "C" int mz_fc_phase_counters(unsigned long long* out, int reset) {
+    cudaError_t e = cudaDeviceSynchronize();
+    void* dev = nullptr;
+    if (e == cudaSuccess) e = cudaGetSymbolAddress(&dev, g_fc_phase);
+    if (e == cudaSuccess && out) {
+        std::vector<unsigned long long> rows((size_t)kPhMaxGames * kPhCount);
+        e = cudaMemcpy(rows.data(), dev, rows.size() * 8, cudaMemcpyDeviceToHost);
+        for (int p = 0; p < kPhCount; ++p) out[p] = 0;
+        for (size_t i = 0; i < rows.size(); ++i) out[i % kPhCount] += rows[i];
+    }
+    if (e == cudaSuccess && reset) e = cudaMemset(dev, 0, sizeof(g_fc_phase));
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    return e == cudaSuccess ? 0 : (int)e;
+}
+#endif
 
 size_t fc_search_smem_bytes(const FcSearchArgs& a, int group, bool teacher) {
     const GameSmem L = game_smem_layout(a.N, a.A, a.net.E, a.net.maxw, !teacher);

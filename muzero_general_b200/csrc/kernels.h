@@ -53,6 +53,7 @@ struct DevTrace {
 struct FcSearchArgs {
     int n_games, N, A, P;
     int threads;           // block size of the launch (multiple of 32)
+    int select_levels;     // tree levels per selection round (set by launch_fc_search)
     double discount, noise_frac, noise_alpha;
     uint64_t seed;
     const double* pbc;

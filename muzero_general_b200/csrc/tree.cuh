@@ -247,6 +247,182 @@ MZ_DEVINL Leaf tree_select(const TreeConst& c, GameTree& t, int sim, int64_t gam
 }
 
 // ------------------------------------------------------------------------------------------
+// Multi-level selection (fused FC kernel).  tree_select spends one dependent chain - loads, table lookup, fp64 division,
+// shuffle max, ballot, broadcast - per tree level, and with few actions most of the group's lanes idle through it.  Here
+// the group scores D levels below the round's start node at once: A + A^2 + ... + A^D <= G lanes, level d (1-based) in
+// lanes [off_d, off_d + A^d), off_1 = 0, off_{d+1} = off_d + A^d; lane off_d + j holds the node reached by the base-A
+// digits of j (most significant first), i.e. child j % A of level-(d-1) candidate j / A.  Every node's score depends only
+// on its own slot, its parent's visit count and lo/hi (constant during a selection), so each lane evaluates exactly
+// tree_select's expression for its node; the levels are then resolved in order from two ballots (ties, expanded) with
+// tree_select's tie rules at the node's absolute depth, and the next round starts from the last expanded pick.  Same
+// scores, same comparisons, same Philox draws: the path is bit-identical to tree_select's.  D = 1 IS tree_select.
+// ------------------------------------------------------------------------------------------
+constexpr int kMaxSelectLevels = 4;
+
+// levels per round for A actions in a group of G lanes: the largest D with A + A^2 + ... + A^D <= G, capped at what A = 2
+// gets (A = 1 would otherwise fill the group)
+__host__ __device__ constexpr int select_levels_for(int A, int G) {
+    int D = 1, lanes = 0, w = 1;
+    for (int d = 1; d <= kMaxSelectLevels; ++d) {
+        w *= (A < 2 ? 2 : A);
+        if (lanes + w > G) break;
+        lanes += w;
+        D = d;
+    }
+    return D;
+}
+
+// this lane's place in the layout (fixed for a launch)
+struct SelectLanes {
+    int D;          // levels per round
+    int level;      // 1..D, 0 = idle lane
+    int act;        // action of this lane's node (last base-A digit)
+    unsigned walk;  // digits 1..level-1 (actions from the round's start node to the parent), 8 bits each
+};
+
+template <int G, int kA>
+MZ_DEVINL SelectLanes select_lanes(int A_rt, int D) {
+    const int A = kA ? kA : A_rt;
+    const int k = LaneGroup<G>::lane();
+    SelectLanes s{D, 0, 0, 0u};
+    int off = 0, w = A, j = 0;
+    for (int d = 1; d <= D; ++d) {
+        if (k >= off && k < off + w) { s.level = d; j = k - off; }
+        off += w;
+        w *= A;
+    }
+    if (s.level > 0) {
+        s.act = j % A;
+        int q = j / A;
+        for (int d = s.level - 1; d >= 1; --d) { s.walk |= (unsigned)(q % A) << (8 * (d - 1)); q /= A; }
+    }
+    return s;
+}
+
+// kMaxD: compile-time bound of sl.D; kA: |A| when fixed at compile time (0 = c.A)
+template <int G, int kMaxD, int kA>
+MZ_DEVINL Leaf tree_select_lookahead(const TreeConst& c, GameTree& t, const SelectLanes& sl, int sim, int64_t game_id,
+                                     int move, int first_index, int& rounds) {
+    if (kMaxD <= 1 || sl.D <= 1) {
+        const Leaf leaf = tree_select<G>(c, t, sim, game_id, move, first_index);
+        rounds = leaf.depth;
+        return leaf;
+    }
+    const int A = kA ? kA : c.A;
+    const int D = sl.D;
+    const int k = LaneGroup<G>::lane();
+    const unsigned gm = LaneGroup<G>::mask();
+    const unsigned seg_mask = (1u << A) - 1u;
+    const bool pow2 = (A & (A - 1)) == 0;
+    int e = 0;
+    int n_parent = t.root_visit;
+    int depth = 0;                                 // levels resolved before this round
+    Leaf leaf;
+    rounds = 0;
+    if (k == 0) { t.path[0] = -1; t.path_reward[0] = t.root_reward; }
+    while (true) {
+        rounds += 1;
+        // this lane's parent: one dependent (expansion, visit) load per level below the first
+        int pe = e, np = n_parent;
+#pragma unroll
+        for (int d = 1; d < kMaxD; ++d) {
+            if (d < sl.level && pe >= 0) {
+                const int s = pe * A + (int)((sl.walk >> (8 * (d - 1))) & 0xffu);
+                np = t.visit[s];
+                pe = t.expansion[s];
+            }
+        }
+        const bool valid = sl.level > 0 && pe >= 0 && (pe != 0 || ((t.legal >> sl.act) & 1u));
+        const int slot = pe * A + sl.act;
+        double score = -INFINITY;
+        int nc = 0, child_exp_k = -1;
+        float reward_k = 0.0f;
+        if (valid) {
+            // tree_select's score, operation for operation
+            nc = t.visit[slot];
+            child_exp_k = t.expansion[slot];
+            const double pr = (pe == 0) ? t.root_prior[sl.act] : (double)t.prior[slot];
+            double pbc;
+            if (c.ucb) {
+                pbc = __ldg(c.ucb + np * (c.N + 2) + nc);
+            } else {
+                const double q = __ddiv_rn(c.sqrtn[np], (double)(nc + 1));
+                pbc = __dmul_rn(c.pbc[np], q);
+            }
+            score = __dmul_rn(pbc, pr);
+            if (nc > 0) {
+                reward_k = t.reward[slot];
+                score = __dadd_rn(score, value_range_normalize(t.mval[slot], t.lo, t.hi));
+            } else {
+                score = __dadd_rn(score, 0.0);
+            }
+        }
+        // maximum over each lane's A siblings, every level at once (exact: no rounding involved)
+        double best = score;
+        if (pow2) {
+            // level offsets are multiples of A: the sibling blocks are aligned
+            for (int o = A >> 1; o > 0; o >>= 1) best = fmax(best, shfl_xor_f64(gm, best, o, G));
+        } else {
+            // reduce towards the block's first lane, then broadcast from it
+            for (int o = 1; o < A; o <<= 1) {
+                const int lo = __shfl_down_sync(gm, __double2loint(best), o, G);
+                const int hi = __shfl_down_sync(gm, __double2hiint(best), o, G);
+                if (sl.act + o < A) best = fmax(best, __hiloint2double(hi, lo));
+            }
+            best = shfl_f64(gm, best, k - sl.act, G);
+        }
+        const unsigned tie_bits = LaneGroup<G>::ballot(valid && score == best);
+        const unsigned exp_bits = LaneGroup<G>::ballot(valid && child_exp_k >= 0);
+        // resolve the levels in order (uniform over the group)
+        int off = 0, w = A, p = 0, last = 0, pick = 0, dl = 0;
+        unsigned picked = 0;
+        bool hit_leaf = false;
+#pragma unroll
+        for (int d = 0; d < kMaxD; ++d) {
+            if (d < D && !hit_leaf) {
+                const int seg = off + p * A;
+                const unsigned tied = (tie_bits >> seg) & seg_mask;
+                const int n_tied = __popc(tied);
+                const int dd = depth + d;          // absolute depth of the parent
+                if (n_tied <= 1) {
+                    pick = max(__ffs(tied) - 1, 0);
+                } else {
+                    int idx;
+                    if (sim == 0 && dd == 0 && first_index >= 0) {
+                        idx = first_index < n_tied ? first_index : n_tied - 1;
+                    } else {
+                        idx = philox_tie_index(c.seed, game_id, move, sim, dd, n_tied);
+                        if (!(sim == 0 && dd == 0)) t.ties += 1;
+                    }
+                    pick = nth_set_bit(tied, idx);
+                }
+                last = seg + pick;
+                picked |= 1u << last;
+                dl = d + 1;
+                hit_leaf = ((exp_bits >> last) & 1u) == 0;
+                off += w;
+                w *= A;
+                p = p * A + pick;
+            }
+        }
+        if ((picked >> k) & 1u) { t.path[depth + sl.level] = slot; t.path_reward[depth + sl.level] = reward_k; }
+        if (hit_leaf) {
+            const int pe_last = LaneGroup<G>::bcast(pe, last);
+            leaf.depth = depth + dl;
+            leaf.parent_exp = pe_last;
+            leaf.action = pick;
+            leaf.slot = pe_last * A + pick;
+            break;
+        }
+        e = LaneGroup<G>::bcast(child_exp_k, last);
+        n_parent = LaneGroup<G>::bcast(nc, last);
+        depth += D;
+    }
+    LaneGroup<G>::sync();
+    return leaf;
+}
+
+// ------------------------------------------------------------------------------------------
 // Expansion of the selected leaf with the network outputs (self_play.py:345-351, 451-465).
 // prior_f32: this lane's fp32 softmax prior (lane k <-> action k).
 // ------------------------------------------------------------------------------------------
