@@ -230,12 +230,21 @@ int mz_kernel_times(MzHandle* h, double* ms, int64_t* count);
 int mz_debug_small_search_plan(int32_t H, int32_t W, int32_t C, int32_t A, int32_t n, int32_t sm_count, int32_t tower_floats,
                                int32_t heads_floats, int32_t scratch_floats, int32_t cap_channels, int64_t* plan);
 
-/* Debug / parity: one conv3x3 (C -> C, stride 1, pad 1; models.py:206-209) with optional bias, residual and
- * ReLU on host NCHW fp32 data, through the CUDA-core kernel (use_tensor_cores = 0) or the wgmma implicit
- * GEMM (C = 64, H <= 6, W <= 7): 1 = fp16 operands, 2 = split fp16+bf16 operands with three partial products
- * (fp32-grade, the default of the search path).  w is [C][C][3][3] as in the reference state_dict. */
-int mz_debug_conv3x3(int device, int32_t n, int32_t C, int32_t H, int32_t W, const float* x, const float* w,
-                     const float* bias, const float* residual, int32_t relu, int32_t use_tensor_cores, float* out);
+/* Debug / tests (host only, no device needed): launch plan of the CUDA-core conv3x3 kernel (csrc/resnet.cu) for n boards of
+ * cin x H x W -> cout channels at stride 1 or 2.  Returns 1 and fills plan[11] = {P (pixels per thread), stride,
+ * MAX_ITEMS (accumulator tiles per thread), row bands, rows per band, boards per CTA, cin chunk, grid x, grid y (cout
+ * tiles of <= 64 channels), grid z, shared-memory bytes}, or 0 with the reason in mz_last_error(NULL) when the shape
+ * cannot be launched.  mz_create refuses a net with such a conv. */
+int mz_debug_conv3x3_plan(int32_t n, int32_t cin, int32_t cout, int32_t H, int32_t W, int32_t stride, int64_t* plan);
+
+/* Debug / parity: one conv3x3 (cin -> cout, stride 1 or 2, pad 1; models.py:206-209) with optional bias, residual and
+ * ReLU on host NCHW fp32 data, through the CUDA-core kernel (use_tensor_cores = 0; cout a multiple of 4) or the wgmma
+ * implicit GEMM (64 -> 64, stride 1, H <= 6, W <= 7, else MZ_EUNSUPPORTED): 1 = fp16 operands, 2 = split fp16 operands
+ * with three partial products (fp32-grade, the default of the search path).  x is [n][cin][H][W], w is [cout][cin][3][3]
+ * as in the reference state_dict, bias [cout], residual and out [n][cout][Ho][Wo] with Ho = (H - 1) / stride + 1 (same
+ * for Wo).  The device output is filled with NaN before the launch, so an element the kernel does not write reads NaN. */
+int mz_debug_conv3x3(int device, int32_t n, int32_t cin, int32_t cout, int32_t H, int32_t W, int32_t stride, const float* x,
+                     const float* w, const float* bias, const float* residual, int32_t relu, int32_t use_tensor_cores, float* out);
 
 /* Arithmetic the handle's search path computes in, e.g. "f32 nets + f64 tree statistics" (bench.py's dtype). */
 const char* mz_numerics(const MzHandle* h);

@@ -139,8 +139,9 @@ SYMBOLS = [
                                     C.POINTER(C.c_void_p)]),
     ("mz_selfplay_peek", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayPeek)]),
     ("mz_debug_small_search_plan", C.c_int, [C.c_int32] * 10 + [C.POINTER(C.c_int64)]),
-    ("mz_debug_conv3x3", C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
-                                   C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
+    ("mz_debug_conv3x3_plan", C.c_int, [C.c_int32] * 6 + [C.POINTER(C.c_int64)]),
+    ("mz_debug_conv3x3", C.c_int, [C.c_int] + [C.c_int32] * 6 + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                                  C.c_int32, C.c_int32, C.c_void_p]),
 ]
 
 _lib = None

@@ -880,16 +880,24 @@ extern "C" int mz_debug_small_search_plan(int32_t H, int32_t W, int32_t C, int32
     return 1;
 }
 
+extern "C" int mz_debug_conv3x3_plan(int32_t n, int32_t cin, int32_t cout, int32_t H, int32_t W, int32_t stride, int64_t* plan) {
+    if (!plan) return fail(nullptr, 0, "mz_debug_conv3x3_plan: null plan");
+    std::string e;
+    if (!resnet_conv_plan(n, cin, cout, H, W, stride, plan, &e)) return fail(nullptr, 0, e);
+    return 1;
+}
+
 // debug: one conv3x3 through either implementation (host NCHW in / out)
 // ------------------------------------------------------------------------------------------
-extern "C" int mz_debug_conv3x3(int device, int32_t n, int32_t C, int32_t H, int32_t W, const float* x, const float* w,
-                                const float* bias, const float* residual, int32_t relu, int32_t use_tensor_cores, float* out) {
+extern "C" int mz_debug_conv3x3(int device, int32_t n, int32_t cin, int32_t cout, int32_t H, int32_t W, int32_t stride, const float* x,
+                                const float* w, const float* bias, const float* residual, int32_t relu, int32_t use_tensor_cores,
+                                float* out) {
     if (!x || !w || !out || n < 1) return fail(nullptr, MZ_EINVAL, "mz_debug_conv3x3: bad argument");
     if (cudaSetDevice(device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_conv3x3: no such device");
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_conv3x3: device query failed");
     std::string e;
-    int rc = resnet_debug_conv(n, C, H, W, x, w, bias, residual, relu, use_tensor_cores, out, prop.multiProcessorCount, &e);
+    int rc = resnet_debug_conv(n, cin, cout, H, W, stride, x, w, bias, residual, relu, use_tensor_cores, out, prop.multiProcessorCount, &e);
     if (rc) return fail(nullptr, rc, "mz_debug_conv3x3: " + e);
     return MZ_OK;
 }

@@ -87,8 +87,9 @@ ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, s
 void resnet_destroy(ResNetDevice* r);
 int resnet_load_weights(ResNetDevice* r, const MzTensor* tensors, int n, std::string* err);
 int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, int64_t* launches, std::string* err);
-int resnet_debug_conv(int n, int C, int H, int W, const float* x, const float* w_oihw, const float* bias,
+int resnet_debug_conv(int n, int cin, int cout, int H, int W, int stride, const float* x, const float* w_oihw, const float* bias,
                       const float* residual, int relu, int use_tc, float* out, int sm_count, std::string* err);
+bool resnet_conv_plan(int n, int cin, int cout, int H, int W, int stride, int64_t* plan, std::string* err);   // host only
 const char* resnet_numerics(const ResNetDevice* r);
 int resnet_take_saturations(ResNetDevice* r, cudaStream_t stream);   // x3 range guard (synchronises)
 bool resnet_can_partition(const ResNetDevice* r);

@@ -71,8 +71,9 @@ __global__ void __launch_bounds__(256) conv3x3_kernel(const __grid_constant__ Co
     const int y_in0 = r0 * STRIDE - 1;
     const int Hp = (a.band_rows - 1) * STRIDE + 3, Wp = a.Win + 2;   // staged (padded) plane of the band
     const int plane = Hp * Wp;
-    const int ct = a.Cout < 64 ? a.Cout : 64;                   // cout tile of this CTA
-    const int cout0 = blockIdx.y * ct;
+    // cout tiles of at most 64 channels; the last one holds the remaining Cout - cout0 (a multiple of 4)
+    const int cout0 = blockIdx.y * 64;
+    const int ct = min(a.Cout - cout0, 64);                     // cout tile of this CTA
     const int cgs = ct / 4;
     const int segs = a.Wo / P;
     const int items_per_board = cgs * nbr * segs;
@@ -97,9 +98,12 @@ __global__ void __launch_bounds__(256) conv3x3_kernel(const __grid_constant__ Co
         const int cc = min(a.cin_chunk, a.Cin - c0);
         __syncthreads();
         // ---- stage weights of this cin chunk / cout tile
-        for (int i = threadIdx.x; i < cc * 9 * ct; i += blockDim.x) {
-            const int co = i % ct, r = i / ct;                  // r = ci*9 + tap
-            s_w[i] = a.w[((size_t)(c0 * 9 + r)) * a.Cout + cout0 + co];
+        // (as float4: Cout, cout0 and ct are multiples of 4 and every layer of the blob starts 16-byte aligned; one
+        // integer division per 4 weights instead of per weight matters when a CTA stages 64 x 9 x 64 of them)
+        for (int i = threadIdx.x; i < cc * 9 * ct / 4; i += blockDim.x) {
+            const int co = (i % (ct / 4)) * 4, r = i / (ct / 4);           // r = ci*9 + tap
+            *reinterpret_cast<float4*>(s_w + r * ct + co) =
+                *reinterpret_cast<const float4*>(a.w + ((size_t)(c0 * 9 + r)) * a.Cout + cout0 + co);
         }
         // ---- stage padded input planes
         for (int i = threadIdx.x; i < nb * cc * plane; i += blockDim.x) {
@@ -386,6 +390,52 @@ struct ResNetDevice {
 
 static int conv_out(int h, int stride) { return (h - 1) / stride + 1; }
 
+// Launch plan of one conv3x3_kernel call: n boards of cin x H x W -> cout x Ho x Wo.  The launcher (Runner::conv),
+// resnet_create's check of every conv layer of a net and mz_debug_conv3x3_plan all take it from conv3x3_plan.
+struct ConvPlan {
+    int P, stride, max_items;      // template arguments: pixels per thread, stride, accumulator tiles per thread (1 or 4)
+    int bands, band_rows;          // output rows split into bands of band_rows rows (the last one may be shorter)
+    int boards, cin_chunk;         // boards per CTA (the last CTA may hold fewer), input channels staged at a time
+    dim3 grid;                     // (board groups, cout tiles of <= 64 channels, bands)
+    size_t smem;                   // dynamic shared memory bytes
+};
+constexpr int kConvThreads = 256;
+
+// false (with the reason in *err) when the shape cannot be launched
+static bool conv3x3_plan(int n, int cin, int cout, int Hin, int Win, int stride, ConvPlan* p, std::string* err) {
+    if (n < 1 || cin < 1 || Hin < 1 || Win < 1) { *err = "conv3x3: empty shape"; return false; }
+    if (cout < 4 || cout % 4 != 0) { *err = "conv3x3: cout must be a positive multiple of 4"; return false; }
+    if (stride != 1 && stride != 2) { *err = "conv3x3: stride must be 1 or 2"; return false; }
+    const int Ho = conv_out(Hin, stride), Wo = conv_out(Win, stride);
+    p->stride = stride;
+    p->P = 1;
+    for (int cand : {8, 7, 6, 4, 3, 2}) if (Wo % cand == 0) { p->P = cand; break; }
+    const int ct = cout < 64 ? cout : 64;          // the widest cout tile sizes the items and the weight slice
+    const int threads = kConvThreads;
+    // large images (e.g. 128 output channels at 48 x 48, games/atari.py): split the output rows into bands, one CTA each
+    int bands = 1;
+    while (bands < Ho && (ct / 4) * ((Ho + bands - 1) / bands) * (Wo / p->P) > threads * 4) ++bands;
+    p->band_rows = (Ho + bands - 1) / bands;
+    p->bands = (Ho + p->band_rows - 1) / p->band_rows;
+    const int items_per_board = (ct / 4) * p->band_rows * (Wo / p->P);
+    int boards = 1;
+    if (items_per_board < threads) boards = threads / items_per_board;
+    if (boards > 32) boards = 32;
+    if (boards > n) boards = n;
+    if (items_per_board * boards > threads * 4) { *err = "conv3x3: image too large for the item budget"; return false; }
+    const size_t plane = (size_t)((p->band_rows - 1) * stride + 3) * (Win + 2);
+    // pick the cin chunk so weights + planes fit comfortably
+    const size_t budget = 200 * 1024 / 4;
+    int chunk = cin;
+    while (chunk > 1 && (size_t)chunk * 9 * ct + (size_t)boards * chunk * plane > budget) chunk = (chunk + 1) / 2;
+    if ((size_t)chunk * 9 * ct + (size_t)boards * chunk * plane > budget) { *err = "conv3x3: tile does not fit in shared memory"; return false; }
+    p->boards = boards; p->cin_chunk = chunk;
+    p->max_items = items_per_board * boards > threads ? 4 : 1;
+    p->smem = ((size_t)chunk * 9 * ct + (size_t)boards * chunk * plane) * 4;
+    p->grid = dim3((n + boards - 1) / boards, (cout + 63) / 64, p->bands);
+    return true;
+}
+
 // Offsets of one head in the head blob, which holds *size floats so far: conv1x1 weight [rc][C] and bias [rc], then per
 // FC layer the weights packed [in/4][out][4] (zero rows pad `in`) and the bias; every part that is read as float4 starts
 // 16-byte aligned.  *size grows by the head.
@@ -438,6 +488,32 @@ ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, s
         max_elems = std::max(max_elems, (size_t)net.channels * H * W);
     }
     max_elems = std::max(max_elems, (size_t)(net.channels + 1) * r->hh * r->hw);
+    // Every conv of the net must have a conv3x3_kernel launch plan (it is the route of the stems and the fallback of
+    // every other tower), so a shape the planner refuses fails here, not part-way through a search.  A plan that exists
+    // for max_batch boards exists for any smaller batch (fewer boards per CTA only shrink the tile).
+    {
+        struct Shape { int cin, cout, H, W, stride; };
+        const int C = net.channels, h = r->hh, w = r->hw;
+        std::vector<Shape> shapes;
+        if (net.downsample) {
+            const int h1 = conv_out(H, 2), w1 = conv_out(W, 2), h2 = conv_out(h1, 2), w2 = conv_out(w1, 2);
+            shapes = {{net.obs_c, C / 2, H, W, 2}, {C / 2, C / 2, h1, w1, 1}, {C / 2, C, h1, w1, 2}, {C, C, h2, w2, 1},
+                      {C, C, conv_out(h2, 2), conv_out(w2, 2), 1}};
+        } else {
+            shapes = {{net.obs_c, C, H, W, 1}};
+        }
+        shapes.push_back({C + 1, C, h, w, 1});                     // dynamics stem (action plane)
+        if (net.blocks > 0) shapes.push_back({C, C, h, w, 1});
+        for (const Shape& s : shapes) {
+            ConvPlan p;
+            std::string why;
+            if (!conv3x3_plan(max_batch, s.cin, s.cout, s.H, s.W, s.stride, &p, &why)) {
+                *err = why + " (" + std::to_string(s.cin) + " -> " + std::to_string(s.cout) + " channels, stride " +
+                       std::to_string(s.stride) + ", " + std::to_string(s.H) + " x " + std::to_string(s.W) + " input)";
+                delete r; return nullptr;
+            }
+        }
+    }
     // MZ_TC_MODE = "off": fp32 CUDA-core towers everywhere; anything else: tensor-core towers where the shape allows
     // (conv_tc.cu).  MZ_NO_TC=1 is the older spelling of "off".
     const char* no_tc = getenv("MZ_NO_TC");
@@ -865,31 +941,13 @@ struct Runner {
         a.gather_parent = gather_parent; a.pool_stride = pool_stride; a.action = action;
         a.n = n; a.Cin = l.cin; a.Cout = l.cout; a.Hin = Hin; a.Win = Win; a.stride = l.stride;
         a.Ho = conv_out(Hin, l.stride); a.Wo = conv_out(Win, l.stride); a.relu = relu; a.A = r->net.action_space;
-        int P = 1;
-        for (int cand : {8, 7, 6, 4, 3, 2}) if (a.Wo % cand == 0) { P = cand; break; }
-        const int ct = l.cout < 64 ? l.cout : 64;
-        const int threads = 256;
-        // large images (e.g. 128 output channels at 48 x 48, games/atari.py): split the output rows into bands, one CTA each
-        int bands = 1;
-        while (bands < a.Ho && (ct / 4) * ((a.Ho + bands - 1) / bands) * (a.Wo / P) > threads * 4) ++bands;
-        a.band_rows = (a.Ho + bands - 1) / bands;
-        bands = (a.Ho + a.band_rows - 1) / a.band_rows;
-        const int items_per_board = (ct / 4) * a.band_rows * (a.Wo / P);
-        int boards = 1;
-        if (items_per_board < threads) boards = threads / items_per_board;
-        if (boards > 32) boards = 32;
-        if (boards > n) boards = n;
-        if (items_per_board * boards > threads * 4) { *err = "conv3x3: image too large for the item budget"; return false; }
-        const size_t plane = (size_t)((a.band_rows - 1) * l.stride + 3) * (Win + 2);
-        // pick the cin chunk so weights + planes fit comfortably
-        const size_t budget = 200 * 1024 / 4;
-        int chunk = l.cin;
-        while (chunk > 1 && (size_t)chunk * 9 * ct + (size_t)boards * chunk * plane > budget) chunk = (chunk + 1) / 2;
-        if ((size_t)chunk * 9 * ct + (size_t)boards * chunk * plane > budget) { *err = "conv3x3: tile does not fit in shared memory"; return false; }
-        a.boards_per_cta = boards; a.cin_chunk = chunk;
-        const size_t smem = ((size_t)chunk * 9 * ct + (size_t)boards * chunk * plane) * 4;
-        dim3 grid((n + boards - 1) / boards, l.cout / ct, bands);
-        const bool multi = items_per_board * boards > threads;
+        ConvPlan plan;
+        if (!conv3x3_plan(n, l.cin, l.cout, Hin, Win, l.stride, &plan, err)) return false;
+        const int P = plan.P, threads = kConvThreads;
+        a.band_rows = plan.band_rows; a.boards_per_cta = plan.boards; a.cin_chunk = plan.cin_chunk;
+        const size_t smem = plan.smem;
+        const dim3 grid = plan.grid;
+        const bool multi = plan.max_items == 4;
 #define MZ_CONV(PP, SS)                                                                                         \
         if (P == PP && l.stride == SS) {                                                                        \
             auto kern = multi ? conv3x3_kernel<PP, SS, 4> : conv3x3_kernel<PP, SS, 1>;                          \
@@ -1188,39 +1246,57 @@ void resnet_use_strict(ResNetDevice* r) {
     r->state_elems = r->C * r->hh * r->hw;           // dense NCHW states: smaller than the board layout, the pool fits
 }
 
+// Launch plan of conv3x3_kernel for a shape (host only, behind mz_debug_conv3x3_plan): plan[11] = {P, stride, MAX_ITEMS,
+// bands, band_rows, boards per CTA, cin chunk, grid x, grid y, grid z, shared-memory bytes}.
+bool resnet_conv_plan(int n, int cin, int cout, int H, int W, int stride, int64_t* plan, std::string* err) {
+    ConvPlan p;
+    if (!conv3x3_plan(n, cin, cout, H, W, stride, &p, err)) return false;
+    const int64_t out[11] = {p.P, p.stride, p.max_items, p.bands, p.band_rows, p.boards, p.cin_chunk,
+                             p.grid.x, p.grid.y, p.grid.z, (int64_t)p.smem};
+    for (int i = 0; i < 11; ++i) plan[i] = out[i];
+    return true;
+}
+
 // Stand-alone conv3x3 (+bias, +residual, +ReLU) on host NCHW data through either implementation.
-// Debug / parity entry point behind mz_debug_conv3x3.
-int resnet_debug_conv(int n, int C, int H, int W, const float* x, const float* w_oihw, const float* bias,
+// Debug / parity entry point behind mz_debug_conv3x3.  The CUDA-core kernel takes any cin, cout (a multiple of 4) and
+// stride 1 or 2; the tensor-core convs take 64 -> 64 at stride 1 on their boards only.
+int resnet_debug_conv(int n, int cin, int cout, int H, int W, int stride, const float* x, const float* w_oihw, const float* bias,
                       const float* residual, int relu, int use_tc, float* out, int sm_count, std::string* err) {
-    if (use_tc && !conv_tc_supported(C, H, W)) { *err = "shape not supported by the tensor-core conv"; return MZ_EUNSUPPORTED; }
-    if (C % 4) { *err = "C must be a multiple of 4"; return MZ_EINVAL; }
+    if (use_tc && (cin != cout || stride != 1 || !conv_tc_supported(cout, H, W))) {
+        *err = "shape not supported by the tensor-core conv"; return MZ_EUNSUPPORTED;
+    }
+    ConvPlan plan;
+    if (!conv3x3_plan(n, cin, cout, H, W, stride, &plan, err)) return MZ_EINVAL;
+    const int C = cout, Ho = conv_out(H, stride), Wo = conv_out(W, stride);
     MzNetDesc nd{};
-    nd.kind = MZ_NET_RESNET; nd.channels = C; nd.obs_c = C; nd.obs_h = H; nd.obs_w = W; nd.action_space = 1;
+    nd.kind = MZ_NET_RESNET; nd.channels = C; nd.obs_c = cin; nd.obs_h = H; nd.obs_w = W; nd.action_space = 1;
     ResNetDevice r{};
-    r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = H; r.hw = W;
+    r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = Ho; r.hw = Wo;
     // fake a one-tensor state_dict for pack_conv
-    MzTensor t{"conv.weight", w_oihw, (int64_t)C * C * 9};
+    MzTensor t{"conv.weight", w_oihw, (int64_t)cout * cin * 9};
     Loader L{&t, 1, err};
     std::vector<float> blob;
     std::vector<ConvLayer> layers;
     r.use_tc = use_tc != 0; r.split = use_tc == 2; r.tc_capable = true;
-    if (!pack_conv(L, "conv", "", C, C, 1, blob, layers, use_tc == 2 ? kLayoutSplit : (use_tc ? kLayoutF16 : 0), H, W)) return MZ_EINVAL;
+    if (!pack_conv(L, "conv", "", cin, cout, stride, blob, layers, use_tc == 2 ? kLayoutSplit : (use_tc ? kLayoutF16 : 0), H, W))
+        return MZ_EINVAL;
     long bias_off = -1;
     if (bias) { bias_off = (long)blob.size(); blob.insert(blob.end(), bias, bias + C); while (blob.size() % 4) blob.push_back(0.f); }
     layers[0].b_off = bias_off;
     const bool split = use_tc == 2;
-    const size_t dense = (size_t)n * C * H * W, packed = (size_t)n * conv_tc_board_elems(split);
+    const size_t dense_in = (size_t)n * cin * H * W, dense = (size_t)n * C * Ho * Wo, packed = (size_t)n * conv_tc_board_elems(split);
     float *d_blob = nullptr, *d_x = nullptr, *d_res = nullptr, *d_out = nullptr, *d_px = nullptr, *d_pres = nullptr, *d_pout = nullptr;
     auto cleanup = [&]() { for (float* p : {d_blob, d_x, d_res, d_out, d_px, d_pres, d_pout}) if (p) cudaFree(p); };
-    bool ok = cudaMalloc(&d_blob, blob.size() * 4) == cudaSuccess && cudaMalloc(&d_x, dense * 4) == cudaSuccess &&
+    bool ok = cudaMalloc(&d_blob, blob.size() * 4) == cudaSuccess && cudaMalloc(&d_x, dense_in * 4) == cudaSuccess &&
               cudaMalloc(&d_out, dense * 4) == cudaSuccess && (!residual || cudaMalloc(&d_res, dense * 4) == cudaSuccess);
     if (ok && use_tc)
         ok = cudaMalloc(&d_px, packed * 4) == cudaSuccess && cudaMalloc(&d_pout, packed * 4) == cudaSuccess &&
              (!residual || cudaMalloc(&d_pres, packed * 4) == cudaSuccess);
     if (!ok) { cleanup(); *err = "allocation failed"; return MZ_ENOMEM; }
     cudaMemcpy(d_blob, blob.data(), blob.size() * 4, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_x, x, dense * 4, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_x, x, dense_in * 4, cudaMemcpyHostToDevice);
     if (residual) cudaMemcpy(d_res, residual, dense * 4, cudaMemcpyHostToDevice);
+    cudaMemset(d_out, 0xFF, dense * 4);                 // NaN: an output element the kernel does not write cannot pass a test
     r.d_conv = d_blob;
     int64_t launches = 0;
     Runner R{&r, nullptr, &launches, err, n};
@@ -1252,9 +1328,10 @@ int resnet_debug_conv(int n, int C, int H, int W, const float* x, const float* w
         cudaEventSynchronize(e1);
         float ms = 0.f;
         cudaEventElapsedTime(&ms, e0, e1);
-        const double flops = 2.0 * n * H * W * (double)C * C * 9;
-        fprintf(stderr, "[mz_debug_conv3x3] %s n=%d C=%d %dx%d residual=%d: %.2f us per launch, %.1f TFLOP/s useful\n",
-                use_tc ? "wgmma" : "cuda-core", n, C, H, W, residual ? 1 : 0, 1000.0 * ms / reps, flops / (ms / reps * 1e-3) / 1e12);
+        const double flops = 2.0 * n * Ho * Wo * (double)cin * cout * 9;
+        fprintf(stderr, "[mz_debug_conv3x3] %s n=%d %d->%d %dx%d stride %d residual=%d: %.2f us per launch, %.1f TFLOP/s useful\n",
+                use_tc ? "wgmma" : "cuda-core", n, cin, cout, H, W, stride, residual ? 1 : 0, 1000.0 * ms / reps,
+                flops / (ms / reps * 1e-3) / 1e12);
         cudaEventDestroy(e0); cudaEventDestroy(e1);
     }
     if (good) cudaMemcpy(out, d_out, dense * 4, cudaMemcpyDeviceToHost);

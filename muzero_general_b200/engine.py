@@ -471,19 +471,29 @@ def parse_staged_games(buf: bytes, index):
     return games
 
 
-def debug_conv3x3(x, w, bias=None, residual=None, relu=False, tensor_cores=False, device=0):
-    """One conv3x3 (pad 1, stride 1) on the device through mz_debug_conv3x3; numpy NCHW in and out.
+def debug_conv3x3(x, w, bias=None, residual=None, relu=False, tensor_cores=False, device=0, stride=1):
+    """One conv3x3 (pad 1, stride 1 or 2) on the device through mz_debug_conv3x3; numpy NCHW in and out.
+    x is [n, Cin, H, W], w [Cout, Cin, 3, 3], bias [Cout], residual and the result [n, Cout, Ho, Wo].
     ``tensor_cores``: False / "off" = CUDA cores, "fp16" = wgmma with fp16 operands, True / "x3" = wgmma on split operands."""
     lib = _lib.load_library()
     x = numpy.ascontiguousarray(x, numpy.float32)
     w = numpy.ascontiguousarray(w, numpy.float32)
-    n, Cc, H, W = x.shape
-    out = numpy.empty_like(x)
+    n, cin, H, W = x.shape
+    cout = w.shape[0]
+    if w.shape != (cout, cin, 3, 3):
+        raise ValueError(f"weights {w.shape} do not fit {cin} input channels")
+    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+    out = numpy.empty((n, cout, Ho, Wo), numpy.float32)
     b = None if bias is None else numpy.ascontiguousarray(bias, numpy.float32)
     r = None if residual is None else numpy.ascontiguousarray(residual, numpy.float32)
+    if b is not None and b.shape != (cout,):
+        raise ValueError(f"bias {b.shape} does not fit {cout} output channels")
+    if r is not None and r.shape != out.shape:
+        raise ValueError(f"residual {r.shape} does not match the output {out.shape}")
     mode = {False: 0, True: 2, "off": 0, "fp16": 1, "x3": 2}[tensor_cores]
-    rc = lib.mz_debug_conv3x3(device, n, Cc, H, W, x.ctypes.data, w.ctypes.data, None if b is None else b.ctypes.data,
-                              None if r is None else r.ctypes.data, int(relu), mode, out.ctypes.data)
+    rc = lib.mz_debug_conv3x3(device, n, cin, cout, H, W, stride, x.ctypes.data, w.ctypes.data,
+                              None if b is None else b.ctypes.data, None if r is None else r.ctypes.data, int(relu), mode,
+                              out.ctypes.data)
     if rc != 0:
         raise _lib.MzError(rc, lib.mz_last_error(None).decode())
     return out

@@ -20,12 +20,14 @@ Routes (``ROUTES``) and the cases that take them:
   small_tower     fused CUDA-core tower (small_tower.cu): st_c32_6x7, st_16x8_c16, st_1x2, st_c32_const,
                   st_c32_tiny, st_1x2_b0 (no blocks)
   per_layer       one conv3x3 launch per conv: pl_9x9_c32, pl_c48_6x7 (48 channels: no tensor cores, and the weights
-                  of a block exceed the fused tower's shared memory), pl_3x3_nofuse (MZ_NO_FUSE=1), pl_9x9_wide
+                  of a block exceed the fused tower's shared memory), pl_3x3_nofuse (MZ_NO_FUSE=1), pl_9x9_wide,
+                  pl_c96_6x7 (96 channels: a full cout tile of 64 and a last one of 32)
   small_search    fused small-network search (small_search.cu): ss_3x3_a2_c8, ss_3x3_a16_c20 (two blocks; with 32
                   channels the weights of two blocks exceed shared memory), ss_5x6_a4, ss_7x3_a12, ss_5x6_tiny
   heads_wide      heads_kernel<128> (C*HW > 1024) on the CUDA-core route: hw_c128_6x7
   heads_big       generic heads route (weights beyond shared memory) on the CUDA-core route: hb_c32_6x7
-  downsample      DownSample stem: ds_20x24 (3 x 20 x 24 frames -> 2 x 2 hidden, 16 channels)
+  downsample      DownSample stem: ds_20x24 (3 x 20 x 24 frames -> 2 x 2 hidden, 16 channels), ds_c96_20x24 (96
+                  channels: the stride-2 48 -> 96 conv and the 96-channel blocks have a 32-channel last cout tile)
 
 Edge weights (``edge_weights``), applied to the representation and dynamics towers:
 
@@ -118,6 +120,7 @@ CASES = [
     NetCase("pl_c48_6x7", "connect4", "per_layer", dict(channels=48)),
     NetCase("pl_3x3_nofuse", "tictactoe", "per_layer", env=dict(MZ_NO_FUSE="1")),
     NetCase("pl_9x9_wide", "connect4", "per_layer", _board(9, 9, 9, c=32, blocks=1), weights="wide"),
+    NetCase("pl_c96_6x7", "connect4", "per_layer", dict(channels=96, blocks=1)),
 
     NetCase("ss_3x3_a2_c8", "tictactoe", "small_search", _board(3, 3, 2, c=8, blocks=1)),
     NetCase("ss_3x3_a16_c20", "tictactoe", "small_search", _board(3, 3, 16, c=20, blocks=2)),
@@ -130,13 +133,15 @@ CASES = [
                                                           resnet_fc_value_layers=[128])),
     NetCase("ds_20x24", "connect4", "downsample", dict(observation_shape=(3, 20, 24), action_space=list(range(4)),
                                                        channels=16, blocks=1, downsample="resnet", **_HEADS16)),
+    NetCase("ds_c96_20x24", "connect4", "downsample", dict(observation_shape=(3, 20, 24), action_space=list(range(4)),
+                                                           channels=96, blocks=1, downsample="resnet", **_HEADS16)),
 ]
 
 BY_NAME = {c.name: c for c in CASES}
 
 # in-search parity: one case per residual route (the tensor-core case in x3 with one and two graph partitions and in
 # fp16; the nets kept off the tensor cores by their heads, in fp16 and x3) and every FC route
-SEARCH_CASES = ["pl_9x9_c32", "st_c32_6x7", "ss_5x6_a4", "ss_7x3_a12", "tc_6x7", "tc_6x7_s300", "tc_6x7_bigheads",
+SEARCH_CASES = ["pl_9x9_c32", "pl_c96_6x7", "st_c32_6x7", "ss_5x6_a4", "ss_7x3_a12", "tc_6x7", "tc_6x7_s300", "tc_6x7_bigheads",
                 "fc_cartpole", "fc_cartpole_s20", "fc_e5_a3", "fc_a40"]
 
 
