@@ -315,11 +315,28 @@ typedef struct MzSelfPlayPeek {
  *   int64 game_id; int32 slot; int32 length T; int32 first_to_play; int32 obs_elems O; int32 actions A; int32 bytes;
  *   double root_value[T]; int32 visit_counts[T][A]; int32 action[T]; float reward[T]; int32 to_play[T] (after the move);
  *   float priority[T] (zeros unless td_steps > 0); float observation[T+1][O] (index 0 = reset observation); padding to 8.
- * = the fields of GameHistory (self_play.py:479-511) minus the dummy first entries. */
+ * = the fields of GameHistory (self_play.py:479-511) minus the dummy first entries.
+ * In test-mode games (mz_selfplay_begin_vs with an opponent) a move the opponent played has root_value NaN and all
+ * visit counts 0 (store_search_statistics(None), self_play.py:496-511: root_values holds None there and child_visits
+ * has no row); its action, reward, to_play and observation are recorded like MuZero's. */
 #define MZ_STAGED_HEADER_BYTES 32
 
 /* replaces the per-move body of SelfPlay.play_game / continuous_self_play for a whole batch (self_play.py:31-183) */
 int mz_selfplay_begin(MzHandle* h, const MzSelfPlayDesc* desc);
+
+/* Opponents of test-mode games (SelfPlay.select_opponent_action, self_play.py:188-220), board games only:
+ *   EXPERT  Game.expert_agent (games/tictactoe.py:308-349, games/connect4.py:307-343): a win, else the last block the
+ *           scan finds, else the random default;
+ *   RANDOM  the random default: the legal action with index floor(u * n_legal) in ascending order, u from the Philox
+ *           stream tag 0x7169E005 at counter (game id, move, 0, game id >> 32). */
+enum { MZ_OPPONENT_SELF = 0, MZ_OPPONENT_EXPERT = 1, MZ_OPPONENT_RANDOM = 2 };
+
+/* play_game(temperature, threshold, False, opponent, muzero_player) (self_play.py:110-183) for a whole batch:
+ * mz_selfplay_begin with the opponent playing every move whose to_play is not muzero_player, in the same step, so
+ * every search is at MuZero's turn (the opponent opens a game when muzero_player is 1).  max_moves counts both sides'
+ * moves, and so does MzSelfPlayStats.env_steps.  mz_selfplay_begin(h, d) is mz_selfplay_begin_vs(h, d, MZ_OPPONENT_SELF, 0).
+ * Refused: an opponent on CartPole, muzero_player outside {0, 1}, td_steps > 0 with an opponent, an unknown opponent. */
+int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* desc, int32_t opponent, int32_t muzero_player);
 int mz_selfplay_moves(MzHandle* h, int32_t n_moves, double temperature, const MzSelfPlayInject* inject, MzSelfPlayStats* stats);
 /* the same in two halves, so the host can work while the device plays: enqueue returns at once, wait synchronises */
 int mz_selfplay_enqueue(MzHandle* h, int32_t n_moves, double temperature);
@@ -330,6 +347,13 @@ int mz_selfplay_wait(MzHandle* h, MzSelfPlayStats* stats);
  * {byte offset of the game's block, (slot << 32) | length}, so a consumer can address any game without walking. */
 int mz_selfplay_drain(MzHandle* h, const void** data, uint64_t* bytes, int32_t* n_games, const uint64_t** index);
 int mz_selfplay_peek(MzHandle* h, const MzSelfPlayPeek* out);
+
+/* Debug / parity: the device opponent (MZ_OPPONENT_EXPERT or MZ_OPPONENT_RANDOM) of env (MZ_ENV_TICTACTOE or
+ * MZ_ENV_CONNECT4) on n host positions.  board is [n][H*W] of +1 / -1 / 0 (row 0 = bottom), player [n] the side to
+ * move (+1 / -1).  The random default is the pick for uniform[i], or default_action[i] when default_action is not NULL
+ * (one of the two must be given).  out [n] receives the actions. */
+int mz_debug_opponent_action(int device, int32_t env, int32_t opponent, int32_t n, const int8_t* board,
+                             const int8_t* player, const double* uniform, const int32_t* default_action, int32_t* out);
 
 #ifdef __cplusplus
 }

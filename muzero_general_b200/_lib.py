@@ -109,6 +109,7 @@ class MzSelfPlayPeek(C.Structure):
 
 
 MZ_ENV_CARTPOLE, MZ_ENV_TICTACTOE, MZ_ENV_CONNECT4 = 0, 1, 2
+MZ_OPPONENT_SELF, MZ_OPPONENT_EXPERT, MZ_OPPONENT_RANDOM = 0, 1, 2
 MZ_STAGED_HEADER_BYTES = 32
 
 # every symbol include/mzb200.h declares: (name, restype, argtypes)
@@ -132,12 +133,15 @@ SYMBOLS = [
     ("mz_kernel_times", C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
     ("mz_numerics", C.c_char_p, [C.c_void_p]),
     ("mz_selfplay_begin", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayDesc)]),
+    ("mz_selfplay_begin_vs", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayDesc), C.c_int32, C.c_int32]),
     ("mz_selfplay_moves", C.c_int, [C.c_void_p, C.c_int32, C.c_double, C.POINTER(MzSelfPlayInject), C.POINTER(MzSelfPlayStats)]),
     ("mz_selfplay_enqueue", C.c_int, [C.c_void_p, C.c_int32, C.c_double]),
     ("mz_selfplay_wait", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayStats)]),
     ("mz_selfplay_drain", C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_int32),
                                     C.POINTER(C.c_void_p)]),
     ("mz_selfplay_peek", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayPeek)]),
+    ("mz_debug_opponent_action", C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]),
     ("mz_debug_small_search_plan", C.c_int, [C.c_int32] * 10 + [C.POINTER(C.c_int64)]),
     ("mz_debug_conv3x3_plan", C.c_int, [C.c_int32] * 6 + [C.POINTER(C.c_int64)]),
     ("mz_debug_conv3x3", C.c_int, [C.c_int] + [C.c_int32] * 6 + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

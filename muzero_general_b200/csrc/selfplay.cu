@@ -15,7 +15,12 @@
 // mapped pinned host memory (no per-move D2H, no host-side bookkeeping per move).
 //
 // Random draws: Philox4x32-10 keyed by (seed, global game id, move): root noise and first-simulation ties inside the
-// search (tree.cuh), the action sample here (tag kTagAction), CartPole's reset state (tag kTagReset).
+// search (tree.cuh), the action sample here (tag kTagAction), CartPole's reset state (tag kTagReset), the opponent's
+// random default move in test-mode games (tag kTagOpponent).
+//
+// Test-mode games (mz_selfplay_begin_vs, the reference's play_game(0, ..., opponent, muzero_player),
+// self_play.py:110-183): the opponent's move is played by the thread that played MuZero's, right after it (or by
+// start_game when the opponent moves first), so every search runs at MuZero's turn.
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -26,10 +31,13 @@
 namespace mz {
 
 constexpr uint32_t kTagReset = 0x7169E004u;
+constexpr uint32_t kTagOpponent = 0x7169E005u;
 constexpr int kMaxCells = 48;              // board cells per slot (Connect4: 42)
 
 struct SpDev {
     int env, B, A, O, H, W, K, max_moves, threshold, reward_scale;
+    int opponent;              // MZ_OPPONENT_*
+    int muzero_player;         // to_play of MuZero's side when opponent != MZ_OPPONENT_SELF
     uint64_t seed;
     int64_t id_stride;         // a slot's next game id = current + id_stride
     int td_steps;              // > 0: PER priorities are computed while packing (replay_buffer.py:33-51)
@@ -190,7 +198,111 @@ MZ_DEVINL void publish(const SpDev& s, int g) {
     }
 }
 
-MZ_DEVINL void start_game(const SpDev& s, int g, int64_t gid) {
+// numpy.random.choice(legal actions) for the uniform u: the legal action with index floor(u * n_legal), ascending
+MZ_DEVINL int uniform_legal_pick(const uint8_t* lg, int A, double u) {
+    int n_legal = 0, last = 0;
+    for (int k = 0; k < A; ++k) if (lg[k]) { ++n_legal; last = k; }
+    int idx = (int)(u * n_legal);
+    if (idx >= n_legal) idx = n_legal - 1;
+    for (int k = 0; k < A; ++k) if (lg[k] && idx-- == 0) return k;
+    return last;
+}
+
+// ------------------------------------------------------------------------------------------
+// the opponent of test-mode games (self_play.py:188-220)
+// ------------------------------------------------------------------------------------------
+// One window of the expert's scan (games/_boards.py::_threat_scan): `len` cells from (y0, x0) in steps (dy, dx).  A
+// window whose stones sum to +-(len - 1) has one empty cell; its action becomes the candidate (a block, which a later
+// window may overwrite) and returns true when the window is the mover's own (a win).  fixed >= 0: Connect4's vertical
+// check, which names its column without looking at the gap.  Connect4 counts a gap only if it is the next free cell
+// of its column (height = stones in the column, numpy.count_nonzero(board[:, x])).
+MZ_DEVINL bool expert_window(const SpDev& s, const int8_t* b, int me, int y0, int x0, int dy, int dx, int len, int fixed,
+                             int* action) {
+    int sum = 0, gy = -1, gx = -1;
+    for (int j = 0; j < len; ++j) {
+        const int y = y0 + j * dy, x = x0 + j * dx;
+        const int v = b[y * s.W + x];
+        sum += v;
+        if (v == 0 && gy < 0) { gy = y; gx = x; }
+    }
+    if (sum != len - 1 && sum != 1 - len) return false;
+    if (fixed >= 0) {
+        *action = fixed;
+    } else if (s.env == MZ_ENV_CONNECT4) {
+        int height = 0;
+        for (int y = 0; y < s.H; ++y) height += b[y * s.W + gx] != 0;
+        if (height != gy) return false;
+        *action = gx;
+    } else {
+        *action = gy * s.W + gx;
+    }
+    return me * sum > 0;
+}
+
+// expert_action of games/tictactoe.py:308-349 and games/connect4.py:307-343 in their scan order; `dflt` is the random
+// legal move the reference draws first
+MZ_DEVINL int expert_action(const SpDev& s, int g, int dflt) {
+    const int8_t* b = s.board + (size_t)g * kMaxCells;
+    const int me = s.player[g];
+    int a = dflt;
+    if (s.env == MZ_ENV_TICTACTOE) {
+        for (int i = 0; i < 3; ++i) {
+            if (expert_window(s, b, me, i, 0, 0, 1, 3, -1, &a)) return a;       // row i
+            if (expert_window(s, b, me, 0, i, 1, 0, 3, -1, &a)) return a;       // column i
+        }
+        if (expert_window(s, b, me, 0, 0, 1, 1, 3, -1, &a)) return a;           // diagonal
+        if (expert_window(s, b, me, 0, 2, 1, -1, 3, -1, &a)) return a;          // numpy.fliplr(board).diagonal()
+        return a;
+    }
+    for (int k = 0; k < 3; ++k)                                                  // 4x4 sub-board rows k.., columns l..
+        for (int l = 0; l < 4; ++l) {
+            for (int i = 0; i < 4; ++i) {
+                if (expert_window(s, b, me, k + i, l, 0, 1, 4, -1, &a)) return a;
+                if (expert_window(s, b, me, k, l + i, 1, 0, 4, l + i, &a)) return a;
+            }
+            if (expert_window(s, b, me, k, l, 1, 1, 4, -1, &a)) return a;
+            if (expert_window(s, b, me, k, l + 3, 1, -1, 4, -1, &a)) return a;
+        }
+    return a;
+}
+
+// the opponent's move in slot g (legal mask published): the random legal default for the uniform u (or `dflt` when
+// >= 0), improved by the expert's scan for MZ_OPPONENT_EXPERT
+MZ_DEVINL int opponent_action(const SpDev& s, int g, double u, int dflt = -1) {
+    const int d = dflt >= 0 ? dflt : uniform_legal_pick(s.legal + (size_t)g * s.A, s.A, u);
+    return s.opponent == MZ_OPPONENT_EXPERT ? expert_action(s, g, d) : d;
+}
+
+// record of move t of slot g, then the slot's search inputs for the next move (store_search_statistics uses the
+// pre-step root, self_play.py:169-175); root NaN and visits nullptr (all zero) mark a move no search chose
+MZ_DEVINL void record_move(const SpDev& s, int g, int t, int action, float reward, double root, const int32_t* visits) {
+    const size_t r = (size_t)g * s.max_moves + t;
+    s.rec_root[r] = root;
+    for (int k = 0; k < s.A; ++k) s.rec_visits[r * s.A + k] = visits ? visits[k] : 0;
+    s.rec_action[r] = action;
+    s.rec_reward[r] = reward;
+    publish(s, g);
+    s.rec_to_play[r] = s.to_play[g];
+    const float* o = s.obs + (size_t)g * s.O;
+    float* ro = s.rec_obs + ((size_t)g * (s.max_moves + 1) + t + 1) * s.O;
+    for (int i = 0; i < s.O; ++i) ro[i] = o[i];
+    s.move[g] = t + 1;
+    s.last_action[g] = action;
+}
+
+// plays and records the opponent's move s.move[g] in slot g; returns done
+MZ_DEVINL bool opponent_move(const SpDev& s, int g) {
+    const int t = s.move[g];
+    const double u = philox_uniform53(s.seed, s.game_id[g], t, 0u, kTagOpponent);
+    const int action = opponent_action(s, g, u);
+    bool won, done;
+    board_step(s, g, action, &won, &done);
+    record_move(s, g, t, action, won ? (float)s.reward_scale : 0.0f, __longlong_as_double(0x7FF8000000000000ll), nullptr);
+    return done;
+}
+
+// starts game gid in slot g; returns the moves played (1 when the opponent opens)
+MZ_DEVINL int start_game(const SpDev& s, int g, int64_t gid) {
     s.game_id[g] = gid;
     s.move[g] = 0;
     s.fin[g] = 0;
@@ -201,12 +313,17 @@ MZ_DEVINL void start_game(const SpDev& s, int g, int64_t gid) {
     const float* o = s.obs + (size_t)g * s.O;
     float* r0 = s.rec_obs + (size_t)g * (s.max_moves + 1) * s.O;
     for (int i = 0; i < s.O; ++i) r0[i] = o[i];
+    if (s.opponent == MZ_OPPONENT_SELF || s.to_play[g] == s.muzero_player) return 0;
+    const bool done = opponent_move(s, g);
+    if (done || s.move[g] >= s.max_moves) s.fin[g] = s.move[g];
+    return 1;
 }
 
 __global__ void selfplay_reset_kernel(const SpDev s, int64_t first_game_id) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= s.B) return;
-    start_game(s, g, first_game_id + g);
+    const int played = start_game(s, g, first_game_id + g);
+    if (played) atomicAdd(&s.counters[0], (unsigned long long)played);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -221,14 +338,7 @@ MZ_DEVINL int sample_action(const SpDev& s, int g, double temperature, double u)
         for (int k = 0; k < A; ++k) if (lg[k] && v[k] > best) { best = v[k]; arg = k; }
         return arg;
     }
-    int n_legal = 0, last = 0;
-    for (int k = 0; k < A; ++k) if (lg[k]) { ++n_legal; last = k; }
-    if (isinf(temperature)) {                                  // numpy.random.choice(actions)
-        int idx = (int)(u * n_legal);
-        if (idx >= n_legal) idx = n_legal - 1;
-        for (int k = 0; k < A; ++k) if (lg[k] && idx-- == 0) return k;
-        return last;
-    }
+    if (isinf(temperature)) return uniform_legal_pick(lg, A, u);   // numpy.random.choice(actions)
     // numpy.random.choice(actions, p=p) with p = visit_counts ** (1 / T) / sum(...): cdf = p.cumsum(), cdf /= cdf[-1],
     // then the number of cdf entries <= u.  Illegal actions carry p = 0 and repeat the previous entry, so counting
     // over the whole action space lands on the same legal action; after the division the last entry is exactly 1 > u.
@@ -254,8 +364,9 @@ MZ_DEVINL int sample_action(const SpDev& s, int g, double temperature, double u)
     return pick;
 }
 
-// select_action + Game.step + record for slot g (one thread)
-MZ_DEVINL void slot_act(const SpDev& s, int g) {
+// select_action + Game.step + record for slot g (one thread), then the opponent's reply in a test-mode game; returns
+// the moves played
+MZ_DEVINL int slot_act(const SpDev& s, int g) {
     const int t = s.move[g];
     const int64_t gid = s.game_id[g];
     int action = s.forced_action ? s.forced_action[g] : -1;
@@ -274,20 +385,15 @@ MZ_DEVINL void slot_act(const SpDev& s, int g) {
         board_step(s, g, action, &won, &done);
         reward = won ? (float)s.reward_scale : 0.0f;
     }
-    // record of move t (store_search_statistics uses the pre-step root, self_play.py:169-175)
-    const size_t r = (size_t)g * s.max_moves + t;
-    s.rec_root[r] = s.root_value[g];
-    for (int k = 0; k < s.A; ++k) s.rec_visits[r * s.A + k] = s.visits[(size_t)g * s.A + k];
-    s.rec_action[r] = action;
-    s.rec_reward[r] = reward;
-    publish(s, g);
-    s.rec_to_play[r] = s.to_play[g];
-    const float* o = s.obs + (size_t)g * s.O;
-    float* ro = s.rec_obs + ((size_t)g * (s.max_moves + 1) + t + 1) * s.O;
-    for (int i = 0; i < s.O; ++i) ro[i] = o[i];
-    s.move[g] = t + 1;
-    s.last_action[g] = action;
-    if (done || t + 1 >= s.max_moves) s.fin[g] = t + 1;
+    record_move(s, g, t, action, reward, s.root_value[g], s.visits + (size_t)g * s.A);
+    int played = 1;
+    // len(action_history) <= max_moves (self_play.py:123) counts both sides' moves
+    if (s.opponent != MZ_OPPONENT_SELF && !done && t + 1 < s.max_moves && s.to_play[g] != s.muzero_player) {
+        done = opponent_move(s, g);
+        ++played;
+    }
+    if (done || s.move[g] >= s.max_moves) s.fin[g] = s.move[g];
+    return played;
 }
 
 __host__ __device__ inline unsigned long long staged_block_bytes(int T, int A, int O) {
@@ -344,8 +450,7 @@ __global__ void __launch_bounds__(kStepThreads) selfplay_step_kernel(const SpDev
         if (lane == 0) {
             T = s.fin[g];
             if (act && T == 0) {
-                slot_act(s, g);
-                atomicAdd(&s_active, 1);
+                atomicAdd(&s_active, slot_act(s, g));
                 T = s.fin[g];
             }
         }
@@ -406,7 +511,10 @@ __global__ void __launch_bounds__(kStepThreads) selfplay_step_kernel(const SpDev
                 for (int i = lane; i < (T + 1) * s.O; i += 32) f[i] = src[i];
             }
             __syncwarp();
-            if (lane == 0) start_game(s, g, s.game_id[g] + s.id_stride);
+            if (lane == 0) {
+                const int played = start_game(s, g, s.game_id[g] + s.id_stride);
+                if (played) atomicAdd(&s_active, played);
+            }
         }
     }
     __syncthreads();
@@ -464,7 +572,20 @@ static bool sp_alloc(MzSelfPlay* sp, T** p, size_t count) {
 }
 
 extern "C" int mz_selfplay_begin(MzHandle* h, const MzSelfPlayDesc* d) {
+    return mz_selfplay_begin_vs(h, d, MZ_OPPONENT_SELF, 0);
+}
+
+extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int32_t muzero_player) {
     if (!h || !d) return fail(h, MZ_EINVAL, "mz_selfplay_begin: null argument");
+    if (opponent != MZ_OPPONENT_SELF && opponent != MZ_OPPONENT_EXPERT && opponent != MZ_OPPONENT_RANDOM)
+        return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin_vs: unknown opponent " + std::to_string(opponent));
+    if (muzero_player != 0 && muzero_player != 1)
+        return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: muzero_player must be 0 or 1, got " + std::to_string(muzero_player));
+    if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_CARTPOLE)
+        return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: CartPole has one player, its opponent is \"self\"");
+    if (opponent != MZ_OPPONENT_SELF && d->td_steps > 0)
+        return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: test-mode games are not saved to a replay buffer, td_steps must be 0 "
+                                  "(an opponent's move has no root value to bootstrap from)");
     MZ_CUDA(h, cudaSetDevice(h->device));
     MZ_CUDA(h, cudaStreamSynchronize(h->stream));
     mz_selfplay_destroy(h);
@@ -484,6 +605,7 @@ extern "C" int mz_selfplay_begin(MzHandle* h, const MzSelfPlayDesc* d) {
     SpDev& s = sp->dev;
     s.env = d->env; s.B = B; s.A = A; s.O = O; s.H = H; s.W = W; s.K = K; s.max_moves = d->max_moves;
     s.threshold = d->temperature_threshold; s.reward_scale = d->reward_scale; s.seed = h->search.seed;
+    s.opponent = opponent; s.muzero_player = muzero_player;
     s.id_stride = d->game_id_stride > 0 ? d->game_id_stride : B;
     s.td_steps = 0; s.per_alpha = 1.0; s.discount_pow = nullptr;
     if (d->td_steps > 0) {
@@ -688,5 +810,68 @@ extern "C" int mz_selfplay_peek(MzHandle* h, const MzSelfPlayPeek* out) {
     if (out->game_id) MZ_CUDA(h, cudaMemcpy(out->game_id, s.game_id, B * 8, cudaMemcpyDeviceToHost));
     if (out->move_index) MZ_CUDA(h, cudaMemcpy(out->move_index, s.move, B * 4, cudaMemcpyDeviceToHost));
     if (out->last_action) MZ_CUDA(h, cudaMemcpy(out->last_action, s.last_action, B * 4, cudaMemcpyDeviceToHost));
+    return MZ_OK;
+}
+
+// debug: opponent_action over host positions, one thread per position
+__global__ void opponent_debug_kernel(const SpDev s, const double* uniform, const int32_t* dflt, int32_t* out) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= s.B) return;
+    board_legal(s, g, s.legal + (size_t)g * s.A);
+    out[g] = opponent_action(s, g, uniform ? uniform[g] : 0.0, dflt ? dflt[g] : -1);
+}
+
+extern "C" int mz_debug_opponent_action(int device, int32_t env, int32_t opponent, int32_t n, const int8_t* board,
+                                        const int8_t* player, const double* uniform, const int32_t* default_action,
+                                        int32_t* out) {
+    SpDev s{};
+    switch (env) {
+        case MZ_ENV_TICTACTOE: s.H = 3; s.W = 3; s.K = 3; s.A = 9; break;
+        case MZ_ENV_CONNECT4: s.H = 6; s.W = 7; s.K = 4; s.A = 7; break;
+        default: return fail(nullptr, MZ_EUNSUPPORTED, "mz_debug_opponent_action: no opponent for this environment");
+    }
+    if (opponent != MZ_OPPONENT_EXPERT && opponent != MZ_OPPONENT_RANDOM)
+        return fail(nullptr, MZ_EUNSUPPORTED, "mz_debug_opponent_action: opponent must be MZ_OPPONENT_EXPERT or MZ_OPPONENT_RANDOM");
+    if (n < 1 || !board || !player || !out || (!uniform && !default_action))
+        return fail(nullptr, MZ_EINVAL, "mz_debug_opponent_action: bad argument");
+    const int cells = s.H * s.W;
+    for (int i = 0; i < n; ++i) {
+        if (player[i] != 1 && player[i] != -1) return fail(nullptr, MZ_EINVAL, "mz_debug_opponent_action: player must be +1 or -1");
+        if (uniform && !(uniform[i] >= 0.0 && uniform[i] < 1.0)) return fail(nullptr, MZ_EINVAL, "mz_debug_opponent_action: uniforms must lie in [0, 1)");
+        if (default_action && (default_action[i] < 0 || default_action[i] >= s.A))
+            return fail(nullptr, MZ_EINVAL, "mz_debug_opponent_action: default action out of range");
+        bool any = false;
+        for (int c = 0; c < cells; ++c) {
+            if (board[(size_t)i * cells + c] < -1 || board[(size_t)i * cells + c] > 1)
+                return fail(nullptr, MZ_EINVAL, "mz_debug_opponent_action: board cells must be +1, -1 or 0");
+            any |= board[(size_t)i * cells + c] == 0 && (env == MZ_ENV_TICTACTOE || c >= (s.H - 1) * s.W);
+        }
+        if (!any) return fail(nullptr, MZ_EINVAL, "mz_debug_opponent_action: a position without a legal action");
+    }
+    if (cudaSetDevice(device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_opponent_action: no such device");
+    s.env = env; s.B = n; s.opponent = opponent;
+    void* mem = nullptr;
+    const size_t nb = (size_t)n * kMaxCells, np = (size_t)n, nl = (size_t)n * s.A, nu = (size_t)n * 8, nd = (size_t)n * 4, no = (size_t)n * 4;
+    const size_t o_player = nb, o_legal = o_player + np, o_u = (o_legal + nl + 7) & ~(size_t)7, o_d = o_u + nu, o_out = o_d + nd;
+    if (cudaMalloc(&mem, o_out + no) != cudaSuccess) { (void)cudaGetLastError(); return fail(nullptr, MZ_ENOMEM, "mz_debug_opponent_action: out of device memory"); }
+    unsigned char* base = static_cast<unsigned char*>(mem);
+    s.board = reinterpret_cast<int8_t*>(base);
+    s.player = reinterpret_cast<int8_t*>(base + o_player);
+    s.legal = base + o_legal;
+    double* d_u = uniform ? reinterpret_cast<double*>(base + o_u) : nullptr;
+    int32_t* d_d = default_action ? reinterpret_cast<int32_t*>(base + o_d) : nullptr;
+    int32_t* d_out = reinterpret_cast<int32_t*>(base + o_out);
+    cudaError_t e = cudaMemset(s.board, 0, nb);
+    if (e == cudaSuccess) e = cudaMemcpy2D(s.board, kMaxCells, board, cells, cells, n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(s.player, player, np, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && d_u) e = cudaMemcpy(d_u, uniform, nu, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && d_d) e = cudaMemcpy(d_d, default_action, nd, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        opponent_debug_kernel<<<(n + 127) / 128, 128>>>(s, d_u, d_d, d_out);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(out, d_out, no, cudaMemcpyDeviceToHost);
+    cudaFree(mem);
+    if (e != cudaSuccess) return fail(nullptr, MZ_ECUDA, std::string("mz_debug_opponent_action: ") + cudaGetErrorString(e));
     return MZ_OK;
 }

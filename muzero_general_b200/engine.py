@@ -362,13 +362,19 @@ class DeviceSelfPlayLoop:
     finished games handed back as packed struct-of-arrays blocks (SURVEY.md 8f-1, include/mzb200.h)."""
 
     ENVS = {"cartpole": _lib.MZ_ENV_CARTPOLE, "tictactoe": _lib.MZ_ENV_TICTACTOE, "connect4": _lib.MZ_ENV_CONNECT4}
+    OPPONENTS = {"self": _lib.MZ_OPPONENT_SELF, "expert": _lib.MZ_OPPONENT_EXPERT, "random": _lib.MZ_OPPONENT_RANDOM}
 
     def __init__(self, engine: SearchEngine, env: str, max_moves: int, temperature_threshold=None, reward_scale: int = 1,
                  first_game_id: int = 0, staging_bytes: int = 0, game_id_stride: int = 0, td_steps: int = 0,
-                 per_alpha: float = 1.0, discount: float = 1.0):
+                 per_alpha: float = 1.0, discount: float = 1.0, opponent: str = "self", muzero_player: int = 0):
+        """``opponent`` "expert" or "random" plays test-mode games (``play_game(..., opponent, muzero_player)``): the
+        opponent's moves are played on the device and recorded with a NaN root value and zero visit counts."""
         if env not in self.ENVS:
             raise NotImplementedError(f"no device-resident environment for {env!r}")
+        if opponent not in self.OPPONENTS:
+            raise NotImplementedError(f"no device opponent {opponent!r} (expected one of {sorted(self.OPPONENTS)})")
         self.engine = engine
+        self.opponent, self.muzero_player = opponent, int(muzero_player)
         d = _lib.MzSelfPlayDesc()
         d.env = self.ENVS[env]
         d.max_moves = int(max_moves)
@@ -383,7 +389,7 @@ class DeviceSelfPlayLoop:
             d.discount_pow = C.cast(self._discount_pow, C.c_void_p)
         self.with_priorities = bool(d.td_steps)
         d.staging_bytes = int(staging_bytes)
-        engine._check(engine.lib.mz_selfplay_begin(engine._h, C.byref(d)))
+        engine._check(engine.lib.mz_selfplay_begin_vs(engine._h, C.byref(d), self.OPPONENTS[opponent], self.muzero_player))
         self.stats = _lib.MzSelfPlayStats()
 
     def moves(self, n_moves: int, temperature: float, forced_action=None, uniform=None, noise=None, first_index=None):
@@ -469,6 +475,30 @@ def parse_staged_games(buf: bytes, index):
     for g, meta in zip(games, index[:, 1]):
         assert (int(meta) >> 32, int(meta) & 0xFFFFFFFF) == (g["slot"], g["length"])
     return games
+
+
+def debug_opponent_action(env, boards, players, uniforms=None, defaults=None, opponent="expert", device=0):
+    """The device opponent of test-mode games on host positions (mz_debug_opponent_action).  ``boards`` is
+    ``[n, H, W]`` (or ``[n, H*W]``) of +1 / -1 / 0 with row 0 at the bottom, ``players`` ``[n]`` the side to move
+    (+1 / -1).  The random default is the legal action with index ``floor(u * n_legal)`` for ``uniforms[i]``, or
+    ``defaults[i]`` when given.  Returns the ``[n]`` int32 actions."""
+    lib = _lib.load_library()
+    codes = {"tictactoe": _lib.MZ_ENV_TICTACTOE, "connect4": _lib.MZ_ENV_CONNECT4}
+    if env not in codes:
+        raise NotImplementedError(f"no device opponent for {env!r}")
+    b = numpy.ascontiguousarray(boards, numpy.int8)
+    n = b.shape[0]
+    b = b.reshape(n, -1)
+    p = numpy.ascontiguousarray(players, numpy.int8).reshape(n)
+    u = None if uniforms is None else numpy.ascontiguousarray(uniforms, numpy.float64).reshape(n)
+    d = None if defaults is None else numpy.ascontiguousarray(defaults, numpy.int32).reshape(n)
+    out = numpy.empty(n, numpy.int32)
+    rc = lib.mz_debug_opponent_action(device, codes[env], DeviceSelfPlayLoop.OPPONENTS[opponent], n, b.ctypes.data,
+                                      p.ctypes.data, None if u is None else u.ctypes.data,
+                                      None if d is None else d.ctypes.data, out.ctypes.data)
+    if rc != 0:
+        raise _lib.MzError(rc, lib.mz_last_error(None).decode())
+    return out
 
 
 def debug_conv3x3(x, w, bias=None, residual=None, relu=False, tensor_cores=False, device=0, stride=1):

@@ -372,9 +372,13 @@ class PackedGameHistory(GameHistory):
         d["action_history"] = [0] + list(g["action"].astype(numpy.int64))
         d["reward_history"] = [0] + [reward_type(r) for r in g["reward"].tolist()]
         d["to_play_history"] = [int(g["first_to_play"])] + g["to_play"].tolist()
-        visits = g["visits"]
+        # a test-mode game's opponent moves carry a NaN root value: store_search_statistics(None) (self_play.py:496-511)
+        # appends None to root_values and no child_visits row
+        root = g["root_value"]
+        searched = ~numpy.isnan(root)
+        visits = g["visits"][searched]
         d["child_visits"] = (visits / visits.sum(1, keepdims=True)).tolist()
-        d["root_values"] = g["root_value"].tolist()
+        d["root_values"] = [v if s else None for v, s in zip(root.tolist(), searched.tolist())]
 
     def __reduce__(self):
         self._materialise()
@@ -423,6 +427,10 @@ class SelfPlay:
         self._stream = None           # across play_games calls (its generator)
         self.played_games = 0
         self.played_steps = 0
+        self._next_test_game_id = self.first_game_id + self.TEST_GAME_IDS
+
+    # test-mode games are numbered from here, so they never share a random stream with a training game
+    TEST_GAME_IDS = 1 << 40
 
     # ------------------------------------------------------------------ reference loop
     def continuous_self_play(self, shared_storage, replay_buffer, test_mode=False):
@@ -631,6 +639,56 @@ class SelfPlay:
             out.extend(self._batched.move())
         return out
 
+    # ------------------------------------------------------------------ evaluation
+    def play_test_games(self, n_games, opponent=None, muzero_player=None, temperature=0):
+        """``n_games`` games of the reference's test worker (self_play.py:54-90), played as one device batch:
+        ``play_game(temperature, config.temperature_threshold, False, opponent, muzero_player)`` with the opponent
+        ("expert", "random" or "self") moving on the GPU.  ``opponent`` and ``muzero_player`` default to the config's,
+        like the test worker ("self" for one-player games).  Returns ``(PackedGames, summary)``: the games have the
+        reference's test-mode shape (``root_values`` is None at opponent moves, ``child_visits`` has rows for MuZero's
+        moves only), and ``summary`` holds the means over the games of what the test worker reports
+        (``episode_length``, ``total_reward``, ``mean_value``; ``muzero_reward`` and ``opponent_reward`` for two
+        players) plus ``games`` and MuZero's ``wins`` / ``draws`` / ``losses``.
+
+        The games returned are the ``n_games`` smallest game ids of the call (slot g plays ids first + g + k * stride),
+        not the first ``n_games`` to finish, which would over-represent short games; games begun past them are
+        discarded.  Every call starts a fresh device loop and later calls use new ids, so the same seed and sequence of
+        calls give the same games.  The device loop replaces the handle's self-play loop: with one running, call
+        ``reset_stream()`` first."""
+        cfg = self.config
+        if self._device_env_name() is None:
+            raise NotImplementedError(
+                "test games on the device need a device environment (CartPole, TicTacToe or Connect4 with "
+                "rng_mode='philox' and stacked_observations=0); play them one at a time with "
+                "play_game(0, config.temperature_threshold, False, opponent, muzero_player)")
+        if self._device_loop is not None:
+            raise RuntimeError("this worker's device self-play loop has games in flight, and starting test games on the "
+                               "same handle would drop them; call reset_stream() first")
+        n_games = int(n_games)
+        if n_games < 1:
+            raise ValueError("n_games must be >= 1")
+        if opponent is None:
+            opponent = "self" if len(cfg.players) == 1 else cfg.opponent
+        if muzero_player is None:
+            muzero_player = cfg.muzero_player
+        B, stride, first = self.num_parallel_games, self.game_id_stride, self._next_test_game_id
+        i = numpy.arange(n_games)
+        wanted = first + (i // B) * stride + i % B
+        dev = DeviceBatchedSelfPlay(self, cfg.temperature_threshold, opponent, muzero_player, first_game_id=first)
+        games = PackedGames(dev.obs_shape, dev.obs_dtype, dev.reward_type)
+        missing = n_games
+        while missing:
+            # a few moves per call: every move past the last wanted game's end is searched for the whole batch
+            for buf, index in dev.moves(min(dev.chunk, 4), temperature)._chunks:
+                ids = numpy.array([int(numpy.frombuffer(buf, numpy.int64, 1, int(off))[0]) for off in index[:, 0]])
+                keep = numpy.isin(ids, wanted)
+                games.add(buf, index[keep])
+                missing -= int(keep.sum())
+        # the next call starts past every id this one began
+        started = int(dev.loop.peek()["game_id"].max())
+        self._next_test_game_id = first + ((started - first) // stride + 1) * stride
+        return games, summarise_test_games(games, muzero_player, len(cfg.players))
+
     def close(self):
         self.model.engine.close()
 
@@ -689,20 +747,24 @@ class DeviceBatchedSelfPlay:
     ``first_game_id + g + k*B``; every random draw is a Philox stream keyed by (seed, global game id, move), so a
     game's history is independent of the batch size and of the number of ranks."""
 
-    def __init__(self, worker, temperature_threshold=None):
+    def __init__(self, worker, temperature_threshold=None, opponent="self", muzero_player=0, first_game_id=None):
         cfg = worker.config
         Game = worker.Game
         vec = getattr(Game, "VECTOR", None)
         self.obs_shape = tuple(cfg.observation_shape)
         self.obs_dtype = getattr(vec, "OBS_DTYPE", numpy.float32)
         self.reward_type = int if vec is not None else float
+        # test-mode games never reach a replay buffer (self_play.py:54-66): no priorities against an opponent
+        priorities = opponent == "self" and getattr(cfg, "PER", False) and getattr(cfg, "device_priorities", True)
         self.loop = DeviceSelfPlayLoop(worker.model.engine, Game.DEVICE_ENV, cfg.max_moves,
                                        temperature_threshold=temperature_threshold,
                                        reward_scale=getattr(vec, "REWARD_SCALE", 1),
-                                       first_game_id=worker.first_game_id, game_id_stride=worker.game_id_stride,
-                                       td_steps=int(cfg.td_steps) if getattr(cfg, "PER", False) and getattr(cfg, "device_priorities", True) else 0,
+                                       first_game_id=worker.first_game_id if first_game_id is None else first_game_id,
+                                       game_id_stride=worker.game_id_stride,
+                                       td_steps=int(cfg.td_steps) if priorities else 0,
                                        per_alpha=cfg.PER_alpha, discount=cfg.discount,
-                                       staging_bytes=int(getattr(cfg, "selfplay_staging_bytes", 0) or 0))
+                                       staging_bytes=int(getattr(cfg, "selfplay_staging_bytes", 0) or 0),
+                                       opponent=opponent, muzero_player=muzero_player)
         self.moves_per_call = int(getattr(cfg, "selfplay_moves_per_call", 64) or 64)   # upper bound of a chunk
         self.chunk = min(4, self.moves_per_call)                                      # adapted to the staging fill below
         self.device_ms = 0.0          # device time of all mz_selfplay_moves calls so far
@@ -804,6 +866,40 @@ class PackedGames:
                 return self._make(buf, index[i, 0])
             i -= len(index)
         raise IndexError("game index out of range")
+
+
+def summarise_test_games(games, muzero_player, num_players):
+    """Means over ``games`` (``PackedGames``) of what the reference's test worker reports per game
+    (self_play.py:67-90), read from the packed blocks without building the histories:
+      episode_length   len(action_history) - 1
+      total_reward     sum(reward_history)
+      mean_value       numpy.mean([v for v in root_values if v]): opponent moves (None) and zero values left out
+      muzero_reward    sum of the rewards of the moves made with to_play == muzero_player (two players)
+      opponent_reward  the same for the other side (two players)
+    plus ``games`` and, for two players, MuZero's ``wins`` / ``draws`` / ``losses`` (its reward above / equal to /
+    below the opponent's)."""
+    per = {"episode_length": [], "total_reward": [], "mean_value": []}
+    if num_players > 1:
+        per.update(muzero_reward=[], opponent_reward=[])
+    for buf, index in games._chunks:
+        for off in index[:, 0]:
+            g = parse_staged_game(buf, int(off))
+            reward = g["reward"].astype(numpy.float64)
+            root = g["root_value"]
+            values = root[~numpy.isnan(root) & (root != 0)]
+            per["episode_length"].append(g["length"])
+            per["total_reward"].append(reward.sum())
+            per["mean_value"].append(values.mean() if values.size else float("nan"))
+            if num_players > 1:
+                mover = numpy.concatenate(([g["first_to_play"]], g["to_play"][:-1]))      # to_play before each move
+                per["muzero_reward"].append(reward[mover == muzero_player].sum())
+                per["opponent_reward"].append(reward[mover != muzero_player].sum())
+    out = {k: float(numpy.mean(v)) for k, v in per.items()}
+    out["games"] = len(per["episode_length"])
+    if num_players > 1:
+        diff = numpy.array(per["muzero_reward"]) - numpy.array(per["opponent_reward"])
+        out.update(wins=int((diff > 0).sum()), draws=int((diff == 0).sum()), losses=int((diff < 0).sum()))
+    return out
 
 
 class BatchedSelfPlay:
