@@ -211,6 +211,9 @@ int64_t mz_launch_count(const MzHandle* h);
 int32_t mz_graph_partitions(const MzHandle* h);
 /* device time of the search kernels of the last mz_search call, ms (CUDA events on the library stream) */
 double mz_last_search_ms(const MzHandle* h);
+/* shape of the handle's last launch of the fused FC search kernel (csrc/fc_search.cu): returns 1 and fills info[5] =
+ * {grid, threads per CTA, lanes per game, shared-memory bytes per CTA, resident CTAs per SM}, or 0 before the first one */
+int mz_fc_last_launch(const MzHandle* h, int64_t* info);
 
 /* Per-kernel-class device timing for the roofline line of bench.py.  While enabled (process-wide), the step-wise
  * pipeline runs launch by launch with a CUDA event pair around every kernel instead of replaying its CUDA graph.
@@ -229,6 +232,17 @@ int mz_kernel_times(MzHandle* h, double* ms, int64_t* count);
  * is not handled (the step-wise pipeline is used then). */
 int mz_debug_small_search_plan(int32_t H, int32_t W, int32_t C, int32_t A, int32_t n, int32_t sm_count, int32_t tower_floats,
                                int32_t heads_floats, int32_t scratch_floats, int32_t cap_channels, int64_t* plan);
+
+/* Debug / tests (host only, no device needed): CTA size of the fused FC search (csrc/fc_search.cu::fc_search_plan) for
+ * N simulations, |A| actions, encoding E, widest layer maxw, blob_floats floats of weights, G lanes per game, the teacher-
+ * forced kernel or not, n games on sm_count SMs with smem_per_sm bytes of shared memory per SM, smem_reserve of it taken
+ * per CTA, smem_cap bytes at most per CTA and regs registers per thread; threads = 0 picks the CTA size (the fewest
+ * passes, then the smallest CTA), else plans that size.  Returns 1 and fills plan[6] = {threads per CTA, games per CTA,
+ * CTAs per SM, resident games, passes, shared-memory bytes per CTA}, or 0 when a game does not fit (the search then
+ * runs step by step). */
+int mz_debug_fc_search_plan(int32_t N, int32_t A, int32_t E, int32_t maxw, int32_t blob_floats, int32_t G, int32_t teacher,
+                            int32_t n, int32_t sm_count, int32_t smem_per_sm, int32_t smem_reserve, int32_t smem_cap,
+                            int32_t regs, int32_t threads, int64_t* plan);
 
 /* Debug / tests (host only, no device needed): launch plan of the CUDA-core conv3x3 kernel (csrc/resnet.cu) for n boards of
  * cin x H x W -> cout channels at stride 1 or 2.  Returns 1 and fills plan[11] = {P (pixels per thread), stride,

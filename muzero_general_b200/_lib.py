@@ -129,6 +129,7 @@ SYMBOLS = [
     ("mz_launch_count", C.c_int64, [C.c_void_p]),
     ("mz_graph_partitions", C.c_int32, [C.c_void_p]),
     ("mz_last_search_ms", C.c_double, [C.c_void_p]),
+    ("mz_fc_last_launch", C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     ("mz_kernel_timing", C.c_int, [C.c_void_p, C.c_int32]),
     ("mz_kernel_times", C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
     ("mz_numerics", C.c_char_p, [C.c_void_p]),
@@ -143,6 +144,7 @@ SYMBOLS = [
     ("mz_debug_opponent_action", C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p]),
     ("mz_debug_small_search_plan", C.c_int, [C.c_int32] * 10 + [C.POINTER(C.c_int64)]),
+    ("mz_debug_fc_search_plan", C.c_int, [C.c_int32] * 14 + [C.POINTER(C.c_int64)]),
     ("mz_debug_conv3x3_plan", C.c_int, [C.c_int32] * 6 + [C.POINTER(C.c_int64)]),
     ("mz_debug_conv3x3", C.c_int, [C.c_int] + [C.c_int32] * 6 + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                                   C.c_int32, C.c_int32, C.c_void_p]),

@@ -93,7 +93,9 @@ extern "C" int mz_create(const MzNetDesc* net, const MzSearchDesc* search, int d
     cudaDeviceProp prop;
     MZ_CREATE_CUDA(cudaGetDeviceProperties(&prop, device));
     h->sm_count = prop.multiProcessorCount;
-    h->smem_cap = prop.sharedMemPerBlockOptin;
+    h->fc_launch.smem_per_sm = prop.sharedMemPerMultiprocessor;
+    h->fc_launch.smem_reserve = prop.reservedSharedMemPerBlock;
+    h->fc_launch.smem_cap = prop.sharedMemPerBlockOptin;
     MZ_CREATE_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     MZ_CREATE_CUDA(cudaEventCreate(&h->ev0));
     MZ_CREATE_CUDA(cudaEventCreate(&h->ev1));
@@ -184,7 +186,7 @@ extern "C" int mz_create(const MzNetDesc* net, const MzSearchDesc* search, int d
     }
     const char* tenv = getenv("MZ_FC_THREADS");
     if (tenv) h->fc_threads = atoi(tenv);
-    if (h->fc_threads < 32 || h->fc_threads > kFcMaxThreads || h->fc_threads % 32) h->fc_threads = 64;
+    if (h->fc_threads < 32 || h->fc_threads > kFcMaxThreads || h->fc_threads % 32) h->fc_threads = 0;
     if ((h->fc_group < A && A <= 32) || (h->fc_group != 4 && h->fc_group != 8 && h->fc_group != 16 && h->fc_group != 32)) {
         fail(nullptr, MZ_EINVAL, "mz_create: MZ_FC_GROUP must be 4, 8, 16 or 32 and >= action_space");
         mz_destroy(h);
@@ -231,6 +233,13 @@ extern "C" int64_t mz_obs_elems(const MzHandle* h) { return h ? h->obs_elems : 0
 extern "C" int64_t mz_launch_count(const MzHandle* h) { return h ? h->launches : 0; }
 extern "C" double mz_last_search_ms(const MzHandle* h) { return h ? h->last_ms : 0.0; }
 extern "C" int32_t mz_graph_partitions(const MzHandle* h) { return h ? h->graph_parts : 1; }
+extern "C" int mz_fc_last_launch(const MzHandle* h, int64_t* info) {
+    if (!h || !info || !h->fc_launch.launched) return 0;
+    const FcLaunchInfo& l = h->fc_launch.last;
+    const int64_t out[5] = {l.grid, l.block, l.group, (int64_t)l.smem, l.ctas_per_sm};
+    for (int i = 0; i < 5; ++i) info[i] = out[i];
+    return 1;
+}
 
 // ------------------------------------------------------------------------------------------
 // weights
@@ -434,8 +443,7 @@ int mz_dispatch_search(MzHandle* h, const SearchCall& call, bool teacher, bool t
         a.max_tree_depth = call.max_tree_depth; a.tie_count = call.tie_count; a.root_priors = call.root_priors;
         a.value_range = call.value_range; a.teacher = call.teacher; a.trace = call.trace;
         if (call.keep_tree) a.pool = h->pool;
-        FcLaunchInfo info{};
-        cudaError_t e = launch_fc_search(a, h->fc_group, teacher, h->sm_count, h->smem_cap, h->stream, &info);
+        cudaError_t e = launch_fc_search(a, h->fc_group, teacher, h->sm_count, &h->fc_launch, h->stream);
         if (e == cudaErrorInvalidConfiguration) {
             // the tree does not fit in shared memory next to the weights: use the HBM node pool
             (void)cudaGetLastError();
@@ -877,6 +885,18 @@ extern "C" int mz_debug_small_search_plan(int32_t H, int32_t W, int32_t C, int32
         return 0;
     const int64_t out[8] = {P, CO, G, tile, threads, (int64_t)smem, row_stride, board_stride};
     for (int i = 0; i < 8; ++i) plan[i] = out[i];
+    return 1;
+}
+
+extern "C" int mz_debug_fc_search_plan(int32_t N, int32_t A, int32_t E, int32_t maxw, int32_t blob_floats, int32_t G, int32_t teacher,
+                                       int32_t n, int32_t sm_count, int32_t smem_per_sm, int32_t smem_reserve, int32_t smem_cap,
+                                       int32_t regs, int32_t threads, int64_t* plan) {
+    FcPlan p;
+    if (!plan || smem_per_sm < 0 || smem_reserve < 0 || smem_cap < 0 ||
+        !fc_search_plan(N, A, E, maxw, blob_floats, G, teacher != 0, n, sm_count, smem_per_sm, smem_reserve, smem_cap, regs, threads, &p))
+        return 0;
+    const int64_t out[6] = {p.threads, p.groups, p.ctas_per_sm, p.slots, p.passes, (int64_t)p.smem};
+    for (int i = 0; i < 6; ++i) plan[i] = out[i];
     return 1;
 }
 

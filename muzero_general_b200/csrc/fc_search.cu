@@ -12,6 +12,7 @@
 #include "kernels.h"
 
 #include <stdlib.h>
+#include <algorithm>
 #include <vector>
 
 namespace mz {
@@ -45,20 +46,32 @@ __host__ __device__ inline GameSmem game_smem_layout(int N, int A, int E, int ma
 
 // Phase split (scripts/fc_phase_split.py builds a copy of the library with -DMZ_FC_PHASES): every group times its game's
 // root, select, network, expand and backup phases with clock() and adds them, with the levels and selection rounds it
-// walked, to device counters that mz_fc_phase_counters reads.  The library built without the macro is unchanged.
-enum { kPhRoot, kPhSelect, kPhNet, kPhExpand, kPhBackup, kPhLevels, kPhRounds, kPhSims, kPhCount };
+// walked, to device counters that mz_fc_phase_counters reads.  It also stores the %globaltimer at which its game started
+// and finished (mz_fc_phase_spans): games that start after others have finished ran in a later pass of the persistent
+// loop.  The library built without the macro is unchanged.
+enum { kPhRoot, kPhSelect, kPhNet, kPhExpand, kPhBackup, kPhLevels, kPhRounds, kPhSims, kPhSums,
+       kPhStart = kPhSums, kPhEnd, kPhCount };
 // The counters are per game and added to in memory as the game goes (fire-and-forget reductions to distinct addresses):
-// accumulators held in registers would push the kernel past 128 registers and change its occupancy.
+// accumulators held in registers would push the kernel past 128 registers and change its occupancy.  The start and end
+// times sit in the same row.
 #ifdef MZ_FC_PHASES
 constexpr int kPhMaxGames = 1 << 16;
 __device__ unsigned long long g_fc_phase[kPhMaxGames][kPhCount];
+MZ_DEVINL unsigned long long global_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
 struct PhaseClock {
     int row = -1;                     // game of this group's lane 0, -1 on the other lanes
     unsigned last = 0;
     MZ_DEVINL void start(int g, bool leader) {
         row = (leader && g < kPhMaxGames) ? g : -1;
+        if (row >= 0) atomicExch(&g_fc_phase[row][kPhStart], global_ns());
         last = (unsigned)clock();
     }
+    // an exchange, like the counters' reductions, leaves the kernel without spills where a plain store did not
+    MZ_DEVINL void finish() { if (row >= 0) atomicExch(&g_fc_phase[row][kPhEnd], global_ns()); }
     MZ_DEVINL void mark(int p) {
         const unsigned now = (unsigned)clock();
         if (row >= 0) atomicAdd(&g_fc_phase[row][p], (unsigned long long)(now - last));
@@ -69,6 +82,7 @@ struct PhaseClock {
 #else
 struct PhaseClock {
     MZ_DEVINL void start(int, bool) {}
+    MZ_DEVINL void finish() {}
     MZ_DEVINL void mark(int) {}
     MZ_DEVINL void count(int, int) {}
 };
@@ -83,7 +97,7 @@ constexpr int fixed_actions() {
 // SH: FcFixedShape<E, H, S, A> runs the per-simulation network call through the fully unrolled fixed-shape code
 // (fc_net.cuh::fc_recurrent_fixed, bit-identical to the generic descriptors walk), FcGenericShape through the latter.
 template <int G, bool kTeacher, typename SH>
-__global__ void __launch_bounds__(kFcMaxThreads) fc_search_kernel(const __grid_constant__ FcSearchArgs a) {
+__global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __grid_constant__ FcSearchArgs a) {
     extern __shared__ __align__(16) unsigned char smem[];
     const int N = a.N, A = a.A;
     // ---- CTA-shared: tables + weights
@@ -269,6 +283,7 @@ __global__ void __launch_bounds__(kFcMaxThreads) fc_search_kernel(const __grid_c
                 a.pool.n_expanded[g] = t.n_expanded;
             }
         }
+        ph.finish();
         LaneGroup<G>::sync();
     }
     (void)F;
@@ -277,46 +292,98 @@ __global__ void __launch_bounds__(kFcMaxThreads) fc_search_kernel(const __grid_c
 // ------------------------------------------------------------------------------------------
 // host launcher
 // ------------------------------------------------------------------------------------------
+// Shared memory of a CTA of `groups` games: the UCB tables and (student kernels) the weight blob, then one region per game.
+static size_t fc_cta_smem(int N, int A, int E, int maxw, int blob_floats, bool teacher, int groups) {
+    const GameSmem L = game_smem_layout(N, A, E, maxw, !teacher);
+    const size_t shared_bytes = ((2 * (size_t)(N + 2) * 8 + (teacher ? 0 : (size_t)blob_floats) * 4) + 15) & ~(size_t)15;
+    return shared_bytes + (size_t)groups * L.bytes;
+}
+
+// The kernel is latency-bound: a game's chain of dependent simulations barely lengthens with the number of games that
+// share its SM, so the launch lasts about one chain per pass and the plan minimises passes.  Resident CTAs per SM follow
+// the occupancy rules of sm_90: shared memory in 128-byte units plus the per-CTA reserve, registers in 256-register
+// units per warp out of 64K, at most 2048 threads and 32 CTAs.
+bool fc_search_plan(int N, int A, int E, int maxw, int blob_floats, int G, bool teacher, int n_games, int sm_count,
+                    size_t smem_per_sm, size_t smem_reserve, size_t smem_cap, int regs, int threads, FcPlan* plan) {
+    if (n_games < 1 || sm_count < 1 || G < 1 || regs < 1 || N < 0 || A < 1 || E < 1 || maxw < 1 || blob_floats < 0) return false;
+    bool found = false;
+    const std::vector<int> sizes = threads != 0 ? std::vector<int>{threads} : std::vector<int>{64, 128, 256};
+    for (int t : sizes) {
+        if (t % 32 != 0 || t < G || t > kFcMaxThreads) continue;
+        const int groups = t / G;
+        const size_t smem = fc_cta_smem(N, A, E, maxw, blob_floats, teacher, groups);
+        const int by_smem = smem > smem_cap ? 0 : (int)(smem_per_sm / ((smem + smem_reserve + 127) & ~(size_t)127));
+        const int by_regs = (65536 / (((regs * 32) + 255) & ~255)) / (t / 32);
+        const int per_sm = std::min(std::min(by_smem, by_regs), std::min(2048 / t, 32));
+        if (per_sm >= 1) {
+            const int slots = per_sm * groups * sm_count;
+            const int passes = (n_games + slots - 1) / slots;
+            if (!found || passes < plan->passes) {
+                *plan = FcPlan{t, groups, per_sm, slots, passes, smem};
+                found = true;
+            }
+        }
+    }
+    return found;
+}
+
 template <int G, bool T, typename SH>
-static cudaError_t launch_one(const FcSearchArgs& a_in, int sm_count, size_t smem_cap, cudaStream_t stream, FcLaunchInfo* info) {
+static cudaError_t launch_one(const FcSearchArgs& a_in, int sm_count, FcLaunchState* st, cudaStream_t stream) {
     FcSearchArgs a = a_in;
     const char* one_level = getenv("MZ_FC_SELECT_LEVELS");    // A/B switch: "1" = one tree level per selection round
     a.select_levels = (one_level && one_level[0] == '1' && one_level[1] == 0) ? 1 : select_levels_for(a.A, G);
-    const GameSmem L = game_smem_layout(a.N, a.A, a.net.E, a.net.maxw, !T);
-    const size_t shared_bytes = ((2 * (size_t)(a.N + 2) * 8 + (T ? 0 : (size_t)a.net.blob_floats) * 4) + 15) & ~(size_t)15;
-    const int threads = a.threads;
-    const int groups = threads / G;
-    if (groups < 1) return cudaErrorInvalidValue;
-    const size_t smem = shared_bytes + (size_t)groups * L.bytes;
-    if (smem > smem_cap) return cudaErrorInvalidConfiguration;
     auto kern = fc_search_kernel<G, T, SH>;
-    cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (err != cudaSuccess) return err;
-    int per_sm = 0;
-    err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem);
-    if (err != cudaSuccess) return err;
+    const void* fn = reinterpret_cast<const void*>(kern);
+    int regs = 0;
+    for (const auto& k : st->kernels) if (k.fn == fn) regs = k.regs;
+    if (regs == 0) {
+        // the driver's default carveout may leave less shared memory per SM than the plan counts on
+        cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)st->smem_cap);
+        if (err == cudaSuccess) err = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncAttributes fa{};
+        if (err == cudaSuccess) err = cudaFuncGetAttributes(&fa, kern);
+        if (err != cudaSuccess) return err;
+        regs = fa.numRegs;
+        st->kernels.push_back({fn, regs});
+    }
+    FcPlan plan;
+    if (!fc_search_plan(a.N, a.A, a.net.E, a.net.maxw, a.net.blob_floats, G, T, a.n_games, sm_count, st->smem_per_sm,
+                        st->smem_reserve, st->smem_cap, regs, a.threads, &plan))
+        return cudaErrorInvalidConfiguration;
+    int per_sm = -1;
+    for (const auto& s : st->shapes) if (s.fn == fn && s.threads == plan.threads && s.smem == plan.smem) per_sm = s.ctas_per_sm;
+    if (per_sm < 0) {
+        cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, plan.threads, plan.smem);
+        if (err != cudaSuccess) return err;
+        st->shapes.push_back({fn, plan.threads, plan.smem, per_sm});
+    }
+    per_sm = std::min(per_sm, plan.ctas_per_sm);      // the device's word when it disagrees with the plan
     if (per_sm < 1) return cudaErrorInvalidConfiguration;
-    const int want = (a.n_games + groups - 1) / groups;
-    const int grid = want < per_sm * sm_count ? want : per_sm * sm_count;
-    if (info) { info->grid = grid; info->block = threads; info->smem = smem; info->ctas_per_sm = per_sm; info->group = G; }
-    kern<<<grid, threads, smem, stream>>>(a);
-    return cudaGetLastError();
+    const int want = (a.n_games + plan.groups - 1) / plan.groups;
+    const int grid = std::min(want, per_sm * sm_count);
+    kern<<<grid, plan.threads, plan.smem, stream>>>(a);
+    const cudaError_t err = cudaGetLastError();
+    if (err == cudaSuccess) {
+        st->launched = true;
+        st->last = FcLaunchInfo{grid, plan.threads, per_sm, G, plan.smem};
+    }
+    return err;
 }
 
 // shapes with a fully unrolled network path: games/cartpole.py (encoding 8, hidden 16, support 10, 2 actions)
 using CartPoleShape = FcFixedShape<8, 16, 10, 2>;
 
-cudaError_t launch_fc_search(const FcSearchArgs& a, int group, bool teacher, int sm_count, size_t smem_cap,
-                             cudaStream_t stream, FcLaunchInfo* info) {
+cudaError_t launch_fc_search(const FcSearchArgs& a, int group, bool teacher, int sm_count, FcLaunchState* state,
+                             cudaStream_t stream) {
     const char* generic = getenv("MZ_FC_GENERIC");             // A/B switch: always walk the layer descriptors
     if (!teacher && !(generic && generic[0] == '1') && fc_matches_fixed<CartPoleShape>(a.net)) {
-        if (group == 16) return launch_one<16, false, CartPoleShape>(a, sm_count, smem_cap, stream, info);
-        if (group == 32) return launch_one<32, false, CartPoleShape>(a, sm_count, smem_cap, stream, info);
+        if (group == 16) return launch_one<16, false, CartPoleShape>(a, sm_count, state, stream);
+        if (group == 32) return launch_one<32, false, CartPoleShape>(a, sm_count, state, stream);
     }
 #define MZ_CASE(GG)                                                                                     \
     case GG:                                                                                            \
-        return teacher ? launch_one<GG, true, FcGenericShape>(a, sm_count, smem_cap, stream, info)      \
-                       : launch_one<GG, false, FcGenericShape>(a, sm_count, smem_cap, stream, info);
+        return teacher ? launch_one<GG, true, FcGenericShape>(a, sm_count, state, stream)               \
+                       : launch_one<GG, false, FcGenericShape>(a, sm_count, state, stream);
     switch (group) {
         MZ_CASE(4)
         MZ_CASE(8)
@@ -337,19 +404,27 @@ extern "C" int mz_fc_phase_counters(unsigned long long* out, int reset) {
     if (e == cudaSuccess && out) {
         std::vector<unsigned long long> rows((size_t)kPhMaxGames * kPhCount);
         e = cudaMemcpy(rows.data(), dev, rows.size() * 8, cudaMemcpyDeviceToHost);
-        for (int p = 0; p < kPhCount; ++p) out[p] = 0;
-        for (size_t i = 0; i < rows.size(); ++i) out[i % kPhCount] += rows[i];
+        for (int p = 0; p < kPhSums; ++p) out[p] = 0;
+        for (size_t i = 0; i < rows.size(); ++i) if (i % kPhCount < kPhSums) out[i % kPhCount] += rows[i];
     }
     if (e == cudaSuccess && reset) e = cudaMemset(dev, 0, sizeof(g_fc_phase));
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
     return e == cudaSuccess ? 0 : (int)e;
 }
-#endif
 
-size_t fc_search_smem_bytes(const FcSearchArgs& a, int group, bool teacher) {
-    const GameSmem L = game_smem_layout(a.N, a.A, a.net.E, a.net.maxw, !teacher);
-    const size_t shared_bytes = ((2 * (size_t)(a.N + 2) * 8 + (teacher ? 0 : (size_t)a.net.blob_floats) * 4) + 15) & ~(size_t)15;
-    return shared_bytes + (size_t)(a.threads / group) * L.bytes;
+// out[2 * g], out[2 * g + 1] = %globaltimer (ns) at which game g < n of the last launch started and finished (read them
+// before mz_fc_phase_counters resets the rows)
+extern "C" int mz_fc_phase_spans(unsigned long long* out, int n) {
+    if (!out || n < 0 || n > kPhMaxGames) return (int)cudaErrorInvalidValue;
+    std::vector<unsigned long long> rows((size_t)n * kPhCount);
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpyFromSymbol(rows.data(), g_fc_phase, rows.size() * 8);
+    for (int g = 0; e == cudaSuccess && g < n; ++g) {
+        out[2 * g] = rows[(size_t)g * kPhCount + kPhStart];
+        out[2 * g + 1] = rows[(size_t)g * kPhCount + kPhEnd];
+    }
+    return e == cudaSuccess ? 0 : (int)e;
 }
+#endif
 
 }  // namespace mz

@@ -16,7 +16,6 @@ struct MzHandle {
     MzSearchDesc search;
     int device = 0;
     int sm_count = 0;
-    size_t smem_cap = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     std::string err;
@@ -31,7 +30,8 @@ struct MzHandle {
     float* d_fc_blob = nullptr;
     bool weights_loaded = false;
     int fc_group = 16;
-    int fc_threads = 64;
+    int fc_threads = 0;                // CTA size of the fused search, 0 = planned per launch (MZ_FC_THREADS overrides)
+    FcLaunchState fc_launch;
     // residual weights + workspace
     ResNetDevice* res = nullptr;
     // pool

@@ -4,13 +4,17 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <vector>
+
 #include "../../include/mzb200.h"
 #include "fc_net.cuh"
 
 namespace mz {
 
 constexpr int kFcThreads = 128;      // fc_inference_kernel block
-constexpr int kFcMaxThreads = 128;   // upper bound of the fused search kernel's block
+// Upper bound of the fused search kernel's block.  Two such CTAs per SM at the 128 registers per thread that
+// __launch_bounds__(kFcMaxThreads, 2) caps the kernel at fill the 64K-register file exactly (fc_search_plan).
+constexpr int kFcMaxThreads = 256;
 
 // HBM node pool, game-major: game g owns slots [g*(N+1)*A, (g+1)*(N+1)*A).
 struct NodePool {
@@ -52,7 +56,7 @@ struct DevTrace {
 
 struct FcSearchArgs {
     int n_games, N, A, P;
-    int threads;           // block size of the launch (multiple of 32)
+    int threads;           // block size of the launch (multiple of 32), 0 = the one fc_search_plan picks
     int select_levels;     // tree levels per selection round (set by launch_fc_search)
     double discount, noise_frac, noise_alpha;
     uint64_t seed;
@@ -100,8 +104,30 @@ cudaError_t launch_fc_inference(const FcInferArgs& a, int group, int sm_count, c
 
 struct FcLaunchInfo { int grid, block, ctas_per_sm, group; size_t smem; };
 
-cudaError_t launch_fc_search(const FcSearchArgs& a, int group, bool teacher, int sm_count, size_t smem_cap,
-                             cudaStream_t stream, FcLaunchInfo* info);
-size_t fc_search_smem_bytes(const FcSearchArgs& a, int group, bool teacher);
+// Launch shape of the fused search: `threads` per CTA of `groups` games and `smem` bytes, `ctas_per_sm` resident per SM,
+// `slots` games resident on the GPU at once, `passes` = ceil(n_games / slots) chains of the persistent loop.
+struct FcPlan { int threads, groups, ctas_per_sm, slots, passes; size_t smem; };
+
+// Host arithmetic only.  Over CTAs of 64, 128 and 256 threads (or `threads` alone when it is not 0), the one whose resident
+// CTAs - limited by shared memory (smem_per_sm, less smem_reserve per CTA), registers (regs per thread) and threads per SM -
+// run n_games in the fewest passes, and the smallest of those.  False when one game's tree does not fit a CTA (smem_cap).
+bool fc_search_plan(int N, int A, int E, int maxw, int blob_floats, int G, bool teacher, int n_games, int sm_count,
+                    size_t smem_per_sm, size_t smem_reserve, size_t smem_cap, int regs, int threads, FcPlan* plan);
+
+// The device limits the plan is made against, and what a handle has set up for the fused search kernel so far: each
+// instantiation gets its attributes set and its register count read once, each (instantiation, block, shared memory)
+// its occupancy confirmed once, so that later searches go straight to the launch.
+struct FcLaunchState {
+    size_t smem_per_sm = 0, smem_reserve = 0, smem_cap = 0;
+    struct Kernel { const void* fn; int regs; };
+    struct Shape { const void* fn; int threads; size_t smem; int ctas_per_sm; };
+    std::vector<Kernel> kernels;
+    std::vector<Shape> shapes;
+    bool launched = false;         // last: the handle's last fused launch (mz_fc_last_launch)
+    FcLaunchInfo last{};
+};
+
+cudaError_t launch_fc_search(const FcSearchArgs& a, int group, bool teacher, int sm_count, FcLaunchState* state,
+                             cudaStream_t stream);
 
 }  // namespace mz

@@ -146,6 +146,14 @@ class SearchEngine:
         return int(self.lib.mz_graph_partitions(self._h))
 
     @property
+    def last_fc_launch(self):
+        """Shape of this handle's last fused FC search launch (grid, block, group, smem, ctas_per_sm), None before one."""
+        info = (C.c_int64 * 5)()
+        if self.lib.mz_fc_last_launch(self._h, info) != 1:
+            return None
+        return dict(zip(("grid", "block", "group", "smem", "ctas_per_sm"), (int(v) for v in info)))
+
+    @property
     def last_search_ms(self):
         return float(self.lib.mz_last_search_ms(self._h))
 
