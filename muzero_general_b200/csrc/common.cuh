@@ -9,25 +9,32 @@ namespace mz {
 
 // ------------------------------------------------------------------------------------------
 // Lane groups: a warp is split into 32/G groups of G consecutive lanes; one game per group.
+//
+// Every group of a warp calls every collective, the same number of times, so that each one takes the constant full mask
+// (kWarp) and the segment width G keeps the groups' data apart.  A mask that depends on the lane (0xffff << 16 for the
+// upper group of G = 16) makes nvcc guard each collective region with a run-time convergence check (MATCH.ANY, REDUX.OR,
+// a divergent-branch fallback); the full mask needs none.  Hence: a loop that contains a collective runs to the largest
+// trip count of the warp's groups (the others predicate their updates off), and a persistent loop over games iterates
+// while the warp still has a game - a group without one runs on a clamped index and stores nothing.
 // ------------------------------------------------------------------------------------------
+constexpr unsigned kWarp = 0xffffffffu;
+
 template <int G>
 struct LaneGroup {
     static_assert(G == 4 || G == 8 || G == 16 || G == 32, "group width");
     MZ_DEVINL static unsigned lane() { return threadIdx.x & (G - 1); }
     MZ_DEVINL static unsigned base() { return (threadIdx.x & 31u) & ~(unsigned)(G - 1); }
-    MZ_DEVINL static unsigned mask() {
-        if constexpr (G == 32) return 0xffffffffu;
-        else return ((1u << G) - 1u) << base();
-    }
-    MZ_DEVINL static void sync() { __syncwarp(mask()); }
+    MZ_DEVINL static void sync() { __syncwarp(kWarp); }
     // ballot restricted to the group, bit i = lane i of the group
     MZ_DEVINL static unsigned ballot(bool p) {
-        unsigned b = __ballot_sync(mask(), p);
+        unsigned b = __ballot_sync(kWarp, p);
         if constexpr (G == 32) return b;
         else return (b >> base()) & ((1u << G) - 1u);
     }
     template <typename T>
-    MZ_DEVINL static T bcast(T v, int src) { return __shfl_sync(mask(), v, src, G); }
+    MZ_DEVINL static T bcast(T v, int src) { return __shfl_sync(kWarp, v, src, G); }
+    // true in every lane while any group of the warp passes p (the trip-count test of a loop that contains collectives)
+    MZ_DEVINL static bool warp_any(bool p) { return __any_sync(kWarp, p); }
 };
 
 MZ_DEVINL double shfl_xor_f64(unsigned mask, double v, int off, int width) {
@@ -57,24 +64,21 @@ MZ_DEVINL void prefetch_l1(const void* p) { asm volatile("prefetch.L1 [%0];" ::"
 
 MZ_DEVINL int pow2_ceil(int n) { return n <= 1 ? 1 : 1 << (32 - __clz(n - 1)); }
 
-// Exact max / min (no rounding involved), NaN-free inputs assumed.
+// Exact max / min (no rounding involved), NaN-free inputs assumed.  `width` must be the same in every group of the warp.
 template <int G>
 MZ_DEVINL double group_max_f64(double v, int width) {
-    const unsigned m = LaneGroup<G>::mask();
-    for (int off = width >> 1; off > 0; off >>= 1) v = fmax(v, shfl_xor_f64(m, v, off, G));
+    for (int off = width >> 1; off > 0; off >>= 1) v = fmax(v, shfl_xor_f64(kWarp, v, off, G));
     return v;
 }
 template <int G>
 MZ_DEVINL double group_min_f64(double v, int width) {
-    const unsigned m = LaneGroup<G>::mask();
-    for (int off = width >> 1; off > 0; off >>= 1) v = fmin(v, shfl_xor_f64(m, v, off, G));
+    for (int off = width >> 1; off > 0; off >>= 1) v = fmin(v, shfl_xor_f64(kWarp, v, off, G));
     return v;
 }
 template <int G>
 MZ_DEVINL float group_max_f32(float v) {
-    const unsigned m = LaneGroup<G>::mask();
 #pragma unroll
-    for (int off = G >> 1; off > 0; off >>= 1) v = fmaxf(v, __shfl_xor_sync(m, v, off, G));
+    for (int off = G >> 1; off > 0; off >>= 1) v = fmaxf(v, __shfl_xor_sync(kWarp, v, off, G));
     return v;
 }
 // The same reductions over the first W lanes of the group only (W a power of two <= G): valid in lanes < W.  With the lanes
@@ -83,23 +87,20 @@ MZ_DEVINL float group_max_f32(float v) {
 constexpr int pow2_ceil_c(int n) { return n <= 1 ? 1 : 2 * pow2_ceil_c((n + 1) / 2); }
 template <int G, int W>
 MZ_DEVINL float group_max_f32_w(float v) {
-    const unsigned m = LaneGroup<G>::mask();
 #pragma unroll
-    for (int off = W >> 1; off > 0; off >>= 1) v = fmaxf(v, __shfl_xor_sync(m, v, off, G));
+    for (int off = W >> 1; off > 0; off >>= 1) v = fmaxf(v, __shfl_xor_sync(kWarp, v, off, G));
     return v;
 }
 template <int G, int W>
 MZ_DEVINL float group_sum_f32_w(float v) {
-    const unsigned m = LaneGroup<G>::mask();
 #pragma unroll
-    for (int off = W >> 1; off > 0; off >>= 1) v += __shfl_xor_sync(m, v, off, G);
+    for (int off = W >> 1; off > 0; off >>= 1) v += __shfl_xor_sync(kWarp, v, off, G);
     return v;
 }
 template <int G>
 MZ_DEVINL float group_sum_f32(float v) {
-    const unsigned m = LaneGroup<G>::mask();
 #pragma unroll
-    for (int off = G >> 1; off > 0; off >>= 1) v += __shfl_xor_sync(m, v, off, G);
+    for (int off = G >> 1; off > 0; off >>= 1) v += __shfl_xor_sync(kWarp, v, off, G);
     return v;
 }
 

@@ -21,7 +21,12 @@ __global__ void __launch_bounds__(kFcThreads) fc_inference_kernel(const __grid_c
     float* base = s_blob + ((a.net.blob_floats + 3) & ~3) + (size_t)gi * (4 * maxw + 4);
     float *s0 = base, *s1 = base + maxw, *s2 = base + 2 * maxw, *sh = base + 3 * maxw;   // maxw % 4 == 0
 
-    for (int g = blockIdx.x * groups_per_cta + gi; g < a.n; g += gridDim.x * groups_per_cta) {
+    // a warp runs while its first group has a sample (see LaneGroup); a group past the last one evaluates that one again (it
+    // belongs to this warp) and stores nothing
+    const int warp_first = (int)blockIdx.x * groups_per_cta + (int)(threadIdx.x & ~31u) / G;
+    for (int g0 = warp_first; g0 < a.n; g0 += gridDim.x * groups_per_cta) {
+        const bool own = g0 + gi - (int)(threadIdx.x & ~31u) / G < a.n;
+        const int g = own ? g0 + gi - (int)(threadIdx.x & ~31u) / G : a.n - 1;
         float reward = 0.0f;
         if (a.recurrent) {
             const int act = a.action[g];
@@ -31,7 +36,7 @@ __global__ void __launch_bounds__(kFcThreads) fc_inference_kernel(const __grid_c
             load_vector<G>(hin, s1, E);
             float* raw = mlp_forward<G>(a.net.dyn, s_blob, s1, s0, s1, s2, act);
             float* rl = mlp_forward<G>(a.net.rew, s_blob, raw, s0, s1, nullptr);
-            if (a.reward_logits) for (int i = lane; i < F; i += G) a.reward_logits[(size_t)g * F + i] = rl[i];
+            if (a.reward_logits && own) for (int i = lane; i < F; i += G) a.reward_logits[(size_t)g * F + i] = rl[i];
             reward = support_to_scalar_group<G>(rl, S);
             LaneGroup<G>::sync();
             rescale_unit_range<G>(raw, sh, E);
@@ -39,20 +44,20 @@ __global__ void __launch_bounds__(kFcThreads) fc_inference_kernel(const __grid_c
             load_vector<G>(a.in + (size_t)g * a.net.obs_elems, s1, a.net.obs_elems);
             float* raw = mlp_forward<G>(a.net.rep, s_blob, s1, s0, s1, s2);
             rescale_unit_range<G>(raw, sh, E);
-            if (a.reward_logits)        // log(one-hot at the centre), models.py:176-183
+            if (a.reward_logits && own)        // log(one-hot at the centre), models.py:176-183
                 for (int i = lane; i < F; i += G) a.reward_logits[(size_t)g * F + i] = (i == S) ? 0.0f : -INFINITY;
             reward = inverse_value_transform(0.0f);
         }
-        if (a.hidden) for (int i = lane; i < E; i += G) a.hidden[(size_t)g * E + i] = sh[i];
-        if (a.pool_hidden)
+        if (a.hidden && own) for (int i = lane; i < E; i += G) a.hidden[(size_t)g * E + i] = sh[i];
+        if (a.pool_hidden && own)
             for (int i = lane; i < E; i += G) a.pool_hidden[((size_t)g * a.pool_stride + a.out_slot) * E + i] = sh[i];
         float* pol = mlp_forward<G>(a.net.pol, s_blob, sh, s0, s1, s2);
-        if (a.policy_logits) for (int i = lane; i < A; i += G) a.policy_logits[(size_t)g * A + i] = pol[i];
+        if (a.policy_logits && own) for (int i = lane; i < A; i += G) a.policy_logits[(size_t)g * A + i] = pol[i];
         LaneGroup<G>::sync();
         float* vl = mlp_forward<G>(a.net.val, s_blob, sh, s0, s1, s2);
-        if (a.value_logits) for (int i = lane; i < F; i += G) a.value_logits[(size_t)g * F + i] = vl[i];
+        if (a.value_logits && own) for (int i = lane; i < F; i += G) a.value_logits[(size_t)g * F + i] = vl[i];
         const float value = support_to_scalar_group<G>(vl, S);
-        if (lane == 0) {
+        if (lane == 0 && own) {
             if (a.value) a.value[g] = value;
             if (a.reward) a.reward[g] = reward;
         }

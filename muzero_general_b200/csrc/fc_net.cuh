@@ -197,7 +197,7 @@ template <int G>
 MZ_DEVINL void support_to_scalar_group2(const float* la, const float* lb, int S, float& ra, float& rb) {
     const int lane = LaneGroup<G>::lane();
     const int F = 2 * S + 1;
-    const unsigned m = LaneGroup<G>::mask();
+    const unsigned m = kWarp;
     float ma = -INFINITY, mb = -INFINITY;
     for (int i = lane; i < F; i += G) { ma = fmaxf(ma, la[i]); mb = fmaxf(mb, lb[i]); }
 #pragma unroll
@@ -325,7 +325,7 @@ MZ_DEVINL void fc_recurrent_fixed(const FcNet& net, const float* blob, const flo
     logit = 0.0f;
     if (lane < A) logit = dot_packed<H>(blob + pl.w_off[1], A, lane, blob[pl.b_off[1] + lane], sp);
     // ---- support_to_scalar of value and reward (support_to_scalar_group2 on registers: same maxima, sums and order)
-    const unsigned m = LaneGroup<G>::mask();
+    const unsigned m = kWarp;
     float ma = -INFINITY, mb = -INFINITY;
 #pragma unroll
     for (int r = 0; r < R; ++r)

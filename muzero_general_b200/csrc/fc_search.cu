@@ -5,8 +5,8 @@
 // expand, backup} - for every game of the batch.  A group of G lanes owns one game from the
 // first to the last simulation: its tree (child slots, hidden states, path) lives in shared
 // memory next to the network weights, so the only HBM traffic is the observation in and
-// the visit counts / root values out.  Groups never synchronise with each other; the grid
-// is persistent (one wave) and groups stride over the games.
+// the visit counts / root values out.  The groups of a warp share its collectives (common.cuh,
+// LaneGroup), warps never synchronise with each other; the grid is persistent (one wave) and warps stride over the games.
 #include "fc_net.cuh"
 #include "tree.cuh"
 #include "kernels.h"
@@ -146,8 +146,14 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
     const SelectLanes sl = select_lanes<G, kA>(A, min(a.select_levels, kMaxD));
     PhaseClock ph;
 
-    for (int g = blockIdx.x * groups_per_cta + gi; g < a.n_games; g += gridDim.x * groups_per_cta) {
-        ph.start(g, lane == 0);
+    // The warp's groups run their games side by side (see LaneGroup): the loop goes on while the warp's first group has a
+    // game, and a group past the last game searches that one again (it belongs to this warp) and stores nothing.
+    const int warp_first = (int)blockIdx.x * groups_per_cta + (int)(threadIdx.x & ~31u) / G;
+    for (int g0 = warp_first; g0 < a.n_games; g0 += gridDim.x * groups_per_cta) {
+        const int g_own = g0 + gi - (int)(threadIdx.x & ~31u) / G;
+        const bool own = g_own < a.n_games;
+        const int g = own ? g_own : a.n_games - 1;
+        ph.start(g, lane == 0 && own);
         const int64_t game_id = a.game_id ? a.game_id[g] : (int64_t)g;
         const int move = a.move_index ? a.move_index[g] : 0;
         const int to_play0 = a.to_play ? a.to_play[g] : 0;
@@ -179,11 +185,11 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
         float prior;
         if (kTeacher) prior = (lane < A) ? a.teacher.root_priors[(size_t)g * A + lane] : 0.0f;
         else prior = group_softmax_masked<G>(logit, lane < A && ((legal >> lane) & 1u));
-        if (a.trace.root_priors_raw && lane < A) a.trace.root_priors_raw[(size_t)g * A + lane] = ((legal >> lane) & 1u) ? prior : 0.0f;
-        if (a.trace.root_reward && lane == 0) a.trace.root_reward[g] = root_reward;
+        if (a.trace.root_priors_raw && lane < A && own) a.trace.root_priors_raw[(size_t)g * A + lane] = ((legal >> lane) & 1u) ? prior : 0.0f;
+        if (a.trace.root_reward && lane == 0 && own) a.trace.root_reward[g] = root_reward;
         tree_init_root<G>(c, t, prior, root_reward,
                           (a.add_noise && a.noise) ? a.noise + (size_t)g * A : nullptr, a.add_noise && !a.noise,
-                          game_id, move, a.trace.noise ? a.trace.noise + (size_t)g * A : nullptr);
+                          game_id, move, (a.trace.noise && own) ? a.trace.noise + (size_t)g * A : nullptr);
         ph.mark(kPhRoot);
 
         // ------------------------------------------------------------------ simulations
@@ -235,7 +241,7 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
                 else prior = group_softmax_masked<G>(logit, lane < A);
             }
             ph.mark(kPhNet);
-            if (a.trace.depth) {
+            if (a.trace.depth && own) {
                 const size_t ti = (size_t)g * N + sim;
                 if (lane == 0) { a.trace.depth[ti] = leaf.depth; a.trace.value[ti] = value; a.trace.reward[ti] = reward; }
                 if (lane < A) a.trace.priors[ti * A + lane] = prior;
@@ -251,19 +257,19 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
         ph.count(kPhSims, N);
 
         // ------------------------------------------------------------------ results
-        if (lane < A) {
+        if (lane < A && own) {
             const bool ok = (legal >> lane) & 1u;
             if (a.visit_counts) a.visit_counts[(size_t)g * A + lane] = ok ? t.visit[lane] : 0;
             if (a.root_priors) a.root_priors[(size_t)g * A + lane] = t.root_prior[lane];
         }
-        if (lane == 0) {
+        if (lane == 0 && own) {
             if (a.root_value) a.root_value[g] = (t.root_visit == 0) ? 0.0 : __ddiv_rn(t.root_vsum, (double)t.root_visit);
             if (a.root_predicted_value) a.root_predicted_value[g] = root_value;
             if (a.max_tree_depth) a.max_tree_depth[g] = max_depth;
             if (a.tie_count) a.tie_count[g] = t.ties;
             if (a.value_range) { a.value_range[2 * g] = t.lo; a.value_range[2 * g + 1] = t.hi; }
         }
-        if (a.pool.visit) {      // MZ_FLAG_KEEP_TREE: spill the shared-memory tree to the HBM node pool
+        if (a.pool.visit && own) {      // MZ_FLAG_KEEP_TREE: spill the shared-memory tree to the HBM node pool
             const int slots = (N + 1) * A;
             const size_t pb = (size_t)g * slots;
             for (int s = lane; s < t.n_expanded * A; s += G) {

@@ -307,16 +307,16 @@ __device__ __forceinline__ void heads_one_sample(const HeadsArgs& a, const float
         }
         if (a.logits[h])
             for (int o = u; o < d.n_out; o += span) a.logits[h][(size_t)g * d.n_out + o] = cur[o];
-        if (a.scalar[h]) {
-            if (span >= 32) {                          // span is a multiple of 32: the head's first warp
-                if (u < 32) {
-                    const float v = support_to_scalar_group<32>(cur, a.S);
-                    if (u == 0) a.scalar[h][g] = v;
-                }
-            } else {                                   // two heads share a warp: 16 lanes each
-                const float v = support_to_scalar_group<16>(cur, a.S);
+        if (span >= 32) {                              // span is a multiple of 32: the head's first warp
+            if (a.scalar[h] && u < 32) {
+                const float v = support_to_scalar_group<32>(cur, a.S);
                 if (u == 0) a.scalar[h][g] = v;
             }
+        } else {
+            // two heads share a warp, 16 lanes each: both call the full-mask reduction (common.cuh, LaneGroup); a head
+            // without a scalar reduces its first logit only (S = 0) and discards the result
+            const float v = support_to_scalar_group<16>(cur, a.scalar[h] ? a.S : 0);
+            if (u == 0 && a.scalar[h]) a.scalar[h][g] = v;
         }
     }
     group_bar<GROUP>(group);

@@ -79,9 +79,11 @@ __global__ void __launch_bounds__(kSmallSearchThreads) small_search_kernel(const
             heads_one_sample<32>(a.heads_pred, hblob, s_scratch, nullptr, a.g0 + b0 + s, warp, lane, 0,
                                  HeadsTile{s_act + out * bufsz + s * bstride, nullptr, s_map, s_xmap});
         __syncthreads();
-        // expand + backup with these outputs, then select the next leaf (self_play.py:318-353); read-out after the last one
-        for (int lg = tid / G; lg < nbt; lg += nthreads / G)
-            tree_step_game<G, true>(a.tree, a.g0 + b0 + lg, sim + 1, 0, 1, sim + 1 < N ? 1 : 0, sim + 1 == N ? 1 : 0);
+        // expand + backup with these outputs, then select the next leaf (self_play.py:318-353); read-out after the last one.
+        // A warp runs while its first group has a game; a group past the tile's last game replays that one (in its warp).
+        for (int lg = tid / G; lg - (lane / G) < nbt; lg += nthreads / G)
+            tree_step_game<G, true>(a.tree, a.g0 + b0 + min(lg, nbt - 1), lg < nbt, sim + 1, 0, 1, sim + 1 < N ? 1 : 0,
+                                    sim + 1 == N ? 1 : 0);
         // (the next dynamics tile starts with a CTA barrier: leaf_parent / leaf_action of every game are visible)
     }
 }

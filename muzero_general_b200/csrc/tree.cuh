@@ -54,6 +54,7 @@ struct GameTree {
     unsigned legal;        // bitmask of legal root actions
     int n_expanded;        // expansions so far (>= 1 after the root expansion)
     int ties;              // exact ties after the first simulation
+    bool own = true;       // false: the group has no game and replays a warp neighbour's without storing (see LaneGroup)
 };
 
 struct Leaf {
@@ -114,13 +115,12 @@ MZ_DEVINL void tree_init_root(const TreeConst& c, GameTree& t, float prior_f32, 
         // Dirichlet(alpha) over the legal actions = normalised Gamma(alpha) draws (numpy.random.dirichlet)
         const double gm = legal ? philox_gamma(c.seed, game_id, move, k, c.noise_alpha) : 0.0;
         double sum = gm;
-        const unsigned m = LaneGroup<G>::mask();
-        for (int off = G >> 1; off > 0; off >>= 1) sum += shfl_xor_f64(m, sum, off, G);
+        for (int off = G >> 1; off > 0; off >>= 1) sum += shfl_xor_f64(kWarp, sum, off, G);
         nz = gm / sum;
         have_noise = true;
     }
-    if (noise_out && k < c.A) noise_out[k] = nz;
-    if (k < c.A) {
+    if (noise_out && k < c.A && t.own) noise_out[k] = nz;
+    if (k < c.A && t.own) {
         double p = (double)prior_f32;
         if (legal && have_noise) {
             // prior * (1 - frac) + n * frac       (self_play.py:476)
@@ -160,10 +160,11 @@ MZ_DEVINL Leaf tree_select(const TreeConst& c, GameTree& t, int sim, int64_t gam
     int n_parent = t.root_visit;
     int depth = 0;
     Leaf leaf;
-    if (k == 0) { t.path[0] = -1; t.path_reward[0] = t.root_reward; }
-    while (true) {
+    bool done = false;                             // the group has reached its leaf: it idles until the warp's last group has
+    if (k == 0 && t.own) { t.path[0] = -1; t.path_reward[0] = t.root_reward; }
+    do {
         const int base = e * c.A;
-        const bool valid = (k < c.A) && (e != 0 || ((t.legal >> k) & 1u));
+        const bool valid = !done && (k < c.A) && (e != 0 || ((t.legal >> k) & 1u));
         double score = -INFINITY;
         int nc = 0, child_exp_k = -1;
         float reward_k = 0.0f;
@@ -213,7 +214,9 @@ MZ_DEVINL Leaf tree_select(const TreeConst& c, GameTree& t, int sim, int64_t gam
         const unsigned tied = LaneGroup<G>::ballot(valid && score == best);
         const int n_tied = __popc(tied);
         int pick;
-        if (n_tied <= 1) {
+        if (done) {
+            pick = 0;
+        } else if (n_tied <= 1) {
             pick = max(__ffs(tied) - 1, 0);        // n_tied == 0 only for a root without legal actions (rejected by the
                                                    // host; the clamp keeps the slot inside the game's pool regardless)
         } else {
@@ -227,21 +230,24 @@ MZ_DEVINL Leaf tree_select(const TreeConst& c, GameTree& t, int sim, int64_t gam
             pick = nth_set_bit(tied, idx);
         }
         const int slot = base + pick;
-        depth += 1;
         // the picked child's fields come from the lane that scored it (no second round of loads)
         const int child_exp = LaneGroup<G>::bcast(child_exp_k, pick);
         const int child_visits = LaneGroup<G>::bcast(nc, pick);
-        if (k == pick) { t.path[depth] = slot; t.path_reward[depth] = reward_k; }
-        if (child_exp < 0) {
-            leaf.depth = depth;
-            leaf.parent_exp = e;
-            leaf.action = pick;
-            leaf.slot = slot;
-            break;
+        if (!done) {
+            depth += 1;
+            if (k == pick && t.own) { t.path[depth] = slot; t.path_reward[depth] = reward_k; }
+            if (child_exp < 0) {
+                leaf.depth = depth;
+                leaf.parent_exp = e;
+                leaf.action = pick;
+                leaf.slot = slot;
+                done = true;
+            } else {
+                n_parent = child_visits;
+                e = child_exp;
+            }
         }
-        n_parent = child_visits;
-        e = child_exp;
-    }
+    } while (LaneGroup<G>::warp_any(!done));
     LaneGroup<G>::sync();
     return leaf;
 }
@@ -311,7 +317,6 @@ MZ_DEVINL Leaf tree_select_lookahead(const TreeConst& c, GameTree& t, const Sele
     const int A = kA ? kA : c.A;
     const int D = sl.D;
     const int k = LaneGroup<G>::lane();
-    const unsigned gm = LaneGroup<G>::mask();
     const unsigned seg_mask = (1u << A) - 1u;
     const bool pow2 = (A & (A - 1)) == 0;
     int e = 0;
@@ -319,11 +324,12 @@ MZ_DEVINL Leaf tree_select_lookahead(const TreeConst& c, GameTree& t, const Sele
     int depth = 0;                                 // levels resolved before this round
     Leaf leaf;
     rounds = 0;
-    if (k == 0) { t.path[0] = -1; t.path_reward[0] = t.root_reward; }
-    while (true) {
-        rounds += 1;
+    bool done = false;                             // as in tree_select
+    if (k == 0 && t.own) { t.path[0] = -1; t.path_reward[0] = t.root_reward; }
+    do {
+        rounds += done ? 0 : 1;
         // this lane's parent: one dependent (expansion, visit) load per level below the first
-        int pe = e, np = n_parent;
+        int pe = done ? -1 : e, np = n_parent;
 #pragma unroll
         for (int d = 1; d < kMaxD; ++d) {
             if (d < sl.level && pe >= 0) {
@@ -361,15 +367,15 @@ MZ_DEVINL Leaf tree_select_lookahead(const TreeConst& c, GameTree& t, const Sele
         double best = score;
         if (pow2) {
             // level offsets are multiples of A: the sibling blocks are aligned
-            for (int o = A >> 1; o > 0; o >>= 1) best = fmax(best, shfl_xor_f64(gm, best, o, G));
+            for (int o = A >> 1; o > 0; o >>= 1) best = fmax(best, shfl_xor_f64(kWarp, best, o, G));
         } else {
             // reduce towards the block's first lane, then broadcast from it
             for (int o = 1; o < A; o <<= 1) {
-                const int lo = __shfl_down_sync(gm, __double2loint(best), o, G);
-                const int hi = __shfl_down_sync(gm, __double2hiint(best), o, G);
+                const int lo = __shfl_down_sync(kWarp, __double2loint(best), o, G);
+                const int hi = __shfl_down_sync(kWarp, __double2hiint(best), o, G);
                 if (sl.act + o < A) best = fmax(best, __hiloint2double(hi, lo));
             }
-            best = shfl_f64(gm, best, k - sl.act, G);
+            best = shfl_f64(kWarp, best, k - sl.act, G);
         }
         const unsigned tie_bits = LaneGroup<G>::ballot(valid && score == best);
         const unsigned exp_bits = LaneGroup<G>::ballot(valid && child_exp_k >= 0);
@@ -379,7 +385,7 @@ MZ_DEVINL Leaf tree_select_lookahead(const TreeConst& c, GameTree& t, const Sele
         bool hit_leaf = false;
 #pragma unroll
         for (int d = 0; d < kMaxD; ++d) {
-            if (d < D && !hit_leaf) {
+            if (d < D && !hit_leaf && !done) {
                 const int seg = off + p * A;
                 const unsigned tied = (tie_bits >> seg) & seg_mask;
                 const int n_tied = __popc(tied);
@@ -405,19 +411,22 @@ MZ_DEVINL Leaf tree_select_lookahead(const TreeConst& c, GameTree& t, const Sele
                 p = p * A + pick;
             }
         }
-        if ((picked >> k) & 1u) { t.path[depth + sl.level] = slot; t.path_reward[depth + sl.level] = reward_k; }
+        if (((picked >> k) & 1u) && t.own) { t.path[depth + sl.level] = slot; t.path_reward[depth + sl.level] = reward_k; }
+        // (picked == 0 once done) the leaf's parent, or the next round's start node and its visit count
+        const int next = LaneGroup<G>::bcast(hit_leaf ? pe : child_exp_k, last);
+        const int next_visits = LaneGroup<G>::bcast(nc, last);
         if (hit_leaf) {
-            const int pe_last = LaneGroup<G>::bcast(pe, last);
             leaf.depth = depth + dl;
-            leaf.parent_exp = pe_last;
+            leaf.parent_exp = next;
             leaf.action = pick;
-            leaf.slot = pe_last * A + pick;
-            break;
+            leaf.slot = next * A + pick;
+            done = true;
+        } else if (!done) {
+            e = next;
+            n_parent = next_visits;
+            depth += D;
         }
-        e = LaneGroup<G>::bcast(child_exp_k, last);
-        n_parent = LaneGroup<G>::bcast(nc, last);
-        depth += D;
-    }
+    } while (LaneGroup<G>::warp_any(!done));
     LaneGroup<G>::sync();
     return leaf;
 }
@@ -430,12 +439,12 @@ template <int G>
 MZ_DEVINL int tree_expand(const TreeConst& c, GameTree& t, const Leaf& leaf, float reward, float prior_f32) {
     const int k = LaneGroup<G>::lane();
     const int e = t.n_expanded;
-    if (k == 0) {
+    if (k == 0 && t.own) {
         t.expansion[leaf.slot] = e;
         t.reward[leaf.slot] = reward;
         t.path_reward[leaf.depth] = reward;
     }
-    if (k < c.A) {
+    if (k < c.A && t.own) {
         const int s = e * c.A + k;
         t.visit[s] = 0;
         t.vsum[s] = 0.0;
@@ -462,8 +471,10 @@ MZ_DEVINL void tree_backup(const TreeConst& c, GameTree& t, const Leaf& leaf, fl
     double v = (double)leaf_value;                    // value seen by node j, starting at j = L
     double root_vsum = t.root_vsum;
     // lane j holds (slot, reward) of path node j when the path fits in the group: the serial recurrence
-    // then runs on shuffles instead of a dependent chain of loads
-    const bool packed = (L < G);
+    // then runs on shuffles instead of a dependent chain of loads.  Its shuffles are collectives, so the choice and the trip
+    // count follow the deepest path of the warp (Lw); the shallower groups' steps j > L change nothing.
+    const int Lw = G < 32 ? (int)__reduce_max_sync(kWarp, (unsigned)L) : L;
+    const bool packed = (Lw < G);
     int my_slot = -1;
     float my_reward = 0.0f;
     if (packed && k <= L) { my_slot = t.path[k]; my_reward = t.path_reward[k]; }
@@ -471,14 +482,15 @@ MZ_DEVINL void tree_backup(const TreeConst& c, GameTree& t, const Leaf& leaf, fl
         // The recurrence runs on shuffles and every lane keeps the value its own node saw; the node updates then happen
         // ONCE, all lanes in parallel (a divergent owner block inside the loop would be issued L + 1 times, one lane each).
         double myv = 0.0;
-        for (int j = L; j >= 0; --j) {
+        for (int j = Lw; j >= 0; --j) {
             const double r = (double)LaneGroup<G>::bcast(my_reward, j);
             const bool same = (c.P == 1) || (((L - j) & 1) == 0);
             if (j == k) myv = v;
             const double rr = (c.P == 1) ? r : (same ? -r : r);
-            v = __dadd_rn(rr, __dmul_rn(c.discount, v));
+            const double vn = __dadd_rn(rr, __dmul_rn(c.discount, v));
+            v = j <= L ? vn : v;
         }
-        if (k <= L) {
+        if (k <= L && t.own) {
             const bool same = (c.P == 1) || (((L - k) & 1) == 0);
             const double add = same ? myv : -myv;
             double q;
@@ -498,13 +510,13 @@ MZ_DEVINL void tree_backup(const TreeConst& c, GameTree& t, const Leaf& leaf, fl
             hi = m;
         }
     } else {
-    for (int j = L; j >= 0; --j) {
+    for (int j = L; j >= 0; --j) {                    // (no collective in this loop: its trip count may differ per group)
         const int slot = t.path[j];
         const float rf = t.path_reward[j];
         const double r = (double)rf;
         // node.to_play == to_play  <=>  (L - j) even (players alternate every level)
         const bool same = (c.P == 1) || (((L - j) & 1) == 0);
-        if ((j % G) == k) {
+        if ((j % G) == k && t.own) {
             const double add = same ? v : -v;
             double q;
             if (j == 0) {
@@ -528,10 +540,10 @@ MZ_DEVINL void tree_backup(const TreeConst& c, GameTree& t, const Leaf& leaf, fl
         v = __dadd_rn(rr, __dmul_rn(c.discount, v));
     }
     }
-    // only lanes 0..L hold candidates: reduce over the smallest power of two covering them,
-    // then broadcast lane 0's result (lanes beyond the reduced width hold partial values)
-    const int width = (L + 1 >= G) ? G : pow2_ceil(L + 1);
-    const unsigned gm = LaneGroup<G>::mask();
+    // only lanes 0..L hold candidates: reduce over the smallest power of two covering the warp's deepest path (the others
+    // hold the neutral +-inf), then broadcast lane 0's result (lanes beyond the reduced width hold partial values)
+    const int width = (Lw + 1 >= G) ? G : pow2_ceil(Lw + 1);
+    const unsigned gm = kWarp;
     if (width >= 2) {
         // minimum and maximum in ONE butterfly: after the first exchange the lower half of the `width` lanes carries minimum
         // candidates and the upper half maximum candidates (each lane sends the one it does not keep), the remaining steps

@@ -23,9 +23,13 @@ template <int G, bool kLatency>
 __global__ void __launch_bounds__(128) tree_step_kernel(const __grid_constant__ TreeStepArgs a) {
     pdl_launch_dependents();
     pdl_wait();                                   // everything below reads what the network kernels just wrote
+    // a warp with a game runs whole: a group past the last game replays the last one (in this warp) and stores nothing
+    const int first = (blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) / G;
+    if (first >= a.n) return;
     const int local = (blockIdx.x * blockDim.x + threadIdx.x) / G;
-    if (local >= a.n) return;
-    tree_step_game<G, kLatency>(a, a.g0 + local, a.sim, a.do_root, a.do_update, a.do_select, a.do_final);   // arrays are addressed by the global game index
+    const bool own = local < a.n;
+    tree_step_game<G, kLatency>(a, a.g0 + (own ? local : a.n - 1), own, a.sim, a.do_root, a.do_update, a.do_select,
+                                a.do_final);   // arrays are addressed by the global game index
 }
 
 // override_root_with (self_play.py:275-277, 310-314): the tree mz_import_tree put into the pool becomes the root of a new
@@ -34,13 +38,16 @@ __global__ void __launch_bounds__(128) tree_step_kernel(const __grid_constant__ 
 // search) so that the per-simulation kernel keeps its register budget.
 template <int G>
 __global__ void __launch_bounds__(128) tree_adopt_root_kernel(const __grid_constant__ TreeStepArgs a) {
+    // a warp with a game runs whole: a group past the last game replays the last one (in this warp) and stores nothing
+    const int first = (blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) / G;
+    if (first >= a.n) return;
     const int local = (blockIdx.x * blockDim.x + threadIdx.x) / G;
-    if (local >= a.n) return;
-    const int g = a.g0 + local;
+    const bool own = local < a.n;
+    const int g = a.g0 + (own ? local : a.n - 1);
     const int lane = LaneGroup<G>::lane();
     const int A = a.A;
     const NodePool& p = a.pool;
-    if (lane == 0) {
+    if (lane == 0 && own) {
         p.range[2 * g] = INFINITY;
         p.range[2 * g + 1] = -INFINITY;
         p.ties[g] = 0;
@@ -52,10 +59,9 @@ __global__ void __launch_bounds__(128) tree_adopt_root_kernel(const __grid_const
         double sum = 0.0;
         if (!a.noise) {                               // drawn here: normalised Gamma(alpha) draws over the whole action space
             for (int k = lane; k < A; k += G) sum += philox_gamma(a.seed, gid, mv, k, a.noise_alpha);
-            const unsigned m = LaneGroup<G>::mask();
-            for (int off = G >> 1; off > 0; off >>= 1) sum += shfl_xor_f64(m, sum, off, G);
+            for (int off = G >> 1; off > 0; off >>= 1) sum += shfl_xor_f64(kWarp, sum, off, G);
         }
-        for (int k = lane; k < A; k += G) {           // lane l owns the actions l, l + G, ...
+        for (int k = lane; k < A && own; k += G) {    // lane l owns the actions l, l + G, ...
             const double nz = a.noise ? a.noise[(size_t)g * A + k] : philox_gamma(a.seed, gid, mv, k, a.noise_alpha) / sum;
             if (a.trace.noise) a.trace.noise[(size_t)g * A + k] = nz;
             double* rp = p.root_prior + (size_t)g * A + k;

@@ -2,7 +2,8 @@
 // and the fused small-network search kernel (small_search.cu) execute the SAME code:
 //   [root expansion] -> [expand + backup of the previous simulation's leaf] -> [selection of the next leaf] -> [read-out]
 // A group of G >= |A| lanes owns game g (global index into the node pool).  `sim` is the simulation selected by this
-// step (do_select); do_update handles sim - 1.
+// step (do_select); do_update handles sim - 1.  own = false: the group has no game of its own and replays game g, which
+// belongs to another group of its warp, without storing anything (the warp's collectives need every group, see LaneGroup).
 #pragma once
 #include "kernels.h"
 #include "pipeline.h"
@@ -11,7 +12,8 @@
 namespace mz {
 
 template <int G, bool kLatency>
-MZ_DEVINL void tree_step_game(const TreeStepArgs& a, int g, int sim, int do_root, int do_update, int do_select, int do_final) {
+MZ_DEVINL void tree_step_game(const TreeStepArgs& a, int g, bool own, int sim, int do_root, int do_update, int do_select,
+                               int do_final) {
     const int lane = LaneGroup<G>::lane();
     const int N = a.N, A = a.A;
     const size_t slots = (size_t)(N + 1) * A;
@@ -31,6 +33,7 @@ MZ_DEVINL void tree_step_game(const TreeStepArgs& a, int g, int sim, int do_root
     t.root_prior = p.root_prior + (size_t)g * A;
     t.path = p.path + (size_t)g * (N + 2);
     t.path_reward = p.path_reward + (size_t)g * (N + 2);
+    t.own = own;
     int max_depth = 0;
 
     if (do_root == 1) {
@@ -43,12 +46,12 @@ MZ_DEVINL void tree_step_game(const TreeStepArgs& a, int g, int sim, int do_root
         if (a.policy_is_prior) prior = (lane < A) ? a.net_policy[(size_t)g * a.policy_stride + lane] : 0.0f;
         else prior = group_softmax_masked<G>((lane < A) ? a.net_policy[(size_t)g * a.policy_stride + lane] : 0.0f, ok);
         const float root_reward = a.net_reward ? a.net_reward[(size_t)g * a.value_stride] : inverse_value_transform(0.0f);
-        if (a.trace.root_priors_raw && lane < A) a.trace.root_priors_raw[(size_t)g * A + lane] = ok ? prior : 0.0f;
-        if (a.trace.root_reward && lane == 0) a.trace.root_reward[g] = root_reward;
+        if (a.trace.root_priors_raw && lane < A && own) a.trace.root_priors_raw[(size_t)g * A + lane] = ok ? prior : 0.0f;
+        if (a.trace.root_reward && lane == 0 && own) a.trace.root_reward[g] = root_reward;
         tree_init_root<G>(c, t, prior, root_reward, (a.add_noise && a.noise) ? a.noise + (size_t)g * A : nullptr,
                           a.add_noise && !a.noise, a.game_id ? a.game_id[g] : (int64_t)g, a.move_index ? a.move_index[g] : 0,
                           a.trace.noise ? a.trace.noise + (size_t)g * A : nullptr);
-        if (lane == 0 && a.root_predicted_value) a.root_predicted_value[g] = a.net_value[(size_t)g * a.value_stride];
+        if (lane == 0 && own && a.root_predicted_value) a.root_predicted_value[g] = a.net_value[(size_t)g * a.value_stride];
     } else {
         t.legal = p.legal[g];
         t.root_visit = p.root_visit[g];
@@ -72,7 +75,7 @@ MZ_DEVINL void tree_step_game(const TreeStepArgs& a, int g, int sim, int do_root
         float prior;
         if (a.policy_is_prior) prior = (lane < A) ? a.net_policy[(size_t)g * a.policy_stride + lane] : 0.0f;
         else prior = group_softmax_masked<G>((lane < A) ? a.net_policy[(size_t)g * a.policy_stride + lane] : 0.0f, lane < A);
-        if (a.trace.depth) {
+        if (a.trace.depth && own) {
             const size_t ti = (size_t)g * N + (sim - 1);
             if (lane == 0) { a.trace.depth[ti] = leaf.depth; a.trace.value[ti] = value; a.trace.reward[ti] = reward; }
             if (lane < A) a.trace.priors[ti * A + lane] = prior;
@@ -89,7 +92,7 @@ MZ_DEVINL void tree_step_game(const TreeStepArgs& a, int g, int sim, int do_root
         const int move = a.move_index ? a.move_index[g] : 0;
         const int first_index = a.first_index ? a.first_index[g] : -1;
         const Leaf leaf = tree_select<G, kLatency>(c, t, sim, game_id, move, first_index);
-        if (lane == 0) {
+        if (lane == 0 && own) {
             p.leaf_depth[g] = leaf.depth;
             p.leaf_parent[g] = leaf.parent_exp;
             p.leaf_action[g] = leaf.action;
@@ -97,7 +100,7 @@ MZ_DEVINL void tree_step_game(const TreeStepArgs& a, int g, int sim, int do_root
         }
     }
 
-    if (lane == 0) {
+    if (lane == 0 && own) {
         p.legal[g] = t.legal;
         p.root_visit[g] = t.root_visit;
         p.root_vsum[g] = t.root_vsum;
@@ -109,7 +112,7 @@ MZ_DEVINL void tree_step_game(const TreeStepArgs& a, int g, int sim, int do_root
         p.max_depth[g] = max_depth;
     }
 
-    if (do_final) {
+    if (do_final && own) {
         if (lane < A) {
             const bool ok = (t.legal >> lane) & 1u;
             if (a.visit_counts) a.visit_counts[(size_t)g * A + lane] = ok ? t.visit[lane] : 0;
