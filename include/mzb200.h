@@ -272,14 +272,23 @@ const char* mz_numerics(const MzHandle* h);
  * finished games only.  Root noise, the first simulation's tie and the action sample come from Philox4x32-10 streams
  * keyed (seed, game id, move), so a game's history does not depend on the batch or on the number of ranks.
  * Requires config.stacked_observations == 0 (the observation is the environment's own). */
-enum { MZ_ENV_CARTPOLE = 0, MZ_ENV_TICTACTOE = 1, MZ_ENV_CONNECT4 = 2 };
+enum { MZ_ENV_CARTPOLE = 0, MZ_ENV_TICTACTOE = 1, MZ_ENV_CONNECT4 = 2, MZ_ENV_GOMOKU = 3, MZ_ENV_TWENTYONE = 4,
+       MZ_ENV_SIMPLE_GRID = 5 };
 
 typedef struct MzSelfPlayDesc {
     int32_t env;                  /* MZ_ENV_*: games/cartpole.py:131-174 (restated cart-pole physics),
-                                     games/tictactoe.py:243-306, games/connect4.py:220-305 */
+                                     games/tictactoe.py:243-306, games/connect4.py:220-305,
+                                     games/gomoku.py:220-292 (11x11, five in a row; the mover is paid reward_scale
+                                     whenever the game ends, a full board included),
+                                     games/twentyone.py:228-303 with Game.step's x10 (one player; cards from the Philox
+                                     stream tag 0x7169E006 at counter (game id, draw k, 0, game id >> 32): card =
+                                     1 + floor(12 u), value min(card, 10); draw 0 = the player's first card, 1 = the
+                                     dealer's, then hits and the dealer's draws in the reference's order),
+                                     games/simple_grid.py:125-229 (one player; 3x3 grid, one-hot observation of 9) */
     int32_t max_moves;            /* config.max_moves */
     int32_t temperature_threshold;/* config.temperature_threshold, 0 = None (self_play.py:153-156) */
-    int32_t reward_scale;         /* board games: reward of the winning move (tictactoe.py:144: 20, connect4.py:144: 10) */
+    int32_t reward_scale;         /* board games: reward of the winning move (tictactoe.py:144: 20, connect4.py:144: 10,
+                                     gomoku: 1); Twenty-One and Simple Grid: Game.step's factor, 10 */
     int64_t first_game_id;        /* slot g plays the global games first_game_id + g + k * game_id_stride, k = 0, 1, ... */
     int64_t game_id_stride;       /* 0 = max_games; world_size * max_games keeps ids unique across ranks */
     /* Initial prioritised-replay priorities |root_value - n-step target| ** PER_alpha of every position of a finished
@@ -338,7 +347,8 @@ typedef struct MzSelfPlayPeek {
 /* replaces the per-move body of SelfPlay.play_game / continuous_self_play for a whole batch (self_play.py:31-183) */
 int mz_selfplay_begin(MzHandle* h, const MzSelfPlayDesc* desc);
 
-/* Opponents of test-mode games (SelfPlay.select_opponent_action, self_play.py:188-220), board games only:
+/* Opponents of test-mode games (SelfPlay.select_opponent_action, self_play.py:188-220), board games only (Gomoku: RANDOM
+ * only, the reference's Gomoku has no expert_agent):
  *   EXPERT  Game.expert_agent (games/tictactoe.py:308-349, games/connect4.py:307-343): a win, else the last block the
  *           scan finds, else the random default;
  *   RANDOM  the random default: the legal action with index floor(u * n_legal) in ascending order, u from the Philox
@@ -349,7 +359,8 @@ enum { MZ_OPPONENT_SELF = 0, MZ_OPPONENT_EXPERT = 1, MZ_OPPONENT_RANDOM = 2 };
  * mz_selfplay_begin with the opponent playing every move whose to_play is not muzero_player, in the same step, so
  * every search is at MuZero's turn (the opponent opens a game when muzero_player is 1).  max_moves counts both sides'
  * moves, and so does MzSelfPlayStats.env_steps.  mz_selfplay_begin(h, d) is mz_selfplay_begin_vs(h, d, MZ_OPPONENT_SELF, 0).
- * Refused: an opponent on CartPole, muzero_player outside {0, 1}, td_steps > 0 with an opponent, an unknown opponent. */
+ * Refused: an opponent on a one-player game (CartPole, Twenty-One, Simple Grid), muzero_player outside {0, 1}, td_steps > 0
+ * with an opponent (MZ_EINVAL); an unknown opponent, EXPERT on Gomoku (MZ_EUNSUPPORTED). */
 int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* desc, int32_t opponent, int32_t muzero_player);
 int mz_selfplay_moves(MzHandle* h, int32_t n_moves, double temperature, const MzSelfPlayInject* inject, MzSelfPlayStats* stats);
 /* the same in two halves, so the host can work while the device plays: enqueue returns at once, wait synchronises */
@@ -362,8 +373,8 @@ int mz_selfplay_wait(MzHandle* h, MzSelfPlayStats* stats);
 int mz_selfplay_drain(MzHandle* h, const void** data, uint64_t* bytes, int32_t* n_games, const uint64_t** index);
 int mz_selfplay_peek(MzHandle* h, const MzSelfPlayPeek* out);
 
-/* Debug / parity: the device opponent (MZ_OPPONENT_EXPERT or MZ_OPPONENT_RANDOM) of env (MZ_ENV_TICTACTOE or
- * MZ_ENV_CONNECT4) on n host positions.  board is [n][H*W] of +1 / -1 / 0 (row 0 = bottom), player [n] the side to
+/* Debug / parity: the device opponent (MZ_OPPONENT_EXPERT or MZ_OPPONENT_RANDOM) of env (MZ_ENV_TICTACTOE,
+ * MZ_ENV_CONNECT4, or MZ_ENV_GOMOKU with MZ_OPPONENT_RANDOM only) on n host positions.  board is [n][H*W] of +1 / -1 / 0 (row 0 = bottom), player [n] the side to
  * move (+1 / -1).  The random default is the pick for uniform[i], or default_action[i] when default_action is not NULL
  * (one of the two must be given).  out [n] receives the actions. */
 int mz_debug_opponent_action(int device, int32_t env, int32_t opponent, int32_t n, const int8_t* board,

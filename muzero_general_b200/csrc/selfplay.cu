@@ -10,13 +10,20 @@
 //   TicTacToe  games/tictactoe.py:243-306; Connect4  games/connect4.py:220-305: planes [own stones of player +1,
 //              stones of player -1, side to move (+1/-1)], player +1 = to_play 0 moves first, reward_scale for the mover
 //              on completing a line, done on a line or a full board; Connect4 actions are columns (gravity)
+//   Gomoku     games/gomoku.py:220-292: the same planes on 11x11, five in a row; the mover is paid reward_scale whenever
+//              the game ends, a full board without a line included
+//   TwentyOne  games/twentyone.py:228-303: hit (0) / stand (1); planes [player's hand, dealer's hand, 0] of 3x3; done on
+//              a bust, a stand or exactly 21, then the dealer draws while at 16 or less unless the player went bust;
+//              reward_scale * get_reward (Game.step's x10)
+//   SimpleGrid games/simple_grid.py:125-229: 3x3 grid from (0, 0), action 0 = row + 1, 1 = column + 1, a move off the
+//              edge changes nothing; one-hot observation of 9; reward_scale and done on reaching (2, 2)
 // State per slot lives in HBM (a few dozen bytes); per-move records go to per-slot struct-of-arrays buffers
 // [B][max_moves] and leave the device only when the game ends, as one packed block written by a warp straight into
 // mapped pinned host memory (no per-move D2H, no host-side bookkeeping per move).
 //
 // Random draws: Philox4x32-10 keyed by (seed, global game id, move): root noise and first-simulation ties inside the
 // search (tree.cuh), the action sample here (tag kTagAction), CartPole's reset state (tag kTagReset), the opponent's
-// random default move in test-mode games (tag kTagOpponent).
+// random default move in test-mode games (tag kTagOpponent), Twenty-One's cards (tag kTagCard, counter (game, draw k)).
 //
 // Test-mode games (mz_selfplay_begin_vs, the reference's play_game(0, ..., opponent, muzero_player),
 // self_play.py:110-183): the opponent's move is played by the thread that played MuZero's, right after it (or by
@@ -32,7 +39,8 @@ namespace mz {
 
 constexpr uint32_t kTagReset = 0x7169E004u;
 constexpr uint32_t kTagOpponent = 0x7169E005u;
-constexpr int kMaxCells = 48;              // board cells per slot (Connect4: 42)
+constexpr uint32_t kTagCard = 0x7169E006u;
+constexpr int kMaxCells = 128;             // board cells per slot (Gomoku: 121)
 
 struct SpDev {
     int env, B, A, O, H, W, K, max_moves, threshold, reward_scale;
@@ -48,6 +56,7 @@ struct SpDev {
     int* cart_steps;           // [B]
     int8_t* board;             // [B][kMaxCells], +1 / -1 / 0
     int8_t* player;            // [B] side to move, +1 / -1
+    int32_t* ints;             // [B][4] Twenty-One: player's hand, dealer's hand, cards drawn; Simple Grid: row, column
     // search inputs / outputs (device)
     float* obs;                // [B][O]
     uint8_t* legal;            // [B][A]
@@ -122,6 +131,45 @@ MZ_DEVINL bool cartpole_step(const SpDev& s, int g, int action) {
     return fabs(st[0]) > kXLimit || fabs(st[2]) > theta_limit || steps >= kEpisodeCap;
 }
 
+// Twenty-One: the slot's next card, 1 + floor(12 u) like randint(1, 13), face cards counting 10
+MZ_DEVINL int twentyone_card(const SpDev& s, int g) {
+    int32_t* st = s.ints + (size_t)g * 4;
+    const double u = philox_uniform53(s.seed, s.game_id[g], st[2]++, 0u, kTagCard);
+    const int card = 1 + (int)(12.0 * u);
+    return card < 10 ? card : 10;
+}
+
+MZ_DEVINL void twentyone_reset(const SpDev& s, int g) {
+    int32_t* st = s.ints + (size_t)g * 4;
+    st[2] = 0;
+    st[0] = twentyone_card(s, g);
+    st[1] = twentyone_card(s, g);
+}
+
+// returns done; *reward = get_reward(done) * reward_scale
+MZ_DEVINL bool twentyone_step(const SpDev& s, int g, int action, float* reward) {
+    int32_t* st = s.ints + (size_t)g * 4;
+    if (action == 0) st[0] += twentyone_card(s, g);
+    const bool done = st[0] > 21 || action == 1 || st[0] == 21;
+    int r = 0;
+    if (done) {
+        if (st[0] <= 21)
+            while (st[1] <= 16) st[1] += twentyone_card(s, g);
+        const int p = st[0], d = st[1];
+        r = (p <= 21 && (d < p || d > 21)) ? 1 : (p > 21 ? -1 : (p == d ? 0 : -1));
+    }
+    *reward = (float)(r * s.reward_scale);
+    return done;
+}
+
+// Simple Grid: returns done (the corner (2, 2) reached)
+MZ_DEVINL bool grid_step(const SpDev& s, int g, int action) {
+    int32_t* st = s.ints + (size_t)g * 4;
+    if (action == 0 && st[0] < 2) ++st[0];
+    if (action == 1 && st[1] < 2) ++st[1];
+    return st[0] == 2 && st[1] == 2;
+}
+
 MZ_DEVINL void board_reset(const SpDev& s, int g) {
     int8_t* b = s.board + (size_t)g * kMaxCells;
     for (int i = 0; i < kMaxCells; ++i) b[i] = 0;
@@ -148,8 +196,8 @@ MZ_DEVINL void board_legal(const SpDev& s, int g, uint8_t* legal) {
     }
 }
 
-// places the mover's stone, returns (won, done); the side to move flips
-MZ_DEVINL void board_step(const SpDev& s, int g, int action, bool* won, bool* done) {
+// places the mover's stone, returns (paid, done): paid = a line, or for Gomoku any end; the side to move flips
+MZ_DEVINL void board_step(const SpDev& s, int g, int action, bool* paid, bool* done) {
     int8_t* b = s.board + (size_t)g * kMaxCells;
     const int me = s.player[g];
     int y = -1, x = -1;
@@ -179,7 +227,7 @@ MZ_DEVINL void board_step(const SpDev& s, int g, int action, bool* won, bool* do
     if (s.env == MZ_ENV_CONNECT4) { for (int c = 0; c < s.W; ++c) any |= b[(s.H - 1) * s.W + c] == 0; }
     else { for (int i = 0; i < s.H * s.W; ++i) any |= b[i] == 0; }
     s.player[g] = (int8_t)(-me);
-    *won = w;
+    *paid = w || (s.env == MZ_ENV_GOMOKU && !any);
     *done = w || !any;
 }
 
@@ -187,8 +235,15 @@ MZ_DEVINL void board_step(const SpDev& s, int g, int action, bool* won, bool* do
 MZ_DEVINL void publish(const SpDev& s, int g) {
     float* o = s.obs + (size_t)g * s.O;
     uint8_t* lg = s.legal + (size_t)g * s.A;
-    if (s.env == MZ_ENV_CARTPOLE) {
-        cartpole_observe(s, g, o);
+    if (s.env == MZ_ENV_CARTPOLE || s.env == MZ_ENV_TWENTYONE || s.env == MZ_ENV_SIMPLE_GRID) {
+        const int32_t* st = s.ints + (size_t)g * 4;
+        if (s.env == MZ_ENV_CARTPOLE) {
+            cartpole_observe(s, g, o);
+        } else if (s.env == MZ_ENV_TWENTYONE) {
+            for (int i = 0; i < 9; ++i) { o[i] = (float)st[0]; o[9 + i] = (float)st[1]; o[18 + i] = 0.0f; }
+        } else {
+            for (int i = 0; i < 9; ++i) o[i] = i == st[0] * 3 + st[1] ? 1.0f : 0.0f;
+        }
         for (int k = 0; k < s.A; ++k) lg[k] = 1;
         s.to_play[g] = 0;
     } else {
@@ -295,9 +350,9 @@ MZ_DEVINL bool opponent_move(const SpDev& s, int g) {
     const int t = s.move[g];
     const double u = philox_uniform53(s.seed, s.game_id[g], t, 0u, kTagOpponent);
     const int action = opponent_action(s, g, u);
-    bool won, done;
-    board_step(s, g, action, &won, &done);
-    record_move(s, g, t, action, won ? (float)s.reward_scale : 0.0f, __longlong_as_double(0x7FF8000000000000ll), nullptr);
+    bool paid, done;
+    board_step(s, g, action, &paid, &done);
+    record_move(s, g, t, action, paid ? (float)s.reward_scale : 0.0f, __longlong_as_double(0x7FF8000000000000ll), nullptr);
     return done;
 }
 
@@ -307,7 +362,10 @@ MZ_DEVINL int start_game(const SpDev& s, int g, int64_t gid) {
     s.move[g] = 0;
     s.fin[g] = 0;
     s.last_action[g] = -1;
-    if (s.env == MZ_ENV_CARTPOLE) cartpole_reset(s, g, gid); else board_reset(s, g);
+    if (s.env == MZ_ENV_CARTPOLE) cartpole_reset(s, g, gid);
+    else if (s.env == MZ_ENV_TWENTYONE) twentyone_reset(s, g);
+    else if (s.env == MZ_ENV_SIMPLE_GRID) { s.ints[(size_t)g * 4] = 0; s.ints[(size_t)g * 4 + 1] = 0; }
+    else board_reset(s, g);
     publish(s, g);
     s.first_to_play[g] = s.to_play[g];
     const float* o = s.obs + (size_t)g * s.O;
@@ -380,10 +438,15 @@ MZ_DEVINL int slot_act(const SpDev& s, int g) {
     if (s.env == MZ_ENV_CARTPOLE) {
         done = cartpole_step(s, g, action);
         reward = 1.0f;
+    } else if (s.env == MZ_ENV_TWENTYONE) {
+        done = twentyone_step(s, g, action, &reward);
+    } else if (s.env == MZ_ENV_SIMPLE_GRID) {
+        done = grid_step(s, g, action);
+        reward = done ? (float)s.reward_scale : 0.0f;
     } else {
-        bool won;
-        board_step(s, g, action, &won, &done);
-        reward = won ? (float)s.reward_scale : 0.0f;
+        bool paid;
+        board_step(s, g, action, &paid, &done);
+        reward = paid ? (float)s.reward_scale : 0.0f;
     }
     record_move(s, g, t, action, reward, s.root_value[g], s.visits + (size_t)g * s.A);
     int played = 1;
@@ -583,6 +646,10 @@ extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_
         return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: muzero_player must be 0 or 1, got " + std::to_string(muzero_player));
     if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_CARTPOLE)
         return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: CartPole has one player, its opponent is \"self\"");
+    if (opponent != MZ_OPPONENT_SELF && (d->env == MZ_ENV_TWENTYONE || d->env == MZ_ENV_SIMPLE_GRID))
+        return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: Twenty-One and Simple Grid have one player, their opponent is \"self\"");
+    if (opponent == MZ_OPPONENT_EXPERT && d->env == MZ_ENV_GOMOKU)
+        return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin_vs: Gomoku has no expert opponent (the reference's Game has no expert_agent)");
     if (opponent != MZ_OPPONENT_SELF && d->td_steps > 0)
         return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: test-mode games are not saved to a replay buffer, td_steps must be 0 "
                                   "(an opponent's move has no root value to bootstrap from)");
@@ -595,6 +662,9 @@ extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_
         case MZ_ENV_CARTPOLE: if (A != 2 || O != 4) return fail(h, MZ_EINVAL, "mz_selfplay_begin: CartPole needs 2 actions and a 4-value observation (stacked_observations must be 0)"); break;
         case MZ_ENV_TICTACTOE: H = 3; W = 3; K = 3; if (A != 9 || O != 27) return fail(h, MZ_EINVAL, "mz_selfplay_begin: TicTacToe needs 9 actions and a 3x3x3 observation (stacked_observations must be 0)"); break;
         case MZ_ENV_CONNECT4: H = 6; W = 7; K = 4; if (A != 7 || O != 126) return fail(h, MZ_EINVAL, "mz_selfplay_begin: Connect4 needs 7 actions and a 3x6x7 observation (stacked_observations must be 0)"); break;
+        case MZ_ENV_GOMOKU: H = 11; W = 11; K = 5; if (A != 121 || O != 363) return fail(h, MZ_EINVAL, "mz_selfplay_begin: Gomoku needs 121 actions and a 3x11x11 observation (stacked_observations must be 0)"); break;
+        case MZ_ENV_TWENTYONE: if (A != 2 || O != 27) return fail(h, MZ_EINVAL, "mz_selfplay_begin: Twenty-One needs 2 actions and a 3x3x3 observation (stacked_observations must be 0)"); break;
+        case MZ_ENV_SIMPLE_GRID: if (A != 2 || O != 9) return fail(h, MZ_EINVAL, "mz_selfplay_begin: Simple Grid needs 2 actions and a 9-value observation (stacked_observations must be 0)"); break;
         default: return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin: unknown environment");
     }
     if (d->max_moves < 1) return fail(h, MZ_EINVAL, "mz_selfplay_begin: max_moves < 1");
@@ -620,6 +690,7 @@ extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_
     }
     const size_t T = (size_t)d->max_moves;
     bool ok = sp_alloc(sp, &s.cart, (size_t)B * 4) && sp_alloc(sp, &s.cart_steps, B) && sp_alloc(sp, &s.board, (size_t)B * kMaxCells) &&
+              sp_alloc(sp, &s.ints, (size_t)B * 4) &&
               sp_alloc(sp, &s.player, B) && sp_alloc(sp, &s.obs, (size_t)B * O) && sp_alloc(sp, &s.legal, (size_t)B * A) &&
               sp_alloc(sp, &s.to_play, B) && sp_alloc(sp, &s.game_id, B) && sp_alloc(sp, &s.move, B) &&
               sp_alloc(sp, &s.visits, (size_t)B * A) && sp_alloc(sp, &s.root_value, B) && sp_alloc(sp, &s.rec_root, B * T) &&
@@ -828,10 +899,13 @@ extern "C" int mz_debug_opponent_action(int device, int32_t env, int32_t opponen
     switch (env) {
         case MZ_ENV_TICTACTOE: s.H = 3; s.W = 3; s.K = 3; s.A = 9; break;
         case MZ_ENV_CONNECT4: s.H = 6; s.W = 7; s.K = 4; s.A = 7; break;
+        case MZ_ENV_GOMOKU: s.H = 11; s.W = 11; s.K = 5; s.A = 121; break;
         default: return fail(nullptr, MZ_EUNSUPPORTED, "mz_debug_opponent_action: no opponent for this environment");
     }
     if (opponent != MZ_OPPONENT_EXPERT && opponent != MZ_OPPONENT_RANDOM)
         return fail(nullptr, MZ_EUNSUPPORTED, "mz_debug_opponent_action: opponent must be MZ_OPPONENT_EXPERT or MZ_OPPONENT_RANDOM");
+    if (opponent == MZ_OPPONENT_EXPERT && env == MZ_ENV_GOMOKU)
+        return fail(nullptr, MZ_EUNSUPPORTED, "mz_debug_opponent_action: Gomoku has no expert opponent");
     if (n < 1 || !board || !player || !out || (!uniform && !default_action))
         return fail(nullptr, MZ_EINVAL, "mz_debug_opponent_action: bad argument");
     const int cells = s.H * s.W;
@@ -844,7 +918,7 @@ extern "C" int mz_debug_opponent_action(int device, int32_t env, int32_t opponen
         for (int c = 0; c < cells; ++c) {
             if (board[(size_t)i * cells + c] < -1 || board[(size_t)i * cells + c] > 1)
                 return fail(nullptr, MZ_EINVAL, "mz_debug_opponent_action: board cells must be +1, -1 or 0");
-            any |= board[(size_t)i * cells + c] == 0 && (env == MZ_ENV_TICTACTOE || c >= (s.H - 1) * s.W);
+            any |= board[(size_t)i * cells + c] == 0 && (env != MZ_ENV_CONNECT4 || c >= (s.H - 1) * s.W);
         }
         if (!any) return fail(nullptr, MZ_EINVAL, "mz_debug_opponent_action: a position without a legal action");
     }

@@ -369,14 +369,16 @@ class DeviceSelfPlayLoop:
     """Python face of mz_selfplay_*: ``max_games`` environments stepped on the GPU, one batched search per move,
     finished games handed back as packed struct-of-arrays blocks (SURVEY.md 8f-1, include/mzb200.h)."""
 
-    ENVS = {"cartpole": _lib.MZ_ENV_CARTPOLE, "tictactoe": _lib.MZ_ENV_TICTACTOE, "connect4": _lib.MZ_ENV_CONNECT4}
+    ENVS = {"cartpole": _lib.MZ_ENV_CARTPOLE, "tictactoe": _lib.MZ_ENV_TICTACTOE, "connect4": _lib.MZ_ENV_CONNECT4,
+            "gomoku": _lib.MZ_ENV_GOMOKU, "twentyone": _lib.MZ_ENV_TWENTYONE, "simple_grid": _lib.MZ_ENV_SIMPLE_GRID}
     OPPONENTS = {"self": _lib.MZ_OPPONENT_SELF, "expert": _lib.MZ_OPPONENT_EXPERT, "random": _lib.MZ_OPPONENT_RANDOM}
 
     def __init__(self, engine: SearchEngine, env: str, max_moves: int, temperature_threshold=None, reward_scale: int = 1,
                  first_game_id: int = 0, staging_bytes: int = 0, game_id_stride: int = 0, td_steps: int = 0,
                  per_alpha: float = 1.0, discount: float = 1.0, opponent: str = "self", muzero_player: int = 0):
         """``opponent`` "expert" or "random" plays test-mode games (``play_game(..., opponent, muzero_player)``): the
-        opponent's moves are played on the device and recorded with a NaN root value and zero visit counts."""
+        opponent's moves are played on the device and recorded with a NaN root value and zero visit counts.  An opponent
+        the game lacks (Gomoku's "expert") raises NotImplementedError."""
         if env not in self.ENVS:
             raise NotImplementedError(f"no device-resident environment for {env!r}")
         if opponent not in self.OPPONENTS:
@@ -397,7 +399,12 @@ class DeviceSelfPlayLoop:
             d.discount_pow = C.cast(self._discount_pow, C.c_void_p)
         self.with_priorities = bool(d.td_steps)
         d.staging_bytes = int(staging_bytes)
-        engine._check(engine.lib.mz_selfplay_begin_vs(engine._h, C.byref(d), self.OPPONENTS[opponent], self.muzero_player))
+        try:
+            engine._check(engine.lib.mz_selfplay_begin_vs(engine._h, C.byref(d), self.OPPONENTS[opponent], self.muzero_player))
+        except _lib.MzError as e:
+            if e.code == _lib.MZ_EUNSUPPORTED:
+                raise NotImplementedError(str(e)) from e
+            raise
         self.stats = _lib.MzSelfPlayStats()
 
     def moves(self, n_moves: int, temperature: float, forced_action=None, uniform=None, noise=None, first_index=None):
@@ -491,7 +498,7 @@ def debug_opponent_action(env, boards, players, uniforms=None, defaults=None, op
     (+1 / -1).  The random default is the legal action with index ``floor(u * n_legal)`` for ``uniforms[i]``, or
     ``defaults[i]`` when given.  Returns the ``[n]`` int32 actions."""
     lib = _lib.load_library()
-    codes = {"tictactoe": _lib.MZ_ENV_TICTACTOE, "connect4": _lib.MZ_ENV_CONNECT4}
+    codes = {"tictactoe": _lib.MZ_ENV_TICTACTOE, "connect4": _lib.MZ_ENV_CONNECT4, "gomoku": _lib.MZ_ENV_GOMOKU}
     if env not in codes:
         raise NotImplementedError(f"no device opponent for {env!r}")
     b = numpy.ascontiguousarray(boards, numpy.int8)

@@ -33,6 +33,7 @@ class GomokuVector(BoardVector):
 
 
 class Game(BoardGame, AbstractGame):
+    DEVICE_ENV = "gomoku"           # csrc/selfplay.cu restates these rules on the device
     VECTOR = GomokuVector
 
     def action_to_string(self, action_number):

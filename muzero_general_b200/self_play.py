@@ -622,7 +622,8 @@ class SelfPlay:
     def play_moves(self, n_moves, temperature, temperature_threshold=None):
         """Advance every game of the lockstep batch by ``n_moves`` moves; returns the games that finished.
 
-        With ``rng_mode="philox"`` and a game that has a device-resident environment (CartPole, TicTacToe, Connect4)
+        With ``rng_mode="philox"`` and a game that has a device-resident environment (CartPole, TicTacToe, Connect4,
+        Gomoku, Twenty-One, Simple Grid)
         the whole loop - observation, search, visit-count sampling, environment step, history records - runs on the
         GPU (``mz_selfplay_moves``) and only finished games cross to the host, as ``PackedGameHistory`` objects.
         Otherwise the host loop (``BatchedSelfPlay.move``) is used."""
@@ -658,8 +659,8 @@ class SelfPlay:
         cfg = self.config
         if self._device_env_name() is None:
             raise NotImplementedError(
-                "test games on the device need a device environment (CartPole, TicTacToe or Connect4 with "
-                "rng_mode='philox' and stacked_observations=0); play them one at a time with "
+                "test games on the device need a device environment (CartPole, TicTacToe, Connect4, Gomoku, Twenty-One "
+                "or Simple Grid with rng_mode='philox' and stacked_observations=0); play them one at a time with "
                 "play_game(0, config.temperature_threshold, False, opponent, muzero_player)")
         if self._device_loop is not None:
             raise RuntimeError("this worker's device self-play loop has games in flight, and starting test games on the "
@@ -682,7 +683,9 @@ class SelfPlay:
             for buf, index in dev.moves(min(dev.chunk, 4), temperature)._chunks:
                 ids = numpy.array([int(numpy.frombuffer(buf, numpy.int64, 1, int(off))[0]) for off in index[:, 0]])
                 keep = numpy.isin(ids, wanted)
-                games.add(buf, index[keep])
+                # in game-id order: the games of one drain are staged in the order their warps reserved space, and
+                # the summary's float means must not depend on it
+                games.add(buf, index[keep][numpy.argsort(ids[keep], kind="stable")])
                 missing -= int(keep.sum())
         # the next call starts past every id this one began
         started = int(dev.loop.peek()["game_id"].max())
