@@ -271,7 +271,11 @@ const char* mz_numerics(const MzHandle* h);
  * kernel that detects it and its slot starts a new game with a fresh global id (old id + game_id_stride); the host reads
  * finished games only.  Root noise, the first simulation's tie and the action sample come from Philox4x32-10 streams
  * keyed (seed, game id, move), so a game's history does not depend on the batch or on the number of ranks.
- * Requires config.stacked_observations == 0 (the observation is the environment's own). */
+ * With stacked_observations = s > 0 the search input is GameHistory.get_stacked_observations(-1, s, A)
+ * (self_play.py:513-550), built on the device from the game's records: the observation of move t, then for
+ * k = 1..s, p = t - k, the observation after move p and a plane filled with (float)((double)action_p / A) (C + 1 zero
+ * planes when p < 0).  The handle's obs_elems must be (C * (s + 1) + s) * H * W for the environment's C planes of
+ * H x W; the records and the staged blocks hold the environment's own C * H * W observation. */
 enum { MZ_ENV_CARTPOLE = 0, MZ_ENV_TICTACTOE = 1, MZ_ENV_CONNECT4 = 2, MZ_ENV_GOMOKU = 3, MZ_ENV_TWENTYONE = 4,
        MZ_ENV_SIMPLE_GRID = 5 };
 
@@ -296,7 +300,7 @@ typedef struct MzSelfPlayDesc {
      * the game.  td_steps = 0: not computed.  discount_pow[k] = config.discount ** k for k = 0..td_steps, computed by the
      * caller (Python's own pow, so the products are the reference's); per_alpha must be 0.5 or 1 (an exact sqrt / identity). */
     int32_t td_steps;
-    int32_t reserved;
+    int32_t stacked_observations; /* config.stacked_observations, >= 0; 0 = the search sees the observation alone */
     double per_alpha;
     const double* discount_pow;
     uint64_t staging_bytes;       /* capacity of the finished-game staging area, 0 = library default (4x the bytes of
@@ -326,7 +330,8 @@ typedef struct MzSelfPlayStats {
 
 /* Current device-side view of the environments (HOST output pointers, any may be NULL). */
 typedef struct MzSelfPlayPeek {
-    float* obs;                   /* [n, obs_elems] observation the next search will see */
+    float* obs;                   /* [n, obs_elems] input the next search will see (the stacked input when
+                                     stacked_observations > 0) */
     uint8_t* legal_mask;          /* [n, A] */
     int32_t* to_play;             /* [n] */
     int64_t* game_id;             /* [n] */
@@ -360,7 +365,9 @@ enum { MZ_OPPONENT_SELF = 0, MZ_OPPONENT_EXPERT = 1, MZ_OPPONENT_RANDOM = 2 };
  * every search is at MuZero's turn (the opponent opens a game when muzero_player is 1).  max_moves counts both sides'
  * moves, and so does MzSelfPlayStats.env_steps.  mz_selfplay_begin(h, d) is mz_selfplay_begin_vs(h, d, MZ_OPPONENT_SELF, 0).
  * Refused: an opponent on a one-player game (CartPole, Twenty-One, Simple Grid), muzero_player outside {0, 1}, td_steps > 0
- * with an opponent (MZ_EINVAL); an unknown opponent, EXPERT on Gomoku (MZ_EUNSUPPORTED). */
+ * with an opponent, stacked_observations < 0, a handle whose action space or obs_elems does not fit the environment and
+ * stacked_observations (MZ_EINVAL); an unknown opponent, EXPERT on Gomoku (MZ_EUNSUPPORTED).  The opponent's moves are
+ * part of the stacked history like MuZero's. */
 int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* desc, int32_t opponent, int32_t muzero_player);
 int mz_selfplay_moves(MzHandle* h, int32_t n_moves, double temperature, const MzSelfPlayInject* inject, MzSelfPlayStats* stats);
 /* the same in two halves, so the host can work while the device plays: enqueue returns at once, wait synchronises */

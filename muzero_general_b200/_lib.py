@@ -89,8 +89,8 @@ class MzInferenceOut(C.Structure):
 class MzSelfPlayDesc(C.Structure):
     _fields_ = [("env", C.c_int32), ("max_moves", C.c_int32), ("temperature_threshold", C.c_int32),
                 ("reward_scale", C.c_int32), ("first_game_id", C.c_int64), ("game_id_stride", C.c_int64),
-                ("td_steps", C.c_int32), ("reserved", C.c_int32), ("per_alpha", C.c_double), ("discount_pow", C.c_void_p),
-                ("staging_bytes", C.c_uint64)]
+                ("td_steps", C.c_int32), ("stacked_observations", C.c_int32), ("per_alpha", C.c_double),
+                ("discount_pow", C.c_void_p), ("staging_bytes", C.c_uint64)]
 
 
 class MzSelfPlayInject(C.Structure):

@@ -28,6 +28,10 @@
 // Test-mode games (mz_selfplay_begin_vs, the reference's play_game(0, ..., opponent, muzero_player),
 // self_play.py:110-183): the opponent's move is played by the thread that played MuZero's, right after it (or by
 // start_game when the opponent moves first), so every search runs at MuZero's turn.
+//
+// Stacked observations (config.stacked_observations = s > 0): the search input of a slot is [B][O_in] with
+// O_in = O + s * (O + plane), the current observation (O floats) followed by the tail that stack_fill builds from the
+// slot's records.  Records, staged blocks and rec_obs keep the environment's own O.
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -44,6 +48,9 @@ constexpr int kMaxCells = 128;             // board cells per slot (Gomoku: 121)
 
 struct SpDev {
     int env, B, A, O, H, W, K, max_moves, threshold, reward_scale;
+    int O_in;                  // floats of a slot's search input: O, plus stack * (O + plane) stacked floats
+    int stack;                 // config.stacked_observations
+    int plane;                 // floats of one observation plane (the action plane of the stack has this size)
     int opponent;              // MZ_OPPONENT_*
     int muzero_player;         // to_play of MuZero's side when opponent != MZ_OPPONENT_SELF
     uint64_t seed;
@@ -58,7 +65,7 @@ struct SpDev {
     int8_t* player;            // [B] side to move, +1 / -1
     int32_t* ints;             // [B][4] Twenty-One: player's hand, dealer's hand, cards drawn; Simple Grid: row, column
     // search inputs / outputs (device)
-    float* obs;                // [B][O]
+    float* obs;                // [B][O_in]
     uint8_t* legal;            // [B][A]
     int32_t* to_play;          // [B]
     int64_t* game_id;          // [B]
@@ -231,9 +238,10 @@ MZ_DEVINL void board_step(const SpDev& s, int g, int action, bool* paid, bool* d
     *done = w || !any;
 }
 
-// writes the search inputs of slot g from its environment state
+// writes the search inputs of slot g from its environment state (the current observation: the first O floats of the
+// slot's input)
 MZ_DEVINL void publish(const SpDev& s, int g) {
-    float* o = s.obs + (size_t)g * s.O;
+    float* o = s.obs + (size_t)g * s.O_in;
     uint8_t* lg = s.legal + (size_t)g * s.A;
     if (s.env == MZ_ENV_CARTPOLE || s.env == MZ_ENV_TWENTYONE || s.env == MZ_ENV_SIMPLE_GRID) {
         const int32_t* st = s.ints + (size_t)g * 4;
@@ -338,7 +346,7 @@ MZ_DEVINL void record_move(const SpDev& s, int g, int t, int action, float rewar
     s.rec_reward[r] = reward;
     publish(s, g);
     s.rec_to_play[r] = s.to_play[g];
-    const float* o = s.obs + (size_t)g * s.O;
+    const float* o = s.obs + (size_t)g * s.O_in;
     float* ro = s.rec_obs + ((size_t)g * (s.max_moves + 1) + t + 1) * s.O;
     for (int i = 0; i < s.O; ++i) ro[i] = o[i];
     s.move[g] = t + 1;
@@ -368,7 +376,7 @@ MZ_DEVINL int start_game(const SpDev& s, int g, int64_t gid) {
     else board_reset(s, g);
     publish(s, g);
     s.first_to_play[g] = s.to_play[g];
-    const float* o = s.obs + (size_t)g * s.O;
+    const float* o = s.obs + (size_t)g * s.O_in;
     float* r0 = s.rec_obs + (size_t)g * (s.max_moves + 1) * s.O;
     for (int i = 0; i < s.O; ++i) r0[i] = o[i];
     if (s.opponent == MZ_OPPONENT_SELF || s.to_play[g] == s.muzero_player) return 0;
@@ -377,10 +385,30 @@ MZ_DEVINL int start_game(const SpDev& s, int g, int64_t gid) {
     return 1;
 }
 
+// The stacked tail of slot g's search input, after its current observation (GameHistory.get_stacked_observations(-1),
+// self_play.py:513-550): for k = 1 .. stack, p = t - k with t the moves played, the observation after move p
+// (rec_obs[p]) and a plane of action_history[p + 1] / A = rec_action[p] / A, or O + plane zeros when p < 0.  The
+// action plane is the fp64 quotient rounded once to fp32, what the reference's float64 plane becomes after .float().
+// Threads lane, lane + step, ... share the floats; the slot's records must be visible to all of them.
+MZ_DEVINL void stack_fill(const SpDev& s, int g, int lane, int step) {
+    const int t = s.move[g];
+    const int block = s.O + s.plane;
+    float* tail = s.obs + (size_t)g * s.O_in + s.O;
+    const float* rec = s.rec_obs + (size_t)g * (s.max_moves + 1) * s.O;
+    const int32_t* act = s.rec_action + (size_t)g * s.max_moves;
+    for (int i = lane; i < s.stack * block; i += step) {
+        const int k = i / block, j = i - k * block, p = t - 1 - k;
+        float v = 0.0f;
+        if (p >= 0) v = j < s.O ? rec[(size_t)p * s.O + j] : __double2float_rn(__ddiv_rn((double)act[p], (double)s.A));
+        tail[i] = v;
+    }
+}
+
 __global__ void selfplay_reset_kernel(const SpDev s, int64_t first_game_id) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= s.B) return;
     const int played = start_game(s, g, first_game_id + g);
+    if (s.stack) stack_fill(s, g, 0, 1);
     if (played) atomicAdd(&s.counters[0], (unsigned long long)played);
 }
 
@@ -499,7 +527,8 @@ MZ_DEVINL float initial_priority(const SpDev& s, int g, int T, int i) {
 // Staging space is reserved with ONE atomicAdd per finished game (a compare-and-swap loop serialises hundreds of
 // finishing warps per move): the cursor may run
 // past the capacity, reservations that end beyond it are void (the game stays parked), and since the cursor only grows
-// the valid reservations are a contiguous prefix whose end is tracked in counters[5].
+// the valid reservations are a contiguous prefix whose end is tracked in counters[5].  With stacked observations, a
+// slot whose move was played or whose game restarted then rebuilds its stacked tail with the whole warp.
 constexpr int kStepThreads = 1024;
 
 __global__ void __launch_bounds__(kStepThreads) selfplay_step_kernel(const SpDev s, int act) {
@@ -509,12 +538,14 @@ __global__ void __launch_bounds__(kStepThreads) selfplay_step_kernel(const SpDev
     const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     int T = 0;
+    int changed = 0;                                  // the slot's move count or records changed in this pass
     if (g < s.B) {
         if (lane == 0) {
             T = s.fin[g];
             if (act && T == 0) {
                 atomicAdd(&s_active, slot_act(s, g));
                 T = s.fin[g];
+                changed = 1;
             }
         }
         T = __shfl_sync(0xffffffffu, T, 0);
@@ -578,7 +609,12 @@ __global__ void __launch_bounds__(kStepThreads) selfplay_step_kernel(const SpDev
                 const int played = start_game(s, g, s.game_id[g] + s.id_stride);
                 if (played) atomicAdd(&s_active, played);
             }
+            changed = 1;
         }
+    }
+    if (s.stack && g < s.B && __any_sync(0xffffffffu, changed)) {
+        __syncwarp();                                 // lane 0's records and move count, visible to the warp
+        stack_fill(s, g, lane, 32);
     }
     __syncthreads();
     if (threadIdx.x == 0 && s_active) atomicAdd(&s.counters[0], (unsigned long long)s_active);
@@ -653,20 +689,33 @@ extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_
     if (opponent != MZ_OPPONENT_SELF && d->td_steps > 0)
         return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: test-mode games are not saved to a replay buffer, td_steps must be 0 "
                                   "(an opponent's move has no root value to bootstrap from)");
+    if (d->stacked_observations < 0)
+        return fail(h, MZ_EINVAL, "mz_selfplay_begin: stacked_observations must be >= 0, got " + std::to_string(d->stacked_observations));
     MZ_CUDA(h, cudaSetDevice(h->device));
     MZ_CUDA(h, cudaStreamSynchronize(h->stream));
     mz_selfplay_destroy(h);
-    const int B = h->search.max_games, A = h->net.action_space, O = (int)h->obs_elems;
-    int H = 1, W = 1, K = 0;
+    const int B = h->search.max_games, A = h->net.action_space;
+    // board H x W and line length K; the observation's C planes of ph x pw; the action space
+    int H = 1, W = 1, K = 0, C = 0, ph = 0, pw = 0, A_env = 0;
+    const char* name = "";
     switch (d->env) {
-        case MZ_ENV_CARTPOLE: if (A != 2 || O != 4) return fail(h, MZ_EINVAL, "mz_selfplay_begin: CartPole needs 2 actions and a 4-value observation (stacked_observations must be 0)"); break;
-        case MZ_ENV_TICTACTOE: H = 3; W = 3; K = 3; if (A != 9 || O != 27) return fail(h, MZ_EINVAL, "mz_selfplay_begin: TicTacToe needs 9 actions and a 3x3x3 observation (stacked_observations must be 0)"); break;
-        case MZ_ENV_CONNECT4: H = 6; W = 7; K = 4; if (A != 7 || O != 126) return fail(h, MZ_EINVAL, "mz_selfplay_begin: Connect4 needs 7 actions and a 3x6x7 observation (stacked_observations must be 0)"); break;
-        case MZ_ENV_GOMOKU: H = 11; W = 11; K = 5; if (A != 121 || O != 363) return fail(h, MZ_EINVAL, "mz_selfplay_begin: Gomoku needs 121 actions and a 3x11x11 observation (stacked_observations must be 0)"); break;
-        case MZ_ENV_TWENTYONE: if (A != 2 || O != 27) return fail(h, MZ_EINVAL, "mz_selfplay_begin: Twenty-One needs 2 actions and a 3x3x3 observation (stacked_observations must be 0)"); break;
-        case MZ_ENV_SIMPLE_GRID: if (A != 2 || O != 9) return fail(h, MZ_EINVAL, "mz_selfplay_begin: Simple Grid needs 2 actions and a 9-value observation (stacked_observations must be 0)"); break;
+        case MZ_ENV_CARTPOLE: name = "CartPole"; C = 1; ph = 1; pw = 4; A_env = 2; break;
+        case MZ_ENV_TICTACTOE: name = "TicTacToe"; H = 3; W = 3; K = 3; C = 3; ph = 3; pw = 3; A_env = 9; break;
+        case MZ_ENV_CONNECT4: name = "Connect4"; H = 6; W = 7; K = 4; C = 3; ph = 6; pw = 7; A_env = 7; break;
+        case MZ_ENV_GOMOKU: name = "Gomoku"; H = 11; W = 11; K = 5; C = 3; ph = 11; pw = 11; A_env = 121; break;
+        case MZ_ENV_TWENTYONE: name = "Twenty-One"; C = 3; ph = 3; pw = 3; A_env = 2; break;
+        case MZ_ENV_SIMPLE_GRID: name = "Simple Grid"; C = 1; ph = 1; pw = 9; A_env = 2; break;
         default: return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin: unknown environment");
     }
+    // the network input: the observation and, per stacked step, an earlier observation and its action plane
+    const int64_t stack = d->stacked_observations, obs_c = (int64_t)C * (stack + 1) + stack;
+    if (A != A_env || h->obs_elems != obs_c * ph * pw)
+        return fail(h, MZ_EINVAL, std::string("mz_selfplay_begin: ") + name + " needs " + std::to_string(A_env) +
+                                  " actions and, with stacked_observations = " + std::to_string(stack) + ", an input of obs_c = " +
+                                  std::to_string(obs_c) + " planes of " + std::to_string(ph) + "x" + std::to_string(pw) +
+                                  " (" + std::to_string(obs_c * ph * pw) + " values); the handle has " + std::to_string(A) +
+                                  " actions and " + std::to_string(h->obs_elems) + " input values");
+    const int O = C * ph * pw;
     if (d->max_moves < 1) return fail(h, MZ_EINVAL, "mz_selfplay_begin: max_moves < 1");
     MzSelfPlay* sp = new (std::nothrow) MzSelfPlay();
     if (!sp) return fail(h, MZ_ENOMEM, "mz_selfplay_begin: out of host memory");
@@ -674,6 +723,7 @@ extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_
     sp->desc = *d;
     SpDev& s = sp->dev;
     s.env = d->env; s.B = B; s.A = A; s.O = O; s.H = H; s.W = W; s.K = K; s.max_moves = d->max_moves;
+    s.O_in = (int)h->obs_elems; s.stack = (int)stack; s.plane = ph * pw;
     s.threshold = d->temperature_threshold; s.reward_scale = d->reward_scale; s.seed = h->search.seed;
     s.opponent = opponent; s.muzero_player = muzero_player;
     s.id_stride = d->game_id_stride > 0 ? d->game_id_stride : B;
@@ -691,7 +741,7 @@ extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_
     const size_t T = (size_t)d->max_moves;
     bool ok = sp_alloc(sp, &s.cart, (size_t)B * 4) && sp_alloc(sp, &s.cart_steps, B) && sp_alloc(sp, &s.board, (size_t)B * kMaxCells) &&
               sp_alloc(sp, &s.ints, (size_t)B * 4) &&
-              sp_alloc(sp, &s.player, B) && sp_alloc(sp, &s.obs, (size_t)B * O) && sp_alloc(sp, &s.legal, (size_t)B * A) &&
+              sp_alloc(sp, &s.player, B) && sp_alloc(sp, &s.obs, (size_t)B * s.O_in) && sp_alloc(sp, &s.legal, (size_t)B * A) &&
               sp_alloc(sp, &s.to_play, B) && sp_alloc(sp, &s.game_id, B) && sp_alloc(sp, &s.move, B) &&
               sp_alloc(sp, &s.visits, (size_t)B * A) && sp_alloc(sp, &s.root_value, B) && sp_alloc(sp, &s.rec_root, B * T) &&
               sp_alloc(sp, &s.rec_visits, B * T * A) && sp_alloc(sp, &s.rec_action, B * T) && sp_alloc(sp, &s.rec_reward, B * T) &&
@@ -875,7 +925,7 @@ extern "C" int mz_selfplay_peek(MzHandle* h, const MzSelfPlayPeek* out) {
     MZ_CUDA(h, cudaStreamSynchronize(h->stream));
     const SpDev& s = h->sp->dev;
     const size_t B = s.B;
-    if (out->obs) MZ_CUDA(h, cudaMemcpy(out->obs, s.obs, B * s.O * 4, cudaMemcpyDeviceToHost));
+    if (out->obs) MZ_CUDA(h, cudaMemcpy(out->obs, s.obs, B * s.O_in * 4, cudaMemcpyDeviceToHost));
     if (out->legal_mask) MZ_CUDA(h, cudaMemcpy(out->legal_mask, s.legal, B * s.A, cudaMemcpyDeviceToHost));
     if (out->to_play) MZ_CUDA(h, cudaMemcpy(out->to_play, s.to_play, B * 4, cudaMemcpyDeviceToHost));
     if (out->game_id) MZ_CUDA(h, cudaMemcpy(out->game_id, s.game_id, B * 8, cudaMemcpyDeviceToHost));

@@ -375,10 +375,13 @@ class DeviceSelfPlayLoop:
 
     def __init__(self, engine: SearchEngine, env: str, max_moves: int, temperature_threshold=None, reward_scale: int = 1,
                  first_game_id: int = 0, staging_bytes: int = 0, game_id_stride: int = 0, td_steps: int = 0,
-                 per_alpha: float = 1.0, discount: float = 1.0, opponent: str = "self", muzero_player: int = 0):
+                 per_alpha: float = 1.0, discount: float = 1.0, opponent: str = "self", muzero_player: int = 0,
+                 stacked_observations: int = 0):
         """``opponent`` "expert" or "random" plays test-mode games (``play_game(..., opponent, muzero_player)``): the
         opponent's moves are played on the device and recorded with a NaN root value and zero visit counts.  An opponent
-        the game lacks (Gomoku's "expert") raises NotImplementedError."""
+        the game lacks (Gomoku's "expert") raises NotImplementedError.  ``stacked_observations`` (the config's; the
+        engine's network must have been built for it) makes every search see the stacked input of
+        ``get_stacked_observations``, built on the device; the staged observations stay the environment's own."""
         if env not in self.ENVS:
             raise NotImplementedError(f"no device-resident environment for {env!r}")
         if opponent not in self.OPPONENTS:
@@ -392,6 +395,7 @@ class DeviceSelfPlayLoop:
         d.reward_scale = int(reward_scale)
         d.first_game_id = int(first_game_id)
         d.game_id_stride = int(game_id_stride)
+        d.stacked_observations = int(stacked_observations)
         if td_steps and per_alpha in (0.5, 1, 1.0):
             # PER priorities on the device: discount ** k evaluated HERE, with Python's pow, like replay_buffer.py:246,260
             self._discount_pow = (C.c_double * (int(td_steps) + 1))(*[discount ** k for k in range(int(td_steps) + 1)])

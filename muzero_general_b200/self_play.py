@@ -602,8 +602,7 @@ class SelfPlay:
         """Name of the device-resident environment for this worker, or None (host environments)."""
         cfg = self.config
         name = getattr(self.Game, "DEVICE_ENV", None)
-        if (name is None or self.rng_mode != "philox" or cfg.stacked_observations
-                or not getattr(cfg, "device_envs", True)):
+        if name is None or self.rng_mode != "philox" or not getattr(cfg, "device_envs", True):
             return None
         return name
 
@@ -660,7 +659,7 @@ class SelfPlay:
         if self._device_env_name() is None:
             raise NotImplementedError(
                 "test games on the device need a device environment (CartPole, TicTacToe, Connect4, Gomoku, Twenty-One "
-                "or Simple Grid with rng_mode='philox' and stacked_observations=0); play them one at a time with "
+                "or Simple Grid with rng_mode='philox' and device_envs on); play them one at a time with "
                 "play_game(0, config.temperature_threshold, False, opponent, muzero_player)")
         if self._device_loop is not None:
             raise RuntimeError("this worker's device self-play loop has games in flight, and starting test games on the "
@@ -767,7 +766,8 @@ class DeviceBatchedSelfPlay:
                                        td_steps=int(cfg.td_steps) if priorities else 0,
                                        per_alpha=cfg.PER_alpha, discount=cfg.discount,
                                        staging_bytes=int(getattr(cfg, "selfplay_staging_bytes", 0) or 0),
-                                       opponent=opponent, muzero_player=muzero_player)
+                                       opponent=opponent, muzero_player=muzero_player,
+                                       stacked_observations=int(cfg.stacked_observations))
         self.moves_per_call = int(getattr(cfg, "selfplay_moves_per_call", 64) or 64)   # upper bound of a chunk
         self.chunk = min(4, self.moves_per_call)                                      # adapted to the staging fill below
         self.device_ms = 0.0          # device time of all mz_selfplay_moves calls so far
