@@ -270,10 +270,10 @@ MZ_DEVINL float dot_packed(const float* __restrict__ W, int out, int o, float bi
 
 // One recurrent inference (models.py:147-170, 128-131) of the group's game.  h: parent state (shared, E floats); hn: where
 // the rescaled next state goes (shared); s0, s1, sr, sp, sv: shared scratch vectors of >= max(E, H) floats.
-// Returns this lane's policy logit (lanes < A), the scalarised value and reward.
+// Returns this lane's fp32 prior (lane k <-> action k, 0 in lanes >= A), the scalarised value and reward.
 template <int G, typename SH>
 MZ_DEVINL void fc_recurrent_fixed(const FcNet& net, const float* blob, const float* h, int action, float* hn,
-                                  float* s0, float* s1, float* sr, float* sp, float* sv, float& logit, float& value, float& reward) {
+                                  float* s0, float* s1, float* sr, float* sp, float* sv, float& prior, float& value, float& reward) {
     constexpr int E = SH::E, H = SH::H, F = SH::F, A = SH::A, S = SH::S;
     static_assert(E <= G && A <= G, "one lane per state element / action");
     const int lane = LaneGroup<G>::lane();
@@ -322,8 +322,38 @@ MZ_DEVINL void fc_recurrent_fixed(const FcNet& net, const float* blob, const flo
             lv[r] = dot_packed<H>(blob + vl.w_off[1], F, o, blob[vl.b_off[1] + o], sv);
         }
     }
-    logit = 0.0f;
-    if (lane < A) logit = dot_packed<H>(blob + pl.w_off[1], A, lane, blob[pl.b_off[1] + lane], sp);
+    // ---- policy: every lane computes all A logits (the weights and sp are broadcast reads) and evaluates the softmax of
+    // tree.cuh::group_softmax_masked over the first W lanes on its own, without shuffles: in each butterfly step entry i
+    // combines with entry i ^ off in the operand order lane i used, so lane k's entry k has the bits lane k computed.
+    constexpr int W = pow2_ceil_c(A);
+    float pe[W], pm[W], ps[W];
+#pragma unroll
+    for (int i = 0; i < W; ++i) {
+        pe[i] = i < A ? dot_packed<H>(blob + pl.w_off[1], A, i, blob[pl.b_off[1] + i], sp) : -INFINITY;
+        pm[i] = pe[i];
+    }
+#pragma unroll
+    for (int off = W >> 1; off > 0; off >>= 1) {
+        float nx[W];
+#pragma unroll
+        for (int i = 0; i < W; ++i) nx[i] = fmaxf(pm[i], pm[i ^ off]);
+#pragma unroll
+        for (int i = 0; i < W; ++i) pm[i] = nx[i];
+    }
+#pragma unroll
+    for (int i = 0; i < W; ++i) { pe[i] = i < A ? expf(pe[i] - pm[i]) : 0.0f; ps[i] = pe[i]; }
+#pragma unroll
+    for (int off = W >> 1; off > 0; off >>= 1) {
+        float nx[W];
+#pragma unroll
+        for (int i = 0; i < W; ++i) nx[i] = ps[i] + ps[i ^ off];
+#pragma unroll
+        for (int i = 0; i < W; ++i) ps[i] = nx[i];
+    }
+    float e_own = 0.0f, s_own = 1.0f;
+#pragma unroll
+    for (int i = 0; i < A; ++i) if (lane == i) { e_own = pe[i]; s_own = ps[i]; }
+    prior = div_pos_or_zero(e_own, s_own);
     // ---- support_to_scalar of value and reward (support_to_scalar_group2 on registers: same maxima, sums and order)
     const unsigned m = kWarp;
     float ma = -INFINITY, mb = -INFINITY;

@@ -96,10 +96,12 @@ constexpr int fixed_actions() {
 
 // SH: FcFixedShape<E, H, S, A> runs the per-simulation network call through the fully unrolled fixed-shape code
 // (fc_net.cuh::fc_recurrent_fixed, bit-identical to the generic descriptors walk), FcGenericShape through the latter.
-template <int G, bool kTeacher, typename SH>
+// The fixed shape also fixes the tree's action count; kP is the number of players when fixed at compile time (0 = a.P).
+template <int G, bool kTeacher, typename SH, int kP>
 __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __grid_constant__ FcSearchArgs a) {
     extern __shared__ __align__(16) unsigned char smem[];
-    const int N = a.N, A = a.A;
+    constexpr int kA = fixed_actions<SH>();
+    const int N = a.N, A = kA ? kA : a.A;
     // ---- CTA-shared: tables + weights
     double* s_pbc = reinterpret_cast<double*>(smem);
     double* s_sqrt = s_pbc + (N + 2);
@@ -141,7 +143,6 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
                              {s_act + 7 * maxw, s_act + 8 * maxw}};
     const bool fused_heads = (a.net.rew.n == a.net.pol.n) && (a.net.pol.n == a.net.val.n);
     // multi-level selection: A fixed at compile time for the fixed network shapes
-    constexpr int kA = fixed_actions<SH>();
     constexpr int kMaxD = select_levels_for(kA ? kA : 2, G);
     const SelectLanes sl = select_lanes<G, kA>(A, min(a.select_levels, kMaxD));
     PhaseClock ph;
@@ -187,9 +188,9 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
         else prior = group_softmax_masked<G>(logit, lane < A && ((legal >> lane) & 1u));
         if (a.trace.root_priors_raw && lane < A && own) a.trace.root_priors_raw[(size_t)g * A + lane] = ((legal >> lane) & 1u) ? prior : 0.0f;
         if (a.trace.root_reward && lane == 0 && own) a.trace.root_reward[g] = root_reward;
-        tree_init_root<G>(c, t, prior, root_reward,
-                          (a.add_noise && a.noise) ? a.noise + (size_t)g * A : nullptr, a.add_noise && !a.noise,
-                          game_id, move, (a.trace.noise && own) ? a.trace.noise + (size_t)g * A : nullptr);
+        tree_init_root<G, kA>(c, t, prior, root_reward,
+                              (a.add_noise && a.noise) ? a.noise + (size_t)g * A : nullptr, a.add_noise && !a.noise,
+                              game_id, move, (a.trace.noise && own) ? a.trace.noise + (size_t)g * A : nullptr);
         ph.mark(kPhRoot);
 
         // ------------------------------------------------------------------ simulations
@@ -210,7 +211,7 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
                 const float* h = s_hidden + (size_t)leaf.parent_exp * Epad;
                 float* hn = s_hidden + (size_t)t.n_expanded * Epad;
                 if constexpr (SH::kEnabled) {
-                    fc_recurrent_fixed<G, SH>(a.net, s_blob, h, leaf.action, hn, s0, s1, hb[0][0], hb[1][0], hb[2][0], logit, value, reward);
+                    fc_recurrent_fixed<G, SH>(a.net, s_blob, h, leaf.action, hn, s0, s1, hb[0][0], hb[1][0], hb[2][0], prior, value, reward);
                 } else {
                 float* raw = mlp_forward<G>(a.net.dyn, s_blob, h, s0, s1, s2, leaf.action);
                 if (fused_heads) {
@@ -237,8 +238,7 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
                     LaneGroup<G>::sync();
                 }
                 }
-                if constexpr (SH::kEnabled) prior = group_softmax_masked_w<G, pow2_ceil_c(SH::A)>(logit, lane < A);
-                else prior = group_softmax_masked<G>(logit, lane < A);
+                if constexpr (!SH::kEnabled) prior = group_softmax_masked<G>(logit, lane < A);
             }
             ph.mark(kPhNet);
             if (a.trace.depth && own) {
@@ -248,9 +248,9 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
                 for (int j = lane; j < leaf.depth && j < a.trace.max_depth; j += G)
                     a.trace.actions[ti * a.trace.max_depth + j] = (uint8_t)(t.path[j + 1] % A);
             }
-            tree_expand<G>(c, t, leaf, reward, prior);
+            tree_expand<G, kA>(c, t, leaf, reward, prior);
             ph.mark(kPhExpand);
-            tree_backup<G>(c, t, leaf, value);
+            tree_backup<G, kP, true>(c, t, leaf, value);
             ph.mark(kPhBackup);
             max_depth = max(max_depth, leaf.depth);
         }
@@ -333,12 +333,12 @@ bool fc_search_plan(int N, int A, int E, int maxw, int blob_floats, int G, bool 
     return found;
 }
 
-template <int G, bool T, typename SH>
+template <int G, bool T, typename SH, int kP = 0>
 static cudaError_t launch_one(const FcSearchArgs& a_in, int sm_count, FcLaunchState* st, cudaStream_t stream) {
     FcSearchArgs a = a_in;
     const char* one_level = getenv("MZ_FC_SELECT_LEVELS");    // A/B switch: "1" = one tree level per selection round
     a.select_levels = (one_level && one_level[0] == '1' && one_level[1] == 0) ? 1 : select_levels_for(a.A, G);
-    auto kern = fc_search_kernel<G, T, SH>;
+    auto kern = fc_search_kernel<G, T, SH, kP>;
     const void* fn = reinterpret_cast<const void*>(kern);
     int regs = 0;
     for (const auto& k : st->kernels) if (k.fn == fn) regs = k.regs;
@@ -383,7 +383,10 @@ cudaError_t launch_fc_search(const FcSearchArgs& a, int group, bool teacher, int
                              cudaStream_t stream) {
     const char* generic = getenv("MZ_FC_GENERIC");             // A/B switch: always walk the layer descriptors
     if (!teacher && !(generic && generic[0] == '1') && fc_matches_fixed<CartPoleShape>(a.net)) {
+        // (a single player: the backup's value recurrence and its signs simplify)
+        if (group == 16 && a.P == 1) return launch_one<16, false, CartPoleShape, 1>(a, sm_count, state, stream);
         if (group == 16) return launch_one<16, false, CartPoleShape>(a, sm_count, state, stream);
+        if (group == 32 && a.P == 1) return launch_one<32, false, CartPoleShape, 1>(a, sm_count, state, stream);
         if (group == 32) return launch_one<32, false, CartPoleShape>(a, sm_count, state, stream);
     }
 #define MZ_CASE(GG)                                                                                     \

@@ -76,6 +76,24 @@ MZ_DEVINL double value_range_normalize(double v, double lo, double hi) {
     return v;
 }
 
+// RN(s / n) for an integer 1 <= n < 2^31 from y = RN(1 / n): q0 = RN(s*y), r = s - q0*n, q = RN(q0 + r*y).
+// Exact - the same bits as __ddiv_rn(s, n) - whenever s / n is a normal number:
+//   * |s*y - s/n| <= 2^-53 |s/n|, so q0 is within 1.5 ulp of s/n.  s and q0*n are multiples of ulp(q0) (s ~ n*q0 has
+//     the larger exponent) and |s - q0*n| <= 1.5 n ulp(q0) < 2^53 ulp(q0): the fma's remainder r is exact.
+//   * then q0 + r*y = s/n + (1 - n*y)(q0 - s/n), and |1 - n*y| <= 2^-53, so the fma rounds s/n + eta with
+//     |eta| <= 3 * 2^-53 ulp(s/n) (a factor 2 covers q0 on the other side of a power of two).
+//   * that rounds like s/n unless s/n lies within |eta| of a midpoint m of two doubles.  s and n*m are multiples of
+//     ulp(s/n)/2, so a non-zero |s/n - m| = |s - n*m| / n is at least ulp(s/n) / (2n), far above |eta|; and s/n = m
+//     would need s = n*m, where m has 54 significant bits and odd n' times it (n = 2^j n') at least as many: no double.
+// In the subnormal range exact midpoints exist (9 * 2^-1074 / 6) and this rounding can miss the even neighbour; there,
+// and for zero (-0 / n must stay -0), infinite or NaN numerators, the IEEE division runs instead.
+MZ_DEVINL double div_by_count(double s, int n, double y) {
+    if (!(fabs(s) >= 0x1p-990 && fabs(s) < INFINITY)) return __ddiv_rn(s, (double)n);     // (s / n > 2^-1021 below)
+    const double q0 = __dmul_rn(s, y);
+    const double r = __fma_rn(-q0, (double)n, s);
+    return __fma_rn(r, y, q0);
+}
+
 // n-th (0-based) set bit of m
 MZ_DEVINL int nth_set_bit(unsigned m, int n) { return (int)__fns(m, 0, n + 1); }
 
@@ -91,21 +109,14 @@ MZ_DEVINL float group_softmax_masked(float logit, bool valid) {
     return div_pos_or_zero(e, s);          // masked lanes (e = 0) must not drag the warp through the division slow path
 }
 
-// the same over the first W lanes only (W = pow2 >= |A|, compile time): valid in lanes < W, same bits
-template <int G, int W>
-MZ_DEVINL float group_softmax_masked_w(float logit, bool valid) {
-    const float m = group_max_f32_w<G, W>(valid ? logit : -INFINITY);
-    const float e = valid ? expf(logit - m) : 0.0f;
-    const float s = group_sum_f32_w<G, W>(e);
-    return div_pos_or_zero(e, s);
-}
-
-template <int G>
+// kA: |A| when fixed at compile time (0 = c.A), as in tree_select_lookahead and tree_expand
+template <int G, int kA = 0>
 MZ_DEVINL void tree_init_root(const TreeConst& c, GameTree& t, float prior_f32, float root_reward,
                               const double* noise /* [A] by action or nullptr */, bool generate_noise = false,
                               int64_t game_id = 0, int move = 0, double* noise_out = nullptr) {
+    const int A = kA ? kA : c.A;
     const int k = LaneGroup<G>::lane();
-    const bool legal = (k < c.A) && ((t.legal >> k) & 1u);
+    const bool legal = (k < A) && ((t.legal >> k) & 1u);
     double nz = 0.0;
     bool have_noise = false;
     if (noise != nullptr) {
@@ -119,8 +130,8 @@ MZ_DEVINL void tree_init_root(const TreeConst& c, GameTree& t, float prior_f32, 
         nz = gm / sum;
         have_noise = true;
     }
-    if (noise_out && k < c.A && t.own) noise_out[k] = nz;
-    if (k < c.A && t.own) {
+    if (noise_out && k < A && t.own) noise_out[k] = nz;
+    if (k < A && t.own) {
         double p = (double)prior_f32;
         if (legal && have_noise) {
             // prior * (1 - frac) + n * frac       (self_play.py:476)
@@ -435,8 +446,9 @@ MZ_DEVINL Leaf tree_select_lookahead(const TreeConst& c, GameTree& t, const Sele
 // Expansion of the selected leaf with the network outputs (self_play.py:345-351, 451-465).
 // prior_f32: this lane's fp32 softmax prior (lane k <-> action k).
 // ------------------------------------------------------------------------------------------
-template <int G>
+template <int G, int kA = 0>
 MZ_DEVINL int tree_expand(const TreeConst& c, GameTree& t, const Leaf& leaf, float reward, float prior_f32) {
+    const int A = kA ? kA : c.A;
     const int k = LaneGroup<G>::lane();
     const int e = t.n_expanded;
     if (k == 0 && t.own) {
@@ -444,8 +456,8 @@ MZ_DEVINL int tree_expand(const TreeConst& c, GameTree& t, const Leaf& leaf, flo
         t.reward[leaf.slot] = reward;
         t.path_reward[leaf.depth] = reward;
     }
-    if (k < c.A && t.own) {
-        const int s = e * c.A + k;
+    if (k < A && t.own) {
+        const int s = e * A + k;
         t.visit[s] = 0;
         t.vsum[s] = 0.0;
         t.reward[s] = 0.0f;
@@ -463,8 +475,21 @@ MZ_DEVINL int tree_expand(const TreeConst& c, GameTree& t, const Leaf& leaf, flo
 // (value_sum, visit, running min/max) are independent: lane j updates node j, all at once, after
 // the recurrence handed every lane the value its node saw.
 // ------------------------------------------------------------------------------------------
-template <int G>
+// RN(s / n), n = a visit count + 1: div_by_count when kRcp, else the IEEE division
+template <bool kRcp>
+MZ_DEVINL double mean_of(double s, int n) {
+    if constexpr (kRcp) return div_by_count(s, n, __drcp_rn((double)n));
+    else return __ddiv_rn(s, (double)n);
+}
+
+// kP: number of players when fixed at compile time (0 = c.P).
+// kRcp: the means divide through div_by_count.  After a shuffled recurrence every lane then reads its node's sum and count
+// and takes RN(1 / count) BEFORE the recurrence (that work overlaps the serial chain instead of following it), evaluates
+// the update (a lane without a node on slot 0, with a numerator of 1) and stores it predicated: three dependent fp64 steps
+// behind the recurrence instead of a division, and no divergent owner block.
+template <int G, int kP = 0, bool kRcp = false>
 MZ_DEVINL void tree_backup(const TreeConst& c, GameTree& t, const Leaf& leaf, float leaf_value) {
+    const int P = kP ? kP : c.P;
     const int k = LaneGroup<G>::lane();
     const int L = leaf.depth;                         // path indices 0..L
     double lo = INFINITY, hi = -INFINITY;
@@ -481,17 +506,36 @@ MZ_DEVINL void tree_backup(const TreeConst& c, GameTree& t, const Leaf& leaf, fl
     if (packed) {
         // The recurrence runs on shuffles and every lane keeps the value its own node saw; the node updates then happen
         // ONCE, all lanes in parallel (a divergent owner block inside the loop would be issued L + 1 times, one lane each).
+        const bool mine = kRcp && k <= L && t.own;  // (kRcp) this lane updates a node
+        const int sl = (mine && k > 0) ? my_slot : 0;
+        double old_sum = 0.0, y = 1.0;
+        int n = 1;
+        if constexpr (kRcp) {
+            old_sum = k == 0 ? t.root_vsum : t.vsum[sl];
+            n = mine ? (k == 0 ? t.root_visit : t.visit[sl]) + 1 : 1;
+            y = __drcp_rn((double)n);
+        }
         double myv = 0.0;
         for (int j = Lw; j >= 0; --j) {
             const double r = (double)LaneGroup<G>::bcast(my_reward, j);
-            const bool same = (c.P == 1) || (((L - j) & 1) == 0);
+            const bool same = (P == 1) || (((L - j) & 1) == 0);
             if (j == k) myv = v;
-            const double rr = (c.P == 1) ? r : (same ? -r : r);
+            const double rr = (P == 1) ? r : (same ? -r : r);
             const double vn = __dadd_rn(rr, __dmul_rn(c.discount, v));
             v = j <= L ? vn : v;
         }
-        if (k <= L && t.own) {
-            const bool same = (c.P == 1) || (((L - k) & 1) == 0);
+        if constexpr (kRcp) {
+            const bool same = (P == 1) || (((L - k) & 1) == 0);
+            const double add = same ? myv : -myv;
+            const double s = __dadd_rn(old_sum, add);
+            const double q = div_by_count(mine ? s : 1.0, n, y);
+            const double m = __dadd_rn((double)my_reward, __dmul_rn(c.discount, (P == 1) ? q : -q));
+            if (mine && k > 0) { t.vsum[sl] = s; t.visit[sl] = n; t.mval[sl] = m; }   // mval: what the next selection normalises
+            if (mine && k == 0) root_vsum = s;
+            lo = mine ? m : lo;
+            hi = mine ? m : hi;
+        } else if (k <= L && t.own) {
+            const bool same = (P == 1) || (((L - k) & 1) == 0);
             const double add = same ? myv : -myv;
             double q;
             if (k == 0) {
@@ -504,7 +548,7 @@ MZ_DEVINL void tree_backup(const TreeConst& c, GameTree& t, const Leaf& leaf, fl
                 t.visit[my_slot] = n;
                 q = __ddiv_rn(s, (double)n);
             }
-            const double m = __dadd_rn((double)my_reward, __dmul_rn(c.discount, (c.P == 1) ? q : -q));
+            const double m = __dadd_rn((double)my_reward, __dmul_rn(c.discount, (P == 1) ? q : -q));
             if (k > 0) t.mval[my_slot] = m;           // what the next selection will normalise for this child
             lo = m;
             hi = m;
@@ -515,28 +559,28 @@ MZ_DEVINL void tree_backup(const TreeConst& c, GameTree& t, const Leaf& leaf, fl
         const float rf = t.path_reward[j];
         const double r = (double)rf;
         // node.to_play == to_play  <=>  (L - j) even (players alternate every level)
-        const bool same = (c.P == 1) || (((L - j) & 1) == 0);
+        const bool same = (P == 1) || (((L - j) & 1) == 0);
         if ((j % G) == k && t.own) {
             const double add = same ? v : -v;
             double q;
             if (j == 0) {
                 root_vsum = __dadd_rn(t.root_vsum, add);
-                q = __ddiv_rn(root_vsum, (double)(t.root_visit + 1));
+                q = mean_of<kRcp>(root_vsum, t.root_visit + 1);
             } else {
                 const double s = __dadd_rn(t.vsum[slot], add);
                 const int n = t.visit[slot] + 1;
                 t.vsum[slot] = s;
                 t.visit[slot] = n;
-                q = __ddiv_rn(s, (double)n);
+                q = mean_of<kRcp>(s, n);
             }
-            const double m = __dadd_rn(r, __dmul_rn(c.discount, (c.P == 1) ? q : -q));
+            const double m = __dadd_rn(r, __dmul_rn(c.discount, (P == 1) ? q : -q));
             if (j > 0) t.mval[slot] = m;           // what the next selection will normalise for this child
             lo = fmin(lo, m);
             hi = fmax(hi, m);
         }
         // value = (same ? -reward : reward) + discount * value     (P == 2)
         // value = reward + discount * value                        (P == 1)
-        const double rr = (c.P == 1) ? r : (same ? -r : r);
+        const double rr = (P == 1) ? r : (same ? -r : r);
         v = __dadd_rn(rr, __dmul_rn(c.discount, v));
     }
     }
