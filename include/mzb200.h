@@ -260,6 +260,24 @@ int mz_debug_conv3x3_plan(int32_t n, int32_t cin, int32_t cout, int32_t H, int32
 int mz_debug_conv3x3(int device, int32_t n, int32_t cin, int32_t cout, int32_t H, int32_t W, int32_t stride, const float* x,
                      const float* w, const float* bias, const float* residual, int32_t relu, int32_t use_tensor_cores, float* out);
 
+/* Call sites of the 64-channel tensor-core towers (site argument of mz_debug_conv_tower) */
+#define MZ_TOWER_REPRESENTATION 0   /* input in a workspace, reusable once read; no stem */
+#define MZ_TOWER_DYNAMICS 1         /* plain recurrent call: input converted into a workspace; stem with the action plane */
+#define MZ_TOWER_DYNAMICS_POOL 2    /* in search: input gathered from the hidden-state pool (read only); stem with the action plane */
+#define MZ_TOWER_PREDICTION 3       /* input in the rescaled-state scratch buffer, reusable; no stem */
+
+/* Debug / parity: one whole tensor-core tower (models.py:213-229 without BN: [stem conv +] `blocks` residual blocks, every
+ * conv with bias and ReLU) of one call site of the network on host NCHW fp32 data, through the launch packing and the
+ * kernels the network runs (mode 1 = fp16 operands, 2 = x3).  H <= 6, W <= 7.  x is [n][64][H][W]; w holds every conv's
+ * [cout 64][cin][3][3] back to back (the dynamics stem first, cin = 65: channel 64 is the action plane action[g] / A), bias
+ * [convs][64] (or NULL); action [n] in [0, A) for the dynamics sites; at MZ_TOWER_DYNAMICS_POOL game g's input sits in slot
+ * parent[g] of its pool_stride slots, the other slots hold NaN, and `parts` (x3 only, 1..4) runs the games in the ranges of
+ * the partitioned replay.  Workspaces and output start as NaN.  out is [n][64][H][W]; *launches gets the number of kernel
+ * launches of the tower and *saturated the x3 range-guard count (stored activations beyond the fp16 range). */
+int mz_debug_conv_tower(int device, int32_t n, int32_t H, int32_t W, int32_t mode, int32_t blocks, int32_t site, int32_t parts,
+                        int32_t A, const float* x, const float* w, const float* bias, const int32_t* action, const int32_t* parent,
+                        int32_t pool_stride, float* out, int64_t* launches, int32_t* saturated);
+
 /* Arithmetic the handle's search path computes in, e.g. "f32 nets + f64 tree statistics" (bench.py's dtype). */
 const char* mz_numerics(const MzHandle* h);
 

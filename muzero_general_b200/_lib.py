@@ -148,6 +148,8 @@ SYMBOLS = [
     ("mz_debug_conv3x3_plan", C.c_int, [C.c_int32] * 6 + [C.POINTER(C.c_int64)]),
     ("mz_debug_conv3x3", C.c_int, [C.c_int] + [C.c_int32] * 6 + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                                   C.c_int32, C.c_int32, C.c_void_p]),
+    ("mz_debug_conv_tower", C.c_int, [C.c_int] + [C.c_int32] * 8 + [C.c_void_p] * 5 + [C.c_int32, C.c_void_p,
+                                                                                      C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
 ]
 
 _lib = None

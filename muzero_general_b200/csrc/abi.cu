@@ -511,7 +511,7 @@ int mz_dispatch_search(MzHandle* h, const SearchCall& call, bool teacher, bool t
             int rc2 = run(root, h->stream);
             if (rc2) return rc2;
             if (cudaEventRecord(h->part_fork, h->stream) != cudaSuccess) return fail(h, MZ_ECUDA, "partitioned replay: fork");
-            const int per = ((n + parts - 1) / parts + 7) & ~7;
+            const int per = partition_games(n, parts);
             for (int p = 0; p < parts; ++p) {
                 SearchCall sc = call_;
                 sc.phases = kPhaseSims;
@@ -919,5 +919,21 @@ extern "C" int mz_debug_conv3x3(int device, int32_t n, int32_t cin, int32_t cout
     std::string e;
     int rc = resnet_debug_conv(n, cin, cout, H, W, stride, x, w, bias, residual, relu, use_tensor_cores, out, prop.multiProcessorCount, &e);
     if (rc) return fail(nullptr, rc, "mz_debug_conv3x3: " + e);
+    return MZ_OK;
+}
+
+// debug: one tensor-core tower of one call site of the network (host NCHW in / out)
+extern "C" int mz_debug_conv_tower(int device, int32_t n, int32_t H, int32_t W, int32_t mode, int32_t blocks, int32_t site,
+                                   int32_t parts, int32_t A, const float* x, const float* w, const float* bias,
+                                   const int32_t* action, const int32_t* parent, int32_t pool_stride, float* out,
+                                   int64_t* launches, int32_t* saturated) {
+    if (!x || !w || !out || !launches) return fail(nullptr, MZ_EINVAL, "mz_debug_conv_tower: bad argument");
+    if (cudaSetDevice(device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_conv_tower: no such device");
+    cudaDeviceProp prop;
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_conv_tower: device query failed");
+    std::string e;
+    int rc = resnet_debug_tower(n, H, W, mode, blocks, site, parts, A, x, w, bias, action, parent, pool_stride, out, launches,
+                                saturated, prop.multiProcessorCount, &e);
+    if (rc) return fail(nullptr, rc, "mz_debug_conv_tower: " + e);
     return MZ_OK;
 }

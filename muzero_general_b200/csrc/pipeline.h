@@ -93,6 +93,13 @@ bool resnet_conv_plan(int n, int cin, int cout, int H, int W, int stride, int64_
 const char* resnet_numerics(const ResNetDevice* r);
 int resnet_take_saturations(ResNetDevice* r, cudaStream_t stream);   // x3 range guard (synchronises)
 bool resnet_can_partition(const ResNetDevice* r);
+// games per range of the partitioned replay (the last range may hold fewer): a multiple of 8
+inline int partition_games(int n, int parts) { return ((n + parts - 1) / parts + 7) & ~7; }
+// Debug / parity entry behind mz_debug_conv_tower: one tensor-core tower of one call site of resnet_inference_tc on host NCHW
+// data (see include/mzb200.h)
+int resnet_debug_tower(int n, int H, int W, int mode, int blocks, int site, int parts, int A, const float* x, const float* w,
+                       const float* bias, const int32_t* action, const int32_t* parent, int pool_stride, float* out,
+                       int64_t* launches, int32_t* saturated, int sm_count, std::string* err);
 // fused search of small residual networks: all simulations in one launch (small_search.cu); MZ_SMALL_SEARCH=0 / 1 switches it off / on
 bool resnet_small_search_supported(ResNetDevice* r, const InferCall& first_recurrent, const TreeStepArgs& tree, int n_sims);
 int resnet_small_search(ResNetDevice* r, const InferCall& first_recurrent, const TreeStepArgs& tree, int n_sims, cudaStream_t stream,

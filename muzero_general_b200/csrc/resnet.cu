@@ -901,7 +901,9 @@ struct Runner {
             if (nb < 4) a.buf[nb++] = nullptr;      // (only two spare workspaces when the input is one of ws)
             a.gather_parent = gather_now; a.pool_stride = pool_stride; a.action = action;
             int cur = 0, nl = 0;
-            const bool reuse0 = ext_reusable && !gather_now;       // the input buffer is dead after its last reader
+            // the input buffer is dead after its last reader: always so for a workspace written by the previous launch,
+            // for the tower's own input only when it is scratch (a gathered pool never is)
+            const bool reuse0 = (ext_reusable || ext_now != ext) && !gather_now;
             auto pick = [&](int avoid1, int avoid2) {
                 for (int i = 1; i < 4; ++i) if (i != avoid1 && i != avoid2 && a.buf[i]) return i;
                 if (reuse0 && avoid1 != 0 && avoid2 != 0) return 0;
@@ -928,6 +930,25 @@ struct Runner {
             ext_now = result; gather_now = nullptr;
         }
         return result;
+    }
+
+    // The four tower call sites of resnet_inference_tc, each with where its input lives (mz_debug_conv_tower runs the same
+    // helpers).  Representation: the CUDA-core stem (rep_trunk[0]) wrote ws[0].
+    const float* representation_tower() {
+        return tower_tc(r->rep_trunk, 1, false, r->net.blocks, r->ws[0], true, r->ws, nullptr, 0, nullptr);
+    }
+    // Dynamics, plain API call: the dense states were converted into dynamics_staging().
+    float* dynamics_staging() const { return r->ws[2]; }
+    const float* dynamics_tower(const int32_t* action) {
+        return tower_tc(r->dyn, 0, true, r->net.blocks, dynamics_staging(), true, r->ws, nullptr, 0, action);
+    }
+    // Dynamics in search: the parents' states are gathered from the pool, which stays read only.
+    const float* dynamics_tower_pool(const float* pool, const int32_t* gather_parent, int pool_stride, const int32_t* action) {
+        return tower_tc(r->dyn, 0, true, r->net.blocks, pool, false, r->ws, gather_parent, pool_stride, action);
+    }
+    // Prediction: the heads wrote the rescaled state into scratch_state.
+    const float* prediction_tower() {
+        return tower_tc(r->pred, 0, false, r->net.blocks, r->scratch_state, true, r->ws, nullptr, 0, nullptr);
     }
 
     bool conv(const ConvLayer& l, const float* in, float* out, const float* residual, bool relu, int Hin, int Win,
@@ -1154,13 +1175,11 @@ static int resnet_inference_tc(ResNetDevice* r, const InferCall& c, cudaStream_t
     const int n = c.n, C = r->C, hh = r->hh, hw = r->hw, F = 2 * nd.support_size + 1;
     Runner R{r, stream, launches, err, n, c.g0};
     if (c.g0 != 0 && (!r->split || !c.recurrent || !c.gather_parent)) { *err = "resnet: partitioned calls need the x3 towers in pool mode"; return MZ_EINVAL; }
-    float *cur = r->ws[0], *tmp = r->ws[1], *spare = r->ws[2];
     float* state = r->scratch_state;                   // rescaled state, P64C4, input of the prediction tower
     if (!c.recurrent) {
-        if (!R.conv(r->rep_trunk[0], c.in, cur, nullptr, true, nd.obs_h, nd.obs_w, nullptr, 0, nullptr, true)) return MZ_ECUDA;
-        const float* x = R.tower_tc(r->rep_trunk, 1, false, nd.blocks, cur, true, r->ws, nullptr, 0, nullptr);
+        if (!R.conv(r->rep_trunk[0], c.in, r->ws[0], nullptr, true, nd.obs_h, nd.obs_w, nullptr, 0, nullptr, true)) return MZ_ECUDA;
+        const float* x = R.representation_tower();
         if (!x) return MZ_ECUDA;
-        // note: layers index from 1 in rep_trunk (0 is the stem, run above on the CUDA cores)
         if (!R.heads(x, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, c.hidden, c.pool_hidden, c.pool_stride, c.out_slot,
                      true, state))
             return MZ_ECUDA;
@@ -1173,25 +1192,26 @@ static int resnet_inference_tc(ResNetDevice* r, const InferCall& c, cudaStream_t
             *launches += 1;
         }
     } else {
-        const float* in = c.pool_hidden;
-        if (!c.gather_parent) {
+        const float* x;
+        if (c.gather_parent) {
+            x = R.dynamics_tower_pool(c.pool_hidden, c.gather_parent, c.pool_stride, c.action);
+        } else {
             // plain API call: dense NCHW hidden states -> P64C4
             const size_t total = (size_t)n * C * hh * hw;
-            nchw_to_p64c4_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(c.in, spare, n, C, hh, hw, r->split ? 1 : 0);
+            nchw_to_p64c4_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(c.in, R.dynamics_staging(), n, C, hh, hw,
+                                                                                       r->split ? 1 : 0);
             *launches += 1;
-            in = spare;
+            x = R.dynamics_tower(c.action);
         }
-        const float* x = R.tower_tc(r->dyn, 0, true, nd.blocks, in, in == spare, r->ws, c.gather_parent, c.pool_stride, c.action);
         if (!x) return MZ_ECUDA;
         if (!R.heads(x, 1, &r->reward_head, nullptr, c.reward_logits, nullptr, c.reward, nullptr, c.hidden, c.pool_hidden,
                      c.pool_stride, c.out_slot, true, state))
             return MZ_ECUDA;
     }
-    const float* x = R.tower_tc(r->pred, 0, false, nd.blocks, state, true, r->ws, nullptr, 0, nullptr);
+    const float* x = R.prediction_tower();
     if (!x) return MZ_ECUDA;
     if (!R.heads(x, 2, &r->value_head, &r->policy_head, c.value_logits, c.policy_logits, c.value, nullptr, nullptr, nullptr, 0, 0, true))
         return MZ_ECUDA;
-    (void)tmp;
     return MZ_OK;
 }
 
@@ -1336,6 +1356,135 @@ int resnet_debug_conv(int n, int cin, int cout, int H, int W, int stride, const 
     }
     if (good) cudaMemcpy(out, d_out, dense * 4, cudaMemcpyDeviceToHost);
     r.d_conv = nullptr;
+    cleanup();
+    return good ? MZ_OK : MZ_ECUDA;
+}
+
+// Stand-alone tensor-core tower of one call site of resnet_inference_tc, through the same Runner helpers, on host NCHW
+// data.  The three workspaces, the prediction site's scratch state, the pool and the output start as NaN bytes (0xFF);
+// only the input boards are written, with the zero padding the board layout promises.  So a layer that reads a board or a
+// padding row nobody wrote produces NaN.
+int resnet_debug_tower(int n, int H, int W, int mode, int blocks, int site, int parts, int A, const float* x, const float* w,
+                       const float* bias, const int32_t* action, const int32_t* parent, int pool_stride, float* out,
+                       int64_t* launches, int32_t* saturated, int sm_count, std::string* err) {
+    constexpr int C = 64;
+    const bool stem = site == MZ_TOWER_DYNAMICS || site == MZ_TOWER_DYNAMICS_POOL;
+    const bool in_pool = site == MZ_TOWER_DYNAMICS_POOL;
+    if (n < 1 || blocks < 0 || (!stem && blocks < 1) || site < MZ_TOWER_REPRESENTATION || site > MZ_TOWER_PREDICTION ||
+        (mode != 1 && mode != 2) || !conv_tc_supported(C, H, W)) {
+        *err = "bad shape, site or mode"; return MZ_EINVAL;
+    }
+    if (parts < 1 || parts > 4 || (parts > 1 && (!in_pool || mode != 2))) {
+        *err = "partitions need the x3 towers at the in-search dynamics site, 1 to 4 of them"; return MZ_EINVAL;
+    }
+    if (stem) {
+        if (A < 1 || !action) { *err = "the dynamics sites need actions and A >= 1"; return MZ_EINVAL; }
+        for (int g = 0; g < n; ++g) if (action[g] < 0 || action[g] >= A) { *err = "action out of range"; return MZ_EINVAL; }
+    }
+    if (in_pool) {
+        if (!parent || pool_stride < 1) { *err = "the in-search site needs parents and pool_stride >= 1"; return MZ_EINVAL; }
+        for (int g = 0; g < n; ++g) if (parent[g] < 0 || parent[g] >= pool_stride) { *err = "parent out of range"; return MZ_EINVAL; }
+    }
+    // a state_dict of plain convolutions for pack_conv: "c<i>.weight", the stem [C][C + 1][3][3] first
+    const int n_convs = (stem ? 1 : 0) + 2 * blocks;
+    std::vector<std::string> names(n_convs);
+    std::vector<MzTensor> tensors(n_convs);
+    size_t w_off = 0;
+    for (int i = 0; i < n_convs; ++i) {
+        const int cin = stem && i == 0 ? C + 1 : C;
+        names[i] = "c" + std::to_string(i) + ".weight";
+        tensors[i] = MzTensor{names[i].c_str(), w + w_off, (int64_t)C * cin * 9};
+        w_off += (size_t)C * cin * 9;
+    }
+    MzNetDesc nd{};
+    nd.kind = MZ_NET_RESNET; nd.channels = C; nd.obs_c = C; nd.obs_h = H; nd.obs_w = W; nd.action_space = stem ? A : 1;
+    nd.blocks = blocks;
+    ResNetDevice r{};
+    r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = H; r.hw = W;
+    r.use_tc = r.tc_capable = true; r.split = mode == 2;
+    Loader L{tensors.data(), n_convs, err};
+    std::vector<float> blob;
+    std::vector<ConvLayer> layers;
+    for (int i = 0; i < n_convs; ++i) {
+        const int cin = stem && i == 0 ? C + 1 : C;
+        if (!pack_conv(L, "c" + std::to_string(i), "", cin, C, 1, blob, layers, r.split ? kLayoutSplit : kLayoutF16, H, W))
+            return MZ_EINVAL;
+        if (bias) {
+            layers[i].b_off = (long)blob.size();
+            blob.insert(blob.end(), bias + (size_t)i * C, bias + (size_t)(i + 1) * C);
+        }
+    }
+    if (site == MZ_TOWER_REPRESENTATION) { r.rep_trunk = layers; r.rep_trunk.insert(r.rep_trunk.begin(), ConvLayer{}); }  // [0]: the CUDA-core stem, not run here
+    else if (stem) r.dyn = layers;
+    else r.pred = layers;
+
+    const size_t board = (size_t)conv_tc_board_elems(r.split), packed = (size_t)n * board, dense = (size_t)n * C * H * W;
+    const size_t pool_boards = in_pool ? (size_t)n * pool_stride : 0;
+    float *d_blob = nullptr, *d_x = nullptr, *d_out = nullptr, *d_stage = nullptr, *d_pool = nullptr;
+    int32_t *d_action = nullptr, *d_parent = nullptr;
+    auto cleanup = [&]() {
+        for (void* p : {(void*)d_blob, (void*)d_x, (void*)d_out, (void*)d_stage, (void*)d_pool, (void*)d_action, (void*)d_parent,
+                        (void*)r.ws[0], (void*)r.ws[1], (void*)r.ws[2], (void*)r.scratch_state, (void*)r.d_sat})
+            if (p) cudaFree(p);
+        r.ws[0] = r.ws[1] = r.ws[2] = r.scratch_state = nullptr; r.d_sat = nullptr; r.d_conv = nullptr;
+    };
+    bool ok = cudaMalloc(&d_blob, blob.size() * 4) == cudaSuccess && cudaMalloc(&d_x, dense * 4) == cudaSuccess &&
+              cudaMalloc(&d_out, dense * 4) == cudaSuccess && cudaMalloc(&d_stage, packed * 4) == cudaSuccess &&
+              cudaMalloc(&r.scratch_state, packed * 4) == cudaSuccess && cudaMalloc(&r.d_sat, 64) == cudaSuccess &&
+              cudaMalloc(&d_action, (size_t)n * 4) == cudaSuccess && cudaMalloc(&d_parent, (size_t)n * 4) == cudaSuccess &&
+              (!in_pool || cudaMalloc(&d_pool, pool_boards * board * 4) == cudaSuccess);
+    for (int i = 0; ok && i < 3; ++i) ok = cudaMalloc(&r.ws[i], packed * 4) == cudaSuccess;
+    if (!ok) { cleanup(); *err = "allocation failed"; return MZ_ENOMEM; }
+    r.d_conv = d_blob;
+    cudaMemcpy(d_blob, blob.data(), blob.size() * 4, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_x, x, dense * 4, cudaMemcpyHostToDevice);
+    if (stem) cudaMemcpy(d_action, action, (size_t)n * 4, cudaMemcpyHostToDevice);
+    if (in_pool) cudaMemcpy(d_parent, parent, (size_t)n * 4, cudaMemcpyHostToDevice);
+    for (int i = 0; i < 3; ++i) cudaMemset(r.ws[i], 0xFF, packed * 4);
+    cudaMemset(r.scratch_state, 0xFF, packed * 4);
+    cudaMemset(d_out, 0xFF, dense * 4);
+    cudaMemset(r.d_sat, 0, 64);
+    // the input boards, zero padded, where the stage before the tower leaves them
+    Runner R0{&r, nullptr, launches, err, n};
+    float* input = site == MZ_TOWER_REPRESENTATION ? r.ws[0] : site == MZ_TOWER_DYNAMICS ? R0.dynamics_staging()
+                 : site == MZ_TOWER_PREDICTION ? r.scratch_state : d_stage;
+    const unsigned cblocks = (unsigned)((dense + 255) / 256);
+    cudaMemset(input, 0, packed * 4);
+    nchw_to_p64c4_kernel<<<cblocks, 256>>>(d_x, input, n, C, H, W, r.split ? 1 : 0);
+    if (in_pool) {
+        cudaMemset(d_pool, 0xFF, pool_boards * board * 4);
+        for (int g = 0; g < n; ++g)
+            cudaMemcpy(d_pool + ((size_t)g * pool_stride + parent[g]) * board, d_stage + (size_t)g * board, board * 4,
+                       cudaMemcpyDeviceToDevice);
+    }
+    *launches = 0;
+    const float* result = nullptr;
+    bool good = true;
+    if (site == MZ_TOWER_REPRESENTATION) result = R0.representation_tower();
+    else if (site == MZ_TOWER_DYNAMICS) result = R0.dynamics_tower(d_action);
+    else if (site == MZ_TOWER_PREDICTION) result = R0.prediction_tower();
+    else {
+        // the ranges of the partitioned replay, each through its own Runner; every array stays addressed by the global game
+        const int per = partition_games(n, parts);
+        for (int p = 0; p < parts && good; ++p) {
+            Runner R{&r, nullptr, launches, err, std::min(per, n - p * per), p * per};
+            if (R.n <= 0) continue;
+            const float* res = R.dynamics_tower_pool(d_pool, d_parent, pool_stride, d_action);
+            if (!res || (result && res != result)) { good = false; if (res) *err = "partitions ended in different buffers"; }
+            result = res;
+        }
+    }
+    good = good && result;
+    cudaError_t e = cudaDeviceSynchronize();
+    if (good && e != cudaSuccess) { good = false; *err = std::string("debug tower: ") + cudaGetErrorString(e); }
+    if (good) {
+        p64c4_to_nchw_kernel<<<cblocks, 256>>>(result, d_out, n, C, H, W, r.split ? 1 : 0);
+        e = cudaMemcpy(out, d_out, dense * 4, cudaMemcpyDeviceToHost);
+        int sat = 0;
+        if (e == cudaSuccess) e = cudaMemcpy(&sat, r.d_sat, 4, cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) { good = false; *err = std::string("debug tower: ") + cudaGetErrorString(e); }
+        if (saturated) *saturated = sat;
+    }
     cleanup();
     return good ? MZ_OK : MZ_ECUDA;
 }

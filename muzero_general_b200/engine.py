@@ -546,3 +546,39 @@ def debug_conv3x3(x, w, bias=None, residual=None, relu=False, tensor_cores=False
     if rc != 0:
         raise _lib.MzError(rc, lib.mz_last_error(None).decode())
     return out
+
+
+TOWER_SITES = {"representation": 0, "dynamics": 1, "dynamics_pool": 2, "prediction": 3}
+
+
+def debug_conv_tower(x, weights, biases=None, mode="x3", site="prediction", actions=None, A=1, parents=None,
+                     pool_stride=1, parts=1, device=0):
+    """One 64-channel tensor-core tower of a network call site through mz_debug_conv_tower; numpy NCHW in and out.
+    x is [n, 64, H, W]; ``weights`` the convs in order ([64, 65, 3, 3] dynamics stem first, then two [64, 64, 3, 3] per
+    block), ``biases`` one [64] per conv.  ``site``: "representation", "dynamics" (plain recurrent call), "dynamics_pool"
+    (in search: game g's input in pool slot ``parents[g]`` of ``pool_stride``; ``parts`` ranges of the partitioned
+    replay) or "prediction".  Returns (out [n, 64, H, W], kernel launches, x3 range-guard count)."""
+    lib = _lib.load_library()
+    x = numpy.ascontiguousarray(x, numpy.float32)
+    n, ch, H, W = x.shape
+    stem = site in ("dynamics", "dynamics_pool")
+    if ch != 64 or (len(weights) - stem) % 2 != 0:
+        raise ValueError(f"{ch} channels / {len(weights)} convs do not make a 64-channel tower at site {site}")
+    for i, w in enumerate(weights):
+        if numpy.shape(w) != (64, 65 if stem and i == 0 else 64, 3, 3):
+            raise ValueError(f"conv {i}: weights {numpy.shape(w)}")
+    wcat = numpy.ascontiguousarray(numpy.concatenate([numpy.asarray(w, numpy.float32).reshape(-1) for w in weights]))
+    b = None if biases is None else numpy.ascontiguousarray(numpy.stack(biases), numpy.float32)
+    if b is not None and b.shape != (len(weights), 64):
+        raise ValueError(f"biases {b.shape} do not fit {len(weights)} convs")
+    act = None if actions is None else numpy.ascontiguousarray(actions, numpy.int32)
+    par = None if parents is None else numpy.ascontiguousarray(parents, numpy.int32)
+    out = numpy.empty_like(x)
+    launches, sat = C.c_int64(0), C.c_int32(0)
+    rc = lib.mz_debug_conv_tower(device, n, H, W, {"fp16": 1, "x3": 2}[mode], (len(weights) - stem) // 2, TOWER_SITES[site],
+                                 parts, A, x.ctypes.data, wcat.ctypes.data, None if b is None else b.ctypes.data,
+                                 None if act is None else act.ctypes.data, None if par is None else par.ctypes.data,
+                                 pool_stride, out.ctypes.data, C.byref(launches), C.byref(sat))
+    if rc != 0:
+        raise _lib.MzError(rc, lib.mz_last_error(None).decode())
+    return out, launches.value, sat.value

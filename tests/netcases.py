@@ -12,7 +12,9 @@ Routes (``ROUTES``) and the cases that take them:
   (fixed versus generic is decided by fc_net.cuh::fc_matches_fixed from the shape alone: tests/test_netcases_cpu.py
   checks the shapes; no kernel counter separates the two)
   tc              64-channel tensor-core towers (x3 and fp16): tc_1x1, tc_1x7, tc_6x1, tc_3x3 (narrow P64C4 heads),
-                  tc_5x4, tc_6x6, tc_6x7, tc_6x7_a1, tc_6x7_a128, tc_6x7_stack2 (11 input planes), tc_6x7_b0 (no blocks)
+                  tc_5x4, tc_6x6, tc_6x7, tc_6x7_a1, tc_6x7_a128, tc_6x7_stack2 (11 input planes), tc_6x7_b0 (no blocks),
+                  tc_6x7_b4 (4 blocks: the representation and prediction towers fill one 8-layer launch), tc_6x7_b6 (6
+                  blocks: every tower is split across launches)
                   and the edge-weight cases tc_6x7_const, tc_6x7_tiny, tc_5x4_tiny, tc_6x7_wide, tc_6x7_sat,
                   tc_3x3_large / tiny_bn / overflow, tc_5x4_large / tiny_bn / overflow
   tc_heads_left   64 channels whose head weights exceed shared memory: kept off the tensor cores from mz_create on
@@ -94,6 +96,8 @@ CASES = [
     NetCase("tc_6x7_a128", "connect4", "tc", dict(action_space=list(range(128)))),
     NetCase("tc_6x7_stack2", "connect4", "tc", dict(stacked_observations=2)),
     NetCase("tc_6x7_b0", "connect4", "tc", dict(blocks=0)),
+    NetCase("tc_6x7_b4", "connect4", "tc", dict(blocks=4)),
+    NetCase("tc_6x7_b6", "connect4", "tc", dict(blocks=6)),
     NetCase("tc_6x7_const", "connect4", "tc", weights="const"),
     NetCase("tc_6x7_tiny", "connect4", "tc", weights="tiny"),
     NetCase("tc_5x4_tiny", "connect4", "tc", _board(5, 4, 6), weights="tiny"),
@@ -140,9 +144,10 @@ CASES = [
 BY_NAME = {c.name: c for c in CASES}
 
 # in-search parity: one case per residual route (the tensor-core case in x3 with one and two graph partitions and in
-# fp16; the nets kept off the tensor cores by their heads, in fp16 and x3) and every FC route
-SEARCH_CASES = ["pl_9x9_c32", "pl_c96_6x7", "st_c32_6x7", "ss_5x6_a4", "ss_7x3_a12", "tc_6x7", "tc_6x7_s300", "tc_6x7_bigheads",
-                "fc_cartpole", "fc_cartpole_s20", "fc_e5_a3", "fc_a40"]
+# fp16; the 6-block tensor-core case, whose gathered dynamics tower is split across launches, with two partitions; the
+# nets kept off the tensor cores by their heads, in fp16 and x3) and every FC route
+SEARCH_CASES = ["pl_9x9_c32", "pl_c96_6x7", "st_c32_6x7", "ss_5x6_a4", "ss_7x3_a12", "tc_6x7", "tc_6x7_b6", "tc_6x7_s300",
+                "tc_6x7_bigheads", "fc_cartpole", "fc_cartpole_s20", "fc_e5_a3", "fc_a40"]
 
 
 def make_config(case: NetCase):

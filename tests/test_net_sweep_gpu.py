@@ -295,7 +295,7 @@ def test_inference_matches_fp64_oracle(name, mode, monkeypatch):
 # (case, tower mode, graph partitions); the small search runs without a trace (a traced search takes the step-wise
 # pipeline), as does the partitioned replay (a traced search is never replayed)
 SEARCH_RUNS = [("pl_9x9_c32", None, None), ("pl_c96_6x7", None, None), ("st_c32_6x7", None, None), ("ss_5x6_a4", None, None),
-               ("ss_7x3_a12", None, None), ("tc_6x7", "x3", 1), ("tc_6x7", "x3", 2), ("tc_6x7", "fp16", 1),
+               ("ss_7x3_a12", None, None), ("tc_6x7", "x3", 1), ("tc_6x7", "x3", 2), ("tc_6x7", "fp16", 1), ("tc_6x7_b6", "x3", 2),
                ("tc_6x7_s300", "fp16", 1), ("tc_6x7_bigheads", "x3", 1), ("fc_cartpole", None, None),
                ("fc_cartpole_s20", None, None), ("fc_e5_a3", None, None), ("fc_a40", None, None)]
 assert {r[0] for r in SEARCH_RUNS} == set(SEARCH_CASES)

@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from muzero_general_b200.netspec import FC
-from netcases import BY_NAME, CASES, ROUTES, case_spec, edge_weights, make_config, small_search_inputs
+from netcases import BY_NAME, CASES, ROUTES, SEARCH_CASES, case_spec, edge_weights, make_config, small_search_inputs
 from oracle.net import OracleNet, support_to_scalar
 
 
@@ -78,6 +78,11 @@ def test_case_table_covers_every_route_with_shapes_that_select_it():
         if c.route == "downsample":
             assert spec.downsample and (H, W) == (2, 2)
     assert any(case_spec(c).blocks == 0 and c.route == "tc" for c in CASES)
+    # tensor-core towers: one 8-layer launch (4 blocks) and towers split across launches (the dynamics tower from 4
+    # blocks on, every tower from 5), the split in-search dynamics tower inside a partitioned search too
+    tc_blocks = {case_spec(c).blocks for c in CASES if c.route == "tc"}
+    assert 4 in tc_blocks and max(tc_blocks) >= 5, tc_blocks
+    assert any(BY_NAME[name].route == "tc" and case_spec(BY_NAME[name]).blocks >= 5 for name in SEARCH_CASES)
     assert any(case_spec(c).blocks == 0 and c.route != "tc" and case_spec(c).kind != FC for c in CASES)
     narrow_tc = [c for c in CASES if c.route == "tc" and case_spec(c).channels * numpy.prod(case_spec(c).hidden_hw) <= 1024]
     assert narrow_tc, "no tensor-core case takes the narrow heads"
