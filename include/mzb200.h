@@ -30,8 +30,10 @@ extern "C" {
 
 #define MZ_ABI_VERSION 2
 #define MZ_MAX_LAYERS 8          /* hidden layers per MLP head */
-#define MZ_MAX_ACTIONS 128       /* |action_space| supported by the tree kernels (one lane per action up to 32,
-                                    four actions per lane above: csrc/tree_wide.cu) */
+#define MZ_MAX_ACTIONS 256       /* |action_space| supported by the tree kernels (one lane per action up to 32; above,
+                                    one warp per game with four actions per lane up to 128 and eight up to 256:
+                                    csrc/tree_wide.cu).  256 is the ceiling of this ABI version: MzTrace.actions is
+                                    uint8_t, so action ids 0..255 are what a trace can record */
 
 enum { MZ_OK = 0, MZ_EINVAL = -1, MZ_ECUDA = -2, MZ_EUNSUPPORTED = -3, MZ_ESTATE = -4, MZ_ENOMEM = -5 };
 enum { MZ_NET_FC = 0, MZ_NET_RESNET = 1 };
@@ -300,8 +302,10 @@ enum { MZ_ENV_CARTPOLE = 0, MZ_ENV_TICTACTOE = 1, MZ_ENV_CONNECT4 = 2, MZ_ENV_GO
 typedef struct MzSelfPlayDesc {
     int32_t env;                  /* MZ_ENV_*: games/cartpole.py:131-174 (restated cart-pole physics),
                                      games/tictactoe.py:243-306, games/connect4.py:220-305,
-                                     games/gomoku.py:220-292 (11x11, five in a row; the mover is paid reward_scale
-                                     whenever the game ends, a full board included),
+                                     games/gomoku.py:220-292 (s x s, five in a row; the mover is paid reward_scale
+                                     whenever the game ends, a full board included; the side is taken from the
+                                     handle, s = isqrt(action_space), which must be a square with 5 <= s <= 16:
+                                     the reference's board_size, 11 by default),
                                      games/twentyone.py:228-303 with Game.step's x10 (one player; cards from the Philox
                                      stream tag 0x7169E006 at counter (game id, draw k, 0, game id >> 32): card =
                                      1 + floor(12 u), value min(card, 10); draw 0 = the player's first card, 1 = the
@@ -399,7 +403,8 @@ int mz_selfplay_drain(MzHandle* h, const void** data, uint64_t* bytes, int32_t* 
 int mz_selfplay_peek(MzHandle* h, const MzSelfPlayPeek* out);
 
 /* Debug / parity: the device opponent (MZ_OPPONENT_EXPERT or MZ_OPPONENT_RANDOM) of env (MZ_ENV_TICTACTOE,
- * MZ_ENV_CONNECT4, or MZ_ENV_GOMOKU with MZ_OPPONENT_RANDOM only) on n host positions.  board is [n][H*W] of +1 / -1 / 0 (row 0 = bottom), player [n] the side to
+ * MZ_ENV_CONNECT4, or MZ_ENV_GOMOKU with MZ_OPPONENT_RANDOM only, on its default 11 x 11 board: this call has no handle
+ * to read another side from) on n host positions.  board is [n][H*W] of +1 / -1 / 0 (row 0 = bottom), player [n] the side to
  * move (+1 / -1).  The random default is the pick for uniform[i], or default_action[i] when default_action is not NULL
  * (one of the two must be given).  out [n] receives the actions. */
 int mz_debug_opponent_action(int device, int32_t env, int32_t opponent, int32_t n, const int8_t* board,

@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libmzb200.so")
 
 MZ_MAX_LAYERS = 8
-MZ_MAX_ACTIONS = 128
+MZ_MAX_ACTIONS = 256
 MZ_MEM_HOST, MZ_MEM_DEVICE = 0, 1
 MZ_FLAG_KEEP_TREE, MZ_FLAG_STEPWISE, MZ_FLAG_CONTINUE = 1, 2, 4
 MZ_EUNSUPPORTED = -3

@@ -63,7 +63,7 @@ extern "C" int mz_create(const MzNetDesc* net, const MzSearchDesc* search, int d
     if (search->num_players < 1 || search->max_games < 1 || search->num_simulations < 0)
         return fail(nullptr, MZ_EINVAL, "mz_create: bad search descriptor");
     if (net->action_space < 1 || net->action_space > MZ_MAX_ACTIONS)
-        return fail(nullptr, MZ_EUNSUPPORTED, "mz_create: action_space must be in [1, 128]");
+        return fail(nullptr, MZ_EUNSUPPORTED, "mz_create: action_space must be in [1, 256]");
     if (net->kind != MZ_NET_FC && net->kind != MZ_NET_RESNET)
         return fail(nullptr, MZ_EUNSUPPORTED, "The network parameter should be \"fullyconnected\" or \"resnet\".");
     if (net->kind == MZ_NET_RESNET && net->downsample > 1)
@@ -156,7 +156,7 @@ extern "C" int mz_create(const MzNetDesc* net, const MzSearchDesc* search, int d
     MZ_CREATE_CUDA(dev_alloc(&p.n_expanded, B));
     MZ_CREATE_CUDA(dev_alloc(&p.ties, B));
     MZ_CREATE_CUDA(dev_alloc(&p.max_depth, B));
-    MZ_CREATE_CUDA(dev_alloc(&p.legal, (size_t)B * (MZ_MAX_ACTIONS / 32)));     // one word per game (|A| <= 32) or four (tree_wide.cu)
+    MZ_CREATE_CUDA(dev_alloc(&p.legal, (size_t)B * (MZ_MAX_ACTIONS / 32)));     // one word per game (|A| <= 32), or a stride of eight of which tree_wide.cu reads four or eight
     MZ_CREATE_CUDA(dev_alloc(&p.path, (size_t)B * (N + 2)));
     MZ_CREATE_CUDA(dev_alloc(&p.path_reward, (size_t)B * (N + 2)));
     MZ_CREATE_CUDA(dev_alloc(&p.leaf_depth, B));
@@ -641,6 +641,10 @@ extern "C" int mz_search(MzHandle* h, const MzSearchIO* io) {
             return fail(h, MZ_EINVAL, "mz_search: incomplete teacher table");
     }
     if (io->trace) {
+        // the kernels address a game's trace rows by the pool's layout size, the caller's arrays hold num_simulations rows
+        // per game: the two agree for one game, and for any number when the pool has no extra room
+        if (n > 1 && h->search.extra_expansions > 0)
+            return fail(h, MZ_EINVAL, "mz_search: a trace of more than one game needs a handle with extra_expansions = 0");
         const MzTrace& t = *io->trace;
         const int D = t.max_depth;
         call.trace.max_depth = D;
@@ -820,7 +824,7 @@ extern "C" int mz_import_tree(MzHandle* h, int32_t game, const MzTreeExport* t) 
     MZ_CUDA(h, cudaMemcpy(p.prior + base, prior.data(), used * 4, cudaMemcpyHostToDevice));
     MZ_CUDA(h, cudaMemcpy(p.expansion + base, t->child_expansion, used * 4, cudaMemcpyHostToDevice));
     MZ_CUDA(h, cudaMemcpy(p.root_prior + (size_t)game * A, rp.data(), A * 8, cudaMemcpyHostToDevice));
-    // children of a non-root node: the whole action space (one mask word per game, four for |A| > 32)
+    // children of a non-root node: the whole action space (one mask word per game, MZ_MAX_ACTIONS / 32 for |A| > 32)
     const double range[2] = {INFINITY, -INFINITY};
     const int zero = 0;
     if (A > 32) {

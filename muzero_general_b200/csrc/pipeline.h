@@ -79,7 +79,7 @@ struct TreeStepArgs {
     DevTrace trace;
 };
 cudaError_t launch_tree_step(const TreeStepArgs& a, cudaStream_t stream);
-cudaError_t launch_tree_step_wide(const TreeStepArgs& a, cudaStream_t stream);      // 32 < |A| <= 128 (tree_wide.cu)
+cudaError_t launch_tree_step_wide(const TreeStepArgs& a, cudaStream_t stream);      // 32 < |A| <= 256 (tree_wide.cu)
 cudaError_t launch_tree_adopt_root(const TreeStepArgs& a, cudaStream_t stream);     // MZ_FLAG_CONTINUE: adopt the imported tree
 
 struct ResNetDevice;

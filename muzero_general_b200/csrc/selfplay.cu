@@ -10,8 +10,9 @@
 //   TicTacToe  games/tictactoe.py:243-306; Connect4  games/connect4.py:220-305: planes [own stones of player +1,
 //              stones of player -1, side to move (+1/-1)], player +1 = to_play 0 moves first, reward_scale for the mover
 //              on completing a line, done on a line or a full board; Connect4 actions are columns (gravity)
-//   Gomoku     games/gomoku.py:220-292: the same planes on 11x11, five in a row; the mover is paid reward_scale whenever
-//              the game ends, a full board without a line included
+//   Gomoku     games/gomoku.py:220-292: the same planes on s x s (5 <= s <= 16, s * s = |A|: the reference's
+//              board_size, 11 by default), five in a row; the mover is paid reward_scale whenever the game ends, a full
+//              board without a line included
 //   TwentyOne  games/twentyone.py:228-303: hit (0) / stand (1); planes [player's hand, dealer's hand, 0] of 3x3; done on
 //              a bust, a stand or exactly 21, then the dealer draws while at 16 or less unless the player went bust;
 //              reward_scale * get_reward (Game.step's x10)
@@ -44,7 +45,7 @@ namespace mz {
 constexpr uint32_t kTagReset = 0x7169E004u;
 constexpr uint32_t kTagOpponent = 0x7169E005u;
 constexpr uint32_t kTagCard = 0x7169E006u;
-constexpr int kMaxCells = 128;             // board cells per slot (Gomoku: 121)
+constexpr int kMaxCells = 256;             // board cells per slot (Gomoku: up to 16 x 16)
 
 struct SpDev {
     int env, B, A, O, H, W, K, max_moves, threshold, reward_scale;
@@ -415,6 +416,8 @@ __global__ void selfplay_reset_kernel(const SpDev s, int64_t first_game_id) {
 // ------------------------------------------------------------------------------------------
 // select_action (self_play.py:222-245) on the visit counts of the search that just finished, then Game.step
 // ------------------------------------------------------------------------------------------
+// kMaxA: the bound on |A| the cdf array is sized for
+template <int kMaxA>
 MZ_DEVINL int sample_action(const SpDev& s, int g, double temperature, double u) {
     const int32_t* v = s.visits + (size_t)g * s.A;
     const uint8_t* lg = s.legal + (size_t)g * s.A;
@@ -431,7 +434,7 @@ MZ_DEVINL int sample_action(const SpDev& s, int g, double temperature, double u)
     // 1/T is 1, 2 or 4 for every reference schedule (games/*.py visit_softmax_temperature_fn): integer powers are exact
     const double inv = 1.0 / temperature;
     double total = 0.0;
-    double p[MZ_MAX_ACTIONS];
+    double p[kMaxA];
     for (int k = 0; k < A; ++k) {
         double x = lg[k] ? (double)v[k] : 0.0;
         if (inv == 2.0) x = x * x;
@@ -452,6 +455,7 @@ MZ_DEVINL int sample_action(const SpDev& s, int g, double temperature, double u)
 
 // select_action + Game.step + record for slot g (one thread), then the opponent's reply in a test-mode game; returns
 // the moves played
+template <int kMaxA>
 MZ_DEVINL int slot_act(const SpDev& s, int g) {
     const int t = s.move[g];
     const int64_t gid = s.game_id[g];
@@ -459,7 +463,7 @@ MZ_DEVINL int slot_act(const SpDev& s, int g) {
     if (action < 0) {
         const double T = (s.threshold == 0 || t + 1 < s.threshold) ? s.temperature : 0.0;
         const double u = s.uniform ? s.uniform[g] : philox_uniform53(s.seed, gid, t, 0u, kTagAction);
-        action = sample_action(s, g, T, u);
+        action = sample_action<kMaxA>(s, g, T, u);
     }
     float reward;
     bool done;
@@ -529,8 +533,11 @@ MZ_DEVINL float initial_priority(const SpDev& s, int g, int T, int i) {
 // past the capacity, reservations that end beyond it are void (the game stays parked), and since the cursor only grows
 // the valid reservations are a contiguous prefix whose end is tracked in counters[5].  With stacked observations, a
 // slot whose move was played or whose game restarted then rebuilds its stacked tail with the whole warp.
+// kMaxA (128 or 256, the least that holds |A|) sizes the sampler's stack array, so the configurations of up to 128
+// actions keep their stack frame.
 constexpr int kStepThreads = 1024;
 
+template <int kMaxA>
 __global__ void __launch_bounds__(kStepThreads) selfplay_step_kernel(const SpDev s, int act) {
     __shared__ int s_active;
     if (threadIdx.x == 0) s_active = 0;
@@ -543,7 +550,7 @@ __global__ void __launch_bounds__(kStepThreads) selfplay_step_kernel(const SpDev
         if (lane == 0) {
             T = s.fin[g];
             if (act && T == 0) {
-                atomicAdd(&s_active, slot_act(s, g));
+                atomicAdd(&s_active, slot_act<kMaxA>(s, g));
                 T = s.fin[g];
                 changed = 1;
             }
@@ -618,6 +625,12 @@ __global__ void __launch_bounds__(kStepThreads) selfplay_step_kernel(const SpDev
     }
     __syncthreads();
     if (threadIdx.x == 0 && s_active) atomicAdd(&s.counters[0], (unsigned long long)s_active);
+}
+
+static void launch_selfplay_step(const SpDev& s, int act, cudaStream_t stream) {
+    const int grid = (s.B * 32 + kStepThreads - 1) / kStepThreads;
+    if (s.A <= 128) selfplay_step_kernel<128><<<grid, kStepThreads, 0, stream>>>(s, act);
+    else selfplay_step_kernel<256><<<grid, kStepThreads, 0, stream>>>(s, act);
 }
 
 }  // namespace mz
@@ -702,7 +715,16 @@ extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_
         case MZ_ENV_CARTPOLE: name = "CartPole"; C = 1; ph = 1; pw = 4; A_env = 2; break;
         case MZ_ENV_TICTACTOE: name = "TicTacToe"; H = 3; W = 3; K = 3; C = 3; ph = 3; pw = 3; A_env = 9; break;
         case MZ_ENV_CONNECT4: name = "Connect4"; H = 6; W = 7; K = 4; C = 3; ph = 6; pw = 7; A_env = 7; break;
-        case MZ_ENV_GOMOKU: name = "Gomoku"; H = 11; W = 11; K = 5; C = 3; ph = 11; pw = 11; A_env = 121; break;
+        case MZ_ENV_GOMOKU: {
+            // the board's side is the reference's Gomoku.board_size; it travels in the handle's action space
+            int side = 0;
+            while ((side + 1) * (side + 1) <= A) ++side;
+            if (side * side != A || side < 5 || side > 16)
+                return fail(h, MZ_EINVAL, "mz_selfplay_begin: Gomoku plays on s x s boards with 5 <= s <= 16, so its action space is "
+                                          "a square in [25, 256]; the handle has " + std::to_string(A) + " actions");
+            name = "Gomoku"; H = side; W = side; K = 5; C = 3; ph = side; pw = side; A_env = A;
+            break;
+        }
         case MZ_ENV_TWENTYONE: name = "Twenty-One"; C = 3; ph = 3; pw = 3; A_env = 2; break;
         case MZ_ENV_SIMPLE_GRID: name = "Simple Grid"; C = 1; ph = 1; pw = 9; A_env = 2; break;
         default: return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin: unknown environment");
@@ -850,14 +872,14 @@ static int sp_enqueue(MzHandle* h, int32_t n_moves, double temperature, const Mz
     call.visit_counts = s.visits; call.root_value = s.root_value;
     MZ_CUDA(h, cudaEventRecord(sp->e0, h->stream));
     if (sp->h_counters[4]) {                           // games parked by the previous call first, so their slots play again
-        selfplay_step_kernel<<<(B * 32 + kStepThreads - 1) / kStepThreads, kStepThreads, 0, h->stream>>>(s, 0);
+        launch_selfplay_step(s, 0, h->stream);
         h->launches += 1;
     }
     MZ_CUDA(h, cudaMemsetAsync(s.counters + 4, 0, 8, h->stream));      // [4] = park events of THIS call
     for (int m = 0; m < n_moves; ++m) {
         int rc = mz_dispatch_search(h, call, false, false, 0);
         if (rc) return rc;
-        selfplay_step_kernel<<<(B * 32 + kStepThreads - 1) / kStepThreads, kStepThreads, 0, h->stream>>>(s, 1);
+        launch_selfplay_step(s, 1, h->stream);
         h->launches += 1;
     }
     MZ_CUDA(h, cudaGetLastError());

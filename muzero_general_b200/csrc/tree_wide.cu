@@ -1,10 +1,11 @@
-// Step-wise tree kernel for wide action spaces, 32 < |A| <= 128 (games/gomoku.py: 121 actions).
+// Step-wise tree kernel for wide action spaces, 32 < |A| <= 256 (games/gomoku.py: 121 actions on 11 x 11, 225 on 15 x 15).
 //
 // Same arithmetic, same operation order and same pool layout as tree_kernels.cu / tree.cuh (select_child / ucb_score
 // self_play.py:363-404, Node.expand :451-465, add_exploration_noise :467-476, backpropagate :406-430); the only change is
-// the mapping of children to lanes: one WARP owns a game and lane l scores the children l, l + 32, l + 64, l + 96, so a
-// level costs up to four rounds of the per-child work and the tie list is four ballot words read in ascending action
-// order.  The backup does not depend on |A| and is tree.cuh's.  Kept apart from the narrow kernel on purpose: the
+// the mapping of children to lanes: one WARP owns a game and lane l scores the children l, l + 32, ..., l + 32 (kJ - 1),
+// so a level costs up to kJ rounds of the per-child work and the tie list is kJ ballot words read in ascending action
+// order.  kJ is a template parameter, 4 for |A| <= 128 and 8 for |A| <= 256, and nothing but trip counts depends on it.
+// The backup does not depend on |A| and is tree.cuh's.  Kept apart from the narrow kernel on purpose: the
 // per-simulation kernel of the BASELINE configs (|A| <= 9) keeps its register budget and its tested code path.
 #include <stdlib.h>
 
@@ -17,10 +18,11 @@ namespace mz {
 
 namespace {
 
-constexpr int kJ = MZ_MAX_ACTIONS / 32;      // children per lane
+constexpr int kLegalWords = MZ_MAX_ACTIONS / 32;      // words of a game's legal mask in the pool, whatever kJ reads of them
 using LG = LaneGroup<32>;
 
 // lowest set bit position across the words in ascending action order, or the n-th (0-based) set bit
+template <int kJ>
 MZ_DEVINL int nth_action(const unsigned (&w)[kJ], int n) {
 #pragma unroll
     for (int j = 0; j < kJ; ++j) {
@@ -33,7 +35,11 @@ MZ_DEVINL int nth_action(const unsigned (&w)[kJ], int n) {
 
 }  // namespace
 
-__global__ void __launch_bounds__(128) tree_step_wide_kernel(const __grid_constant__ TreeStepArgs a) {
+// kJ: children per lane.  With eight, the register allocator's default target leaves five of the legal-mask words in
+// local memory; one resident CTA per SM as the stated minimum lifts that target (189 registers, no spills) and leaves
+// the kJ = 4 instantiation, which states none, as it was (128 registers).
+template <int kJ>
+__global__ void __launch_bounds__(128, kJ > 4 ? 1 : 0) tree_step_wide_kernel(const __grid_constant__ TreeStepArgs a) {
     pdl_launch_dependents();
     pdl_wait();
     const int local = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -132,7 +138,7 @@ __global__ void __launch_bounds__(128) tree_step_wide_kernel(const __grid_consta
         __syncwarp();
     } else {
 #pragma unroll
-        for (int j = 0; j < kJ; ++j) legal[j] = p.legal[(size_t)g * kJ + j];
+        for (int j = 0; j < kJ; ++j) legal[j] = p.legal[(size_t)g * kLegalWords + j];
         t.root_visit = p.root_visit[g];
         t.root_vsum = p.root_vsum[g];
         t.root_reward = p.root_reward[g];
@@ -279,7 +285,7 @@ __global__ void __launch_bounds__(128) tree_step_wide_kernel(const __grid_consta
 
     if (lane == 0) {
 #pragma unroll
-        for (int j = 0; j < kJ; ++j) p.legal[(size_t)g * kJ + j] = legal[j];
+        for (int j = 0; j < kJ; ++j) p.legal[(size_t)g * kLegalWords + j] = legal[j];
         p.root_visit[g] = t.root_visit;
         p.root_vsum[g] = t.root_vsum;
         p.root_reward[g] = t.root_reward;
@@ -310,7 +316,8 @@ __global__ void __launch_bounds__(128) tree_step_wide_kernel(const __grid_consta
 
 cudaError_t launch_tree_step_wide(const TreeStepArgs& a, cudaStream_t stream) {
     const int grid = (a.n * 32 + 127) / 128;
-    cudaError_t e = launch_chained(tree_step_wide_kernel, dim3(grid), dim3(128), 0, stream, a);
+    cudaError_t e = a.A <= 128 ? launch_chained(tree_step_wide_kernel<4>, dim3(grid), dim3(128), 0, stream, a)
+                               : launch_chained(tree_step_wide_kernel<8>, dim3(grid), dim3(128), 0, stream, a);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 
