@@ -262,7 +262,7 @@ int mz_debug_conv3x3_plan(int32_t n, int32_t cin, int32_t cout, int32_t H, int32
 int mz_debug_conv3x3(int device, int32_t n, int32_t cin, int32_t cout, int32_t H, int32_t W, int32_t stride, const float* x,
                      const float* w, const float* bias, const float* residual, int32_t relu, int32_t use_tensor_cores, float* out);
 
-/* Call sites of the 64-channel tensor-core towers (site argument of mz_debug_conv_tower) */
+/* Call sites of the towers (site argument of mz_debug_conv_tower and mz_debug_small_tower) */
 #define MZ_TOWER_REPRESENTATION 0   /* input in a workspace, reusable once read; no stem */
 #define MZ_TOWER_DYNAMICS 1         /* plain recurrent call: input converted into a workspace; stem with the action plane */
 #define MZ_TOWER_DYNAMICS_POOL 2    /* in search: input gathered from the hidden-state pool (read only); stem with the action plane */
@@ -279,6 +279,28 @@ int mz_debug_conv3x3(int device, int32_t n, int32_t cin, int32_t cout, int32_t H
 int mz_debug_conv_tower(int device, int32_t n, int32_t H, int32_t W, int32_t mode, int32_t blocks, int32_t site, int32_t parts,
                         int32_t A, const float* x, const float* w, const float* bias, const int32_t* action, const int32_t* parent,
                         int32_t pool_stride, float* out, int64_t* launches, int32_t* saturated);
+
+/* Launch plan of the fused CUDA-core tower (host only): n boards of H x W through [a stem conv reading in_channels planes,
+ * C + 1 for the dynamics stem with its action plane, if stem] + `blocks` residual blocks of C channels.  Fills plan[6] =
+ * {P pixels per thread, CO output channels per thread, boards per CTA, threads per CTA, persistent grid, dynamic shared-memory
+ * bytes} and returns 1; returns 0 with the reason in mz_last_error(NULL) when the fused tower refuses the shape (the network
+ * then runs one conv3x3 launch per conv). */
+int mz_debug_small_tower_plan(int32_t n, int32_t in_channels, int32_t C, int32_t H, int32_t W, int32_t blocks, int32_t stem,
+                              int32_t sm_count, int64_t* plan);
+
+/* Debug / parity: one fused CUDA-core tower (models.py:206-231 without BN: [stem conv +] `blocks` residual blocks, every conv
+ * with bias and ReLU, the residual added before the second ReLU of a block) of one call site of resnet_inference on host NCHW
+ * fp32 data, through the helper the network calls.  MZ_TOWER_REPRESENTATION: stem from x [n][in_channels][H][W];
+ * MZ_TOWER_DYNAMICS: stem of C + 1 planes, channel C the action plane action[g] / A, x [n][C][H][W] dense;
+ * MZ_TOWER_DYNAMICS_POOL: the same with game g's input in slot parent[g] of its pool_stride slots, the other slots NaN, and
+ * `parts` (1..4) runs the games in the ranges of the partitioned replay; MZ_TOWER_PREDICTION: no stem, blocks >= 1
+ * (in_channels is C at every site but the representation).  w holds every conv's [C][cin][3][3] back to back, bias [convs][C]
+ * (or NULL).  The output starts as NaN.  out is [n][C][H][W]; plan (or NULL) gets the plan of the launch as
+ * mz_debug_small_tower_plan fills it (of the first range when partitioned).  MZ_EUNSUPPORTED when the fused tower refuses the
+ * shape. */
+int mz_debug_small_tower(int device, int32_t n, int32_t in_channels, int32_t C, int32_t H, int32_t W, int32_t blocks, int32_t site,
+                         int32_t parts, int32_t A, const float* x, const float* w, const float* bias, const int32_t* action,
+                         const int32_t* parent, int32_t pool_stride, float* out, int64_t* plan);
 
 /* Arithmetic the handle's search path computes in, e.g. "f32 nets + f64 tree statistics" (bench.py's dtype). */
 const char* mz_numerics(const MzHandle* h);

@@ -150,6 +150,9 @@ SYMBOLS = [
                                                                   C.c_int32, C.c_int32, C.c_void_p]),
     ("mz_debug_conv_tower", C.c_int, [C.c_int] + [C.c_int32] * 8 + [C.c_void_p] * 5 + [C.c_int32, C.c_void_p,
                                                                                       C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
+    ("mz_debug_small_tower_plan", C.c_int, [C.c_int32] * 8 + [C.POINTER(C.c_int64)]),
+    ("mz_debug_small_tower", C.c_int, [C.c_int] + [C.c_int32] * 9 + [C.c_void_p] * 5 + [C.c_int32, C.c_void_p,
+                                                                                       C.POINTER(C.c_int64)]),
 ]
 
 _lib = None

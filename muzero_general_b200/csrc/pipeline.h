@@ -100,6 +100,13 @@ inline int partition_games(int n, int parts) { return ((n + parts - 1) / parts +
 int resnet_debug_tower(int n, int H, int W, int mode, int blocks, int site, int parts, int A, const float* x, const float* w,
                        const float* bias, const int32_t* action, const int32_t* parent, int pool_stride, float* out,
                        int64_t* launches, int32_t* saturated, int sm_count, std::string* err);
+// Host-only plan of the fused CUDA-core tower (plan[6], see include/mzb200.h, mz_debug_small_tower_plan) and the debug /
+// parity entry behind mz_debug_small_tower: one fused CUDA-core tower of one call site of resnet_inference on host NCHW data
+bool resnet_small_tower_plan(int n, int in_channels, int C, int H, int W, int blocks, bool stem, int sm_count, int64_t* plan,
+                             std::string* err);
+int resnet_debug_small_tower(int n, int in_channels, int C, int H, int W, int blocks, int site, int parts, int A, const float* x,
+                             const float* w, const float* bias, const int32_t* action, const int32_t* parent, int pool_stride,
+                             float* out, int64_t* plan, int sm_count, std::string* err);
 // fused search of small residual networks: all simulations in one launch (small_search.cu); MZ_SMALL_SEARCH=0 / 1 switches it off / on
 bool resnet_small_search_supported(ResNetDevice* r, const InferCall& first_recurrent, const TreeStepArgs& tree, int n_sims);
 int resnet_small_search(ResNetDevice* r, const InferCall& first_recurrent, const TreeStepArgs& tree, int n_sims, cudaStream_t stream,

@@ -813,6 +813,7 @@ namespace {
 struct Runner {
     ResNetDevice* r; cudaStream_t stream; int64_t* launches; std::string* err; int n;
     int g0 = 0;                // games [g0, g0 + n) of the batch (partitioned replay); buffers are addressed by the global index
+    SmallTowerPlan* small_plan = nullptr;   // when set, small_tower reports the plan of its launch here (mz_debug_small_tower)
     bool fail(const char* what, cudaError_t e) { *err = std::string(what) + ": " + cudaGetErrorString(e); return false; }
 
     // conv: in -> out. `in` may be gathered from the pool; action adds the constant plane.
@@ -1020,11 +1021,29 @@ struct Runner {
         if (!small_tower_supported(a)) return 0;
         if (dry_run) return 1;
         kt_begin(KT_SMALL, stream);
-        cudaError_t e = launch_small_tower(a, r->sm_count, stream);
+        cudaError_t e = launch_small_tower(a, r->sm_count, stream, small_plan);
         kt_end(stream);
         if (e != cudaSuccess) { fail("small_tower launch", e); return -1; }
         *launches += 1;
         return 1;
+    }
+
+    // The four fused CUDA-core tower call sites of resnet_inference, each with the input it reads (mz_debug_small_tower runs
+    // the same helpers); each returns what small_tower returns.  Representation: stem from the observation planes.
+    int representation_small_tower(const float* obs, float* out) {
+        return small_tower(r->rep_trunk, 0, true, r->net.blocks, obs, out, r->net.obs_c, r->net.obs_h, r->net.obs_w);
+    }
+    // Dynamics, plain API call: dense hidden states plus the action plane.
+    int dynamics_small_tower(const float* states, float* out, const int32_t* action) {
+        return small_tower(r->dyn, 0, true, r->net.blocks, states, out, r->C, r->hh, r->hw, nullptr, 0, action);
+    }
+    // Dynamics in search: the parents' states gathered from the pool, plus the action plane.
+    int dynamics_small_tower_pool(const float* pool, const int32_t* gather_parent, int pool_stride, float* out, const int32_t* action) {
+        return small_tower(r->dyn, 0, true, r->net.blocks, pool, out, r->C, r->hh, r->hw, gather_parent, pool_stride, action);
+    }
+    // Prediction: the rescaled hidden state, no stem (a net without blocks has no prediction tower).
+    int prediction_small_tower(const float* hidden, float* out) {
+        return r->net.blocks > 0 ? small_tower(r->pred, 0, false, r->net.blocks, hidden, out, r->C, r->hh, r->hw) : 0;
     }
 
     // residual tower: layers[2k], layers[2k+1] are one block; x ends up in `*cur`
@@ -1489,6 +1508,148 @@ int resnet_debug_tower(int n, int H, int W, int mode, int blocks, int site, int 
     return good ? MZ_OK : MZ_ECUDA;
 }
 
+// Launch plan of the fused CUDA-core tower (host only, behind mz_debug_small_tower_plan): plan[6] = {P, CO, boards per
+// CTA, threads, grid, shared-memory bytes} of n boards through [a stem conv reading in_channels planes +] `blocks`
+// residual blocks of C channels, from the same Runner::small_tower_args and planner the launch takes.  false with the
+// reason in *err when the fused tower refuses the shape (the network then runs one conv3x3_kernel launch per conv).
+bool resnet_small_tower_plan(int n, int in_channels, int C, int H, int W, int blocks, bool stem, int sm_count, int64_t* plan,
+                             std::string* err) {
+    if (blocks < 0 || in_channels < 1) { *err = "bad shape"; return false; }
+    if (!stem && in_channels != C) { *err = "without a stem the tower input has C channels"; return false; }
+    if ((stem ? 1 : 0) + 2 * blocks < 1 || (stem ? 1 : 0) + 2 * blocks > kSmallTowerMaxLayers) { *err = "1 to 10 layers"; return false; }
+    ResNetDevice r{};
+    r.C = C; r.hh = H; r.hw = W; r.sm_count = sm_count; r.net.action_space = 1;
+    std::vector<ConvLayer> layers((stem ? 1 : 0) + 2 * (size_t)blocks);
+    for (size_t i = 0; i < layers.size(); ++i) {
+        ConvLayer& l = layers[i];
+        l.cin = stem && i == 0 ? in_channels : C; l.cout = C; l.stride = 1;
+        l.w_off = 0; l.b_off = -1; l.tc_off = l.tc_table_off = l.tc_scale_off = -1;
+    }
+    int64_t launches = 0;
+    Runner R{&r, nullptr, &launches, err, n};
+    SmallTowerArgs a{};
+    if (!R.small_tower_args(a, layers, 0, stem, (size_t)blocks, nullptr, nullptr, in_channels, H, W, nullptr, 0, nullptr)) {
+        *err = "layers the fused tower does not take"; return false;
+    }
+    SmallTowerPlan p;
+    const char* why = "";
+    if (!small_tower_plan(a, sm_count, &p, &why)) { *err = why; return false; }
+    const int64_t out[6] = {p.P, p.CO, p.boards_per_cta, p.threads, p.grid, (int64_t)p.smem};
+    for (int i = 0; i < 6; ++i) plan[i] = out[i];
+    return true;
+}
+
+// Stand-alone fused CUDA-core tower of one call site of resnet_inference, through the same Runner helpers, on host NCHW
+// data.  The output and the pool's other slots start as NaN bytes (0xFF), so a board the tower does not write, or one read
+// from the wrong slot, produces NaN.
+int resnet_debug_small_tower(int n, int in_channels, int C, int H, int W, int blocks, int site, int parts, int A, const float* x,
+                             const float* w, const float* bias, const int32_t* action, const int32_t* parent, int pool_stride,
+                             float* out, int64_t* plan, int sm_count, std::string* err) {
+    const bool stem = site != MZ_TOWER_PREDICTION;
+    const bool dyn = site == MZ_TOWER_DYNAMICS || site == MZ_TOWER_DYNAMICS_POOL;
+    const bool in_pool = site == MZ_TOWER_DYNAMICS_POOL;
+    if (n < 1 || C < 4 || blocks < 0 || (!stem && blocks < 1) || site < MZ_TOWER_REPRESENTATION || site > MZ_TOWER_PREDICTION ||
+        (site == MZ_TOWER_REPRESENTATION ? in_channels < 1 : in_channels != C)) {
+        *err = "bad shape or site"; return MZ_EINVAL;
+    }
+    if (parts < 1 || parts > 4 || (parts > 1 && !in_pool)) { *err = "partitions need the in-search dynamics site, 1 to 4 of them"; return MZ_EINVAL; }
+    if (dyn) {
+        if (A < 1 || !action) { *err = "the dynamics sites need actions and A >= 1"; return MZ_EINVAL; }
+        for (int g = 0; g < n; ++g) if (action[g] < 0 || action[g] >= A) { *err = "action out of range"; return MZ_EINVAL; }
+    }
+    if (in_pool) {
+        if (!parent || pool_stride < 1) { *err = "the in-search site needs parents and pool_stride >= 1"; return MZ_EINVAL; }
+        for (int g = 0; g < n; ++g) if (parent[g] < 0 || parent[g] >= pool_stride) { *err = "parent out of range"; return MZ_EINVAL; }
+    }
+    // a state_dict of plain convolutions for pack_conv: "c<i>.weight", the stem first
+    const int cin0 = site == MZ_TOWER_REPRESENTATION ? in_channels : dyn ? C + 1 : C;
+    const int n_convs = (stem ? 1 : 0) + 2 * blocks;
+    std::vector<std::string> names(n_convs);
+    std::vector<MzTensor> tensors(n_convs);
+    size_t w_off = 0;
+    for (int i = 0; i < n_convs; ++i) {
+        const int cin = i == 0 ? cin0 : C;
+        names[i] = "c" + std::to_string(i) + ".weight";
+        tensors[i] = MzTensor{names[i].c_str(), w + w_off, (int64_t)C * cin * 9};
+        w_off += (size_t)C * cin * 9;
+    }
+    MzNetDesc nd{};
+    nd.kind = MZ_NET_RESNET; nd.channels = C; nd.obs_c = site == MZ_TOWER_REPRESENTATION ? in_channels : C; nd.obs_h = H; nd.obs_w = W;
+    nd.action_space = dyn ? A : 1; nd.blocks = blocks;
+    ResNetDevice r{};
+    r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = H; r.hw = W;
+    Loader L{tensors.data(), n_convs, err};
+    std::vector<float> blob;
+    std::vector<ConvLayer> layers;
+    for (int i = 0; i < n_convs; ++i) {
+        if (!pack_conv(L, "c" + std::to_string(i), "", i == 0 ? cin0 : C, C, 1, blob, layers)) return MZ_EINVAL;
+        if (bias) {
+            layers[i].b_off = (long)blob.size();
+            blob.insert(blob.end(), bias + (size_t)i * C, bias + (size_t)(i + 1) * C);      // (C % 4 == 0: stays aligned)
+        }
+    }
+    if (site == MZ_TOWER_REPRESENTATION) r.rep_trunk = layers;
+    else if (dyn) r.dyn = layers;
+    else r.pred = layers;
+
+    const size_t in_elems = (size_t)nd.obs_c * H * W, dense = (size_t)n * C * H * W;
+    const size_t in_total = in_pool ? (size_t)n * pool_stride * in_elems : (size_t)n * in_elems;
+    float *d_blob = nullptr, *d_in = nullptr, *d_out = nullptr;
+    int32_t *d_action = nullptr, *d_parent = nullptr;
+    auto cleanup = [&]() { for (void* p : {(void*)d_blob, (void*)d_in, (void*)d_out, (void*)d_action, (void*)d_parent}) if (p) cudaFree(p); };
+    const bool ok = cudaMalloc(&d_blob, blob.size() * 4) == cudaSuccess && cudaMalloc(&d_in, in_total * 4) == cudaSuccess &&
+                    cudaMalloc(&d_out, dense * 4) == cudaSuccess && cudaMalloc(&d_action, (size_t)n * 4) == cudaSuccess &&
+                    cudaMalloc(&d_parent, (size_t)n * 4) == cudaSuccess;
+    if (!ok) { cleanup(); *err = "allocation failed"; return MZ_ENOMEM; }
+    r.d_conv = d_blob;
+    cudaMemcpy(d_blob, blob.data(), blob.size() * 4, cudaMemcpyHostToDevice);
+    if (in_pool) {
+        cudaMemset(d_in, 0xFF, in_total * 4);
+        for (int g = 0; g < n; ++g)
+            cudaMemcpy(d_in + ((size_t)g * pool_stride + parent[g]) * in_elems, x + (size_t)g * in_elems, in_elems * 4,
+                       cudaMemcpyHostToDevice);
+        cudaMemcpy(d_parent, parent, (size_t)n * 4, cudaMemcpyHostToDevice);
+    } else {
+        cudaMemcpy(d_in, x, in_total * 4, cudaMemcpyHostToDevice);
+    }
+    if (dyn) cudaMemcpy(d_action, action, (size_t)n * 4, cudaMemcpyHostToDevice);
+    cudaMemset(d_out, 0xFF, dense * 4);
+    int64_t launches = 0;
+    SmallTowerPlan used{}, first{};
+    int rc = MZ_OK;
+    // the ranges of the partitioned replay, each through its own Runner (one range unless in the pool); every array stays
+    // addressed by the global game.  The plan reported is the first range's.
+    const int per = in_pool ? partition_games(n, parts) : n;
+    for (int p = 0; p * per < n && rc == MZ_OK; ++p) {
+        Runner R{&r, nullptr, &launches, err, std::min(per, n - p * per), p * per};
+        R.small_plan = &used;
+        int fused;
+        if (site == MZ_TOWER_REPRESENTATION) fused = R.representation_small_tower(d_in, d_out);
+        else if (site == MZ_TOWER_DYNAMICS) fused = R.dynamics_small_tower(d_in, d_out, d_action);
+        else if (site == MZ_TOWER_DYNAMICS_POOL) fused = R.dynamics_small_tower_pool(d_in, d_parent, pool_stride, d_out, d_action);
+        else fused = R.prediction_small_tower(d_in, d_out);
+        if (fused == 0) {
+            int64_t unused[6];
+            std::string why = "no fused launch";
+            resnet_small_tower_plan(R.n, cin0, C, H, W, blocks, stem, sm_count, unused, &why);
+            *err = "the fused tower refuses the shape: " + why; rc = MZ_EUNSUPPORTED;
+        }
+        else if (fused < 0) rc = MZ_ECUDA;
+        if (p == 0) first = used;
+    }
+    cudaError_t e = cudaDeviceSynchronize();
+    if (rc == MZ_OK && e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug small tower: ") + cudaGetErrorString(e); }
+    if (rc == MZ_OK) {
+        e = cudaMemcpy(out, d_out, dense * 4, cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug small tower: ") + cudaGetErrorString(e); }
+        const int64_t pl[6] = {first.P, first.CO, first.boards_per_cta, first.threads, first.grid, (int64_t)first.smem};
+        if (plan) for (int i = 0; i < 6; ++i) plan[i] = pl[i];
+    }
+    r.d_conv = nullptr;
+    cleanup();
+    return rc;
+}
+
 // stored hidden states (pool layout) -> dense NCHW, device to device
 int resnet_states_to_nchw(ResNetDevice* r, const float* states, int count, float* out, cudaStream_t stream) {
     const size_t total = (size_t)count * r->C * r->hh * r->hw;
@@ -1613,7 +1774,7 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
             if (fused) { float* t = cur; cur = tmp; tmp = t; }
             else if (!R.blocks(r->rep_trunk, 0, nd.blocks, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
         } else {
-            const int fused = R.small_tower(r->rep_trunk, 0, true, nd.blocks, c.in, cur, nd.obs_c, H, W);
+            const int fused = R.representation_small_tower(c.in, cur);
             if (fused < 0) return MZ_ECUDA;
             if (!fused) {
                 if (!R.conv(r->rep_trunk[0], c.in, cur, nullptr, true, H, W)) return MZ_ECUDA;
@@ -1633,7 +1794,8 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
         }
     } else {
         const float* in = c.gather_parent ? c.pool_hidden : c.in;
-        const int fused = R.small_tower(r->dyn, 0, true, nd.blocks, in, cur, C, hh, hw, c.gather_parent, c.pool_stride, c.action);
+        const int fused = c.gather_parent ? R.dynamics_small_tower_pool(c.pool_hidden, c.gather_parent, c.pool_stride, cur, c.action)
+                                          : R.dynamics_small_tower(c.in, cur, c.action);
         if (fused < 0) return MZ_ECUDA;
         if (!fused) {
             if (!R.conv(r->dyn[0], in, cur, nullptr, true, hh, hw, c.gather_parent, c.pool_stride, c.action)) return MZ_ECUDA;
@@ -1649,7 +1811,7 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
         float* x = hidden_out;
         // the tower must not overwrite the hidden state: first conv reads it, writes workspace
         float *pc = cur, *pt = tmp, *ps = spare;
-        const int fused = nd.blocks > 0 ? R.small_tower(r->pred, 0, false, nd.blocks, x, pt, C, hh, hw) : 0;
+        const int fused = R.prediction_small_tower(x, pt);
         if (fused < 0) return MZ_ECUDA;
         if (fused) {
             x = pt;

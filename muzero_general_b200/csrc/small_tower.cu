@@ -37,21 +37,23 @@ __global__ void __launch_bounds__(kMaxThreads) small_tower_kernel(const __grid_c
         small_tower_tile<P, CO, false>(a, s_w, s_act, tile * nb, min(nb, a.n - tile * nb), threadIdx.x, blockDim.x);
 }
 
-struct Plan { int P, CO, nb, threads, grid; size_t smem; bool ok; };
 }  // namespace
 
 // Shared-memory layout of the tower's weights (w_smem_off / b_smem_off / w_floats) and the channel capacity of its
-// activation buffers; false when the shape is outside what the kernels handle.
-bool small_tower_layout(SmallTowerArgs& a) {
-    if (a.n_layers < 1 || a.n_layers > kSmallTowerMaxLayers) return false;
-    if (a.W < 2 || a.W > 8 || a.H < 1 || a.H > 16 || a.C % 4 != 0 || a.C < 4) return false;
+// activation buffers; false (with the reason in *why) when the shape is outside what the kernels handle.
+bool small_tower_layout(SmallTowerArgs& a, const char** why) {
+    const char* dummy;
+    if (!why) why = &dummy;
+    if (a.n_layers < 1 || a.n_layers > kSmallTowerMaxLayers) { *why = "1 to 10 layers"; return false; }
+    if (a.W < 2 || a.W > 8 || a.H < 1 || a.H > 16) { *why = "boards of 1..16 rows x 2..8 columns"; return false; }
+    if (a.C % 4 != 0 || a.C < 4) { *why = "channels must be a positive multiple of 4"; return false; }
     int cap = a.C, w_floats = 0;
     for (int l = 0; l < a.n_layers; ++l) {
         cap = std::max(cap, a.layer[l].cin);
         a.w_smem_off[l] = w_floats; w_floats += a.layer[l].cin * 9 * a.C;
         a.b_smem_off[l] = w_floats; w_floats += a.C;
     }
-    if (a.layer[0].cin != a.in_channels + (a.action ? 1 : 0)) return false;
+    if (a.layer[0].cin != a.in_channels + (a.action ? 1 : 0)) { *why = "the first layer does not read the tower input"; return false; }
     a.cap_channels = cap; a.w_floats = w_floats;
     a.row_stride = a.W + 2; a.board_stride = cap * (a.H + 2) * (a.W + 2);
     return true;
@@ -59,10 +61,11 @@ bool small_tower_layout(SmallTowerArgs& a) {
 
 namespace {
 
-Plan make_plan(SmallTowerArgs& a, int sm_count) {
-    Plan pl{};
-    pl.ok = false;
-    if (a.n < 1 || !small_tower_layout(a)) return pl;
+// false (with the reason in *why) when the fused tower cannot take the shape
+bool make_plan(SmallTowerArgs& a, int sm_count, SmallTowerPlan& pl, const char** why) {
+    pl = SmallTowerPlan{};
+    if (a.n < 1) { *why = "empty batch"; return false; }
+    if (!small_tower_layout(a, why)) return false;
     const int cap = a.cap_channels, w_floats = a.w_floats;
     const int plane = (a.H + 2) * (a.W + 2);
     // CO = 4 only when that still gives every SM a few hundred threads
@@ -72,7 +75,7 @@ Plan make_plan(SmallTowerArgs& a, int sm_count) {
     int P = a.W;
     if (CO == 1 && a.W >= 4 && a.W % 2 == 0 && (a.C / CO) * a.H * 2 <= kMaxThreads) P = a.W / 2;
     const int items = (a.C / CO) * a.H * (a.W / P);
-    if (items > kMaxThreads) return pl;
+    if (items > kMaxThreads) { *why = "one board needs more threads than a CTA holds"; return false; }
     auto bytes = [&](int boards) { return ((size_t)w_floats + 2ull * boards * cap * plane) * 4; };
     // c CTAs per SM, each with as many boards as its threads and its share of shared memory allow: take the split that
     // keeps most of an SM's share of the batch in flight at once (ties: fewer CTAs, the weights are staged per CTA)
@@ -86,7 +89,7 @@ Plan make_plan(SmallTowerArgs& a, int sm_count) {
         const int cover = std::min(c * nb_c, want);
         if (cover > best_cover) { best_cover = cover; best_c = c; best_nb = nb_c; }
     }
-    if (best_c == 0) return pl;
+    if (best_c == 0) { *why = "the weights and one board exceed shared memory"; return false; }
     // persistent grid; spread the boards evenly over the resident CTAs
     int nb = best_nb;
     int grid = sm_count * best_c;
@@ -94,13 +97,12 @@ Plan make_plan(SmallTowerArgs& a, int sm_count) {
     nb = std::min(nb, (a.n + grid * rounds - 1) / (grid * rounds));
     grid = std::min((a.n + nb - 1) / nb, grid);
     a.boards_per_cta = nb; a.cap_channels = cap; a.w_floats = w_floats;
-    pl.P = P; pl.CO = CO; pl.nb = nb; pl.threads = ((nb * items + 31) / 32) * 32; pl.grid = grid; pl.smem = bytes(nb);
-    pl.ok = true;
-    return pl;
+    pl.P = P; pl.CO = CO; pl.boards_per_cta = nb; pl.threads = ((nb * items + 31) / 32) * 32; pl.grid = grid; pl.smem = bytes(nb);
+    return true;
 }
 
 template <int P, int CO>
-cudaError_t launch(const SmallTowerArgs& a, const Plan& pl, cudaStream_t stream) {
+cudaError_t launch(const SmallTowerArgs& a, const SmallTowerPlan& pl, cudaStream_t stream) {
     static size_t attr = 0;
     if (attr < pl.smem) {
         cudaError_t e = cudaFuncSetAttribute(small_tower_kernel<P, CO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
@@ -113,13 +115,20 @@ cudaError_t launch(const SmallTowerArgs& a, const Plan& pl, cudaStream_t stream)
 }  // namespace
 
 bool small_tower_supported(const SmallTowerArgs& a) {
-    SmallTowerArgs copy = a;
-    return make_plan(copy, 132).ok;
+    SmallTowerPlan pl;
+    return small_tower_plan(a, 132, &pl, nullptr);      // (whether a plan exists does not depend on the SM count)
 }
 
-cudaError_t launch_small_tower(SmallTowerArgs a, int sm_count, cudaStream_t stream) {
-    const Plan pl = make_plan(a, sm_count);
-    if (!pl.ok) return cudaErrorInvalidValue;
+bool small_tower_plan(SmallTowerArgs a, int sm_count, SmallTowerPlan* plan, const char** why) {
+    const char* dummy;
+    return make_plan(a, sm_count, *plan, why ? why : &dummy);
+}
+
+cudaError_t launch_small_tower(SmallTowerArgs a, int sm_count, cudaStream_t stream, SmallTowerPlan* used) {
+    SmallTowerPlan pl;
+    const char* why;
+    if (!make_plan(a, sm_count, pl, &why)) return cudaErrorInvalidValue;
+    if (used) *used = pl;
 #define MZ_ST(PP)                                                                             \
     if (pl.P == PP) return pl.CO == 4 ? launch<PP, 4>(a, pl, stream) : launch<PP, 1>(a, pl, stream);
     MZ_ST(2) MZ_ST(3) MZ_ST(4) MZ_ST(5) MZ_ST(6) MZ_ST(7) MZ_ST(8)

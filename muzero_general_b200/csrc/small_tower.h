@@ -35,11 +35,19 @@ struct SmallTowerArgs {
     int w_smem_off[kSmallTowerMaxLayers], b_smem_off[kSmallTowerMaxLayers];
 };
 
-// fills cap_channels, w_floats, w_smem_off, b_smem_off and the plain strides (row W + 2, board cap * plane); false when
-// the shape is outside what the kernels handle
-bool small_tower_layout(SmallTowerArgs& a);
+// Launch of small_tower_kernel<P, CO>: P pixels and CO output channels per thread, boards per CTA, threads per CTA,
+// persistent grid (a CTA takes tiles grid apart) and dynamic shared memory
+struct SmallTowerPlan { int P, CO, boards_per_cta, threads, grid; size_t smem; };
+
+// fills cap_channels, w_floats, w_smem_off, b_smem_off and the plain strides (row W + 2, board cap * plane); false (with
+// the reason in *why, when given) when the shape is outside what the kernels handle
+bool small_tower_layout(SmallTowerArgs& a, const char** why = nullptr);
 // true when the whole tower (all weights + two activation buffers of a board tile) fits on chip
 bool small_tower_supported(const SmallTowerArgs& a);
-cudaError_t launch_small_tower(SmallTowerArgs a, int sm_count, cudaStream_t stream);
+// the plan launch_small_tower takes for `a` on sm_count SMs (host only); false with the reason in *why when the fused
+// tower refuses the shape
+bool small_tower_plan(SmallTowerArgs a, int sm_count, SmallTowerPlan* plan, const char** why);
+// `used`, when given, receives the plan of the launch
+cudaError_t launch_small_tower(SmallTowerArgs a, int sm_count, cudaStream_t stream, SmallTowerPlan* used = nullptr);
 
 }  // namespace mz

@@ -582,3 +582,51 @@ def debug_conv_tower(x, weights, biases=None, mode="x3", site="prediction", acti
     if rc != 0:
         raise _lib.MzError(rc, lib.mz_last_error(None).decode())
     return out, launches.value, sat.value
+
+
+SMALL_TOWER_PLAN = ("P", "CO", "boards", "threads", "grid", "smem")
+
+
+def debug_small_tower_plan(n, in_channels, channels, H, W, blocks, stem, sm_count):
+    """Launch plan of the fused CUDA-core tower (mz_debug_small_tower_plan, host only): (a dict of P, CO, boards per CTA,
+    threads, grid and smem, "") or (None, the reason) when the fused tower refuses the shape.  ``in_channels``: planes
+    the stem reads (C + 1 for the dynamics stem); without a stem, ``channels``."""
+    lib = _lib.load_library()
+    out = (C.c_int64 * 6)()
+    if not lib.mz_debug_small_tower_plan(n, in_channels, channels, H, W, blocks, int(stem), sm_count, out):
+        return None, lib.mz_last_error(None).decode()
+    return dict(zip(SMALL_TOWER_PLAN, out)), ""
+
+def debug_small_tower(x, weights, biases=None, site="prediction", actions=None, A=1, parents=None, pool_stride=1, parts=1,
+                      device=0):
+    """One fused CUDA-core tower of a network call site through mz_debug_small_tower; numpy NCHW in and out.  ``weights``
+    are the convs in order ([C, cin, 3, 3]: the stem first, cin = x's planes at "representation" and C + 1 at the dynamics
+    sites, then two [C, C, 3, 3] per block), ``biases`` one [C] per conv.  ``site``: "representation", "dynamics" (plain
+    recurrent call), "dynamics_pool" (in search: game g's input in pool slot ``parents[g]`` of ``pool_stride``; ``parts``
+    ranges of the partitioned replay) or "prediction".  Returns (out [n, C, H, W], the plan of the launch as a dict)."""
+    lib = _lib.load_library()
+    x = numpy.ascontiguousarray(x, numpy.float32)
+    n, cin, H, W = x.shape
+    stem = site != "prediction"
+    ch = numpy.shape(weights[0])[0]
+    if (len(weights) - stem) % 2 != 0 or (site != "representation" and cin != ch):
+        raise ValueError(f"{cin} input planes / {len(weights)} convs do not make a {ch}-channel tower at site {site}")
+    for i, w in enumerate(weights):
+        want = (ch, (cin + (site != "representation") if stem else ch) if i == 0 else ch, 3, 3)
+        if numpy.shape(w) != want:
+            raise ValueError(f"conv {i}: weights {numpy.shape(w)}, expected {want}")
+    wcat = numpy.ascontiguousarray(numpy.concatenate([numpy.asarray(w, numpy.float32).reshape(-1) for w in weights]))
+    b = None if biases is None else numpy.ascontiguousarray(numpy.stack(biases), numpy.float32)
+    if b is not None and b.shape != (len(weights), ch):
+        raise ValueError(f"biases {b.shape} do not fit {len(weights)} convs")
+    act = None if actions is None else numpy.ascontiguousarray(actions, numpy.int32)
+    par = None if parents is None else numpy.ascontiguousarray(parents, numpy.int32)
+    out = numpy.empty((n, ch, H, W), numpy.float32)
+    plan = (C.c_int64 * 6)()
+    rc = lib.mz_debug_small_tower(device, n, cin, ch, H, W, (len(weights) - stem) // 2, TOWER_SITES[site], parts, A,
+                                  x.ctypes.data, wcat.ctypes.data, None if b is None else b.ctypes.data,
+                                  None if act is None else act.ctypes.data, None if par is None else par.ctypes.data,
+                                  pool_stride, out.ctypes.data, plan)
+    if rc != 0:
+        raise _lib.MzError(rc, lib.mz_last_error(None).decode())
+    return out, dict(zip(SMALL_TOWER_PLAN, plan))

@@ -405,15 +405,57 @@ def test_partitioned_replay_does_not_change_results(name, n, N, parts, game_conf
     assert (b.visit_counts.sum(1) == N).all()
 
 
-@pytest.mark.parametrize("name,n,N", [("tictactoe", 1, 25), ("tictactoe", 700, 50), ("tictactoe", 3001, 12), ("tictactoe", 8192, 10), ("breakout", 5, 20), ("breakout", 300, 12)])
+# TicTacToe configs with other boards and action spaces (16 channels, 1 block, heads of 4 reduced channels and 16 hidden
+# units, so that several 6x6 games fit in a CTA) for the fused search's instantiations (P, CO, G): G = 4 lanes per game
+# for |A| <= 4, 16 up to |A| = 16; P = 3 on 3-wide boards, and on 6-wide ones with CO = 1 (half rows); P = 6 with CO = 4
+# on 6-wide boards.  "co4" sizes the batch with the planner: the smallest batch that gets CO = 4 on this device, plus 3.
+SEARCH_BOARDS = {"ss_3x3_a9": (3, 3, 9), "ss_3x3_a4": (3, 3, 4), "ss_6x6_a4": (6, 6, 4), "ss_6x6_a16": (6, 6, 16)}
+SEARCH_HEADS = dict(reduced_channels_reward=4, reduced_channels_value=4, reduced_channels_policy=4,
+                    resnet_fc_reward_layers=[16], resnet_fc_value_layers=[16], resnet_fc_policy_layers=[16])
+
+
+def _search_board_config(name):
+    from netcases import NetCase, make_config
+    h, w, a = SEARCH_BOARDS[name]
+    return make_config(NetCase(name, "tictactoe", "small_search", dict(observation_shape=(3, h, w), action_space=list(range(a)),
+                                                                       channels=16, blocks=1, **SEARCH_HEADS)))
+
+
+def _small_search_plan(spec, n, S):
+    import ctypes
+    from muzero_general_b200 import _lib
+    from netcases import small_search_inputs
+    p = small_search_inputs(spec)
+    out = (ctypes.c_int64 * 8)()
+    if not _lib.load_library().mz_debug_small_search_plan(p["H"], p["W"], p["C"], p["A"], n, S, p["tower"], p["heads"],
+                                                           p["scratch"], p["cap"], out):
+        return None
+    return tuple(out[:3])          # (P, CO, G)
+
+
+@pytest.mark.parametrize("name,n,N", [("tictactoe", 1, 25), ("tictactoe", 700, 50), ("tictactoe", 3001, 12), ("tictactoe", 8192, 10),
+                                      ("breakout", 5, 20), ("breakout", 300, 12),
+                                      ("ss_3x3_a9", 7, 20), ("ss_3x3_a9", "co4", 8), ("ss_3x3_a4", "co4", 8),
+                                      ("ss_6x6_a4", 5, 16), ("ss_6x6_a4", "co4", 8), ("ss_6x6_a16", "co4", 8)])
 def test_fused_small_search_equals_stepwise_pipeline(name, n, N, game_configs, monkeypatch):
     """Small residual networks run ALL simulations of a search in one launch (csrc/small_search.cu): a CTA takes its
     games through dynamics tower -> reward head + rescale -> prediction tower -> value / policy heads -> tree step with the
     very device functions of the stand-alone kernels.  Visit counts, root values, value ranges, tree depths and the
-    exported trees (hidden states included) equal the step-wise pipeline's (MZ_SMALL_SEARCH=0), bit for bit."""
-    cfg = game_configs[name]
+    exported trees (hidden states included) equal the step-wise pipeline's (MZ_SMALL_SEARCH=0), bit for bit.  The
+    ss_* cases reach all six instantiations (P, CO, G) of the kernel; each asserts the one the planner gives it."""
+    import torch
+    S = torch.cuda.get_device_properties(0).multi_processor_count
+    cfg = _search_board_config(name) if name in SEARCH_BOARDS else game_configs[name]
     spec = netspec_from_config(cfg)
     A = spec.action_space
+    co4 = n == "co4"
+    if co4:
+        n = next(m for m in range(1, 20000) if (_small_search_plan(spec, m, S) or (0, 0))[1] == 4) + 3
+    inst = _small_search_plan(spec, n, S)
+    print(f"[fused small search] {name} n={n}: (P, CO, G) = {inst} on {S} SMs")
+    if name in SEARCH_BOARDS:
+        G = 4 if A <= 4 else 16
+        assert inst == ((spec.hidden_hw[1], 4, G) if co4 else (3, 1, G)), (name, n, inst)
     rs = numpy.random.RandomState(5)
     obs = rs.random_sample((n, spec.obs_elems)).astype(numpy.float32)
     noise = rs.dirichlet([cfg.root_dirichlet_alpha] * A, size=n)
