@@ -302,6 +302,45 @@ int mz_debug_small_tower(int device, int32_t n, int32_t in_channels, int32_t C, 
                          int32_t parts, int32_t A, const float* x, const float* w, const float* bias, const int32_t* action,
                          const int32_t* parent, int32_t pool_stride, float* out, int64_t* plan);
 
+/* Routes of the residual heads (route argument of mz_debug_heads_plan and mz_debug_heads, plan[0]).  The network always
+ * takes MZ_HEADS_PLANNED: heads_kernel<32> (one warp per sample) when C*H*W <= 1024, heads_kernel<128> (128 threads per
+ * sample) otherwise, the generic route (one plain kernel per stage) when the head weights and one sample's tile exceed
+ * shared memory. */
+#define MZ_HEADS_PLANNED 0
+#define MZ_HEADS_WARP 1             /* heads_kernel<32> */
+#define MZ_HEADS_WIDE 2             /* heads_kernel<128> */
+#define MZ_HEADS_GENERIC 3          /* big_*_kernel: dense states, one range only */
+/* State layouts of a heads call (layout argument): dense NCHW fp32, or the tensor-core board layout (64 channels, boards up to
+ * 6 x 7) of one fp16 plane or of split fp16 planes x = x_h + x_l / 2^11 */
+#define MZ_LAYOUT_DENSE 0
+#define MZ_LAYOUT_F16 1
+#define MZ_LAYOUT_SPLIT 2
+
+/* Launch plan of one heads call (host only) of the samples [g0, g0 + n) at a call site (MZ_TOWER_REPRESENTATION: rescale
+ * only; MZ_TOWER_DYNAMICS / MZ_TOWER_DYNAMICS_POOL: reward head + rescale; MZ_TOWER_PREDICTION: value + policy heads) of C
+ * channels on an H x W board.  shapes holds one row of 3 + MZ_MAX_LAYERS int32 per head of the site: {reduced channels,
+ * logits, hidden layers, hidden widths...}; the first head of a site is scalarised, so its logits are 2 S + 1.  Fills plan[5]
+ * = {route (MZ_HEADS_WARP / _WIDE / _GENERIC), groups per CTA, threads per CTA, grid, dynamic shared-memory bytes; the last
+ * four 0 on the generic route} and returns 1; returns 0 with the reason in mz_last_error(NULL) when the shape or the forced
+ * route is refused (the generic route on a board layout or with g0 != 0, a forced group that does not fit). */
+int mz_debug_heads_plan(int32_t n, int32_t g0, int32_t C, int32_t H, int32_t W, int32_t site, int32_t layout, int32_t route,
+                        const int32_t* shapes, int32_t sm_count, int64_t* plan);
+
+/* Debug / parity: the heads call of one call site of resnet_inference (models.py:530-553 rescale, conv1x1 -> flatten -> MLP
+ * with ELU -> logits, models.py:645-666 support_to_scalar) on host NCHW fp32 data x [n][C][H][W], encoded into `layout`,
+ * through the helper the network calls.  The heads are packed from `tensors`: "h<i>.conv.weight" [rc][C] and ".bias" [rc],
+ * "h<i>.fc.<2l>.weight" [out][in] and ".bias" [out] as in the reference state_dict, shaped by `shapes` (as above).  `parts`
+ * (1..4, MZ_TOWER_DYNAMICS_POOL only) runs the samples in the ranges of the partitioned replay.  Outputs (NULL: not copied
+ * back), each filled with NaN bytes before the launch: logits0 / logits1 [n][logits] of the site's heads, scalar [2][n]
+ * (row 0 the first head's support_to_scalar), and at the rescaling sites rescaled [n][C][H][W], pool [n][pool_stride][state]
+ * (the rescaled state in slot out_slot, 0 <= out_slot < pool_stride, in the layout: C*H*W floats dense, 2048 floats of
+ * fp16 or 4096 of split fp16 per board) and, on the board layouts, state [n][state] (the prediction tower's input).  plan gets
+ * the plan of the launch (of the first range).  MZ_EUNSUPPORTED when a range's plan is refused. */
+int mz_debug_heads(int device, int32_t n, int32_t C, int32_t H, int32_t W, int32_t site, int32_t layout, int32_t route,
+                   int32_t parts, const int32_t* shapes, const MzTensor* tensors, int32_t n_tensors, const float* x,
+                   int32_t pool_stride, int32_t out_slot, float* logits0, float* logits1, float* scalar, float* rescaled,
+                   float* pool, float* state, int64_t* plan);
+
 /* Arithmetic the handle's search path computes in, e.g. "f32 nets + f64 tree statistics" (bench.py's dtype). */
 const char* mz_numerics(const MzHandle* h);
 

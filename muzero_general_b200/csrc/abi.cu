@@ -965,3 +965,27 @@ extern "C" int mz_debug_small_tower(int device, int32_t n, int32_t in_channels, 
     if (rc) return fail(nullptr, rc, "mz_debug_small_tower: " + e);
     return MZ_OK;
 }
+
+extern "C" int mz_debug_heads_plan(int32_t n, int32_t g0, int32_t C, int32_t H, int32_t W, int32_t site, int32_t layout, int32_t route,
+                                   const int32_t* shapes, int32_t sm_count, int64_t* plan) {
+    if (!plan || sm_count < 1) return fail(nullptr, 0, "mz_debug_heads_plan: bad argument");
+    std::string e;
+    if (!resnet_heads_plan(n, g0, C, H, W, site, layout, route, shapes, sm_count, plan, &e)) return fail(nullptr, 0, "mz_debug_heads_plan: " + e);
+    return 1;
+}
+
+// debug: the heads of one call site of the network (host NCHW in, every output back)
+extern "C" int mz_debug_heads(int device, int32_t n, int32_t C, int32_t H, int32_t W, int32_t site, int32_t layout, int32_t route,
+                              int32_t parts, const int32_t* shapes, const MzTensor* tensors, int32_t n_tensors, const float* x,
+                              int32_t pool_stride, int32_t out_slot, float* logits0, float* logits1, float* scalar, float* rescaled,
+                              float* pool, float* state, int64_t* plan) {
+    if (!x || (n_tensors > 0 && !tensors)) return fail(nullptr, MZ_EINVAL, "mz_debug_heads: bad argument");
+    if (cudaSetDevice(device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_heads: no such device");
+    cudaDeviceProp prop;
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_heads: device query failed");
+    std::string e;
+    int rc = resnet_debug_heads(n, C, H, W, site, layout, route, parts, shapes, tensors, n_tensors, x, pool_stride, out_slot, logits0,
+                                logits1, scalar, rescaled, pool, state, plan, prop.multiProcessorCount, &e);
+    if (rc) return fail(nullptr, rc, "mz_debug_heads: " + e);
+    return MZ_OK;
+}

@@ -93,7 +93,8 @@ __device__ __forceinline__ void heads_one_sample(const HeadsArgs& a, const float
     float* s_part = s_sc + C;                                        // [2][2][C] partial extrema
     float* s_act = s_part + 4 * C;                                   // per head: ping | pong
     constexpr int cj = 8;                                            // 8-channel chunks per position (board layout: C = 64)
-    // i / HW without a division: __umulhi(i, ceil(2^32 / HW)) is exact for 2 <= HW <= 1024 and i < 2^17 (checked exhaustively)
+    // i / HW without a division: __umulhi(i, ceil(2^32 / HW)) is exact for every HW and index a group's tile can hold
+    // (tests/test_heads_plan_cpu.py::test_hw_inv_division_is_exact_for_every_index_heads_kernel_takes)
     const unsigned hw_inv = a.hw_inv;                                // filled by the host (0: HW == 1)
     auto div_hw = [&](int i) { return hw_inv ? (int)__umulhi((unsigned)i, hw_inv) : i; };
     const int c_shift = (C & (C - 1)) == 0 ? 31 - __clz(C) : -1;     // C is a power of two for every bundled network

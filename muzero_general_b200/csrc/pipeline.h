@@ -107,6 +107,14 @@ bool resnet_small_tower_plan(int n, int in_channels, int C, int H, int W, int bl
 int resnet_debug_small_tower(int n, int in_channels, int C, int H, int W, int blocks, int site, int parts, int A, const float* x,
                              const float* w, const float* bias, const int32_t* action, const int32_t* parent, int pool_stride,
                              float* out, int64_t* plan, int sm_count, std::string* err);
+// Host-only plan of one heads call (plan[5], see include/mzb200.h, mz_debug_heads_plan) and the debug / parity entry behind
+// mz_debug_heads: the heads of one call site of resnet_inference on host NCHW data, in any of the three state layouts
+bool resnet_heads_plan(int n, int g0, int C, int H, int W, int site, int layout, int route, const int32_t* shapes, int sm_count,
+                       int64_t* plan, std::string* err);
+int resnet_debug_heads(int n, int C, int H, int W, int site, int layout, int route, int parts, const int32_t* shapes,
+                       const MzTensor* tensors, int n_tensors, const float* x, int pool_stride, int out_slot, float* logits0,
+                       float* logits1, float* scalar, float* rescaled, float* pool, float* state, int64_t* plan, int sm_count,
+                       std::string* err);
 // fused search of small residual networks: all simulations in one launch (small_search.cu); MZ_SMALL_SEARCH=0 / 1 switches it off / on
 bool resnet_small_search_supported(ResNetDevice* r, const InferCall& first_recurrent, const TreeStepArgs& tree, int n_sims);
 int resnet_small_search(ResNetDevice* r, const InferCall& first_recurrent, const TreeStepArgs& tree, int n_sims, cudaStream_t stream,

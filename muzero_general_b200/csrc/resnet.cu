@@ -236,8 +236,12 @@ __global__ void __launch_bounds__(kHeadThreads) heads_kernel(const __grid_consta
 // ------------------------------------------------------------------------------------------
 // Generic heads for nets whose head weights do not fit in shared memory (games/atari.py: 256 reduced channels x 36
 // positions -> FC 9216 -> 256 -> 256 -> 601, 9.4 MB for the first FC layer alone): the same operations as heads_kernel,
-// one plain kernel per stage, every dot product accumulated in the same ascending order (so the two routes agree bit
-// for bit where both apply).  Throughput is not the point here - availability of the large configuration is.
+// one plain kernel per stage, every dot product accumulated in ascending order from the bias.  The two routes agree bit
+// for bit on the rescaled state always; on the logits of a layer where heads_kernel adds with one lane per output
+// (heads_kernel<128>, and heads_kernel<32> where the split-K width ks is 1); on the scalar where heads_kernel reduces it
+// with 32 lanes (heads_kernel<128>, and heads_kernel<32> with one head per warp) - not where two heads share a warp, 16
+// lanes each (tests/test_heads_gpu.py::test_forced_routes_agree).  Throughput is not the point here - availability of the
+// large configuration is.
 // ------------------------------------------------------------------------------------------
 __global__ void big_rescale_kernel(const float* x, int n, int C, int HW, float* rescaled, float* pool_hidden, int pool_stride, int out_slot) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;           // (sample, channel)
@@ -809,11 +813,16 @@ int resnet_load_weights(ResNetDevice* r, const MzTensor* tensors, int n, std::st
     return MZ_OK;
 }
 
+// launch plan of one heads call (Runner::plan_heads); groups / threads / grid / smem are 0 on the generic route
+struct HeadsPlan { int route = 0, groups = 0, threads = 0, grid = 0; size_t smem = 0; };
+
 namespace {
 struct Runner {
     ResNetDevice* r; cudaStream_t stream; int64_t* launches; std::string* err; int n;
     int g0 = 0;                // games [g0, g0 + n) of the batch (partitioned replay); buffers are addressed by the global index
     SmallTowerPlan* small_plan = nullptr;   // when set, small_tower reports the plan of its launch here (mz_debug_small_tower)
+    int heads_route = MZ_HEADS_PLANNED;     // mz_debug_heads only: force a heads route; the network never sets it
+    HeadsPlan* heads_plan_out = nullptr;    // when set, heads reports the plan of its launch here (mz_debug_heads)
     bool fail(const char* what, cudaError_t e) { *err = std::string(what) + ": " + cudaGetErrorString(e); return false; }
 
     // conv: in -> out. `in` may be gathered from the pool; action adds the constant plane.
@@ -1134,24 +1143,49 @@ struct Runner {
         return a;
     }
 
-    bool heads(const float* x, int n_heads, const HeadDesc* h0, const HeadDesc* h1, float* l0, float* l1, float* s0, float* s1,
-               float* rescaled, float* pool_hidden, int pool_stride, int out_slot, bool p64c4 = false, float* state_p64c4 = nullptr) {
-        HeadsArgs a = heads_args(x, n_heads, h0, h1, l0, l1, s0, s1, rescaled, pool_hidden, pool_stride, out_slot, p64c4, state_p64c4);
-        const HeadDesc* hs[2] = {h0, h1};
-        // one warp per sample when a sample is small (and, for small batches, only as many groups per CTA as it takes
-        // to give every SM work); 128 threads per sample otherwise
-        const bool narrow = a.C * a.HW <= 1024 && n_heads <= 2;
+    // Launch plan of one heads call (host only; the launch and mz_debug_heads_plan both take it from here).  One warp per
+    // sample when a sample is small, 128 threads per sample otherwise; only as many groups per CTA as it takes to give
+    // every SM work (1024 Connect4 boards: 147 CTAs x 7 groups, not 128 x 8), fewer while the weights and the groups' tiles
+    // exceed shared memory; the generic route (dense layout, one range) when even one group does not fit.  heads_route
+    // forces a route; false with the reason in *err when the forced route cannot take the call.
+    bool plan_heads(const HeadsArgs& a, HeadsPlan* p) const {
+        *p = HeadsPlan{};
+        if (heads_route == MZ_HEADS_GENERIC) {
+            if (a.p64c4) { *err = "heads: the generic route reads dense states only, not the tensor-core board layout"; return false; }
+            if (a.g0 != 0) { *err = "heads (generic route): partitioned calls are not supported"; return false; }
+            p->route = MZ_HEADS_GENERIC;
+            return true;
+        }
+        const bool narrow = heads_route == MZ_HEADS_PLANNED ? a.C * a.HW <= 1024 && a.n_heads <= 2 : heads_route == MZ_HEADS_WARP;
         const int group = narrow ? 32 : 128;
         int groups = kHeadThreads / group;
-        // only as many groups per CTA as it takes to give every SM work (1024 Connect4 boards: 147 CTAs x 7 groups, not 128 x 8)
         groups = std::max(1, std::min(groups, (n + r->sm_count - 1) / r->sm_count));
         size_t smem = ((size_t)a.w_floats + (size_t)groups * a.warp_floats) * 4;
         while (groups > 1 && smem > 227 * 1024) { --groups; smem = ((size_t)a.w_floats + (size_t)groups * a.warp_floats) * 4; }
         if (smem > 227 * 1024) {
-            if (p64c4) { *err = "heads: weights + tiles exceed shared memory"; return false; }
-            return heads_big(x, n_heads, hs, l0, l1, s0, s1, rescaled, pool_hidden, pool_stride, out_slot);
+            if (heads_route != MZ_HEADS_PLANNED) { *err = "heads: the forced group's weights + tile exceed shared memory"; return false; }
+            if (a.p64c4) { *err = "heads: weights + tiles exceed shared memory"; return false; }
+            if (a.g0 != 0) { *err = "heads (generic route): partitioned calls are not supported"; return false; }
+            p->route = MZ_HEADS_GENERIC;
+            return true;
         }
-        const int threads = groups * group;
+        p->route = narrow ? MZ_HEADS_WARP : MZ_HEADS_WIDE;
+        p->groups = groups; p->threads = groups * group; p->smem = smem;
+        p->grid = std::min((n + groups - 1) / groups, r->sm_count);
+        return true;
+    }
+
+    bool heads(const float* x, int n_heads, const HeadDesc* h0, const HeadDesc* h1, float* l0, float* l1, float* s0, float* s1,
+               float* rescaled, float* pool_hidden, int pool_stride, int out_slot, bool p64c4 = false, float* state_p64c4 = nullptr) {
+        HeadsArgs a = heads_args(x, n_heads, h0, h1, l0, l1, s0, s1, rescaled, pool_hidden, pool_stride, out_slot, p64c4, state_p64c4);
+        const HeadDesc* hs[2] = {h0, h1};
+        HeadsPlan plan;
+        if (!plan_heads(a, &plan)) return false;
+        if (heads_plan_out) *heads_plan_out = plan;
+        if (plan.route == MZ_HEADS_GENERIC) return heads_big(x, n_heads, hs, l0, l1, s0, s1, rescaled, pool_hidden, pool_stride, out_slot);
+        const bool narrow = plan.route == MZ_HEADS_WARP;
+        const size_t smem = plan.smem;
+        const int threads = plan.threads, grid = plan.grid;
         static size_t attr_smem[2] = {0, 0};
         if (attr_smem[narrow] < smem) {
             cudaError_t e0 = narrow ? cudaFuncSetAttribute(heads_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
@@ -1159,8 +1193,6 @@ struct Runner {
             if (e0 != cudaSuccess) return fail("heads attr", e0);
             attr_smem[narrow] = smem;
         }
-        int grid = (n + groups - 1) / groups;
-        if (grid > r->sm_count) grid = r->sm_count;
         kt_begin(KT_HEADS, stream);
         cudaError_t e = narrow ? launch_chained(heads_kernel<32>, dim3(grid), dim3(threads), smem, stream, a)
                                : launch_chained(heads_kernel<128>, dim3(grid), dim3(threads), smem, stream, a);
@@ -1169,6 +1201,24 @@ struct Runner {
         if (e != cudaSuccess) return fail("heads launch", e);
         *launches += 1;
         return true;
+    }
+
+    // The three heads calls of resnet_inference / resnet_inference_tc (mz_debug_heads runs the same helpers).  On the
+    // tensor-core route the input and the pool are in the board layout and the rescaled state is also written into
+    // scratch_state, the prediction tower's input.  Representation: rescale only (no heads on the root state).
+    bool representation_heads(const float* x, float* hidden, float* pool_hidden, int pool_stride, int out_slot) {
+        return heads(x, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, hidden, pool_hidden, pool_stride, out_slot,
+                     r->use_tc, r->use_tc ? r->scratch_state : nullptr);
+    }
+    // Dynamics (plain API call and in search): reward head on the raw state + rescale.
+    bool dynamics_heads(const float* x, float* reward_logits, float* reward, float* hidden, float* pool_hidden, int pool_stride,
+                        int out_slot) {
+        return heads(x, 1, &r->reward_head, nullptr, reward_logits, nullptr, reward, nullptr, hidden, pool_hidden, pool_stride,
+                     out_slot, r->use_tc, r->use_tc ? r->scratch_state : nullptr);
+    }
+    // Prediction: value and policy heads on the prediction tower's output (a scalar for the value only).
+    bool prediction_heads(const float* x, float* value_logits, float* policy_logits, float* value) {
+        return heads(x, 2, &r->value_head, &r->policy_head, value_logits, policy_logits, value, nullptr, nullptr, nullptr, 0, 0, r->use_tc);
     }
 };
 }  // namespace
@@ -1199,9 +1249,7 @@ static int resnet_inference_tc(ResNetDevice* r, const InferCall& c, cudaStream_t
         if (!R.conv(r->rep_trunk[0], c.in, r->ws[0], nullptr, true, nd.obs_h, nd.obs_w, nullptr, 0, nullptr, true)) return MZ_ECUDA;
         const float* x = R.representation_tower();
         if (!x) return MZ_ECUDA;
-        if (!R.heads(x, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, c.hidden, c.pool_hidden, c.pool_stride, c.out_slot,
-                     true, state))
-            return MZ_ECUDA;
+        if (!R.representation_heads(x, c.hidden, c.pool_hidden, c.pool_stride, c.out_slot)) return MZ_ECUDA;
         if (c.reward_logits) {
             fill_root_reward_logits_kernel<<<(n * F + 255) / 256, 256, 0, stream>>>(c.reward_logits, n, F, nd.support_size);
             *launches += 1;
@@ -1223,14 +1271,11 @@ static int resnet_inference_tc(ResNetDevice* r, const InferCall& c, cudaStream_t
             x = R.dynamics_tower(c.action);
         }
         if (!x) return MZ_ECUDA;
-        if (!R.heads(x, 1, &r->reward_head, nullptr, c.reward_logits, nullptr, c.reward, nullptr, c.hidden, c.pool_hidden,
-                     c.pool_stride, c.out_slot, true, state))
-            return MZ_ECUDA;
+        if (!R.dynamics_heads(x, c.reward_logits, c.reward, c.hidden, c.pool_hidden, c.pool_stride, c.out_slot)) return MZ_ECUDA;
     }
     const float* x = R.prediction_tower();
     if (!x) return MZ_ECUDA;
-    if (!R.heads(x, 2, &r->value_head, &r->policy_head, c.value_logits, c.policy_logits, c.value, nullptr, nullptr, nullptr, 0, 0, true))
-        return MZ_ECUDA;
+    if (!R.prediction_heads(x, c.value_logits, c.policy_logits, c.value)) return MZ_ECUDA;
     return MZ_OK;
 }
 
@@ -1650,6 +1695,146 @@ int resnet_debug_small_tower(int n, int in_channels, int C, int H, int W, int bl
     return rc;
 }
 
+// The heads of one call site of the network as a ResNetDevice holds them: C channels on an H x W board, states in `layout`
+// (kLayoutDense / kLayoutF16 / kLayoutSplit), head descriptors laid out as pack_head lays them from shapes[h] = {reduced
+// channels, n_out, hidden layers, widths...}.  The representation site has no head, the dynamics sites the reward head,
+// the prediction site the value and the policy head; the first head of a site is scalarised (n_out = 2 S + 1).
+static bool debug_heads_device(ResNetDevice& r, int C, int H, int W, int site, int layout, const int32_t* shapes, int sm_count,
+                               int* n_heads, std::string* err) {
+    if (C < 4 || C % 4 || H < 1 || W < 1 || site < MZ_TOWER_REPRESENTATION || site > MZ_TOWER_PREDICTION ||
+        layout < kLayoutDense || layout > kLayoutSplit) {
+        *err = "bad shape, site or layout"; return false;
+    }
+    if (layout != kLayoutDense && (C != 64 || H > 6 || W > 7)) { *err = "the board layouts hold 64 channels on boards up to 6 x 7"; return false; }
+    *n_heads = site == MZ_TOWER_REPRESENTATION ? 0 : site == MZ_TOWER_PREDICTION ? 2 : 1;
+    if (*n_heads > 0 && !shapes) { *err = "head shapes missing"; return false; }
+    r = ResNetDevice{};
+    r.C = C; r.hh = H; r.hw = W; r.sm_count = sm_count; r.max_batch = 0;
+    r.use_tc = layout != kLayoutDense; r.split = layout == kLayoutSplit;
+    HeadDesc* dst[2] = {site == MZ_TOWER_PREDICTION ? &r.value_head : &r.reward_head, &r.policy_head};
+    size_t size = 0;
+    for (int h = 0; h < *n_heads; ++h) {
+        const int32_t* s = shapes + (size_t)h * (3 + MZ_MAX_LAYERS);
+        bool ok = s[0] >= 1 && s[1] >= 1 && s[2] >= 0 && s[2] <= MZ_MAX_LAYERS;
+        for (int l = 0; ok && l < s[2]; ++l) ok = s[3 + l] >= 1;
+        if (!ok) { *err = "bad head shape"; return false; }
+        if (h == 0 && s[1] % 2 == 0) { *err = "the scalarised head has 2 S + 1 logits"; return false; }
+        layout_head(C, s[0], H * W, s + 3, s[2], s[1], &size, *dst[h]);
+    }
+    r.net.support_size = *n_heads > 0 ? shapes[1] / 2 : 0;
+    return true;
+}
+
+// arguments of the heads launch of `site` (what the Runner helper of the site passes to Runner::heads)
+static HeadsArgs debug_heads_args(Runner& R, int site, int n_heads) {
+    ResNetDevice* r = R.r;
+    const HeadDesc* h0 = site == MZ_TOWER_PREDICTION ? &r->value_head : &r->reward_head;
+    return R.heads_args(nullptr, n_heads, n_heads > 0 ? h0 : nullptr, n_heads > 1 ? &r->policy_head : nullptr, nullptr, nullptr,
+                        nullptr, nullptr, nullptr, nullptr, 0, 0, r->use_tc);
+}
+
+// Launch plan of one heads call (host only, behind mz_debug_heads_plan): plan[5] = {route, groups per CTA, threads, grid,
+// shared-memory bytes} of the samples [g0, g0 + n) from Runner::plan_heads, the planner the launch takes; false with the
+// reason in *err when the shape or the forced route is refused.
+bool resnet_heads_plan(int n, int g0, int C, int H, int W, int site, int layout, int route, const int32_t* shapes, int sm_count,
+                       int64_t* plan, std::string* err) {
+    if (n < 1 || g0 < 0 || route < MZ_HEADS_PLANNED || route > MZ_HEADS_GENERIC) { *err = "bad batch or route"; return false; }
+    ResNetDevice r;
+    int n_heads;
+    if (!debug_heads_device(r, C, H, W, site, layout, shapes, sm_count, &n_heads, err)) return false;
+    int64_t launches = 0;
+    Runner R{&r, nullptr, &launches, err, n, g0};
+    R.heads_route = route;
+    HeadsPlan p;
+    if (!R.plan_heads(debug_heads_args(R, site, n_heads), &p)) return false;
+    const int64_t out[5] = {p.route, p.groups, p.threads, p.grid, (int64_t)p.smem};
+    for (int i = 0; i < 5; ++i) plan[i] = out[i];
+    return true;
+}
+
+// Stand-alone heads call of one call site of resnet_inference, through the same Runner helpers, on host NCHW data encoded
+// into `layout`.  Every output starts as NaN bytes (0xFF): so do the pool's other slots and the board layouts' padding.
+int resnet_debug_heads(int n, int C, int H, int W, int site, int layout, int route, int parts, const int32_t* shapes,
+                       const MzTensor* tensors, int n_tensors, const float* x, int pool_stride, int out_slot, float* logits0,
+                       float* logits1, float* scalar, float* rescaled, float* pool, float* state, int64_t* plan, int sm_count,
+                       std::string* err) {
+    ResNetDevice r;
+    int n_heads;
+    if (n < 1 || !debug_heads_device(r, C, H, W, site, layout, shapes, sm_count, &n_heads, err)) {
+        if (n < 1) *err = "bad batch";
+        return MZ_EINVAL;
+    }
+    const bool pooled = site != MZ_TOWER_PREDICTION;
+    if (parts < 1 || parts > 4 || (parts > 1 && site != MZ_TOWER_DYNAMICS_POOL)) { *err = "partitions need the in-search dynamics site, 1 to 4 of them"; return MZ_EINVAL; }
+    if (pooled && (pool_stride < 1 || out_slot < 0 || out_slot >= pool_stride)) { *err = "the rescaling sites need pool_stride >= 1 and 0 <= out_slot < pool_stride"; return MZ_EINVAL; }
+    // pack the heads from the state_dict: "h<i>.conv.{weight,bias}", "h<i>.fc.<2l>.{weight,bias}"
+    Loader L{tensors, n_tensors, err};
+    std::vector<float> blob;
+    HeadDesc* dst[2] = {site == MZ_TOWER_PREDICTION ? &r.value_head : &r.reward_head, &r.policy_head};
+    for (int h = 0; h < n_heads; ++h) {
+        const int32_t* s = shapes + (size_t)h * (3 + MZ_MAX_LAYERS);
+        const std::string p = "h" + std::to_string(h);
+        if (!pack_head(L, p + ".conv", p + ".fc", C, s[0], H * W, s + 3, s[2], s[1], blob, *dst[h])) return MZ_EINVAL;
+    }
+    // every range's plan first: a refused route is MZ_EUNSUPPORTED, not a failed launch
+    const int per = site == MZ_TOWER_DYNAMICS_POOL ? partition_games(n, parts) : n;
+    for (int g0 = 0; g0 < n; g0 += per) {
+        int64_t unused[5];
+        if (!resnet_heads_plan(std::min(per, n - g0), g0, C, H, W, site, layout, route, shapes, sm_count, unused, err)) return MZ_EUNSUPPORTED;
+    }
+    const size_t dense = (size_t)n * C * H * W;
+    const size_t elems = layout != kLayoutDense ? (size_t)conv_tc_board_elems(r.split) : (size_t)C * H * W;
+    const int n_out0 = n_heads > 0 ? shapes[1] : 0, n_out1 = n_heads > 1 ? shapes[3 + MZ_MAX_LAYERS + 1] : 0;
+    float *d_blob = nullptr, *d_x = nullptr, *d_in = nullptr, *d_l0 = nullptr, *d_l1 = nullptr, *d_sc = nullptr, *d_resc = nullptr,
+          *d_pool = nullptr, *d_state = nullptr;
+    auto cleanup = [&]() {
+        for (void* p : {(void*)d_blob, (void*)d_x, (void*)d_in, (void*)d_l0, (void*)d_l1, (void*)d_sc, (void*)d_resc, (void*)d_pool,
+                        (void*)d_state, (void*)r.big_scratch})
+            if (p) cudaFree(p);
+    };
+    auto alloc = [](float** p, size_t floats) { return cudaMalloc(p, floats * 4 + 64) == cudaSuccess && cudaMemset(*p, 0xFF, floats * 4 + 64) == cudaSuccess; };
+    const bool ok = alloc(&d_blob, blob.size()) && alloc(&d_x, dense) && alloc(&d_in, (size_t)n * elems) && alloc(&d_l0, (size_t)n * n_out0) &&
+                    alloc(&d_l1, (size_t)n * n_out1) && alloc(&d_sc, 2 * (size_t)n) && alloc(&d_resc, dense) &&
+                    alloc(&d_pool, (size_t)n * std::max(pool_stride, 1) * elems) && alloc(&d_state, (size_t)n * elems);
+    if (!ok) { cleanup(); *err = "allocation failed"; return MZ_ENOMEM; }
+    cudaMemcpy(d_blob, blob.data(), blob.size() * 4, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_x, x, dense * 4, cudaMemcpyHostToDevice);
+    if (layout != kLayoutDense) {
+        cudaMemset(d_in, 0, (size_t)n * elems * 4);                    // padding positions read as zero, as in the workspaces
+        nchw_to_p64c4_kernel<<<(unsigned)((dense + 255) / 256), 256>>>(d_x, d_in, n, C, H, W, r.split ? 1 : 0);
+    } else {
+        cudaMemcpy(d_in, x, dense * 4, cudaMemcpyHostToDevice);
+    }
+    r.d_head = d_blob; r.scratch_state = d_state;
+    int64_t launches = 0;
+    HeadsPlan used{}, first{};
+    bool good = true;
+    for (int g0 = 0; g0 < n && good; g0 += per) {
+        Runner R{&r, nullptr, &launches, err, std::min(per, n - g0), g0};
+        R.heads_route = route; R.heads_plan_out = &used;
+        if (site == MZ_TOWER_REPRESENTATION) good = R.representation_heads(d_in, d_resc, d_pool, pool_stride, out_slot);
+        else if (site == MZ_TOWER_PREDICTION) good = R.prediction_heads(d_in, d_l0, d_l1, d_sc);
+        else good = R.dynamics_heads(d_in, d_l0, d_sc, d_resc, d_pool, pool_stride, out_slot);
+        if (g0 == 0) first = used;
+    }
+    cudaError_t e = cudaDeviceSynchronize();
+    if (good && e != cudaSuccess) { good = false; *err = std::string("debug heads: ") + cudaGetErrorString(e); }
+    auto back = [&](float* host, const float* dev, size_t floats) {
+        if (host && e == cudaSuccess) e = cudaMemcpy(host, dev, floats * 4, cudaMemcpyDeviceToHost);
+    };
+    if (good) {
+        back(logits0, d_l0, (size_t)n * n_out0); back(logits1, d_l1, (size_t)n * n_out1); back(scalar, d_sc, 2 * (size_t)n);
+        if (pooled) { back(rescaled, d_resc, dense); back(pool, d_pool, (size_t)n * pool_stride * elems); }
+        if (pooled && layout != kLayoutDense) back(state, d_state, (size_t)n * elems);
+        if (e != cudaSuccess) { good = false; *err = std::string("debug heads: ") + cudaGetErrorString(e); }
+        const int64_t pl[5] = {first.route, first.groups, first.threads, first.grid, (int64_t)first.smem};
+        if (plan) for (int i = 0; i < 5; ++i) plan[i] = pl[i];
+    }
+    r.d_head = nullptr; r.scratch_state = nullptr;
+    cleanup();
+    return good ? MZ_OK : MZ_ECUDA;
+}
+
 // stored hidden states (pool layout) -> dense NCHW, device to device
 int resnet_states_to_nchw(ResNetDevice* r, const float* states, int count, float* out, cudaStream_t stream) {
     const size_t total = (size_t)count * r->C * r->hh * r->hw;
@@ -1782,8 +1967,7 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
             }
         }
         // rescale -> hidden (no heads on the raw state at the root)
-        if (!R.heads(cur, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, hidden_out, c.pool_hidden, c.pool_stride, c.out_slot))
-            return MZ_ECUDA;
+        if (!R.representation_heads(cur, hidden_out, c.pool_hidden, c.pool_stride, c.out_slot)) return MZ_ECUDA;
         if (c.reward_logits) {
             fill_root_reward_logits_kernel<<<(n * F + 255) / 256, 256, 0, stream>>>(c.reward_logits, n, F, nd.support_size);
             *launches += 1;
@@ -1802,9 +1986,7 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
             if (!R.blocks(r->dyn, 1, nd.blocks, &cur, &tmp, &spare, hh, hw)) return MZ_ECUDA;
         }
         // reward head on the raw state + rescale -> hidden
-        if (!R.heads(cur, 1, &r->reward_head, nullptr, c.reward_logits, nullptr, c.reward, nullptr, hidden_out, c.pool_hidden,
-                     c.pool_stride, c.out_slot))
-            return MZ_ECUDA;
+        if (!R.dynamics_heads(cur, c.reward_logits, c.reward, hidden_out, c.pool_hidden, c.pool_stride, c.out_slot)) return MZ_ECUDA;
     }
     // prediction on the rescaled state
     {
@@ -1822,8 +2004,7 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
             if (!R.blocks(r->pred, 2, nd.blocks - 1, &pc, &pt, &ps, hh, hw)) return MZ_ECUDA;
             x = pc;
         }
-        if (!R.heads(x, 2, &r->value_head, &r->policy_head, c.value_logits, c.policy_logits, c.value, nullptr, nullptr, nullptr, 0, 0))
-            return MZ_ECUDA;
+        if (!R.prediction_heads(x, c.value_logits, c.policy_logits, c.value)) return MZ_ECUDA;
     }
     return MZ_OK;
 }

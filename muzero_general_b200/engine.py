@@ -630,3 +630,89 @@ def debug_small_tower(x, weights, biases=None, site="prediction", actions=None, 
     if rc != 0:
         raise _lib.MzError(rc, lib.mz_last_error(None).decode())
     return out, dict(zip(SMALL_TOWER_PLAN, plan))
+
+
+HEADS_ROUTES = {"planned": 0, "warp": 1, "wide": 2, "generic": 3}
+HEADS_ROUTE_NAMES = {1: "warp", 2: "wide", 3: "generic"}
+LAYOUTS = {"dense": 0, "f16": 1, "split": 2}
+HEADS_PLAN = ("route", "groups", "threads", "grid", "smem")
+
+
+def _head_shapes(shapes, site):
+    """int32 rows {reduced channels, logits, hidden layers, widths...} of (rc, hidden widths, n_out) head shapes."""
+    want = {"representation": 0, "prediction": 2}.get(site, 1)
+    if len(shapes) != want:
+        raise ValueError(f"site {site} has {want} heads, got {len(shapes)}")
+    rows = numpy.zeros((max(len(shapes), 1), 3 + _lib.MZ_MAX_LAYERS), numpy.int32)
+    for i, (rc, hidden, n_out) in enumerate(shapes):
+        if len(hidden) > _lib.MZ_MAX_LAYERS:
+            raise ValueError(f"head {i}: {len(hidden)} hidden layers, at most {_lib.MZ_MAX_LAYERS}")
+        rows[i, :3] = (rc, n_out, len(hidden))
+        rows[i, 3:3 + len(hidden)] = hidden
+    return rows
+
+
+def debug_heads_plan(n, channels, H, W, heads, site, layout="dense", route="planned", g0=0, sm_count=132):
+    """Launch plan of one heads call (mz_debug_heads_plan, host only): (a dict of route ("warp" = heads_kernel<32>, "wide" =
+    heads_kernel<128>, "generic"), groups per CTA, threads, grid and smem, "") or (None, the reason) when the shape or the
+    forced ``route`` is refused.  ``heads``: the (reduced channels, hidden widths, logits) of the site's heads - none at
+    "representation", the reward head at "dynamics" / "dynamics_pool", value then policy at "prediction"."""
+    lib = _lib.load_library()
+    rows = _head_shapes(heads, site)
+    out = (C.c_int64 * 5)()
+    if not lib.mz_debug_heads_plan(n, g0, channels, H, W, TOWER_SITES[site], LAYOUTS[layout], HEADS_ROUTES[route],
+                                   rows.ctypes.data, sm_count, out):
+        return None, lib.mz_last_error(None).decode()
+    plan = dict(zip(HEADS_PLAN, out))
+    plan["route"] = HEADS_ROUTE_NAMES[plan["route"]]
+    return plan, ""
+
+
+def debug_heads(x, heads, site, layout="dense", route="planned", parts=1, pool_stride=1, out_slot=0, device=0):
+    """The heads call of one network call site through mz_debug_heads; numpy in and out.  ``x`` [n, C, H, W] (dense; encoded
+    into ``layout`` by the entry).  ``heads``: one dict per head of the site (see debug_heads_plan) with "conv_w" [rc, C],
+    "conv_b" [rc] and "fc", a list of (weight [out, in], bias [out]) as in the reference state_dict.  Returns a dict: "logits"
+    (one [n, n_out] per head), "scalar" [2, n], and at the rescaling sites "rescaled" [n, C, H, W], "pool" (float32
+    [n, pool_stride, state floats]) and on the board layouts "state" [n, state floats]; "plan" as debug_heads_plan gives it.
+    Outputs the kernels do not write keep the NaN bytes they start with."""
+    lib = _lib.load_library()
+    x = numpy.ascontiguousarray(x, numpy.float32)
+    n, ch, H, W = x.shape
+    shapes, keep, tensors = [], [], []
+    for i, h in enumerate(heads):
+        conv_w = numpy.ascontiguousarray(h["conv_w"], numpy.float32)
+        shapes.append((conv_w.shape[0], [numpy.shape(w)[0] for w, _ in h["fc"][:-1]], numpy.shape(h["fc"][-1][0])[0]))
+        named = [(f"h{i}.conv.weight", conv_w), (f"h{i}.conv.bias", h["conv_b"])]
+        for l, (w, b) in enumerate(h["fc"]):
+            named += [(f"h{i}.fc.{2 * l}.weight", w), (f"h{i}.fc.{2 * l}.bias", b)]
+        for name, a in named:
+            a = numpy.ascontiguousarray(a, numpy.float32)
+            keep.append(a)
+            tensors.append((name.encode(), a))
+    arr = (_lib.MzTensor * max(len(tensors), 1))()
+    for i, (name, a) in enumerate(tensors):
+        arr[i].name, arr[i].data, arr[i].numel = name, a.ctypes.data, a.size
+    rows = _head_shapes(shapes, site)
+    logits = [numpy.empty((n, s[2]), numpy.float32) for s in shapes]
+    scalar = numpy.empty((2, n), numpy.float32)
+    pooled = site != "prediction"
+    elems = ch * H * W if layout == "dense" else (2048 if layout == "f16" else 4096)
+    rescaled = numpy.empty((n, ch, H, W), numpy.float32) if pooled else None
+    pool = numpy.empty((n, pool_stride, elems), numpy.float32) if pooled else None
+    state = numpy.empty((n, elems), numpy.float32) if pooled and layout != "dense" else None
+    plan = (C.c_int64 * 5)()
+    ptr = lambda a: None if a is None else a.ctypes.data        # noqa: E731
+    rc = lib.mz_debug_heads(device, n, ch, H, W, TOWER_SITES[site], LAYOUTS[layout], HEADS_ROUTES[route], parts, rows.ctypes.data,
+                            arr, len(tensors), x.ctypes.data, pool_stride, out_slot, ptr(logits[0] if logits else None),
+                            ptr(logits[1] if len(logits) > 1 else None), scalar.ctypes.data, ptr(rescaled), ptr(pool), ptr(state),
+                            plan)
+    if rc != 0:
+        raise _lib.MzError(rc, lib.mz_last_error(None).decode())
+    p = dict(zip(HEADS_PLAN, plan))
+    p["route"] = HEADS_ROUTE_NAMES[p["route"]]
+    out = {"logits": logits, "scalar": scalar, "plan": p}
+    if pooled:
+        out.update(rescaled=rescaled, pool=pool)
+    if state is not None:
+        out["state"] = state
+    return out
