@@ -58,7 +58,7 @@ typedef struct MzNetDesc {
     int32_t n_res_fc_reward, res_fc_reward[MZ_MAX_LAYERS];
     int32_t n_res_fc_value, res_fc_value[MZ_MAX_LAYERS];
     int32_t n_res_fc_policy, res_fc_policy[MZ_MAX_LAYERS];
-    int32_t downsample;           /* 0 = none, 1 = "resnet" (models.py:233-275) */
+    int32_t downsample;           /* 0 = none, 1 = "resnet" (models.py:233-275), 2 = "CNN" (models.py:278-297) */
 } MzNetDesc;
 
 /* The MuZeroConfig attributes MCTS reads (self_play.py:249-430). */
@@ -340,6 +340,23 @@ int mz_debug_heads(int device, int32_t n, int32_t C, int32_t H, int32_t W, int32
                    int32_t parts, const int32_t* shapes, const MzTensor* tensors, int32_t n_tensors, const float* x,
                    int32_t pool_stride, int32_t out_slot, float* logits0, float* logits1, float* scalar, float* rescaled,
                    float* pool, float* state, int64_t* plan);
+
+/* Launch plan of the DownsampleCNN stem (downsample = 2, models.py:278-297; host only) for n boards of `in` planes of H x W
+ * and C channels on sm_count SMs.  Fills plan[36] = {h, w (hidden board, ceil(H / 16) x ceil(W / 16)), mid (conv1's
+ * channels, (in + C) / 2)}, then per stage (conv1 + pool1 at plan[3], conv2 + pool2 + average at plan[19]) {kernel, stride,
+ * conv rows, conv columns, pooled rows, pooled columns, output channels per CTA, pooled rows per band, bands (grid z), boards
+ * per CTA, cin chunk, conv pixels per thread, threads per CTA, grid x, grid y, dynamic shared-memory bytes}, and returns 1;
+ * returns 0 with the reason, naming the failing stage, in mz_last_error(NULL) when the reference's module cannot run the
+ * geometry (mz_create refuses such a net). */
+int mz_debug_cnn_stem_plan(int32_t n, int32_t in, int32_t C, int32_t H, int32_t W, int32_t sm_count, int64_t* plan);
+
+/* Debug / parity: the DownsampleCNN stem alone on host NCHW fp32 data, through the launcher of the network: x
+ * [n][in][H][W]; w1 [mid][in][k][k] with k = 2 ceil(H / 16), b1 [mid], w2 [C][mid][5][5], b2 [C] as in the reference
+ * state_dict (features.0 and features.3); out [n][C][ceil(H / 16)][ceil(W / 16)], filled with NaN on the device before the
+ * launch.  plan (or NULL) gets the plan launched, as mz_debug_cnn_stem_plan fills it.  MZ_EUNSUPPORTED for a geometry the
+ * plan refuses. */
+int mz_debug_cnn_stem(int device, int32_t n, int32_t in, int32_t C, int32_t H, int32_t W, const float* x, const float* w1,
+                      const float* b1, const float* w2, const float* b2, float* out, int64_t* plan);
 
 /* Arithmetic the handle's search path computes in, e.g. "f32 nets + f64 tree statistics" (bench.py's dtype). */
 const char* mz_numerics(const MzHandle* h);

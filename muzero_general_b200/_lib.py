@@ -156,6 +156,8 @@ SYMBOLS = [
     ("mz_debug_heads_plan", C.c_int, [C.c_int32] * 8 + [C.c_void_p, C.c_int32, C.POINTER(C.c_int64)]),
     ("mz_debug_heads", C.c_int, [C.c_int] + [C.c_int32] * 8 + [C.c_void_p, C.POINTER(MzTensor), C.c_int32, C.c_void_p,
                                                               C.c_int32, C.c_int32] + [C.c_void_p] * 6 + [C.POINTER(C.c_int64)]),
+    ("mz_debug_cnn_stem_plan", C.c_int, [C.c_int32] * 6 + [C.POINTER(C.c_int64)]),
+    ("mz_debug_cnn_stem", C.c_int, [C.c_int] + [C.c_int32] * 5 + [C.c_void_p] * 6 + [C.POINTER(C.c_int64)]),
 ]
 
 _lib = None

@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "handle.h"
+#include "cnn_stem.h"
 #include "small_search.h"
 
 using namespace mz;
@@ -66,8 +67,8 @@ extern "C" int mz_create(const MzNetDesc* net, const MzSearchDesc* search, int d
         return fail(nullptr, MZ_EUNSUPPORTED, "mz_create: action_space must be in [1, 256]");
     if (net->kind != MZ_NET_FC && net->kind != MZ_NET_RESNET)
         return fail(nullptr, MZ_EUNSUPPORTED, "The network parameter should be \"fullyconnected\" or \"resnet\".");
-    if (net->kind == MZ_NET_RESNET && net->downsample > 1)
-        return fail(nullptr, MZ_EUNSUPPORTED, "downsample=\"CNN\" is not supported");
+    if (net->kind == MZ_NET_RESNET && (net->downsample < 0 || net->downsample > 2))
+        return fail(nullptr, MZ_EUNSUPPORTED, "downsample should be \"resnet\" or \"CNN\".");
 
     int n_dev = 0;
     if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev <= device)
@@ -963,6 +964,28 @@ extern "C" int mz_debug_small_tower(int device, int32_t n, int32_t in_channels, 
     int rc = resnet_debug_small_tower(n, in_channels, C, H, W, blocks, site, parts, A, x, w, bias, action, parent, pool_stride, out,
                                       plan, prop.multiProcessorCount, &e);
     if (rc) return fail(nullptr, rc, "mz_debug_small_tower: " + e);
+    return MZ_OK;
+}
+
+extern "C" int mz_debug_cnn_stem_plan(int32_t n, int32_t in, int32_t C, int32_t H, int32_t W, int32_t sm_count, int64_t* plan) {
+    if (!plan) return fail(nullptr, 0, "mz_debug_cnn_stem_plan: null plan");
+    std::string e;
+    CnnStemPlan p;
+    if (!cnn_stem_plan(n, in, C, H, W, sm_count, &p, &e)) return fail(nullptr, 0, "mz_debug_cnn_stem_plan: " + e);
+    cnn_stem_plan_export(p, plan);
+    return 1;
+}
+
+// debug: the DownsampleCNN stem alone (host NCHW in / out)
+extern "C" int mz_debug_cnn_stem(int device, int32_t n, int32_t in, int32_t C, int32_t H, int32_t W, const float* x, const float* w1,
+                                 const float* b1, const float* w2, const float* b2, float* out, int64_t* plan) {
+    if (!x || !w1 || !b1 || !w2 || !b2 || !out || n < 1) return fail(nullptr, MZ_EINVAL, "mz_debug_cnn_stem: bad argument");
+    if (cudaSetDevice(device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_cnn_stem: no such device");
+    cudaDeviceProp prop;
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_cnn_stem: device query failed");
+    std::string e;
+    int rc = cnn_stem_debug(n, in, C, H, W, x, w1, b1, w2, b2, out, plan, prop.multiProcessorCount, &e);
+    if (rc) return fail(nullptr, rc, "mz_debug_cnn_stem: " + e);
     return MZ_OK;
 }
 

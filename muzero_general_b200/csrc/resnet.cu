@@ -32,6 +32,7 @@
 #include "small_search.h"
 #include "launch.h"
 #include "conv_tc.h"
+#include "cnn_stem.h"
 #include "pipeline.h"
 
 namespace mz {
@@ -370,6 +371,7 @@ struct ResNetDevice {
     // layers in execution order
     std::vector<ConvLayer> rep_down;   // conv1, rb1 x2 (2 convs each), conv2, rb2 x3, rb3 x3   (downsample only)
     std::vector<ConvLayer> rep_trunk;  // [stem conv if no downsample] + blocks x 2
+    CnnStemWeights cnn{};              // downsample = 2: DownsampleCNN's two convs in the conv blob (cnn_stem.cu)
     std::vector<ConvLayer> dyn;        // conv + blocks x 2
     std::vector<ConvLayer> pred;       // blocks x 2
     HeadDesc reward_head, value_head, policy_head;
@@ -469,13 +471,25 @@ ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, s
     ResNetDevice* r = new ResNetDevice();
     r->net = net; r->max_batch = max_batch; r->sm_count = sm_count;
     r->C = net.channels;
-    if (net.channels % 4 != 0 || (net.downsample && (net.channels / 2) % 4 != 0)) {
-        *err = "channels must be a multiple of 4 (8 with downsample)";
+    if (net.channels % 4 != 0 || (net.downsample == 1 && (net.channels / 2) % 4 != 0)) {
+        *err = "channels must be a multiple of 4 (8 with downsample=\"resnet\")";
         delete r; return nullptr;
     }
     int H = net.obs_h, W = net.obs_w;
     size_t max_elems = (size_t)net.obs_c * H * W;
-    if (net.downsample) {
+    if (net.downsample == 2) {
+        // DownsampleCNN: every geometry the reference's module cannot run is refused here, naming the stage
+        CnnStemPlan p;
+        std::string why;
+        if (!cnn_stem_plan(max_batch, net.obs_c, net.channels, H, W, sm_count, &p, &why)) {
+            *err = "downsample=\"CNN\" (" + std::to_string(net.obs_c) + " x " + std::to_string(H) + " x " + std::to_string(W) +
+                   " observation): " + why;
+            delete r; return nullptr;
+        }
+        r->hh = p.h; r->hw = p.w;
+        max_elems = std::max(max_elems, (size_t)p.mid * p.s[0].Hp * p.s[0].Wp);
+        max_elems = std::max(max_elems, (size_t)net.channels * p.h * p.w);
+    } else if (net.downsample) {
         int h1 = conv_out(H, 2), w1 = conv_out(W, 2);
         int h2 = conv_out(h1, 2), w2 = conv_out(w1, 2);
         int h3 = conv_out(h2, 2), w3 = conv_out(w2, 2);
@@ -499,10 +513,12 @@ ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, s
         struct Shape { int cin, cout, H, W, stride; };
         const int C = net.channels, h = r->hh, w = r->hw;
         std::vector<Shape> shapes;
-        if (net.downsample) {
+        if (net.downsample == 1) {
             const int h1 = conv_out(H, 2), w1 = conv_out(W, 2), h2 = conv_out(h1, 2), w2 = conv_out(w1, 2);
             shapes = {{net.obs_c, C / 2, H, W, 2}, {C / 2, C / 2, h1, w1, 1}, {C / 2, C, h1, w1, 2}, {C, C, h2, w2, 1},
                       {C, C, conv_out(h2, 2), conv_out(w2, 2), 1}};
+        } else if (net.downsample == 2) {
+            // the stem was planned above; the representation trunk is blocks only
         } else {
             shapes = {{net.obs_c, C, H, W, 1}};
         }
@@ -778,7 +794,17 @@ int resnet_load_weights(ResNetDevice* r, const MzTensor* tensors, int n, std::st
     r->rep_down.clear(); r->rep_trunk.clear(); r->dyn.clear(); r->pred.clear();
     const std::string rp = "representation_network.module";
     bool ok = true;
-    if (nd.downsample) {
+    if (nd.downsample == 2) {
+        // DownsampleCNN (models.py:278-297): features.0 = conv1, features.3 = conv2, both with bias and no BN
+        const std::string fp = rp + ".downsample_net.features.";
+        const int k = 2 * r->hh, mid = (nd.obs_c + C) / 2;
+        const MzTensor* w1 = L.get(fp + "0.weight", (int64_t)mid * nd.obs_c * k * k);
+        const MzTensor* b1 = L.get(fp + "0.bias", mid);
+        const MzTensor* w2 = L.get(fp + "3.weight", (int64_t)C * mid * 25);
+        const MzTensor* b2 = L.get(fp + "3.bias", C);
+        ok = w1 && b1 && w2 && b2;
+        if (ok) r->cnn = cnn_stem_pack(w1->data, b1->data, w2->data, b2->data, nd.obs_c, mid, C, k, conv);
+    } else if (nd.downsample) {
         const std::string dp = rp + ".downsample_net";
         ok = ok && pack_conv(L, dp + ".conv1", "", nd.obs_c, C / 2, 2, conv, r->rep_down);
         for (int i = 0; ok && i < 2; ++i) ok = pack_resblock(L, dp + ".resblocks1." + std::to_string(i), C / 2, conv, r->rep_down);
@@ -998,6 +1024,18 @@ struct Runner {
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return fail("conv3x3 launch", e);
         *launches += 1;
+        return true;
+    }
+
+    // DownsampleCNN stem of the observations `in`: stage 1 into `pooled`, stage 2 into `out` (cnn_stem.cu)
+    bool cnn_stem(const float* in, float* pooled, float* out) {
+        CnnStemPlan p;
+        if (!cnn_stem_plan(n, r->net.obs_c, r->C, r->net.obs_h, r->net.obs_w, r->sm_count, &p, err)) return false;
+        kt_begin(KT_CONV, stream);
+        cudaError_t e = cnn_stem_launch(p, r->d_conv, r->cnn, in, pooled, out, n, stream);
+        kt_end(stream);
+        if (e != cudaSuccess) return fail("cnn stem launch", e);
+        *launches += 2;
         return true;
     }
 
@@ -1936,7 +1974,14 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
 
     if (!c.recurrent) {
         int H = nd.obs_h, W = nd.obs_w;
-        if (nd.downsample) {
+        if (nd.downsample == 2) {
+            if (!R.cnn_stem(c.in, tmp, cur)) return MZ_ECUDA;
+            H = hh; W = hw;
+            const int fused = R.small_tower(r->rep_trunk, 0, false, nd.blocks, cur, tmp, C, H, W);
+            if (fused < 0) return MZ_ECUDA;
+            if (fused) { float* t = cur; cur = tmp; tmp = t; }
+            else if (!R.blocks(r->rep_trunk, 0, nd.blocks, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
+        } else if (nd.downsample) {
             const auto& d = r->rep_down;
             if (!R.conv(d[0], c.in, cur, nullptr, false, H, W)) return MZ_ECUDA;
             H = conv_out(H, 2); W = conv_out(W, 2);

@@ -47,7 +47,7 @@ class NetSpec:
     res_fc_reward: List[int] = field(default_factory=list)
     res_fc_value: List[int] = field(default_factory=list)
     res_fc_policy: List[int] = field(default_factory=list)
-    downsample: int = 0             # 0 none, 1 "resnet" (models.py:233-275), 2 "CNN" (unsupported)
+    downsample: int = 0             # 0 none, 1 "resnet" (models.py:233-275), 2 "CNN" (models.py:278-297)
 
     @property
     def full_support(self) -> int:
@@ -173,7 +173,11 @@ def weights_spec(spec: NetSpec):
         for i in range(3):
             keys += _resblock_keys(f"{dp}.resblocks3.{i}", C)
     elif spec.downsample == 2:
-        raise NotImplementedError('downsample="CNN" (models.py:278-297) is not on any BASELINE config')
+        # DownsampleCNN (models.py:278-297): conv k x k (k = 2 * ceil(H / 16)) to (in + C) // 2 channels, conv 5 x 5 to C
+        mid, k = (spec.in_channels + C) // 2, 2 * hh
+        dp = f"{rp}.downsample_net.features"
+        keys += [(f"{dp}.0.weight", (mid, spec.in_channels, k, k)), (f"{dp}.0.bias", (mid,)),
+                 (f"{dp}.3.weight", (C, mid, 5, 5)), (f"{dp}.3.bias", (C,))]
     keys += [(f"{rp}.conv.weight", (C, spec.in_channels, 3, 3))]
     keys += _bn_keys(f"{rp}.bn", C)
     for i in range(spec.blocks):
