@@ -144,6 +144,28 @@ typedef struct MzSearchIO {
     const MzTrace* trace;         /* NULL = no trace */
 } MzSearchIO;
 
+/* Arguments of mz_search_device: the search of MzSearchIO with mem = MZ_MEM_DEVICE, flags = 0 and neither teacher nor
+ * trace.  Every pointer is device memory with the meaning of the MzSearchIO field of the same name. */
+typedef struct MzDeviceSearchIO {
+    int32_t n_games;              /* <= max_games */
+    int32_t add_exploration_noise;
+    const float* obs;             /* required */
+    const double* noise;
+    const int64_t* game_id;
+    const int32_t* move_index;
+    const uint8_t* legal_mask;
+    const int32_t* to_play;
+    const int32_t* first_index;
+    int32_t* visit_counts;
+    double* root_value;
+    float* root_predicted_value;
+    int32_t* max_tree_depth;
+    int32_t* tie_count;
+    double* root_priors;
+    double* value_range;
+    double device_ms;             /* out: mz_last_search_ms of this call */
+} MzDeviceSearchIO;
+
 #define MZ_FLAG_KEEP_TREE 1       /* leave the full tree in the HBM node pool for mz_export_tree */
 #define MZ_FLAG_STEPWISE  2       /* force the generic select/infer/expand+backup pipeline */
 #define MZ_FLAG_CONTINUE  4       /* MCTS.run(..., override_root_with=node), self_play.py:275-277: no root inference; the
@@ -190,6 +212,13 @@ int mz_load_weights(MzHandle* h, const MzTensor* tensors, int32_t n_tensors);
 
 /* replaces MCTS.run for a batch of games (self_play.py:260-361; called from self_play.py:144-150) */
 int mz_search(MzHandle* h, const MzSearchIO* io);
+/* The same search on device buffers in two calls, with less host work: mz_search_device enqueues it and returns (no
+ * staging or debug outputs; the fused FC route launches the kernel its handle prepared for the last n_games and A/B
+ * switches it saw), mz_search_device_wait waits for it and sets io->device_ms.  The outputs are complete after the wait;
+ * work the caller does in between overlaps the search.  Every mz_search_device must be followed by its wait before the
+ * next call on the handle.  Results are mz_search's. */
+int mz_search_device(MzHandle* h, MzDeviceSearchIO* io);
+int mz_search_device_wait(MzHandle* h, MzDeviceSearchIO* io);
 
 /* replaces model.initial_inference / recurrent_inference (models.py:172-195, 601-623) */
 int mz_initial_inference(MzHandle* h, int32_t n, int32_t mem, const float* obs, const MzInferenceOut* out);
@@ -213,9 +242,16 @@ int64_t mz_launch_count(const MzHandle* h);
 int32_t mz_graph_partitions(const MzHandle* h);
 /* device time of the search kernels of the last mz_search call, ms (CUDA events on the library stream) */
 double mz_last_search_ms(const MzHandle* h);
+/* host side of the last search call: out[4] = CLOCK_MONOTONIC ns (Python's time.perf_counter_ns) at its entry, when the
+ * search was enqueued, when the stream synchronisation returned, and at its return (scripts/search_host_split.py) */
+int mz_debug_host_split(const MzHandle* h, int64_t* out);
 /* shape of the handle's last launch of the fused FC search kernel (csrc/fc_search.cu): returns 1 and fills info[5] =
  * {grid, threads per CTA, lanes per game, shared-memory bytes per CTA, resident CTAs per SM}, or 0 before the first one */
 int mz_fc_last_launch(const MzHandle* h, int64_t* info);
+/* the fused FC launch the handle keeps for its next search: returns 1 and fills info[7] = {games, lanes per game, fixed
+ * CTA size (0 = planned), MZ_FC_GENERIC=1, MZ_FC_SELECT_LEVELS=1, tree levels per selection round, 1 = the fixed-shape
+ * network instantiation}, or 0 when there is none (no fused launch yet, or the weights were loaded since) */
+int mz_debug_fc_prepared(const MzHandle* h, int64_t* info);
 
 /* Per-kernel-class device timing for the roofline line of bench.py.  While enabled (process-wide), the step-wise
  * pipeline runs launch by launch with a CUDA event pair around every kernel instead of replaying its CUDA graph.

@@ -13,7 +13,7 @@ MZ_MAX_LAYERS = 8
 MZ_MAX_ACTIONS = 256
 MZ_MEM_HOST, MZ_MEM_DEVICE = 0, 1
 MZ_FLAG_KEEP_TREE, MZ_FLAG_STEPWISE, MZ_FLAG_CONTINUE = 1, 2, 4
-MZ_EUNSUPPORTED = -3
+MZ_EUNSUPPORTED, MZ_ESTATE = -3, -4
 
 _L = C.c_int32 * MZ_MAX_LAYERS
 
@@ -74,6 +74,17 @@ class MzSearchIO(C.Structure):
     ]
 
 
+class MzDeviceSearchIO(C.Structure):
+    _fields_ = [
+        ("n_games", C.c_int32), ("add_exploration_noise", C.c_int32),
+        ("obs", C.c_void_p), ("noise", C.c_void_p), ("game_id", C.c_void_p), ("move_index", C.c_void_p),
+        ("legal_mask", C.c_void_p), ("to_play", C.c_void_p), ("first_index", C.c_void_p),
+        ("visit_counts", C.c_void_p), ("root_value", C.c_void_p), ("root_predicted_value", C.c_void_p),
+        ("max_tree_depth", C.c_void_p), ("tie_count", C.c_void_p), ("root_priors", C.c_void_p),
+        ("value_range", C.c_void_p), ("device_ms", C.c_double),
+    ]
+
+
 class MzTreeExport(C.Structure):
     _fields_ = [("n_expansions", C.c_int32), ("child_visit", C.c_void_p), ("child_value_sum", C.c_void_p),
                 ("child_reward", C.c_void_p), ("child_prior", C.c_void_p), ("child_expansion", C.c_void_p),
@@ -120,6 +131,8 @@ SYMBOLS = [
     ("mz_abi_version", C.c_int, []),
     ("mz_load_weights", C.c_int, [C.c_void_p, C.POINTER(MzTensor), C.c_int32]),
     ("mz_search", C.c_int, [C.c_void_p, C.POINTER(MzSearchIO)]),
+    ("mz_search_device", C.c_int, [C.c_void_p, C.POINTER(MzDeviceSearchIO)]),
+    ("mz_search_device_wait", C.c_int, [C.c_void_p, C.POINTER(MzDeviceSearchIO)]),
     ("mz_initial_inference", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(MzInferenceOut)]),
     ("mz_recurrent_inference", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(MzInferenceOut)]),
     ("mz_export_tree", C.c_int, [C.c_void_p, C.c_int32, C.POINTER(MzTreeExport)]),
@@ -129,7 +142,9 @@ SYMBOLS = [
     ("mz_launch_count", C.c_int64, [C.c_void_p]),
     ("mz_graph_partitions", C.c_int32, [C.c_void_p]),
     ("mz_last_search_ms", C.c_double, [C.c_void_p]),
+    ("mz_debug_host_split", C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     ("mz_fc_last_launch", C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
+    ("mz_debug_fc_prepared", C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     ("mz_kernel_timing", C.c_int, [C.c_void_p, C.c_int32]),
     ("mz_kernel_times", C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
     ("mz_numerics", C.c_char_p, [C.c_void_p]),

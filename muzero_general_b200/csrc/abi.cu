@@ -242,6 +242,15 @@ extern "C" int mz_fc_last_launch(const MzHandle* h, int64_t* info) {
     return 1;
 }
 
+extern "C" int mz_debug_fc_prepared(const MzHandle* h, int64_t* info) {
+    if (!h || !info || !h->fc_launch.prepared.valid) return 0;
+    const FcPrepared& p = h->fc_launch.prepared;
+    const int64_t out[7] = {p.key.n_games, p.key.group, p.key.threads, p.key.generic, p.key.one_level, p.select_levels,
+                            p.fixed_shape};
+    for (int i = 0; i < 7; ++i) info[i] = out[i];
+    return 1;
+}
+
 // ------------------------------------------------------------------------------------------
 // weights
 // ------------------------------------------------------------------------------------------
@@ -315,6 +324,7 @@ static int load_fc_weights(MzHandle* h, const MzTensor* t, int n) {
     MZ_CUDA(h, dev_alloc(&h->d_fc_blob, blob.size()));
     MZ_CUDA(h, cudaMemcpy(h->d_fc_blob, blob.data(), blob.size() * 4, cudaMemcpyHostToDevice));
     h->fc = fc;
+    h->fc_launch.prepared.valid = false;
     return MZ_OK;
 }
 
@@ -578,8 +588,50 @@ int mz_dispatch_search(MzHandle* h, const SearchCall& call, bool teacher, bool t
     return MZ_OK;
 }
 
+// The handle's device current on the calling thread (cudaSetDevice only when another one is).
+static int use_device(MzHandle* h) {
+    int cur = -1;
+    if (cudaGetDevice(&cur) != cudaSuccess || cur != h->device) MZ_CUDA(h, cudaSetDevice(h->device));
+    return MZ_OK;
+}
+
+// Enqueues the search between the handle's two events, then the D2H copies of a host-memory call (out_bytes of the
+// output arena, the debug outputs).
+static int enqueue_search(MzHandle* h, const SearchCall& call, bool teacher, bool trace, int flags, size_t out_bytes,
+                          const std::vector<DebugOut>& dbg_outs) {
+    int rc;
+    MZ_CUDA(h, cudaEventRecord(h->ev0, h->stream));
+    if ((rc = mz_dispatch_search(h, call, teacher, trace, flags))) return rc;
+    h->host_ns[1] = mz_host_ns();
+    MZ_CUDA(h, cudaEventRecord(h->ev1, h->stream));
+    if (out_bytes) MZ_CUDA(h, cudaMemcpyAsync(h->h_out, h->d_out, out_bytes, cudaMemcpyDeviceToHost, h->stream));
+    for (const DebugOut& d : dbg_outs)
+        MZ_CUDA(h, cudaMemcpyAsync(d.user, d.dev, d.bytes, cudaMemcpyDeviceToHost, h->stream));
+    return MZ_OK;
+}
+
+// Waits for the search enqueue_search enqueued with the same arguments; a search whose tensor-core towers left the fp16
+// range is redone on the fp32 towers.  Sets last_ms.
+static int wait_search(MzHandle* h, const SearchCall& call, bool teacher, bool trace, int flags, size_t out_bytes,
+                       const std::vector<DebugOut>& dbg_outs) {
+    int rc;
+    MZ_CUDA(h, cudaStreamSynchronize(h->stream));
+    h->host_ns[2] = mz_host_ns();
+    if (h->res && !teacher && resnet_take_saturations(h->res, h->stream) > 0) {
+        // an activation left the fp16 range inside the tensor-core towers: the results above are outside the accuracy
+        // contract.  Switch this handle to the fp32 CUDA-core towers for good and redo the search.
+        mz_switch_to_strict(h);
+        if ((rc = enqueue_search(h, call, teacher, trace, flags, out_bytes, dbg_outs))) return rc;
+        MZ_CUDA(h, cudaStreamSynchronize(h->stream));
+    }
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, h->ev0, h->ev1) == cudaSuccess) h->last_ms = ms;
+    return MZ_OK;
+}
+
 extern "C" int mz_search(MzHandle* h, const MzSearchIO* io) {
     if (!h || !io) return fail(h, MZ_EINVAL, "mz_search: null argument");
+    h->host_ns[0] = mz_host_ns();
     const int n = io->n_games, N = h->search.num_simulations, A = h->net.action_space;
     if (n < 1 || n > h->search.max_games) return fail(h, MZ_EINVAL, "mz_search: n_games out of range");
     const bool teacher = io->teacher != nullptr;
@@ -592,7 +644,8 @@ extern "C" int mz_search(MzHandle* h, const MzSearchIO* io) {
         if (h->imported_expansions + h->search.num_simulations > h->pool_n + 1)
             return fail(h, MZ_EINVAL, "mz_search: the imported tree plus num_simulations exceeds the pool (raise extra_expansions)");
     }
-    MZ_CUDA(h, cudaSetDevice(h->device));
+    int rc;
+    if ((rc = use_device(h))) return rc;
 
     SearchCall call{};
     call.n = n;
@@ -628,7 +681,6 @@ extern "C" int mz_search(MzHandle* h, const MzSearchIO* io) {
         call.tie_count = io->tie_count; call.root_priors = io->root_priors; call.value_range = io->value_range;
     }
     call.add_noise = io->add_exploration_noise;
-    int rc;
     if (teacher) {
         const MzTeacher& t = *io->teacher;
         if ((rc = debug_in(h, "t.root_value", t.root_value, n, io->mem, &call.teacher.root_value))) return rc;
@@ -662,30 +714,58 @@ extern "C" int mz_search(MzHandle* h, const MzSearchIO* io) {
     }
     call.keep_tree = (io->flags & MZ_FLAG_KEEP_TREE) != 0;
 
-    MZ_CUDA(h, cudaEventRecord(h->ev0, h->stream));
-    if ((rc = mz_dispatch_search(h, call, teacher, io->trace != nullptr, io->flags))) return rc;
-    MZ_CUDA(h, cudaEventRecord(h->ev1, h->stream));
-    if (host && call.out_bytes)
-        MZ_CUDA(h, cudaMemcpyAsync(h->h_out, h->d_out, call.out_bytes, cudaMemcpyDeviceToHost, h->stream));
-    for (const DebugOut& d : dbg_outs)
-        MZ_CUDA(h, cudaMemcpyAsync(d.user, d.dev, d.bytes, cudaMemcpyDeviceToHost, h->stream));
-    MZ_CUDA(h, cudaStreamSynchronize(h->stream));
-    if (h->res && !teacher && resnet_take_saturations(h->res, h->stream) > 0) {
-        // an activation left the fp16 range inside the tensor-core towers: the results above are outside the accuracy
-        // contract.  Switch this handle to the fp32 CUDA-core towers for good and redo the search.
-        mz_switch_to_strict(h);
-        MZ_CUDA(h, cudaEventRecord(h->ev0, h->stream));
-        if ((rc = mz_dispatch_search(h, call, teacher, io->trace != nullptr, io->flags))) return rc;
-        MZ_CUDA(h, cudaEventRecord(h->ev1, h->stream));
-        if (host && call.out_bytes)
-            MZ_CUDA(h, cudaMemcpyAsync(h->h_out, h->d_out, call.out_bytes, cudaMemcpyDeviceToHost, h->stream));
-        for (const DebugOut& d : dbg_outs)
-            MZ_CUDA(h, cudaMemcpyAsync(d.user, d.dev, d.bytes, cudaMemcpyDeviceToHost, h->stream));
-        MZ_CUDA(h, cudaStreamSynchronize(h->stream));
-    }
+    const bool trace = io->trace != nullptr;
+    const size_t out_bytes = host ? call.out_bytes : 0;
+    if ((rc = enqueue_search(h, call, teacher, trace, io->flags, out_bytes, dbg_outs))) return rc;
+    if ((rc = wait_search(h, call, teacher, trace, io->flags, out_bytes, dbg_outs))) return rc;
     for (const OutSlot& s : outs) memcpy(s.user, h->h_out + s.off, s.bytes);
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, h->ev0, h->ev1) == cudaSuccess) h->last_ms = ms;
+    h->host_ns[3] = mz_host_ns();
+    return MZ_OK;
+}
+
+// The lean entry point of a search on device memory, in two calls so that the caller's own work overlaps the search:
+// mz_search_device enqueues (no staging, no debug outputs; the fused FC route goes straight to the launch its prepared
+// state holds, launch_fc_search), mz_search_device_wait waits.  Every route is mz_search's.
+extern "C" int mz_search_device(MzHandle* h, MzDeviceSearchIO* io) {
+    if (!h || !io) return fail(h, MZ_EINVAL, "mz_search_device: null argument");
+    h->host_ns[0] = mz_host_ns();
+    const int n = io->n_games;
+    if (h->device_pending) return fail(h, MZ_ESTATE, "mz_search_device: the previous search was not waited for");
+    if (n < 1 || n > h->search.max_games) return fail(h, MZ_EINVAL, "mz_search_device: n_games out of range");
+    if (!h->weights_loaded) return fail(h, MZ_ESTATE, "mz_search_device: weights not loaded");
+    if (!io->obs) return fail(h, MZ_EINVAL, "mz_search_device: obs is null");
+    int rc;
+    if ((rc = use_device(h))) return rc;
+    SearchCall& call = h->device_call;
+    call = SearchCall{};
+    call.n = n;
+    call.obs = io->obs; call.legal_mask = io->legal_mask; call.to_play = io->to_play;
+    call.add_noise = io->add_exploration_noise;
+    call.noise = io->add_exploration_noise ? io->noise : nullptr;
+    call.first_index = io->first_index; call.game_id = io->game_id; call.move_index = io->move_index;
+    call.visit_counts = io->visit_counts; call.root_value = io->root_value;
+    call.root_predicted_value = io->root_predicted_value; call.max_tree_depth = io->max_tree_depth;
+    call.tie_count = io->tie_count; call.root_priors = io->root_priors; call.value_range = io->value_range;
+    if ((rc = enqueue_search(h, call, false, false, 0, 0, {}))) return rc;
+    h->device_pending = true;
+    return MZ_OK;
+}
+
+extern "C" int mz_search_device_wait(MzHandle* h, MzDeviceSearchIO* io) {
+    if (!h || !io) return fail(h, MZ_EINVAL, "mz_search_device_wait: null argument");
+    if (!h->device_pending) return fail(h, MZ_ESTATE, "mz_search_device_wait: no search enqueued by mz_search_device");
+    h->device_pending = false;
+    int rc;
+    if ((rc = use_device(h))) return rc;
+    if ((rc = wait_search(h, h->device_call, false, false, 0, 0, {}))) return rc;
+    io->device_ms = h->last_ms;
+    h->host_ns[3] = mz_host_ns();
+    return MZ_OK;
+}
+
+extern "C" int mz_debug_host_split(const MzHandle* h, int64_t* out) {
+    if (!h || !out) return MZ_EINVAL;
+    for (int i = 0; i < 4; ++i) out[i] = h->host_ns[i];
     return MZ_OK;
 }
 

@@ -333,11 +333,16 @@ bool fc_search_plan(int N, int A, int E, int maxw, int blob_floats, int G, bool 
     return found;
 }
 
+template <int G, bool T, typename SH, int kP>
+static cudaError_t launch_kernel(const FcSearchArgs& a, const FcLaunchInfo& l, cudaStream_t stream) {
+    fc_search_kernel<G, T, SH, kP><<<l.grid, l.block, l.smem, stream>>>(a);
+    return cudaGetLastError();
+}
+
+// Picks the launch of instantiation <G, T, SH, kP> for a.n_games games into *p: selection levels, plan and grid.
 template <int G, bool T, typename SH, int kP = 0>
-static cudaError_t launch_one(const FcSearchArgs& a_in, int sm_count, FcLaunchState* st, cudaStream_t stream) {
-    FcSearchArgs a = a_in;
-    const char* one_level = getenv("MZ_FC_SELECT_LEVELS");    // A/B switch: "1" = one tree level per selection round
-    a.select_levels = (one_level && one_level[0] == '1' && one_level[1] == 0) ? 1 : select_levels_for(a.A, G);
+static cudaError_t prepare_one(const FcSearchArgs& a, bool one_level, int sm_count, FcLaunchState* st, FcPrepared* p) {
+    p->select_levels = one_level ? 1 : select_levels_for(a.A, G);
     auto kern = fc_search_kernel<G, T, SH, kP>;
     const void* fn = reinterpret_cast<const void*>(kern);
     int regs = 0;
@@ -367,32 +372,28 @@ static cudaError_t launch_one(const FcSearchArgs& a_in, int sm_count, FcLaunchSt
     if (per_sm < 1) return cudaErrorInvalidConfiguration;
     const int want = (a.n_games + plan.groups - 1) / plan.groups;
     const int grid = std::min(want, per_sm * sm_count);
-    kern<<<grid, plan.threads, plan.smem, stream>>>(a);
-    const cudaError_t err = cudaGetLastError();
-    if (err == cudaSuccess) {
-        st->launched = true;
-        st->last = FcLaunchInfo{grid, plan.threads, per_sm, G, plan.smem};
-    }
-    return err;
+    p->launch = launch_kernel<G, T, SH, kP>;
+    p->fixed_shape = SH::kEnabled;
+    p->info = FcLaunchInfo{grid, plan.threads, per_sm, G, plan.smem};
+    return cudaSuccess;
 }
 
 // shapes with a fully unrolled network path: games/cartpole.py (encoding 8, hidden 16, support 10, 2 actions)
 using CartPoleShape = FcFixedShape<8, 16, 10, 2>;
 
-cudaError_t launch_fc_search(const FcSearchArgs& a, int group, bool teacher, int sm_count, FcLaunchState* state,
-                             cudaStream_t stream) {
-    const char* generic = getenv("MZ_FC_GENERIC");             // A/B switch: always walk the layer descriptors
-    if (!teacher && !(generic && generic[0] == '1') && fc_matches_fixed<CartPoleShape>(a.net)) {
+static cudaError_t prepare_fc_search(const FcSearchArgs& a, int group, bool teacher, bool generic, bool one_level,
+                                     int sm_count, FcLaunchState* st, FcPrepared* p) {
+    if (!teacher && !generic && fc_matches_fixed<CartPoleShape>(a.net)) {
         // (a single player: the backup's value recurrence and its signs simplify)
-        if (group == 16 && a.P == 1) return launch_one<16, false, CartPoleShape, 1>(a, sm_count, state, stream);
-        if (group == 16) return launch_one<16, false, CartPoleShape>(a, sm_count, state, stream);
-        if (group == 32 && a.P == 1) return launch_one<32, false, CartPoleShape, 1>(a, sm_count, state, stream);
-        if (group == 32) return launch_one<32, false, CartPoleShape>(a, sm_count, state, stream);
+        if (group == 16 && a.P == 1) return prepare_one<16, false, CartPoleShape, 1>(a, one_level, sm_count, st, p);
+        if (group == 16) return prepare_one<16, false, CartPoleShape>(a, one_level, sm_count, st, p);
+        if (group == 32 && a.P == 1) return prepare_one<32, false, CartPoleShape, 1>(a, one_level, sm_count, st, p);
+        if (group == 32) return prepare_one<32, false, CartPoleShape>(a, one_level, sm_count, st, p);
     }
 #define MZ_CASE(GG)                                                                                     \
     case GG:                                                                                            \
-        return teacher ? launch_one<GG, true, FcGenericShape>(a, sm_count, state, stream)               \
-                       : launch_one<GG, false, FcGenericShape>(a, sm_count, state, stream);
+        return teacher ? prepare_one<GG, true, FcGenericShape>(a, one_level, sm_count, st, p)           \
+                       : prepare_one<GG, false, FcGenericShape>(a, one_level, sm_count, st, p);
     switch (group) {
         MZ_CASE(4)
         MZ_CASE(8)
@@ -401,6 +402,32 @@ cudaError_t launch_fc_search(const FcSearchArgs& a, int group, bool teacher, int
     }
 #undef MZ_CASE
     return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_fc_search(const FcSearchArgs& a_in, int group, bool teacher, int sm_count, FcLaunchState* st,
+                             cudaStream_t stream) {
+    // A/B switches, read per launch so that a caller may flip them between searches of one handle:
+    // MZ_FC_GENERIC=1 always walks the layer descriptors, MZ_FC_SELECT_LEVELS=1 resolves one tree level per round
+    const char* generic = getenv("MZ_FC_GENERIC");
+    const char* levels = getenv("MZ_FC_SELECT_LEVELS");
+    FcPreparedKey key{a_in.n_games, group, a_in.threads, teacher, generic && generic[0] == '1',
+                      levels && levels[0] == '1' && levels[1] == 0};
+    FcPrepared& p = st->prepared;
+    if (!p.valid || !(p.key == key)) {
+        p.valid = false;
+        const cudaError_t err = prepare_fc_search(a_in, group, teacher, key.generic, key.one_level, sm_count, st, &p);
+        if (err != cudaSuccess) return err;
+        p.key = key;
+        p.valid = true;
+    }
+    FcSearchArgs a = a_in;
+    a.select_levels = p.select_levels;
+    const cudaError_t err = p.launch(a, p.info, stream);
+    if (err == cudaSuccess) {
+        st->launched = true;
+        st->last = p.info;
+    }
+    return err;
 }
 
 #ifdef MZ_FC_PHASES

@@ -1,5 +1,7 @@
 // The library handle and the helpers shared by the entry-point files (abi.cu, selfplay.cu).
 #pragma once
+#include <time.h>
+
 #include <map>
 #include <string>
 #include <vector>
@@ -70,7 +72,19 @@ struct MzHandle {
     int pool_n = 0;                    // layout "N" of the node pool and tables: num_simulations + extra_expansions
     int imported_expansions = 0;       // expansions of the tree mz_import_tree seeded last (MZ_FLAG_CONTINUE)
     int range_fallbacks = 0;           // times the x3 range guard switched this handle to the fp32 towers (0 or 1)
+    // the search mz_search_device enqueued and mz_search_device_wait has not waited for yet
+    mz::SearchCall device_call{};
+    bool device_pending = false;
+    // CLOCK_MONOTONIC ns of the last search call: entry, search enqueued, stream synchronised, return
+    // (mz_debug_host_split; scripts/search_host_split.py)
+    int64_t host_ns[4] = {0, 0, 0, 0};
 };
+
+static inline int64_t mz_host_ns() {
+    timespec ts;
+    clock_gettime(CLOCK_MONOTONIC, &ts);
+    return (int64_t)ts.tv_sec * 1000000000 + ts.tv_nsec;
+}
 
 int mz_fail(MzHandle* h, int code, const std::string& msg);
 static inline int fail(MzHandle* h, int code, const std::string& msg) { return mz_fail(h, code, msg); }

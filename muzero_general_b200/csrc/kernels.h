@@ -114,15 +114,38 @@ struct FcPlan { int threads, groups, ctas_per_sm, slots, passes; size_t smem; };
 bool fc_search_plan(int N, int A, int E, int maxw, int blob_floats, int G, bool teacher, int n_games, int sm_count,
                     size_t smem_per_sm, size_t smem_reserve, size_t smem_cap, int regs, int threads, FcPlan* plan);
 
+// What decides a fused launch besides the handle's fixed network and tree shape: the games, the lanes per game, a fixed
+// CTA size (0 = planned), teacher forcing and the two A/B switches (MZ_FC_GENERIC, MZ_FC_SELECT_LEVELS).
+struct FcPreparedKey {
+    int n_games, group, threads;
+    bool teacher, generic, one_level;
+    bool operator==(const FcPreparedKey& o) const {
+        return n_games == o.n_games && group == o.group && threads == o.threads && teacher == o.teacher &&
+               generic == o.generic && one_level == o.one_level;
+    }
+};
+
+// The launch made for `key`: instantiation, selection levels and shape.  A search with the same key only copies its
+// pointers into the arguments and launches.
+struct FcPrepared {
+    bool valid = false;
+    FcPreparedKey key{};
+    int select_levels = 1;
+    bool fixed_shape = false;      // the instantiation with the unrolled network of FcFixedShape
+    cudaError_t (*launch)(const FcSearchArgs&, const FcLaunchInfo&, cudaStream_t) = nullptr;
+    FcLaunchInfo info{};
+};
+
 // The device limits the plan is made against, and what a handle has set up for the fused search kernel so far: each
 // instantiation gets its attributes set and its register count read once, each (instantiation, block, shared memory)
-// its occupancy confirmed once, so that later searches go straight to the launch.
+// its occupancy confirmed once, and the launch of the last key is kept, so that later searches go straight to the launch.
 struct FcLaunchState {
     size_t smem_per_sm = 0, smem_reserve = 0, smem_cap = 0;
     struct Kernel { const void* fn; int regs; };
     struct Shape { const void* fn; int threads; size_t smem; int ctas_per_sm; };
     std::vector<Kernel> kernels;
     std::vector<Shape> shapes;
+    FcPrepared prepared;           // invalidated when the weights load (the network descriptors are replaced)
     bool launched = false;         // last: the handle's last fused launch (mz_fc_last_launch)
     FcLaunchInfo last{};
 };

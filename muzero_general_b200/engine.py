@@ -71,6 +71,32 @@ class SearchOutput:
     device_ms: float = 0.0
 
 
+# SearchOutput's arrays in field order: (dtype, columns per game: 0 = one value, -1 = one per action)
+_OUT_FIELDS = (("int32", -1), ("float64", 0), ("float32", 0), ("int32", 0), ("int32", 0), ("float64", -1), ("float64", 2))
+
+
+def output_layout(n, A):
+    """Where a device-memory search puts SearchOutput's seven arrays in the one buffer it allocates for them: per field
+    (dtype, shape, strides, byte offset), offsets 16-byte aligned, and the buffer's size in bytes (a multiple of 16)."""
+    fields, off = [], 0
+    for dt, cols in _OUT_FIELDS:
+        shape = (n,) if cols == 0 else (n, A if cols < 0 else cols)
+        fields.append((dt, shape, (1,) if cols == 0 else (shape[1], 1), off))
+        off += (numpy.dtype(dt).itemsize * math.prod(shape) + 15) & ~15
+    return tuple(fields), off
+
+
+def carve_outputs(buf, fields):
+    """SearchOutput whose arrays are views of ``buf``, a float64 torch tensor of output_layout's size."""
+    import torch
+    views = {"float64": buf, "float32": buf.view(torch.float32), "int32": buf.view(torch.int32)}
+    return SearchOutput(*[views[dt].as_strided(shape, strides, off // (8 if dt == "float64" else 4))
+                          for dt, shape, strides, off in fields])
+
+
+_TORCH_DTYPES = {}
+
+
 class SearchEngine:
     def __init__(self, config, max_games: int = 1, device: int = 0, seed: Optional[int] = None,
                  num_simulations: Optional[int] = None, extra_expansions: int = 0):
@@ -119,6 +145,9 @@ class SearchEngine:
         self._h = handle
         self.hidden_elems = int(self.lib.mz_hidden_elems(self._h))
         self.obs_elems = int(self.lib.mz_obs_elems(self._h))
+        self._dio = _lib.MzDeviceSearchIO()            # one argument struct for every mz_search_device call
+        self._dio_ref = C.byref(self._dio)
+        self._layouts = {}                              # n_games -> output_layout
 
     # ------------------------------------------------------------------ plumbing
     def close(self):
@@ -154,6 +183,15 @@ class SearchEngine:
         return dict(zip(("grid", "block", "group", "smem", "ctas_per_sm"), (int(v) for v in info)))
 
     @property
+    def fc_prepared(self):
+        """The fused FC launch kept for the next search (mz_debug_fc_prepared), None when there is none."""
+        info = (C.c_int64 * 7)()
+        if self.lib.mz_debug_fc_prepared(self._h, info) != 1:
+            return None
+        return dict(zip(("games", "group", "threads", "generic", "one_level", "select_levels", "fixed_shape"),
+                        (int(v) for v in info)))
+
+    @property
     def last_search_ms(self):
         return float(self.lib.mz_last_search_ms(self._h))
 
@@ -183,9 +221,11 @@ class SearchEngine:
         if x is None:
             return None
         if _is_torch(x):
-            import torch
-            want = {numpy.float32: torch.float32, numpy.float64: torch.float64, numpy.int32: torch.int32,
-                    numpy.int64: torch.int64, numpy.uint8: torch.uint8}[dtype]
+            if not _TORCH_DTYPES:
+                import torch
+                _TORCH_DTYPES.update({numpy.float32: torch.float32, numpy.float64: torch.float64, numpy.int32: torch.int32,
+                                      numpy.int64: torch.int64, numpy.uint8: torch.uint8})
+            want = _TORCH_DTYPES[dtype]
             if x.dtype != want or not x.is_contiguous():
                 x = x.to(want).contiguous()
             keep.append(x)
@@ -229,6 +269,14 @@ class SearchEngine:
             n_games = 1 if (src is None and continue_tree) else int(src.shape[0])
         n = n_games
         device_mem = _is_torch(obs)
+        if legal_mask is not None and not _is_torch(legal_mask):
+            # the reference asserts this per game (self_play.py:296); a row without a legal action would also
+            # index the node pool out of bounds on the device
+            assert numpy.asarray(legal_mask).reshape(n, -1).any(axis=1).all(), \
+                "Legal actions should not be an empty array."
+        if device_mem and teacher is None and not (trace or keep_tree or stepwise or continue_tree):
+            return self._search_device(n, obs, legal_mask, to_play, add_exploration_noise, noise, first_index, game_id,
+                                       move_index)
         io = _lib.MzSearchIO()
         io.n_games = n
         io.mem = _lib.MZ_MEM_DEVICE if device_mem else _lib.MZ_MEM_HOST
@@ -238,11 +286,6 @@ class SearchEngine:
                 if obs.shape[1] != self.obs_elems:
                     raise ValueError(f"observation has {obs.shape[1]} elements, expected {self.obs_elems}")
             io.obs = self._ptr(obs, numpy.float32, keep)
-        if legal_mask is not None and not _is_torch(legal_mask):
-            # the reference asserts this per game (self_play.py:296); a row without a legal action would also
-            # index the node pool out of bounds on the device
-            assert numpy.asarray(legal_mask).reshape(n, -1).any(axis=1).all(), \
-                "Legal actions should not be an empty array."
         io.legal_mask = self._ptr(legal_mask, numpy.uint8, keep)
         io.to_play = self._ptr(to_play, numpy.int32, keep)
         io.add_exploration_noise = int(bool(add_exploration_noise))
@@ -293,6 +336,36 @@ class SearchEngine:
             out.trace = tr
         self._check(self.lib.mz_search(self._h, C.byref(io)))
         out.device_ms = self.last_search_ms
+        return out
+
+    def _search_device(self, n, obs, legal_mask, to_play, add_noise, noise, first_index, game_id, move_index):
+        """search() on device tensors through mz_search_device: the seven outputs are views of one fresh buffer, made
+        while the search runs."""
+        import torch
+        keep, io = [], self._dio
+        io.n_games = n
+        io.add_exploration_noise = 1 if add_noise else 0
+        io.obs = self._ptr(obs, numpy.float32, keep)
+        io.noise = self._ptr(noise, numpy.float64, keep)
+        io.game_id = self._ptr(game_id, numpy.int64, keep)
+        io.move_index = self._ptr(move_index, numpy.int32, keep)
+        io.legal_mask = self._ptr(legal_mask, numpy.uint8, keep)
+        io.to_play = self._ptr(to_play, numpy.int32, keep)
+        io.first_index = self._ptr(first_index, numpy.int32, keep)
+        layout = self._layouts.get(n)
+        if layout is None:
+            layout = self._layouts[n] = output_layout(n, self.A)
+        fields, nbytes = layout
+        buf = torch.empty(nbytes // 8, dtype=torch.float64, device=obs.device)
+        base = buf.data_ptr()
+        (io.visit_counts, io.root_value, io.root_predicted_value, io.max_tree_depth, io.tie_count, io.root_priors,
+         io.value_range) = (base + f[3] for f in fields)
+        self._check(self.lib.mz_search_device(self._h, self._dio_ref))
+        try:
+            out = carve_outputs(buf, fields)
+        finally:
+            self._check(self.lib.mz_search_device_wait(self._h, self._dio_ref))
+        out.device_ms = io.device_ms
         return out
 
     # ------------------------------------------------------------------ networks
