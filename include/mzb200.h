@@ -338,6 +338,28 @@ int mz_debug_small_tower(int device, int32_t n, int32_t in_channels, int32_t C, 
                          int32_t parts, int32_t A, const float* x, const float* w, const float* bias, const int32_t* action,
                          const int32_t* parent, int32_t pool_stride, float* out, int64_t* plan);
 
+/* Launch plan of the wide tower (host only; the route MZ_TC_WIDE=1 opts 128-channel nets into): n boards of C x H x W
+ * through [a stem conv, C + 1 planes with the action plane, if stem] + `blocks` residual blocks as x3 tensor-core MMAs, one
+ * board per CTA.  Fills plan[9] = {M-tiles of 64 board rows, threads per CTA, dynamic shared-memory bytes, weight ring
+ * stages, layers, CTAs per SM, boards per wave, launches per tower call, registers per thread assumed} and returns 1;
+ * returns 0 with the reason in mz_last_error(NULL) when the wide towers refuse the shape (C != 128, a board beyond the
+ * shared-memory or M-tile budget, more than 10 blocks): the network then keeps the CUDA-core towers. */
+int mz_debug_wide_tower_plan(int32_t n, int32_t C, int32_t H, int32_t W, int32_t blocks, int32_t stem, int32_t sm_count,
+                             int64_t* plan);
+
+/* Debug / parity: one wide tower (128 channels, models.py:206-231 without BN: [stem conv +] `blocks` residual blocks, every
+ * conv with bias and ReLU) of one call site of resnet_inference on host NCHW fp32 data, through the helper and the weight
+ * packing the network uses.  x is [n][128][H][W] (at MZ_TOWER_REPRESENTATION the output of the CUDA-core stem); w holds
+ * every conv's [128][cin][3][3] back to back (the dynamics stem first, cin = 129: channel 128 is the action plane
+ * action[g] / A), bias [convs][128] (or NULL); at MZ_TOWER_DYNAMICS_POOL game g's input sits in slot parent[g] of its
+ * pool_stride slots, the other slots hold NaN, and `parts` (1..4) runs the games in the ranges of the partitioned replay.
+ * The output starts as NaN.  out is [n][128][H][W]; *launches gets the kernel launches, *saturated the range-guard count
+ * (activations read or stored beyond the fp16 range) and plan (or NULL) the plan of the first range as
+ * mz_debug_wide_tower_plan fills it.  MZ_EUNSUPPORTED when the wide towers refuse the shape. */
+int mz_debug_wide_tower(int device, int32_t n, int32_t H, int32_t W, int32_t blocks, int32_t site, int32_t parts, int32_t A,
+                        const float* x, const float* w, const float* bias, const int32_t* action, const int32_t* parent,
+                        int32_t pool_stride, float* out, int64_t* launches, int32_t* saturated, int64_t* plan);
+
 /* Routes of the residual heads (route argument of mz_debug_heads_plan and mz_debug_heads, plan[0]).  The network always
  * takes MZ_HEADS_PLANNED: heads_kernel<32> (one warp per sample) when C*H*W <= 1024, heads_kernel<128> (128 threads per
  * sample) otherwise, the generic route (one plain kernel per stage) when the head weights and one sample's tile exceed

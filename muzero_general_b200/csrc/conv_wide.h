@@ -1,0 +1,52 @@
+// 128-channel residual towers on the tensor cores at fp32-grade accuracy, dense NCHW fp32 in and out (conv_wide.cu).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+namespace mz {
+
+constexpr int kWideC = 128;
+constexpr int kWideMaxLayers = 21;          // a stem + 10 residual blocks (Gomoku's dynamics tower is 13 layers)
+
+struct WideLayer {
+    const float* w;               // x3 image [9 taps][2 K-halves][256 rows: w_h cout 0..127 | w_l cout 0..127][64 cin] fp16,
+                                  // 128B-swizzled (typed float*): w = (w_h + w_l) / s, s a power of two per output channel
+    const float* scale;           // [128] 1 / s
+    const float* bias;            // [128] folded BN shift, or nullptr
+    const float* action_table;    // dynamics stem: add (action/A) * table[y * W + x][cout]; nullptr otherwise
+};
+
+// [stem conv +] residual blocks of 128 channels, every conv followed by bias (+ residual) (+ action term) + ReLU
+struct WideTowerArgs {
+    const float* in;              // [n][128][H][W] dense fp32, or the hidden-state pool when gather_parent is set
+    float* out;                   // [n][128][H][W]
+    const int32_t* gather_parent; // board g reads in + (g * pool_stride + gather_parent[g]) * 128 * H * W
+    int pool_stride;
+    const int32_t* action;        // [n] for a stem with an action table
+    int n, H, W, A;
+    int g0;                       // boards [g0, g0 + n): every array is addressed by the global index
+    int stem;                     // layer 0 is a stem; the layers after it are blocks of two convs
+    int n_layers;
+    WideLayer layer[kWideMaxLayers];
+    int* sat_count;               // bumped when an activation read or stored exceeds the fp16 range
+    // filled by the launcher from the plan
+    int S, plane_bytes, res_off, bar_off;
+};
+
+// Launch plan of one wide tower (host only; the launcher and mz_debug_wide_tower_plan both take it from here)
+struct WideTowerPlan {
+    int m_tiles, threads;         // 64-row M-tiles of the H x (W + 1) board rows, one warpgroup each
+    int rows;                     // shared-memory rows of one activation plane (guard + zero rows + board, multiple of 8)
+    int stages;                   // weight ring stages (one tap x one 64-channel K-half each)
+    size_t smem;                  // dynamic shared-memory bytes
+    int layers;
+    int ctas_per_sm, wave;        // resident CTAs (one board each) per SM and on the device
+    int launches;                 // kernel launches per tower call
+    int reg_cap;                  // registers per thread the plan assumes (__launch_bounds__ of the kernel)
+};
+
+// false with the reason in *why when the wide tower refuses the shape (the network then keeps the CUDA-core towers)
+bool wide_tower_plan(int n, int C, int H, int W, int layers, int sm_count, WideTowerPlan* p, const char** why);
+cudaError_t launch_wide_tower(WideTowerArgs a, const WideTowerPlan& p, cudaStream_t stream);
+
+}  // namespace mz

@@ -32,6 +32,7 @@
 #include "small_search.h"
 #include "launch.h"
 #include "conv_tc.h"
+#include "conv_wide.h"
 #include "cnn_stem.h"
 #include "pipeline.h"
 
@@ -359,8 +360,8 @@ struct ConvLayer {
     int cin, cout, stride;
     size_t w_off;             // into the conv blob: [cin][9][cout]
     long b_off;               // folded BN bias [cout], -1 = none
-    long tc_off;              // tensor-core image [9][C/4][C][4] (tf32), -1 = none
-    long tc_table_off;        // dynamics first conv: action-plane table [64][C], -1 = none
+    long tc_off;              // tensor-core image [9][C/4][C][4] (tf32), or the wide towers' x3 image (conv_wide.h), -1 = none
+    long tc_table_off;        // dynamics first conv: action-plane table [64][C] ([H * W][C] on the wide towers), -1 = none
     long tc_scale_off;        // x3 mode: [C] per-output-channel power of two undoing the weight prescale, -1 = none
 };
 
@@ -392,6 +393,8 @@ struct ResNetDevice {
     bool heads_off_tc = false;         // a 64-channel board net kept off the tensor cores because its heads exceed shared memory
     bool fuse_small = true;            // CUDA-core towers as one fused launch where they fit (small_tower.cu); MZ_NO_FUSE=1: per layer
     int state_elems = 0;               // float slots per stored hidden state (dense C*H*W, or 2048 = 4096 fp16 for P64C8)
+    bool wide = false;                 // MZ_TC_WIDE=1: 128-channel towers on the tensor cores, x3 numerics, dense states (conv_wide.cu)
+    std::string wide_refused;          // MZ_TC_WIDE=1 on a 128-channel net whose board the wide towers refuse: numerics with the reason
 };
 
 static int conv_out(int h, int stride) { return (h - 1) / stride + 1; }
@@ -560,6 +563,16 @@ ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, s
             r->heads_off_tc = true;
         }
     }
+    // MZ_TC_WIDE=1 (opt-in until measured): the towers of a 128-channel net as x3 tensor-core launches on the dense states
+    // (conv_wide.cu), when the planner accepts the hidden board.  The stems and the heads stay on the CUDA cores.
+    const char* wide_env = getenv("MZ_TC_WIDE");
+    if (wide_env && wide_env[0] == '1' && !tc_off && !(tc_mode && strcmp(tc_mode, "fp16") == 0) && net.channels == kWideC &&
+        !net.downsample) {
+        WideTowerPlan p;
+        const char* why = "";
+        r->wide = wide_tower_plan(max_batch, net.channels, r->hh, r->hw, 1 + 2 * net.blocks, sm_count, &p, &why);
+        if (!r->wide) r->wide_refused = std::string("f32 nets + f64 tree statistics (128-channel towers stay on the CUDA cores: ") + why + ")";
+    }
     const char* no_fuse = getenv("MZ_NO_FUSE");
     r->fuse_small = !(no_fuse && no_fuse[0] == '1');
     r->state_elems = r->use_tc ? conv_tc_board_elems(r->split) : r->C * r->hh * r->hw;
@@ -642,6 +655,8 @@ float f16_to_float(uint16_t h) {
     return f;
 }
 
+constexpr int kWideImage = 3;       // pack_conv's `tc` for the x3 image of the wide towers (conv_wide.cu)
+
 bool pack_conv(Loader& L, const std::string& conv, const std::string& bn, int cin, int cout, int stride,
                std::vector<float>& blob, std::vector<ConvLayer>& layers, int tc = 0, int H = 0, int W = 0) {
     const MzTensor* w = L.get(conv + ".weight", (int64_t)cout * cin * 9);
@@ -675,13 +690,15 @@ bool pack_conv(Loader& L, const std::string& conv, const std::string& bn, int ci
     }
     while (blob.size() % 4) blob.push_back(0.0f);           // keep every layer 16-byte aligned
     l.tc_off = l.tc_table_off = l.tc_scale_off = -1;
-    if (tc == kLayoutSplit) {
-        // x3 image [tap][128 rows][cin 64]: rows 0..63 = w_h of cout 0..63, rows 64..127 = w_l; w' = w * 2^k with k per
-        // output channel such that the row's largest |w'| lies in [1, 2); w_h = fp16(w'), w_l = fp16(w' - w_h).
-        // The 16-byte chunks of a row are XOR-ed with row % 8 (wgmma K-major SWIZZLE_128B).
+    if (tc == kLayoutSplit || tc == kWideImage) {
+        // x3 image [tap][K-half][2C rows][cin 64]: rows 0..C-1 = w_h of cout 0..C-1, rows C..2C-1 = w_l; w' = w * 2^k with
+        // k per output channel such that the row's largest |w'| lies in [1, 2); w_h = fp16(w'), w_l = fp16(w' - w_h).
+        // The 16-byte chunks of a row are XOR-ed with row % 8 (wgmma K-major SWIZZLE_128B).  64 channels (conv_x3.cu): one
+        // K-half; 128 (conv_wide.cu): two, each (tap, K-half) one 32 KB stage of the kernel's weight ring.
         const int C = cout;
+        const bool wide = tc == kWideImage;
         l.tc_off = (long)blob.size();
-        blob.resize(blob.size() + (size_t)9 * 128 * C / 2);
+        blob.resize(blob.size() + (size_t)9 * 2 * C * C / 2);
         l.tc_scale_off = (long)blob.size();
         blob.resize(blob.size() + (size_t)C, 1.0f);
         uint16_t* img = reinterpret_cast<uint16_t*>(blob.data() + l.tc_off);
@@ -703,14 +720,17 @@ bool pack_conv(Loader& L, const std::string& conv, const std::string& bn, int ci
                     const uint16_t hb = to_f16(ws);
                     const float back = f16_to_float(hb);
                     const uint16_t lb = to_f16(ws - back);
-                    const size_t col = (size_t)((((ci >> 3) ^ (co & 7))) << 3) + (ci & 7);
-                    img[((size_t)tap * 128 + co) * C + col] = hb;
-                    img[((size_t)tap * 128 + 64 + co) * C + col] = lb;
+                    const int cl = ci & 63;
+                    const size_t col = (size_t)((((cl >> 3) ^ (co & 7))) << 3) + (cl & 7);
+                    const size_t stage = (size_t)tap * (C / 64) + (ci >> 6);
+                    img[(stage * 2 * C + co) * 64 + col] = hb;
+                    img[(stage * 2 * C + C + co) * 64 + col] = lb;
                 }
         }
         if (cin == C + 1) {
+            // per board position (P64 row (y + 1) * 8 + x, or y * W + x on the wide towers' dense boards)
             l.tc_table_off = (long)blob.size();
-            blob.resize(blob.size() + (size_t)64 * C, 0.0f);
+            blob.resize(blob.size() + (size_t)(wide ? H * W : 64) * C, 0.0f);
             float* tab = blob.data() + l.tc_table_off;
             for (int y = 0; y < H; ++y)
                 for (int x = 0; x < W; ++x)
@@ -720,7 +740,7 @@ bool pack_conv(Loader& L, const std::string& conv, const std::string& bn, int ci
                             for (int dx = -1; dx <= 1; ++dx)
                                 if (y + dy >= 0 && y + dy < H && x + dx >= 0 && x + dx < W)
                                     acc += (double)w->data[((size_t)co * cin + C) * 9 + (dy + 1) * 3 + (dx + 1)] * scale[co];
-                        tab[((y + 1) * 8 + x) * C + co] = (float)acc;
+                        tab[(size_t)(wide ? y * W + x : (y + 1) * 8 + x) * C + co] = (float)acc;
                     }
         }
     } else if (tc) {
@@ -816,7 +836,7 @@ int resnet_load_weights(ResNetDevice* r, const MzTensor* tensors, int n, std::st
     }
     // the tensor-core images are packed whenever the shape allows them (both the fp16 and the x3 image are cheap), so the
     // range guard can switch paths without reloading; which one is used is decided per launch
-    const int tc = !r->tc_capable ? 0 : (r->split ? kLayoutSplit : kLayoutF16);
+    const int tc = r->wide ? kWideImage : !r->tc_capable ? 0 : (r->split ? kLayoutSplit : kLayoutF16);
     for (int i = 0; ok && i < nd.blocks; ++i) ok = pack_resblock(L, rp + ".resblocks." + std::to_string(i), C, conv, r->rep_trunk, tc);
     const std::string dp = "dynamics_network.module";
     ok = ok && pack_conv(L, dp + ".conv", dp + ".bn", C + 1, C, 1, conv, r->dyn, tc, r->hh, r->hw);
@@ -849,6 +869,7 @@ struct Runner {
     SmallTowerPlan* small_plan = nullptr;   // when set, small_tower reports the plan of its launch here (mz_debug_small_tower)
     int heads_route = MZ_HEADS_PLANNED;     // mz_debug_heads only: force a heads route; the network never sets it
     HeadsPlan* heads_plan_out = nullptr;    // when set, heads reports the plan of its launch here (mz_debug_heads)
+    WideTowerPlan* wide_plan_out = nullptr; // when set, wide_tower reports the plan of its launch here (mz_debug_wide_tower)
     bool fail(const char* what, cudaError_t e) { *err = std::string(what) + ": " + cudaGetErrorString(e); return false; }
 
     // conv: in -> out. `in` may be gathered from the pool; action adds the constant plane.
@@ -1093,6 +1114,54 @@ struct Runner {
         return r->net.blocks > 0 ? small_tower(r->pred, 0, false, r->net.blocks, hidden, out, r->C, r->hh, r->hw) : 0;
     }
 
+    // [optional stem conv] + `count` residual blocks of a 128-channel net as ONE x3 tensor-core launch (conv_wide.cu), dense
+    // NCHW in and out.  Returns what small_tower returns: 1 = launched, 0 = not the wide route, -1 = error.
+    int wide_tower(const std::vector<ConvLayer>& layers, size_t first, bool stem, size_t count, const float* in, float* out,
+                   const int32_t* gather_parent = nullptr, int pool_stride = 0, const int32_t* action = nullptr) {
+        const int nl = (stem ? 1 : 0) + 2 * (int)count;
+        if (!r->wide || nl == 0) return 0;
+        WideTowerPlan p;
+        const char* why = "";
+        if (!wide_tower_plan(n, r->C, r->hh, r->hw, nl, r->sm_count, &p, &why)) return 0;
+        WideTowerArgs a{};
+        a.in = in; a.out = out; a.gather_parent = gather_parent; a.pool_stride = pool_stride; a.action = action;
+        a.n = n; a.H = r->hh; a.W = r->hw; a.A = r->net.action_space; a.g0 = g0; a.stem = stem ? 1 : 0; a.n_layers = nl;
+        a.sat_count = r->d_sat;
+        for (int i = 0; i < nl; ++i) {
+            const ConvLayer& l = layers[first + i];
+            WideLayer& t = a.layer[i];
+            t.w = r->d_conv + l.tc_off;
+            t.scale = r->d_conv + l.tc_scale_off;
+            t.bias = l.b_off >= 0 ? r->d_conv + l.b_off : nullptr;
+            t.action_table = i == 0 && stem && action && l.tc_table_off >= 0 ? r->d_conv + l.tc_table_off : nullptr;
+        }
+        if (wide_plan_out) *wide_plan_out = p;
+        kt_begin(KT_TOWER, stream);
+        cudaError_t e = launch_wide_tower(a, p, stream);
+        kt_end(stream);
+        if (e != cudaSuccess) { fail("wide tower launch", e); return -1; }
+        *launches += p.launches;
+        return 1;
+    }
+
+    // The four wide-tower call sites of resnet_inference (mz_debug_wide_tower runs the same helpers).  Representation: the
+    // blocks after the CUDA-core stem, which wrote `in`.
+    int representation_wide_tower(const float* in, float* out) {
+        return wide_tower(r->rep_trunk, 1, false, r->net.blocks, in, out);
+    }
+    // Dynamics, plain API call: dense hidden states plus the action plane.
+    int dynamics_wide_tower(const float* states, float* out, const int32_t* action) {
+        return wide_tower(r->dyn, 0, true, r->net.blocks, states, out, nullptr, 0, action);
+    }
+    // Dynamics in search: the parents' states gathered from the pool, which stays read only.
+    int dynamics_wide_tower_pool(const float* pool, const int32_t* gather_parent, int pool_stride, float* out, const int32_t* action) {
+        return wide_tower(r->dyn, 0, true, r->net.blocks, pool, out, gather_parent, pool_stride, action);
+    }
+    // Prediction: the rescaled hidden state.
+    int prediction_wide_tower(const float* hidden, float* out) {
+        return wide_tower(r->pred, 0, false, r->net.blocks, hidden, out);
+    }
+
     // residual tower: layers[2k], layers[2k+1] are one block; x ends up in `*cur`
     bool blocks(const std::vector<ConvLayer>& layers, size_t first, size_t count, float** cur, float** tmp, float** spare, int H, int W) {
         for (size_t b = 0; b < count; ++b) {
@@ -1331,8 +1400,9 @@ bool resnet_can_partition(const ResNetDevice* r0) {
     Runner R{r, nullptr, &launches, &err, r->max_batch, 0};
     const int nb = r->net.blocks;
     if (nb < 1) return false;
-    if (R.small_tower(r->dyn, 0, true, nb, nullptr, nullptr, r->C, r->hh, r->hw, nullptr, 0, &kDryRunAction, true) != 1) return false;
-    if (R.small_tower(r->pred, 0, false, nb, nullptr, nullptr, r->C, r->hh, r->hw, nullptr, 0, nullptr, true) != 1) return false;
+    // the wide towers honour g0 (resnet_create accepted the board); otherwise the fused small towers must take both towers
+    if (!r->wide && R.small_tower(r->dyn, 0, true, nb, nullptr, nullptr, r->C, r->hh, r->hw, nullptr, 0, &kDryRunAction, true) != 1) return false;
+    if (!r->wide && R.small_tower(r->pred, 0, false, nb, nullptr, nullptr, r->C, r->hh, r->hw, nullptr, 0, nullptr, true) != 1) return false;
     // heads_kernel route (not heads_big): the head weights plus one group's tile fit in shared memory
     const int HW = r->hh * r->hw;
     int hi = 0, lo = 1 << 30, maxw = 32;
@@ -1346,6 +1416,11 @@ bool resnet_can_partition(const ResNetDevice* r0) {
     return ((size_t)(hi - lo) + warp_floats) * 4 <= 227 * 1024;
 }
 const char* resnet_numerics(const ResNetDevice* r) {
+    if (r->wide)
+        return "f32-grade nets (128-channel towers on the tensor cores, split fp16 operands x = x_h + x_l/2^11, 3 partial "
+               "products, f32 accumulate; f32 stems and heads) + f64 tree statistics";
+    if (r->fell_back == 2) return "f32 nets + f64 tree statistics (128-channel tensor-core towers left after an activation exceeded the fp16 range)";
+    if (!r->wide_refused.empty()) return r->wide_refused.c_str();
     if (!r->use_tc) return r->heads_off_tc ? "f32 nets + f64 tree statistics (no tensor-core towers: the head weights exceed shared memory)"
                          : r->fell_back ? "f32 nets + f64 tree statistics (tensor-core towers left after an activation exceeded the fp16 range)"
                                         : "f32 nets + f64 tree statistics";
@@ -1356,7 +1431,7 @@ const char* resnet_numerics(const ResNetDevice* r) {
 // Range guard of the x3 towers: number of epilogue threads that stored an activation beyond the fp16 range since the
 // last call (synchronises the stream).  resnet_use_strict switches the handle to the fp32 CUDA-core towers for good.
 int resnet_take_saturations(ResNetDevice* r, cudaStream_t stream) {
-    if (!r->use_tc || !r->split || !r->d_sat) return 0;
+    if (!((r->use_tc && r->split) || r->wide) || !r->d_sat) return 0;
     int count = 0;
     if (cudaMemcpyAsync(&count, r->d_sat, 4, cudaMemcpyDeviceToHost, stream) != cudaSuccess) return 0;
     if (cudaStreamSynchronize(stream) != cudaSuccess) return 0;
@@ -1364,7 +1439,8 @@ int resnet_take_saturations(ResNetDevice* r, cudaStream_t stream) {
     return count;
 }
 void resnet_use_strict(ResNetDevice* r) {
-    r->use_tc = false; r->split = false; r->fell_back = 1;
+    r->fell_back = r->wide ? 2 : 1;
+    r->use_tc = false; r->split = false; r->wide = false;
     r->state_elems = r->C * r->hh * r->hw;           // dense NCHW states: smaller than the board layout, the pool fits
 }
 
@@ -1733,6 +1809,135 @@ int resnet_debug_small_tower(int n, int in_channels, int C, int H, int W, int bl
     return rc;
 }
 
+// Launch plan of the wide tower (host only, behind mz_debug_wide_tower_plan): plan[9] = {M-tiles, threads, shared-memory bytes,
+// weight ring stages, layers, CTAs per SM, boards per wave, launches, registers per thread assumed} of n boards of C x H x W
+// through [a stem conv +] `blocks` residual blocks.  false with the reason in *err when the wide towers refuse the shape.
+bool resnet_wide_tower_plan(int n, int C, int H, int W, int blocks, bool stem, int sm_count, int64_t* plan, std::string* err) {
+    if (blocks < 0) { *err = "bad shape"; return false; }
+    WideTowerPlan p;
+    const char* why = "";
+    if (!wide_tower_plan(n, C, H, W, (stem ? 1 : 0) + 2 * blocks, sm_count, &p, &why)) { *err = why; return false; }
+    const int64_t out[9] = {p.m_tiles, p.threads, (int64_t)p.smem, p.stages, p.layers, p.ctas_per_sm, p.wave, p.launches, p.reg_cap};
+    for (int i = 0; i < 9; ++i) plan[i] = out[i];
+    return true;
+}
+
+// Stand-alone wide tower of one call site of resnet_inference, through the same Runner helpers and weight packing, on host
+// NCHW data (128 channels).  The output and the pool's other slots start as NaN bytes (0xFF), so a board the tower does not
+// write, or one read from the wrong slot, produces NaN.
+int resnet_debug_wide_tower(int n, int H, int W, int blocks, int site, int parts, int A, const float* x, const float* w,
+                            const float* bias, const int32_t* action, const int32_t* parent, int pool_stride, float* out,
+                            int64_t* launches, int32_t* saturated, int64_t* plan, int sm_count, std::string* err) {
+    constexpr int C = kWideC;
+    const bool stem = site == MZ_TOWER_DYNAMICS || site == MZ_TOWER_DYNAMICS_POOL;
+    const bool in_pool = site == MZ_TOWER_DYNAMICS_POOL;
+    if (n < 1 || blocks < 0 || (!stem && blocks < 1) || site < MZ_TOWER_REPRESENTATION || site > MZ_TOWER_PREDICTION) {
+        *err = "bad shape or site"; return MZ_EINVAL;
+    }
+    if (parts < 1 || parts > 4 || (parts > 1 && !in_pool)) { *err = "partitions need the in-search dynamics site, 1 to 4 of them"; return MZ_EINVAL; }
+    if (stem) {
+        if (A < 1 || !action) { *err = "the dynamics sites need actions and A >= 1"; return MZ_EINVAL; }
+        for (int g = 0; g < n; ++g) if (action[g] < 0 || action[g] >= A) { *err = "action out of range"; return MZ_EINVAL; }
+    }
+    if (in_pool) {
+        if (!parent || pool_stride < 1) { *err = "the in-search site needs parents and pool_stride >= 1"; return MZ_EINVAL; }
+        for (int g = 0; g < n; ++g) if (parent[g] < 0 || parent[g] >= pool_stride) { *err = "parent out of range"; return MZ_EINVAL; }
+    }
+    {
+        int64_t unused[9];
+        std::string why;
+        if (!resnet_wide_tower_plan(n, C, H, W, blocks, stem, sm_count, unused, &why)) {
+            *err = "the wide tower refuses the shape: " + why; return MZ_EUNSUPPORTED;
+        }
+    }
+    const int n_convs = (stem ? 1 : 0) + 2 * blocks;
+    std::vector<std::string> names(n_convs);
+    std::vector<MzTensor> tensors(n_convs);
+    size_t w_off = 0;
+    for (int i = 0; i < n_convs; ++i) {
+        const int cin = stem && i == 0 ? C + 1 : C;
+        names[i] = "c" + std::to_string(i) + ".weight";
+        tensors[i] = MzTensor{names[i].c_str(), w + w_off, (int64_t)C * cin * 9};
+        w_off += (size_t)C * cin * 9;
+    }
+    MzNetDesc nd{};
+    nd.kind = MZ_NET_RESNET; nd.channels = C; nd.obs_c = C; nd.obs_h = H; nd.obs_w = W; nd.action_space = stem ? A : 1;
+    nd.blocks = blocks;
+    ResNetDevice r{};
+    r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = H; r.hw = W; r.wide = true;
+    Loader L{tensors.data(), n_convs, err};
+    std::vector<float> blob;
+    std::vector<ConvLayer> layers;
+    for (int i = 0; i < n_convs; ++i) {
+        if (!pack_conv(L, "c" + std::to_string(i), "", stem && i == 0 ? C + 1 : C, C, 1, blob, layers, kWideImage, H, W)) return MZ_EINVAL;
+        if (bias) {
+            layers[i].b_off = (long)blob.size();
+            blob.insert(blob.end(), bias + (size_t)i * C, bias + (size_t)(i + 1) * C);
+        }
+    }
+    if (site == MZ_TOWER_REPRESENTATION) { r.rep_trunk = layers; r.rep_trunk.insert(r.rep_trunk.begin(), ConvLayer{}); }  // [0]: the CUDA-core stem, not run here
+    else if (stem) r.dyn = layers;
+    else r.pred = layers;
+
+    const size_t board = (size_t)C * H * W, dense = (size_t)n * board;
+    const size_t in_total = in_pool ? (size_t)n * pool_stride * board : dense;
+    float *d_blob = nullptr, *d_in = nullptr, *d_out = nullptr;
+    int32_t *d_action = nullptr, *d_parent = nullptr;
+    auto cleanup = [&]() {
+        for (void* p : {(void*)d_blob, (void*)d_in, (void*)d_out, (void*)d_action, (void*)d_parent, (void*)r.d_sat}) if (p) cudaFree(p);
+        r.d_sat = nullptr; r.d_conv = nullptr;
+    };
+    const bool ok = cudaMalloc(&d_blob, blob.size() * 4) == cudaSuccess && cudaMalloc(&d_in, in_total * 4) == cudaSuccess &&
+                    cudaMalloc(&d_out, dense * 4) == cudaSuccess && cudaMalloc(&d_action, (size_t)n * 4) == cudaSuccess &&
+                    cudaMalloc(&d_parent, (size_t)n * 4) == cudaSuccess && cudaMalloc(&r.d_sat, 64) == cudaSuccess;
+    if (!ok) { cleanup(); *err = "allocation failed"; return MZ_ENOMEM; }
+    r.d_conv = d_blob;
+    cudaMemcpy(d_blob, blob.data(), blob.size() * 4, cudaMemcpyHostToDevice);
+    if (in_pool) {
+        cudaMemset(d_in, 0xFF, in_total * 4);
+        for (int g = 0; g < n; ++g)
+            cudaMemcpy(d_in + ((size_t)g * pool_stride + parent[g]) * board, x + (size_t)g * board, board * 4, cudaMemcpyHostToDevice);
+        cudaMemcpy(d_parent, parent, (size_t)n * 4, cudaMemcpyHostToDevice);
+    } else {
+        cudaMemcpy(d_in, x, dense * 4, cudaMemcpyHostToDevice);
+    }
+    if (stem) cudaMemcpy(d_action, action, (size_t)n * 4, cudaMemcpyHostToDevice);
+    cudaMemset(d_out, 0xFF, dense * 4);
+    cudaMemset(r.d_sat, 0, 64);
+    *launches = 0;
+    WideTowerPlan used{}, first{};
+    int rc = MZ_OK;
+    // the ranges of the partitioned replay, each through its own Runner (one range unless in the pool); every array stays
+    // addressed by the global game.  The plan reported is the first range's.
+    const int per = in_pool ? partition_games(n, parts) : n;
+    for (int p = 0; p * per < n && rc == MZ_OK; ++p) {
+        Runner R{&r, nullptr, launches, err, std::min(per, n - p * per), p * per};
+        R.wide_plan_out = &used;
+        int done;
+        if (site == MZ_TOWER_REPRESENTATION) done = R.representation_wide_tower(d_in, d_out);
+        else if (site == MZ_TOWER_DYNAMICS) done = R.dynamics_wide_tower(d_in, d_out, d_action);
+        else if (site == MZ_TOWER_DYNAMICS_POOL) done = R.dynamics_wide_tower_pool(d_in, d_parent, pool_stride, d_out, d_action);
+        else done = R.prediction_wide_tower(d_in, d_out);
+        if (done == 0) { *err = "no wide launch"; rc = MZ_EUNSUPPORTED; }
+        else if (done < 0) rc = MZ_ECUDA;
+        if (p == 0) first = used;
+    }
+    cudaError_t e = cudaDeviceSynchronize();
+    if (rc == MZ_OK && e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug wide tower: ") + cudaGetErrorString(e); }
+    if (rc == MZ_OK) {
+        int sat = 0;
+        e = cudaMemcpy(out, d_out, dense * 4, cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess) e = cudaMemcpy(&sat, r.d_sat, 4, cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug wide tower: ") + cudaGetErrorString(e); }
+        if (saturated) *saturated = sat;
+        const int64_t pl[9] = {first.m_tiles, first.threads, (int64_t)first.smem, first.stages, first.layers, first.ctas_per_sm,
+                               first.wave, first.launches, first.reg_cap};
+        if (plan) for (int i = 0; i < 9; ++i) plan[i] = pl[i];
+    }
+    cleanup();
+    return rc;
+}
+
 // The heads of one call site of the network as a ResNetDevice holds them: C channels on an H x W board, states in `layout`
 // (kLayoutDense / kLayoutF16 / kLayoutSplit), head descriptors laid out as pack_head lays them from shapes[h] = {reduced
 // channels, n_out, hidden layers, widths...}.  The representation site has no head, the dynamics sites the reward head,
@@ -1898,7 +2103,7 @@ int resnet_states_from_nchw(ResNetDevice* r, const float* dense, int count, floa
 // arguments of the towers and the heads are the ones resnet_inference would launch with, simulation after simulation.
 static bool small_search_build(ResNetDevice* r, const InferCall& c, const TreeStepArgs& tree, int n_sims, SmallSearchArgs* out,
                                int* P, int* CO, int* G, int* threads, size_t* smem) {
-    if (r->use_tc || !r->loaded || !r->fuse_small || !c.recurrent || !c.gather_parent || c.hidden || r->net.blocks < 1) return false;
+    if (r->use_tc || r->wide || !r->loaded || !r->fuse_small || !c.recurrent || !c.gather_parent || c.hidden || r->net.blocks < 1) return false;
     if (c.value_logits || c.reward_logits) return false;
     std::string err; int64_t launches = 0;
     Runner R{r, nullptr, &launches, &err, c.n, c.g0};
@@ -2003,6 +2208,13 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
             if (fused < 0) return MZ_ECUDA;
             if (fused) { float* t = cur; cur = tmp; tmp = t; }
             else if (!R.blocks(r->rep_trunk, 0, nd.blocks, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
+        } else if (r->wide && nd.blocks > 0) {
+            // the stem on the CUDA cores, the blocks as one wide launch
+            if (!R.conv(r->rep_trunk[0], c.in, cur, nullptr, true, H, W)) return MZ_ECUDA;
+            const int wide = R.representation_wide_tower(cur, tmp);
+            if (wide < 0) return MZ_ECUDA;
+            if (wide) { float* t = cur; cur = tmp; tmp = t; }
+            else if (!R.blocks(r->rep_trunk, 1, nd.blocks, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
         } else {
             const int fused = R.representation_small_tower(c.in, cur);
             if (fused < 0) return MZ_ECUDA;
@@ -2023,8 +2235,11 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
         }
     } else {
         const float* in = c.gather_parent ? c.pool_hidden : c.in;
-        const int fused = c.gather_parent ? R.dynamics_small_tower_pool(c.pool_hidden, c.gather_parent, c.pool_stride, cur, c.action)
-                                          : R.dynamics_small_tower(c.in, cur, c.action);
+        int fused = c.gather_parent ? R.dynamics_wide_tower_pool(c.pool_hidden, c.gather_parent, c.pool_stride, cur, c.action)
+                                    : R.dynamics_wide_tower(c.in, cur, c.action);
+        if (fused == 0)
+            fused = c.gather_parent ? R.dynamics_small_tower_pool(c.pool_hidden, c.gather_parent, c.pool_stride, cur, c.action)
+                                    : R.dynamics_small_tower(c.in, cur, c.action);
         if (fused < 0) return MZ_ECUDA;
         if (!fused) {
             if (!R.conv(r->dyn[0], in, cur, nullptr, true, hh, hw, c.gather_parent, c.pool_stride, c.action)) return MZ_ECUDA;
@@ -2038,7 +2253,8 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
         float* x = hidden_out;
         // the tower must not overwrite the hidden state: first conv reads it, writes workspace
         float *pc = cur, *pt = tmp, *ps = spare;
-        const int fused = R.prediction_small_tower(x, pt);
+        int fused = R.prediction_wide_tower(x, pt);
+        if (fused == 0) fused = R.prediction_small_tower(x, pt);
         if (fused < 0) return MZ_ECUDA;
         if (fused) {
             x = pt;

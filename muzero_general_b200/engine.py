@@ -705,6 +705,52 @@ def debug_small_tower(x, weights, biases=None, site="prediction", actions=None, 
     return out, dict(zip(SMALL_TOWER_PLAN, plan))
 
 
+WIDE_TOWER_PLAN = ("m_tiles", "threads", "smem", "stages", "layers", "ctas_per_sm", "wave", "launches", "reg_cap")
+
+
+def debug_wide_tower_plan(n, channels, H, W, blocks, stem, sm_count):
+    """Launch plan of the 128-channel x3 tensor-core tower (mz_debug_wide_tower_plan, host only): (a dict of
+    WIDE_TOWER_PLAN, "") or (None, the reason) when the wide towers refuse the shape."""
+    lib = _lib.load_library()
+    out = (C.c_int64 * 9)()
+    if not lib.mz_debug_wide_tower_plan(n, channels, H, W, blocks, int(stem), sm_count, out):
+        return None, lib.mz_last_error(None).decode()
+    return dict(zip(WIDE_TOWER_PLAN, out)), ""
+
+
+def debug_wide_tower(x, weights, biases=None, site="prediction", actions=None, A=1, parents=None, pool_stride=1, parts=1,
+                     device=0):
+    """One 128-channel x3 tensor-core tower of a network call site through mz_debug_wide_tower; numpy NCHW in and out.
+    x is [n, 128, H, W]; ``weights`` the convs in order ([128, 129, 3, 3] dynamics stem first, then two [128, 128, 3, 3]
+    per block), ``biases`` one [128] per conv.  ``site`` as for debug_conv_tower.  Returns (out [n, 128, H, W], kernel
+    launches, range-guard count, the plan of the launch as a dict)."""
+    lib = _lib.load_library()
+    x = numpy.ascontiguousarray(x, numpy.float32)
+    n, ch, H, W = x.shape
+    stem = site in ("dynamics", "dynamics_pool")
+    if ch != 128 or (len(weights) - stem) % 2 != 0:
+        raise ValueError(f"{ch} channels / {len(weights)} convs do not make a 128-channel tower at site {site}")
+    for i, w in enumerate(weights):
+        if numpy.shape(w) != (128, 129 if stem and i == 0 else 128, 3, 3):
+            raise ValueError(f"conv {i}: weights {numpy.shape(w)}")
+    wcat = numpy.ascontiguousarray(numpy.concatenate([numpy.asarray(w, numpy.float32).reshape(-1) for w in weights]))
+    b = None if biases is None else numpy.ascontiguousarray(numpy.stack(biases), numpy.float32)
+    if b is not None and b.shape != (len(weights), 128):
+        raise ValueError(f"biases {b.shape} do not fit {len(weights)} convs")
+    act = None if actions is None else numpy.ascontiguousarray(actions, numpy.int32)
+    par = None if parents is None else numpy.ascontiguousarray(parents, numpy.int32)
+    out = numpy.empty_like(x)
+    launches, sat = C.c_int64(0), C.c_int32(0)
+    plan = (C.c_int64 * 9)()
+    rc = lib.mz_debug_wide_tower(device, n, H, W, (len(weights) - stem) // 2, TOWER_SITES[site], parts, A, x.ctypes.data,
+                                 wcat.ctypes.data, None if b is None else b.ctypes.data,
+                                 None if act is None else act.ctypes.data, None if par is None else par.ctypes.data,
+                                 pool_stride, out.ctypes.data, C.byref(launches), C.byref(sat), plan)
+    if rc != 0:
+        raise _lib.MzError(rc, lib.mz_last_error(None).decode())
+    return out, launches.value, sat.value, dict(zip(WIDE_TOWER_PLAN, plan))
+
+
 HEADS_ROUTES = {"planned": 0, "warp": 1, "wide": 2, "generic": 3}
 HEADS_ROUTE_NAMES = {1: "warp", 2: "wide", 3: "generic"}
 LAYOUTS = {"dense": 0, "f16": 1, "split": 2}
