@@ -360,6 +360,24 @@ int mz_debug_wide_tower(int device, int32_t n, int32_t H, int32_t W, int32_t blo
                         const float* x, const float* w, const float* bias, const int32_t* action, const int32_t* parent,
                         int32_t pool_stride, float* out, int64_t* launches, int32_t* saturated, int64_t* plan);
 
+/* Launch plan of the wide tower on CTA pairs (host only; the route MZ_TC_WIDE=2 adds for boards the one-CTA plan refuses,
+ * e.g. 15 x 15 and 16 x 16): each board split across a cluster of two CTAs, CTA 0 taking rows [0, ceil(H / 2)) and CTA 1
+ * the rest, the boundary rows exchanged through distributed shared memory after every layer.  Same arguments as
+ * mz_debug_wide_tower_plan.  Fills plan[9] = {board rows of CTA 0, M-tiles per CTA, threads per CTA, dynamic shared-memory
+ * bytes per CTA, weight ring stages, layers, boards (CTA pairs) per wave as planned (CTAs per SM x SMs / 2), launches per
+ * tower call, registers per thread assumed} and returns 1; returns 0 with the reason in mz_last_error(NULL) when the pair
+ * refuses the shape (C != 128, H < 2, a half beyond the shared-memory or M-tile budget, more than 10 blocks).  It accepts
+ * every board the one-CTA plan accepts with H >= 2. */
+int mz_debug_wide_pair_tower_plan(int32_t n, int32_t C, int32_t H, int32_t W, int32_t blocks, int32_t stem, int32_t sm_count,
+                                  int64_t* plan);
+
+/* Debug / parity: mz_debug_wide_tower with every board split across a CTA pair: the same arguments, data and outputs (plan
+ * as mz_debug_wide_pair_tower_plan fills it).  It always runs the pair kernel on a shape its planner accepts, including
+ * boards one CTA could hold.  MZ_EUNSUPPORTED when the pair refuses the shape. */
+int mz_debug_wide_pair_tower(int device, int32_t n, int32_t H, int32_t W, int32_t blocks, int32_t site, int32_t parts, int32_t A,
+                             const float* x, const float* w, const float* bias, const int32_t* action, const int32_t* parent,
+                             int32_t pool_stride, float* out, int64_t* launches, int32_t* saturated, int64_t* plan);
+
 /* Routes of the residual heads (route argument of mz_debug_heads_plan and mz_debug_heads, plan[0]).  The network always
  * takes MZ_HEADS_PLANNED: heads_kernel<32> (one warp per sample) when C*H*W <= 1024, heads_kernel<128> (128 threads per
  * sample) otherwise, the generic route (one plain kernel per stage) when the head weights and one sample's tile exceed

@@ -33,20 +33,26 @@ struct WideTowerArgs {
     int S, plane_bytes, res_off, bar_off;
 };
 
-// Launch plan of one wide tower (host only; the launcher and mz_debug_wide_tower_plan both take it from here)
+// Launch plan of one wide tower (host only; the launchers, mz_debug_wide_tower_plan and mz_debug_wide_pair_tower_plan take it
+// from here).  On CTA pairs every per-CTA field describes one CTA holding pair_rows0 = ceil(H / 2) board rows.
 struct WideTowerPlan {
-    int m_tiles, threads;         // 64-row M-tiles of the H x (W + 1) board rows, one warpgroup each
+    int m_tiles, threads;         // 64-row M-tiles of the (per-CTA) board rows x (W + 1), one warpgroup each
     int rows;                     // shared-memory rows of one activation plane (guard + zero rows + board, multiple of 8)
     int stages;                   // weight ring stages (one tap x one 64-channel K-half each)
     size_t smem;                  // dynamic shared-memory bytes
     int layers;
-    int ctas_per_sm, wave;        // resident CTAs (one board each) per SM and on the device
+    int ctas_per_sm, wave;        // resident CTAs per SM; boards per wave on the device (CTA pairs: ctas_per_sm x SMs / 2)
     int launches;                 // kernel launches per tower call
     int reg_cap;                  // registers per thread the plan assumes (__launch_bounds__ of the kernel)
+    int pair_rows0;               // CTA pairs: board rows of CTA 0 (CTA 1 takes the rest); 0 on the one-CTA route
 };
 
 // false with the reason in *why when the wide tower refuses the shape (the network then keeps the CUDA-core towers)
 bool wide_tower_plan(int n, int C, int H, int W, int layers, int sm_count, WideTowerPlan* p, const char** why);
 cudaError_t launch_wide_tower(WideTowerArgs a, const WideTowerPlan& p, cudaStream_t stream);
+// The same tower with each board split across a cluster of two CTAs (rows [0, pair_rows0) and the rest), for boards one CTA
+// cannot hold (15 x 15, 16 x 16); it accepts every board with H >= 2 whose half fits the one-CTA budget.
+bool wide_pair_plan(int n, int C, int H, int W, int layers, int sm_count, WideTowerPlan* p, const char** why);
+cudaError_t launch_wide_pair_tower(WideTowerArgs a, const WideTowerPlan& p, cudaStream_t stream);
 
 }  // namespace mz

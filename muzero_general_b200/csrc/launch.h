@@ -36,4 +36,19 @@ cudaError_t launch_chained(void (*kernel)(KArgs...), dim3 grid, dim3 block, size
     return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
+// launch_chained for a kernel launched in thread-block clusters of `cluster` CTAs (the grid a multiple of it)
+template <typename... KArgs, typename... Args>
+cudaError_t launch_chained_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, dim3 cluster, size_t smem, cudaStream_t stream,
+                                   Args&&... args) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+    cudaLaunchAttribute attr[2];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+    attr[1].id = cudaLaunchAttributeClusterDimension;
+    attr[1].val.clusterDim.x = cluster.x; attr[1].val.clusterDim.y = cluster.y; attr[1].val.clusterDim.z = cluster.z;
+    cfg.attrs = attr; cfg.numAttrs = 2;
+    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
+
 }  // namespace mz

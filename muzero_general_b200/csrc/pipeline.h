@@ -107,12 +107,14 @@ bool resnet_small_tower_plan(int n, int in_channels, int C, int H, int W, int bl
 int resnet_debug_small_tower(int n, int in_channels, int C, int H, int W, int blocks, int site, int parts, int A, const float* x,
                              const float* w, const float* bias, const int32_t* action, const int32_t* parent, int pool_stride,
                              float* out, int64_t* plan, int sm_count, std::string* err);
-// Host-only plan of the wide 128-channel tower (plan[9], see include/mzb200.h, mz_debug_wide_tower_plan) and the debug / parity
-// entry behind mz_debug_wide_tower: one wide tower of one call site of resnet_inference on host NCHW data
-bool resnet_wide_tower_plan(int n, int C, int H, int W, int blocks, bool stem, int sm_count, int64_t* plan, std::string* err);
+// Host-only plan of the wide 128-channel tower (plan[9], see include/mzb200.h, mz_debug_wide_tower_plan; with `pair`
+// mz_debug_wide_pair_tower_plan) and the debug / parity entry behind mz_debug_wide_tower (mz_debug_wide_pair_tower): one wide
+// tower of one call site of resnet_inference on host NCHW data, one CTA (a CTA pair) per board
+bool resnet_wide_tower_plan(int n, int C, int H, int W, int blocks, bool stem, int sm_count, int64_t* plan, std::string* err,
+                            bool pair = false);
 int resnet_debug_wide_tower(int n, int H, int W, int blocks, int site, int parts, int A, const float* x, const float* w,
                             const float* bias, const int32_t* action, const int32_t* parent, int pool_stride, float* out,
-                            int64_t* launches, int32_t* saturated, int64_t* plan, int sm_count, std::string* err);
+                            int64_t* launches, int32_t* saturated, int64_t* plan, int sm_count, std::string* err, bool pair = false);
 // Host-only plan of one heads call (plan[5], see include/mzb200.h, mz_debug_heads_plan) and the debug / parity entry behind
 // mz_debug_heads: the heads of one call site of resnet_inference on host NCHW data, in any of the three state layouts
 bool resnet_heads_plan(int n, int g0, int C, int H, int W, int site, int layout, int route, const int32_t* shapes, int sm_count,

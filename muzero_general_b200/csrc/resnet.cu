@@ -395,6 +395,7 @@ struct ResNetDevice {
     int state_elems = 0;               // float slots per stored hidden state (dense C*H*W, or 2048 = 4096 fp16 for P64C8)
     bool wide = false;                 // MZ_TC_WIDE=1: 128-channel towers on the tensor cores, x3 numerics, dense states (conv_wide.cu)
     std::string wide_refused;          // MZ_TC_WIDE=1 on a 128-channel net whose board the wide towers refuse: numerics with the reason
+    bool wide_pair = false;            // with `wide`: each board split across a CTA pair (MZ_TC_WIDE=2, boards one CTA refuses)
 };
 
 static int conv_out(int h, int stride) { return (h - 1) / stride + 1; }
@@ -565,13 +566,20 @@ ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, s
     }
     // MZ_TC_WIDE=1 (opt-in until measured): the towers of a 128-channel net as x3 tensor-core launches on the dense states
     // (conv_wide.cu), when the planner accepts the hidden board.  The stems and the heads stay on the CUDA cores.
+    // MZ_TC_WIDE=2: the same, and a board the one-CTA plan refuses (15 x 15, 16 x 16) is split across CTA pairs.
     const char* wide_env = getenv("MZ_TC_WIDE");
-    if (wide_env && wide_env[0] == '1' && !tc_off && !(tc_mode && strcmp(tc_mode, "fp16") == 0) && net.channels == kWideC &&
-        !net.downsample) {
+    if (wide_env && (wide_env[0] == '1' || wide_env[0] == '2') && !tc_off && !(tc_mode && strcmp(tc_mode, "fp16") == 0) &&
+        net.channels == kWideC && !net.downsample) {
         WideTowerPlan p;
         const char* why = "";
         r->wide = wide_tower_plan(max_batch, net.channels, r->hh, r->hw, 1 + 2 * net.blocks, sm_count, &p, &why);
-        if (!r->wide) r->wide_refused = std::string("f32 nets + f64 tree statistics (128-channel towers stay on the CUDA cores: ") + why + ")";
+        std::string reasons = why;
+        if (!r->wide && wide_env[0] == '2') {
+            const char* why_pair = "";
+            r->wide = r->wide_pair = wide_pair_plan(max_batch, net.channels, r->hh, r->hw, 1 + 2 * net.blocks, sm_count, &p, &why_pair);
+            reasons = std::string("one CTA: ") + why + "; CTA pairs: " + why_pair;
+        }
+        if (!r->wide) r->wide_refused = "f32 nets + f64 tree statistics (128-channel towers stay on the CUDA cores: " + reasons + ")";
     }
     const char* no_fuse = getenv("MZ_NO_FUSE");
     r->fuse_small = !(no_fuse && no_fuse[0] == '1');
@@ -1115,14 +1123,14 @@ struct Runner {
     }
 
     // [optional stem conv] + `count` residual blocks of a 128-channel net as ONE x3 tensor-core launch (conv_wide.cu), dense
-    // NCHW in and out.  Returns what small_tower returns: 1 = launched, 0 = not the wide route, -1 = error.
+    // NCHW in and out, one CTA or (r->wide_pair) one CTA pair per board.  Returns what small_tower returns: 1 = launched, 0 = not the wide route, -1 = error.
     int wide_tower(const std::vector<ConvLayer>& layers, size_t first, bool stem, size_t count, const float* in, float* out,
                    const int32_t* gather_parent = nullptr, int pool_stride = 0, const int32_t* action = nullptr) {
         const int nl = (stem ? 1 : 0) + 2 * (int)count;
         if (!r->wide || nl == 0) return 0;
         WideTowerPlan p;
         const char* why = "";
-        if (!wide_tower_plan(n, r->C, r->hh, r->hw, nl, r->sm_count, &p, &why)) return 0;
+        if (!(r->wide_pair ? wide_pair_plan : wide_tower_plan)(n, r->C, r->hh, r->hw, nl, r->sm_count, &p, &why)) return 0;
         WideTowerArgs a{};
         a.in = in; a.out = out; a.gather_parent = gather_parent; a.pool_stride = pool_stride; a.action = action;
         a.n = n; a.H = r->hh; a.W = r->hw; a.A = r->net.action_space; a.g0 = g0; a.stem = stem ? 1 : 0; a.n_layers = nl;
@@ -1137,7 +1145,7 @@ struct Runner {
         }
         if (wide_plan_out) *wide_plan_out = p;
         kt_begin(KT_TOWER, stream);
-        cudaError_t e = launch_wide_tower(a, p, stream);
+        cudaError_t e = r->wide_pair ? launch_wide_pair_tower(a, p, stream) : launch_wide_tower(a, p, stream);
         kt_end(stream);
         if (e != cudaSuccess) { fail("wide tower launch", e); return -1; }
         *launches += p.launches;
@@ -1416,6 +1424,9 @@ bool resnet_can_partition(const ResNetDevice* r0) {
     return ((size_t)(hi - lo) + warp_floats) * 4 <= 227 * 1024;
 }
 const char* resnet_numerics(const ResNetDevice* r) {
+    if (r->wide && r->wide_pair)
+        return "f32-grade nets (128-channel towers on the tensor cores, boards split across CTA pairs, split fp16 operands "
+               "x = x_h + x_l/2^11, 3 partial products, f32 accumulate; f32 stems and heads) + f64 tree statistics";
     if (r->wide)
         return "f32-grade nets (128-channel towers on the tensor cores, split fp16 operands x = x_h + x_l/2^11, 3 partial "
                "products, f32 accumulate; f32 stems and heads) + f64 tree statistics";
@@ -1440,7 +1451,7 @@ int resnet_take_saturations(ResNetDevice* r, cudaStream_t stream) {
 }
 void resnet_use_strict(ResNetDevice* r) {
     r->fell_back = r->wide ? 2 : 1;
-    r->use_tc = false; r->split = false; r->wide = false;
+    r->use_tc = false; r->split = false; r->wide = false; r->wide_pair = false;
     r->state_elems = r->C * r->hh * r->hw;           // dense NCHW states: smaller than the board layout, the pool fits
 }
 
@@ -1812,22 +1823,30 @@ int resnet_debug_small_tower(int n, int in_channels, int C, int H, int W, int bl
 // Launch plan of the wide tower (host only, behind mz_debug_wide_tower_plan): plan[9] = {M-tiles, threads, shared-memory bytes,
 // weight ring stages, layers, CTAs per SM, boards per wave, launches, registers per thread assumed} of n boards of C x H x W
 // through [a stem conv +] `blocks` residual blocks.  false with the reason in *err when the wide towers refuse the shape.
-bool resnet_wide_tower_plan(int n, int C, int H, int W, int blocks, bool stem, int sm_count, int64_t* plan, std::string* err) {
+// With `pair`, the plan of the CTA-pair tower (mz_debug_wide_pair_tower_plan): plan[9] = {board rows of CTA 0, M-tiles per
+// CTA, threads per CTA, shared-memory bytes per CTA, weight ring stages, layers, boards (clusters) per wave, launches,
+// registers per thread assumed}.
+static void wide_plan_export(const WideTowerPlan& p, bool pair, int64_t* plan) {
+    const int64_t one[9] = {p.m_tiles, p.threads, (int64_t)p.smem, p.stages, p.layers, p.ctas_per_sm, p.wave, p.launches, p.reg_cap};
+    const int64_t two[9] = {p.pair_rows0, p.m_tiles, p.threads, (int64_t)p.smem, p.stages, p.layers, p.wave, p.launches, p.reg_cap};
+    for (int i = 0; i < 9; ++i) plan[i] = pair ? two[i] : one[i];
+}
+bool resnet_wide_tower_plan(int n, int C, int H, int W, int blocks, bool stem, int sm_count, int64_t* plan, std::string* err,
+                            bool pair) {
     if (blocks < 0) { *err = "bad shape"; return false; }
     WideTowerPlan p;
     const char* why = "";
-    if (!wide_tower_plan(n, C, H, W, (stem ? 1 : 0) + 2 * blocks, sm_count, &p, &why)) { *err = why; return false; }
-    const int64_t out[9] = {p.m_tiles, p.threads, (int64_t)p.smem, p.stages, p.layers, p.ctas_per_sm, p.wave, p.launches, p.reg_cap};
-    for (int i = 0; i < 9; ++i) plan[i] = out[i];
+    if (!(pair ? wide_pair_plan : wide_tower_plan)(n, C, H, W, (stem ? 1 : 0) + 2 * blocks, sm_count, &p, &why)) { *err = why; return false; }
+    wide_plan_export(p, pair, plan);
     return true;
 }
 
 // Stand-alone wide tower of one call site of resnet_inference, through the same Runner helpers and weight packing, on host
-// NCHW data (128 channels).  The output and the pool's other slots start as NaN bytes (0xFF), so a board the tower does not
+// NCHW data (128 channels); with `pair` always on the CTA-pair kernel.  The output and the pool's other slots start as NaN bytes (0xFF), so a board the tower does not
 // write, or one read from the wrong slot, produces NaN.
 int resnet_debug_wide_tower(int n, int H, int W, int blocks, int site, int parts, int A, const float* x, const float* w,
                             const float* bias, const int32_t* action, const int32_t* parent, int pool_stride, float* out,
-                            int64_t* launches, int32_t* saturated, int64_t* plan, int sm_count, std::string* err) {
+                            int64_t* launches, int32_t* saturated, int64_t* plan, int sm_count, std::string* err, bool pair) {
     constexpr int C = kWideC;
     const bool stem = site == MZ_TOWER_DYNAMICS || site == MZ_TOWER_DYNAMICS_POOL;
     const bool in_pool = site == MZ_TOWER_DYNAMICS_POOL;
@@ -1846,8 +1865,8 @@ int resnet_debug_wide_tower(int n, int H, int W, int blocks, int site, int parts
     {
         int64_t unused[9];
         std::string why;
-        if (!resnet_wide_tower_plan(n, C, H, W, blocks, stem, sm_count, unused, &why)) {
-            *err = "the wide tower refuses the shape: " + why; return MZ_EUNSUPPORTED;
+        if (!resnet_wide_tower_plan(n, C, H, W, blocks, stem, sm_count, unused, &why, pair)) {
+            *err = std::string(pair ? "the wide pair tower" : "the wide tower") + " refuses the shape: " + why; return MZ_EUNSUPPORTED;
         }
     }
     const int n_convs = (stem ? 1 : 0) + 2 * blocks;
@@ -1864,7 +1883,7 @@ int resnet_debug_wide_tower(int n, int H, int W, int blocks, int site, int parts
     nd.kind = MZ_NET_RESNET; nd.channels = C; nd.obs_c = C; nd.obs_h = H; nd.obs_w = W; nd.action_space = stem ? A : 1;
     nd.blocks = blocks;
     ResNetDevice r{};
-    r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = H; r.hw = W; r.wide = true;
+    r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = H; r.hw = W; r.wide = true; r.wide_pair = pair;
     Loader L{tensors.data(), n_convs, err};
     std::vector<float> blob;
     std::vector<ConvLayer> layers;
@@ -1930,9 +1949,7 @@ int resnet_debug_wide_tower(int n, int H, int W, int blocks, int site, int parts
         if (e == cudaSuccess) e = cudaMemcpy(&sat, r.d_sat, 4, cudaMemcpyDeviceToHost);
         if (e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug wide tower: ") + cudaGetErrorString(e); }
         if (saturated) *saturated = sat;
-        const int64_t pl[9] = {first.m_tiles, first.threads, (int64_t)first.smem, first.stages, first.layers, first.ctas_per_sm,
-                               first.wave, first.launches, first.reg_cap};
-        if (plan) for (int i = 0; i < 9; ++i) plan[i] = pl[i];
+        if (plan) wide_plan_export(first, pair, plan);
     }
     cleanup();
     return rc;

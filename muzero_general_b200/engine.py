@@ -708,14 +708,27 @@ def debug_small_tower(x, weights, biases=None, site="prediction", actions=None, 
 WIDE_TOWER_PLAN = ("m_tiles", "threads", "smem", "stages", "layers", "ctas_per_sm", "wave", "launches", "reg_cap")
 
 
+WIDE_PAIR_TOWER_PLAN = ("rows0", "m_tiles", "threads", "smem", "stages", "layers", "wave", "launches", "reg_cap")
+
+
 def debug_wide_tower_plan(n, channels, H, W, blocks, stem, sm_count):
     """Launch plan of the 128-channel x3 tensor-core tower (mz_debug_wide_tower_plan, host only): (a dict of
     WIDE_TOWER_PLAN, "") or (None, the reason) when the wide towers refuse the shape."""
+    return _wide_plan("mz_debug_wide_tower_plan", WIDE_TOWER_PLAN, n, channels, H, W, blocks, stem, sm_count)
+
+
+def debug_wide_pair_tower_plan(n, channels, H, W, blocks, stem, sm_count):
+    """Launch plan of the same tower with each board split across a CTA pair (mz_debug_wide_pair_tower_plan, host only):
+    (a dict of WIDE_PAIR_TOWER_PLAN, per-CTA figures except ``wave``, the boards per wave), "") or (None, the reason)."""
+    return _wide_plan("mz_debug_wide_pair_tower_plan", WIDE_PAIR_TOWER_PLAN, n, channels, H, W, blocks, stem, sm_count)
+
+
+def _wide_plan(entry, fields, n, channels, H, W, blocks, stem, sm_count):
     lib = _lib.load_library()
     out = (C.c_int64 * 9)()
-    if not lib.mz_debug_wide_tower_plan(n, channels, H, W, blocks, int(stem), sm_count, out):
+    if not getattr(lib, entry)(n, channels, H, W, blocks, int(stem), sm_count, out):
         return None, lib.mz_last_error(None).decode()
-    return dict(zip(WIDE_TOWER_PLAN, out)), ""
+    return dict(zip(fields, out)), ""
 
 
 def debug_wide_tower(x, weights, biases=None, site="prediction", actions=None, A=1, parents=None, pool_stride=1, parts=1,
@@ -724,6 +737,19 @@ def debug_wide_tower(x, weights, biases=None, site="prediction", actions=None, A
     x is [n, 128, H, W]; ``weights`` the convs in order ([128, 129, 3, 3] dynamics stem first, then two [128, 128, 3, 3]
     per block), ``biases`` one [128] per conv.  ``site`` as for debug_conv_tower.  Returns (out [n, 128, H, W], kernel
     launches, range-guard count, the plan of the launch as a dict)."""
+    return _wide_tower("mz_debug_wide_tower", WIDE_TOWER_PLAN, x, weights, biases, site, actions, A, parents, pool_stride,
+                       parts, device)
+
+
+def debug_wide_pair_tower(x, weights, biases=None, site="prediction", actions=None, A=1, parents=None, pool_stride=1,
+                          parts=1, device=0):
+    """debug_wide_tower with every board split across a CTA pair (mz_debug_wide_pair_tower), on any board the pair's
+    planner accepts; the plan is a dict of WIDE_PAIR_TOWER_PLAN."""
+    return _wide_tower("mz_debug_wide_pair_tower", WIDE_PAIR_TOWER_PLAN, x, weights, biases, site, actions, A, parents,
+                       pool_stride, parts, device)
+
+
+def _wide_tower(entry, fields, x, weights, biases, site, actions, A, parents, pool_stride, parts, device):
     lib = _lib.load_library()
     x = numpy.ascontiguousarray(x, numpy.float32)
     n, ch, H, W = x.shape
@@ -742,13 +768,13 @@ def debug_wide_tower(x, weights, biases=None, site="prediction", actions=None, A
     out = numpy.empty_like(x)
     launches, sat = C.c_int64(0), C.c_int32(0)
     plan = (C.c_int64 * 9)()
-    rc = lib.mz_debug_wide_tower(device, n, H, W, (len(weights) - stem) // 2, TOWER_SITES[site], parts, A, x.ctypes.data,
-                                 wcat.ctypes.data, None if b is None else b.ctypes.data,
-                                 None if act is None else act.ctypes.data, None if par is None else par.ctypes.data,
-                                 pool_stride, out.ctypes.data, C.byref(launches), C.byref(sat), plan)
+    rc = getattr(lib, entry)(device, n, H, W, (len(weights) - stem) // 2, TOWER_SITES[site], parts, A, x.ctypes.data,
+                             wcat.ctypes.data, None if b is None else b.ctypes.data,
+                             None if act is None else act.ctypes.data, None if par is None else par.ctypes.data,
+                             pool_stride, out.ctypes.data, C.byref(launches), C.byref(sat), plan)
     if rc != 0:
         raise _lib.MzError(rc, lib.mz_last_error(None).decode())
-    return out, launches.value, sat.value, dict(zip(WIDE_TOWER_PLAN, plan))
+    return out, launches.value, sat.value, dict(zip(fields, plan))
 
 
 HEADS_ROUTES = {"planned": 0, "warp": 1, "wide": 2, "generic": 3}

@@ -11,6 +11,11 @@ process, with synthetic weights (seed 0; the rates do not depend on them):
             of one more search with mz_kernel_timing on.
   selfplay  SelfPlay.play_moves env-steps/s on the device loop, 128 games, N = 400, 1 warm-up move + 3 timed moves.
 
+--side S (default 11) puts the net on S x S boards (games.gomoku.MuZeroConfig(board_size=S)).  --route pair measures the CTA-pair
+kernel (conv_tower_wide_pair_kernel through mz_debug_wide_pair_tower; MZ_TC_WIDE=2 for the search and the device loop) in
+place of the one-CTA kernel: at sides the one-CTA plan refuses (15, 16) against the CUDA cores as above, and at 11 x 11, for
+information, its tower alone against the one-CTA kernel's, in two rounds that alternate the routes.
+
 Prints one JSON line per measurement and a last line with the card's name and power limit."""
 import argparse
 import json
@@ -25,7 +30,8 @@ sys.path[:0] = [ROOT, os.path.join(ROOT, "scripts")]
 
 from device_games_rate import card, rate  # noqa: E402
 
-C, H, W, BLOCKS = 128, 11, 11, 6
+C, BLOCKS = 128, 6
+H = W = 11
 
 
 def tower_flops(n):
@@ -43,26 +49,35 @@ def _timed(eng, fn, reps, cls):
     return out
 
 
-def towers(eng, reps):
-    from muzero_general_b200.engine import debug_conv3x3, debug_wide_tower
+def towers(eng, reps, routes=("wide_x3", "cuda_core"), rounds=1):
+    from muzero_general_b200.engine import debug_conv3x3, debug_wide_pair_tower, debug_wide_tower
     rs = numpy.random.RandomState(0)
+    A = H * W
     for n in (128, 1024):
         x = rs.standard_normal((n, C, H, W)).astype(numpy.float32)
         ws = [(rs.standard_normal((C, C + 1 if i == 0 else C, 3, 3)) / 34).astype(numpy.float32) for i in range(1 + 2 * BLOCKS)]
         bs = [numpy.zeros(C, numpy.float32) for _ in ws]
-        act = rs.randint(0, 121, n).astype(numpy.int32)
+        act = rs.randint(0, A, n).astype(numpy.int32)
         par = numpy.zeros(n, numpy.int32)
-        wide = _timed(eng, lambda: debug_wide_tower(x, ws, bs, site="dynamics_pool", actions=act, A=121, parents=par,
-                                                    pool_stride=1), reps, "conv_tower_tc_kernel")
         xs = numpy.concatenate([x, numpy.zeros((n, 1, H, W), numpy.float32)], 1)
-        stem = _timed(eng, lambda: debug_conv3x3(xs, ws[0], bs[0], relu=True), reps, "conv3x3_kernel")
-        body = _timed(eng, lambda: debug_conv3x3(x, ws[1], bs[1], relu=True), reps, "conv3x3_kernel")
-        core = [s + 2 * BLOCKS * b for s, b in zip(stem, body)]
-        for route, ms in (("wide_x3", wide), ("cuda_core", core)):
-            med = float(numpy.median(ms))
-            print(json.dumps({"measure": "tower_dynamics_pool", "route": route, "boards": n, "reps": reps,
-                              "ms_median": round(med, 4), "ms_min": round(min(ms), 4), "ms_max": round(max(ms), 4),
-                              "tflops": round(tower_flops(n) / (med * 1e-3) / 1e12, 2)}), flush=True)
+
+        def timed(route):
+            if route == "cuda_core":
+                stem = _timed(eng, lambda: debug_conv3x3(xs, ws[0], bs[0], relu=True), reps, "conv3x3_kernel")
+                body = _timed(eng, lambda: debug_conv3x3(x, ws[1], bs[1], relu=True), reps, "conv3x3_kernel")
+                return [s + 2 * BLOCKS * b for s, b in zip(stem, body)]
+            fn = debug_wide_pair_tower if route == "pair_x3" else debug_wide_tower
+            return _timed(eng, lambda: fn(x, ws, bs, site="dynamics_pool", actions=act, A=A, parents=par, pool_stride=1),
+                          reps, "conv_tower_tc_kernel")
+
+        for k in range(rounds):
+            for route in routes:
+                ms = timed(route)
+                med = float(numpy.median(ms))
+                print(json.dumps({"measure": "tower_dynamics_pool", "route": route, **({"side": H} if H != 11 else {}), "boards": n, "reps": reps,
+                                  **({"round": k} if rounds > 1 else {}),
+                                  "ms_median": round(med, 4), "ms_min": round(min(ms), 4), "ms_max": round(max(ms), 4),
+                                  "tflops": round(tower_flops(n) / (med * 1e-3) / 1e12, 2)}), flush=True)
 
 
 def search(cfg, weights, route):
@@ -88,31 +103,42 @@ def search(cfg, weights, route):
 
 
 def main():
+    global H, W
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=7)
     ap.add_argument("--skip-selfplay", action="store_true")
+    ap.add_argument("--side", type=int, default=11, help="board side of the Gomoku net (11, 15 or 16)")
+    ap.add_argument("--route", choices=("wide", "pair"), default="wide",
+                    help="tensor-core route: the one-CTA kernel (MZ_TC_WIDE=1) or CTA pairs (MZ_TC_WIDE=2)")
     args = ap.parse_args()
     from muzero_general_b200.engine import SearchEngine
     from muzero_general_b200.games import load_game_module
     from muzero_general_b200.netspec import netspec_from_config, synthetic_weights
 
+    H = W = args.side
     name, power = card()
     mod = load_game_module("gomoku")
-    cfg = mod.MuZeroConfig()
+    cfg = mod.MuZeroConfig(board_size=args.side)
     weights = synthetic_weights(netspec_from_config(cfg), 0)
+    tc_route, switch = ("pair_x3", "2") if args.route == "pair" else ("wide_x3", "1")
     probe = SearchEngine(cfg, max_games=1, num_simulations=1)       # a handle to switch mz_kernel_timing on
     probe.kernel_timing(True)
-    towers(probe, args.reps)
+    if args.route == "pair" and args.side == 11:                    # for information: the pair against one CTA
+        towers(probe, args.reps, ("pair_x3", "wide_x3"), rounds=2)
+    else:
+        towers(probe, args.reps, (tc_route, "cuda_core"))
     probe.kernel_timing(False)
     probe.close()
-    for route in ("wide_x3", "cuda_core"):
-        if route == "wide_x3":
-            os.environ["MZ_TC_WIDE"] = "1"
+    for route in (tc_route, "cuda_core"):
+        if args.route == "pair" and args.side == 11:
+            break
+        if route == tc_route:
+            os.environ["MZ_TC_WIDE"] = switch
         else:
             os.environ.pop("MZ_TC_WIDE", None)
         search(cfg, weights, route)
         if not args.skip_selfplay:
-            c = mod.MuZeroConfig()
+            c = mod.MuZeroConfig(board_size=args.side)
             c.rng_mode, c.num_parallel_games = "philox", 128
             r, steps, dt = rate(mod, c, weights, True, 1, 3, 0.0)
             print(json.dumps({"measure": "selfplay_device_128x400", "route": route, "env_steps_per_s": round(r, 2),
