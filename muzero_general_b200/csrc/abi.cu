@@ -19,6 +19,7 @@
 
 #include "handle.h"
 #include "cnn_stem.h"
+#include "conv_wide.h"
 #include "small_search.h"
 
 using namespace mz;
@@ -1016,9 +1017,10 @@ extern "C" int mz_debug_conv_tower(int device, int32_t n, int32_t H, int32_t W, 
     if (cudaSetDevice(device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_conv_tower: no such device");
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_conv_tower: device query failed");
+    if (mode != 1 && mode != 2) return fail(nullptr, MZ_EINVAL, "mz_debug_conv_tower: bad shape, site or mode");
     std::string e;
-    int rc = resnet_debug_tower(n, H, W, mode, blocks, site, parts, A, x, w, bias, action, parent, pool_stride, out, launches,
-                                saturated, prop.multiProcessorCount, &e);
+    int rc = resnet_debug_tower(mode == 2 ? TowerRoute::TcX3 : TowerRoute::TcF16, n, 64, 64, H, W, blocks, site, parts, A, x, w,
+                                bias, action, parent, pool_stride, out, launches, saturated, nullptr, prop.multiProcessorCount, &e);
     if (rc) return fail(nullptr, rc, "mz_debug_conv_tower: " + e);
     return MZ_OK;
 }
@@ -1041,8 +1043,8 @@ extern "C" int mz_debug_small_tower(int device, int32_t n, int32_t in_channels, 
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_small_tower: device query failed");
     std::string e;
-    int rc = resnet_debug_small_tower(n, in_channels, C, H, W, blocks, site, parts, A, x, w, bias, action, parent, pool_stride, out,
-                                      plan, prop.multiProcessorCount, &e);
+    int rc = resnet_debug_tower(TowerRoute::CudaCore, n, in_channels, C, H, W, blocks, site, parts, A, x, w, bias, action, parent,
+                                pool_stride, out, nullptr, nullptr, plan, prop.multiProcessorCount, &e);
     if (rc) return fail(nullptr, rc, "mz_debug_small_tower: " + e);
     return MZ_OK;
 }
@@ -1065,8 +1067,8 @@ extern "C" int mz_debug_wide_tower(int device, int32_t n, int32_t H, int32_t W, 
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_wide_tower: device query failed");
     std::string e;
-    int rc = resnet_debug_wide_tower(n, H, W, blocks, site, parts, A, x, w, bias, action, parent, pool_stride, out, launches,
-                                     saturated, plan, prop.multiProcessorCount, &e);
+    int rc = resnet_debug_tower(TowerRoute::Wide, n, kWideC, kWideC, H, W, blocks, site, parts, A, x, w, bias, action, parent,
+                                pool_stride, out, launches, saturated, plan, prop.multiProcessorCount, &e);
     if (rc) return fail(nullptr, rc, "mz_debug_wide_tower: " + e);
     return MZ_OK;
 }
@@ -1090,8 +1092,8 @@ extern "C" int mz_debug_wide_pair_tower(int device, int32_t n, int32_t H, int32_
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_wide_pair_tower: device query failed");
     std::string e;
-    int rc = resnet_debug_wide_tower(n, H, W, blocks, site, parts, A, x, w, bias, action, parent, pool_stride, out, launches,
-                                     saturated, plan, prop.multiProcessorCount, &e, true);
+    int rc = resnet_debug_tower(TowerRoute::WidePair, n, kWideC, kWideC, H, W, blocks, site, parts, A, x, w, bias, action, parent,
+                                pool_stride, out, launches, saturated, plan, prop.multiProcessorCount, &e);
     if (rc) return fail(nullptr, rc, "mz_debug_wide_pair_tower: " + e);
     return MZ_OK;
 }

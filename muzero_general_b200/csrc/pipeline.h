@@ -82,6 +82,14 @@ cudaError_t launch_tree_step(const TreeStepArgs& a, cudaStream_t stream);
 cudaError_t launch_tree_step_wide(const TreeStepArgs& a, cudaStream_t stream);      // 32 < |A| <= 256 (tree_wide.cu)
 cudaError_t launch_tree_adopt_root(const TreeStepArgs& a, cudaStream_t stream);     // MZ_FLAG_CONTINUE: adopt the imported tree
 
+// How a residual net runs its towers, chosen once at resnet_create (resnet_use_strict moves a guarded route to CudaCore).
+//   CudaCore  fp32 conv3x3_kernel / fused small towers, dense NCHW states
+//   TcF16     64-channel tensor-core towers on fp16 operands (MZ_TC_MODE=fp16), P64C8 board states
+//   TcX3      64-channel tensor-core towers on split operands (default where the board allows), x_h | x_l board states
+//   Wide      128-channel x3 tensor-core towers, one CTA per board (MZ_TC_WIDE=1), dense states
+//   WidePair  the same, each board split across a CTA pair (MZ_TC_WIDE=2), dense states
+enum class TowerRoute { CudaCore, TcF16, TcX3, Wide, WidePair };
+
 struct ResNetDevice;
 ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, std::string* err);
 void resnet_destroy(ResNetDevice* r);
@@ -90,31 +98,26 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
 int resnet_debug_conv(int n, int cin, int cout, int H, int W, int stride, const float* x, const float* w_oihw, const float* bias,
                       const float* residual, int relu, int use_tc, float* out, int sm_count, std::string* err);
 bool resnet_conv_plan(int n, int cin, int cout, int H, int W, int stride, int64_t* plan, std::string* err);   // host only
-const char* resnet_numerics(const ResNetDevice* r);
+const char* resnet_numerics(const ResNetDevice* r);                  // arithmetic of the residual towers (bench.py dtype)
 int resnet_take_saturations(ResNetDevice* r, cudaStream_t stream);   // x3 range guard (synchronises)
 bool resnet_can_partition(const ResNetDevice* r);
 // games per range of the partitioned replay (the last range may hold fewer): a multiple of 8
 inline int partition_games(int n, int parts) { return ((n + parts - 1) / parts + 7) & ~7; }
-// Debug / parity entry behind mz_debug_conv_tower: one tensor-core tower of one call site of resnet_inference_tc on host NCHW
-// data (see include/mzb200.h)
-int resnet_debug_tower(int n, int H, int W, int mode, int blocks, int site, int parts, int A, const float* x, const float* w,
-                       const float* bias, const int32_t* action, const int32_t* parent, int pool_stride, float* out,
-                       int64_t* launches, int32_t* saturated, int sm_count, std::string* err);
-// Host-only plan of the fused CUDA-core tower (plan[6], see include/mzb200.h, mz_debug_small_tower_plan) and the debug /
-// parity entry behind mz_debug_small_tower: one fused CUDA-core tower of one call site of resnet_inference on host NCHW data
+// Debug / parity entry behind mz_debug_conv_tower (route TcF16 / TcX3, C = 64), mz_debug_small_tower (CudaCore: the fused
+// CUDA-core tower), mz_debug_wide_tower (Wide, C = 128) and mz_debug_wide_pair_tower (WidePair): one tower of one call site
+// of the network on host NCHW data (see include/mzb200.h).  `in_channels` is the planes the representation stem reads
+// (CudaCore only; C otherwise); `launches`, `saturated` and `plan` (plan[6] fused, plan[9] wide) may be null.
+int resnet_debug_tower(TowerRoute route, int n, int in_channels, int C, int H, int W, int blocks, int site, int parts, int A,
+                       const float* x, const float* w, const float* bias, const int32_t* action, const int32_t* parent,
+                       int pool_stride, float* out, int64_t* launches, int32_t* saturated, int64_t* plan, int sm_count,
+                       std::string* err);
+// Host-only plan of the fused CUDA-core tower (plan[6], see include/mzb200.h, mz_debug_small_tower_plan)
 bool resnet_small_tower_plan(int n, int in_channels, int C, int H, int W, int blocks, bool stem, int sm_count, int64_t* plan,
                              std::string* err);
-int resnet_debug_small_tower(int n, int in_channels, int C, int H, int W, int blocks, int site, int parts, int A, const float* x,
-                             const float* w, const float* bias, const int32_t* action, const int32_t* parent, int pool_stride,
-                             float* out, int64_t* plan, int sm_count, std::string* err);
 // Host-only plan of the wide 128-channel tower (plan[9], see include/mzb200.h, mz_debug_wide_tower_plan; with `pair`
-// mz_debug_wide_pair_tower_plan) and the debug / parity entry behind mz_debug_wide_tower (mz_debug_wide_pair_tower): one wide
-// tower of one call site of resnet_inference on host NCHW data, one CTA (a CTA pair) per board
+// mz_debug_wide_pair_tower_plan), one CTA (a CTA pair) per board
 bool resnet_wide_tower_plan(int n, int C, int H, int W, int blocks, bool stem, int sm_count, int64_t* plan, std::string* err,
                             bool pair = false);
-int resnet_debug_wide_tower(int n, int H, int W, int blocks, int site, int parts, int A, const float* x, const float* w,
-                            const float* bias, const int32_t* action, const int32_t* parent, int pool_stride, float* out,
-                            int64_t* launches, int32_t* saturated, int64_t* plan, int sm_count, std::string* err, bool pair = false);
 // Host-only plan of one heads call (plan[5], see include/mzb200.h, mz_debug_heads_plan) and the debug / parity entry behind
 // mz_debug_heads: the heads of one call site of resnet_inference on host NCHW data, in any of the three state layouts
 bool resnet_heads_plan(int n, int g0, int C, int H, int W, int site, int layout, int route, const int32_t* shapes, int sm_count,
@@ -127,8 +130,8 @@ int resnet_debug_heads(int n, int C, int H, int W, int site, int layout, int rou
 bool resnet_small_search_supported(ResNetDevice* r, const InferCall& first_recurrent, const TreeStepArgs& tree, int n_sims);
 int resnet_small_search(ResNetDevice* r, const InferCall& first_recurrent, const TreeStepArgs& tree, int n_sims, cudaStream_t stream,
                         int64_t* launches, std::string* err);
-bool resnet_uses_tensor_cores(const ResNetDevice* r);                    // recurrent inference honours InferCall::g0 (x3 towers / fused small towers)
-void resnet_use_strict(ResNetDevice* r);                             // fp32 CUDA-core towers from now on   // arithmetic of the residual towers (bench.py dtype)
+bool resnet_uses_tensor_cores(const ResNetDevice* r);   // the 64-channel tensor-core towers (TcF16 / TcX3)
+void resnet_use_strict(ResNetDevice* r);                // fp32 CUDA-core towers from now on (the range guard fired)
 int resnet_state_elems(const ResNetDevice* r);        // floats per stored hidden state in the pool
 int resnet_states_to_nchw(ResNetDevice* r, const float* states, int count, float* out, cudaStream_t stream);
 

@@ -383,20 +383,26 @@ struct ResNetDevice {
     float* scratch_hidden = nullptr;   // [B, C*hh*hw] rescaled state when no pool is given (dense NCHW)
     float* scratch_state = nullptr;    // [B, 4096 fp16] same state in P64C8 (tensor-core path)
     bool loaded = false;
-    bool use_tc = false;               // residual towers on the tensor cores (conv_tc.cu / conv_x3.cu)
-    bool split = false;                // x3 mode: split operands, fp32-grade accuracy (conv_x3.cu); false = plain fp16 operands
-    bool tc_capable = false;           // the shape allows the tensor-core towers at all
+    TowerRoute route = TowerRoute::CudaCore;
+    std::string note;                  // CudaCore only: mz_numerics when a tensor-core route was wanted and not taken, or left
     float* big_scratch = nullptr;      // activations of the generic heads route (heads_big)
     size_t big_elems = 0;
     int* d_sat = nullptr;              // x3 mode: number of epilogue threads that stored an activation beyond the fp16 range
-    int fell_back = 0;                 // set when the range guard switched this net to the fp32 CUDA-core towers
-    bool heads_off_tc = false;         // a 64-channel board net kept off the tensor cores because its heads exceed shared memory
     bool fuse_small = true;            // CUDA-core towers as one fused launch where they fit (small_tower.cu); MZ_NO_FUSE=1: per layer
-    int state_elems = 0;               // float slots per stored hidden state (dense C*H*W, or 2048 = 4096 fp16 for P64C8)
-    bool wide = false;                 // MZ_TC_WIDE=1: 128-channel towers on the tensor cores, x3 numerics, dense states (conv_wide.cu)
-    std::string wide_refused;          // MZ_TC_WIDE=1 on a 128-channel net whose board the wide towers refuse: numerics with the reason
-    bool wide_pair = false;            // with `wide`: each board split across a CTA pair (MZ_TC_WIDE=2, boards one CTA refuses)
 };
+
+static bool is_tc(TowerRoute t) { return t == TowerRoute::TcF16 || t == TowerRoute::TcX3; }
+static bool is_wide(TowerRoute t) { return t == TowerRoute::Wide || t == TowerRoute::WidePair; }
+// layout of the stored hidden states and of the tensor-core towers' workspaces
+static int state_layout(TowerRoute t) {
+    return t == TowerRoute::TcX3 ? kLayoutSplit : t == TowerRoute::TcF16 ? kLayoutF16 : kLayoutDense;
+}
+// the x3 range guard counts saturated activations on these routes (conv_x3.cu, conv_wide.cu)
+static bool range_guarded(TowerRoute t) { return t == TowerRoute::TcX3 || is_wide(t); }
+// float slots per stored hidden state: dense C*H*W, or a board of the tensor-core layout (2048 or 4096)
+static int state_elems(const ResNetDevice* r) {
+    return is_tc(r->route) ? conv_tc_board_elems(r->route == TowerRoute::TcX3) : r->C * r->hh * r->hw;
+}
 
 static int conv_out(int h, int stride) { return (h - 1) / stride + 1; }
 
@@ -469,7 +475,75 @@ static void layout_head(int C, int rc, int HW, const int32_t* hidden, int n_hidd
     *size = (o + 3) & ~(size_t)3;
 }
 
-static bool tc_heads_fit(ResNetDevice* r);
+// Shared memory of one heads_kernel launch over the heads hs[0, n_heads): the slice [w_lo, w_lo + w_floats) of the head
+// blob covering them, and per group of threads an x tile + channel stats + (ping, pong) rows as wide as the widest layer.
+struct HeadsFootprint { int w_lo, w_floats, smem_floats, warp_floats; };
+static HeadsFootprint heads_footprint(int C, int HW, int n_heads, const HeadDesc* const* hs) {
+    int maxw = 32, lo = 1 << 30, hi = 0;
+    for (int i = 0; i < n_heads; ++i) {
+        const HeadDesc& d = *hs[i];
+        maxw = std::max(maxw, d.rc * HW + 4);
+        for (int l = 0; l < d.mlp.n; ++l) maxw = std::max(maxw, d.mlp.out[l] + 4);
+        lo = std::min(lo, d.w1_off);
+        hi = std::max(hi, d.mlp.b_off[d.mlp.n - 1] + d.mlp.out[d.mlp.n - 1]);
+    }
+    if (n_heads == 0) { lo = 0; hi = 0; }
+    HeadsFootprint f;
+    f.w_lo = lo; f.w_floats = ((hi - lo) + 3) & ~3;
+    f.smem_floats = (maxw + 3) & ~3;
+    f.warp_floats = (HW * (C + 4) + 6 * C + 4 * f.smem_floats + 3) & ~3;
+    return f;
+}
+static bool heads_fit_one_group(const HeadsFootprint& f) { return ((size_t)f.w_floats + f.warp_floats) * 4 <= 227 * 1024; }
+
+// The tower route of a net at max_batch boards, from its shape and MZ_TC_MODE / MZ_NO_TC / MZ_TC_WIDE; *note as
+// ResNetDevice::note.  Allocates nothing.
+static TowerRoute choose_route(const MzNetDesc& net, int max_batch, int sm_count, std::string* note) {
+    // MZ_TC_MODE = "off": fp32 CUDA-core towers everywhere; anything else: tensor-core towers where the shape allows
+    // (conv_tc.cu).  MZ_NO_TC=1 is the older spelling of "off".
+    const char* no_tc = getenv("MZ_NO_TC");
+    const char* tc_mode = getenv("MZ_TC_MODE");
+    if ((no_tc && no_tc[0] == '1') || (tc_mode && strcmp(tc_mode, "off") == 0)) return TowerRoute::CudaCore;
+    // default "x3": split 16-bit operands, three partial products, fp32-grade accuracy; "fp16": plain fp16 operands
+    // (3x fewer MMAs, ~1e-2 hidden-state error: opt-in)
+    const bool fp16 = tc_mode && strcmp(tc_mode, "fp16") == 0;
+    if (!net.downsample && conv_tc_supported(net.channels, net.obs_h, net.obs_w)) {
+        // The heads of the tensor-core route read the board layout and have no generic (global-memory) variant.  A net
+        // whose head weights do not fit in shared memory next to one sample's tile (e.g. support 300, or a 128-wide value
+        // layer over 16 reduced channels) runs on the fp32 CUDA-core towers and the generic heads route instead.
+        const int C = net.channels, HW = net.obs_h * net.obs_w, F = 2 * net.support_size + 1;
+        HeadDesc reward, value, policy;
+        size_t size = 0;
+        layout_head(C, net.reduced_reward, HW, net.res_fc_reward, net.n_res_fc_reward, F, &size, reward);
+        layout_head(C, net.reduced_value, HW, net.res_fc_value, net.n_res_fc_value, F, &size, value);
+        layout_head(C, net.reduced_policy, HW, net.res_fc_policy, net.n_res_fc_policy, net.action_space, &size, policy);
+        const HeadDesc* calls[3][2] = {{nullptr, nullptr}, {&reward, nullptr}, {&value, &policy}};
+        for (int n_heads = 0; n_heads < 3; ++n_heads)
+            if (!heads_fit_one_group(heads_footprint(C, HW, n_heads, calls[n_heads]))) {
+                *note = "f32 nets + f64 tree statistics (no tensor-core towers: the head weights exceed shared memory)";
+                return TowerRoute::CudaCore;
+            }
+        return fp16 ? TowerRoute::TcF16 : TowerRoute::TcX3;
+    }
+    // MZ_TC_WIDE=1 (opt-in until measured): the towers of a 128-channel net as x3 tensor-core launches on the dense states
+    // (conv_wide.cu), when the planner accepts the hidden board.  The stems and the heads stay on the CUDA cores.
+    // MZ_TC_WIDE=2: the same, and a board the one-CTA plan refuses (15 x 15, 16 x 16) is split across CTA pairs.
+    const char* wide_env = getenv("MZ_TC_WIDE");
+    if (!wide_env || (wide_env[0] != '1' && wide_env[0] != '2') || fp16 || net.channels != kWideC || net.downsample)
+        return TowerRoute::CudaCore;
+    const int layers = 1 + 2 * net.blocks;
+    WideTowerPlan p;
+    const char* why = "";
+    if (wide_tower_plan(max_batch, net.channels, net.obs_h, net.obs_w, layers, sm_count, &p, &why)) return TowerRoute::Wide;
+    std::string reasons = why;
+    if (wide_env[0] == '2') {
+        const char* why_pair = "";
+        if (wide_pair_plan(max_batch, net.channels, net.obs_h, net.obs_w, layers, sm_count, &p, &why_pair)) return TowerRoute::WidePair;
+        reasons = std::string("one CTA: ") + why + "; CTA pairs: " + why_pair;
+    }
+    *note = "f32 nets + f64 tree statistics (128-channel towers stay on the CUDA cores: " + reasons + ")";
+    return TowerRoute::CudaCore;
+}
 
 ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, std::string* err) {
     ResNetDevice* r = new ResNetDevice();
@@ -538,63 +612,21 @@ ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, s
             }
         }
     }
-    // MZ_TC_MODE = "off": fp32 CUDA-core towers everywhere; anything else: tensor-core towers where the shape allows
-    // (conv_tc.cu).  MZ_NO_TC=1 is the older spelling of "off".
-    const char* no_tc = getenv("MZ_NO_TC");
-    const char* tc_mode = getenv("MZ_TC_MODE");
-    const bool tc_off = (no_tc && no_tc[0] == '1') || (tc_mode && strcmp(tc_mode, "off") == 0);
-    r->tc_capable = !net.downsample && conv_tc_supported(net.channels, r->hh, r->hw);
-    r->use_tc = r->tc_capable && !tc_off;
-    // default "x3": split 16-bit operands, three partial products, fp32-grade accuracy; "fp16": plain fp16 operands
-    // (3x fewer MMAs, ~1e-2 hidden-state error: opt-in)
-    r->split = r->use_tc && !(tc_mode && strcmp(tc_mode, "fp16") == 0);
-    // The heads of the tensor-core route read the board layout and have no generic (global-memory) variant.  A net whose
-    // head weights do not fit in shared memory next to one sample's tile (e.g. support 300, or a 128-wide value layer
-    // over 16 reduced channels) runs on the fp32 CUDA-core towers and the generic heads route instead.  The head shapes
-    // are known here, so the hidden-state pool and the workspaces are sized for the route that will run.
-    if (r->use_tc) {
-        const int HW = r->hh * r->hw, F = 2 * net.support_size + 1;
-        size_t size = 0;
-        layout_head(net.channels, net.reduced_reward, HW, net.res_fc_reward, net.n_res_fc_reward, F, &size, r->reward_head);
-        layout_head(net.channels, net.reduced_value, HW, net.res_fc_value, net.n_res_fc_value, F, &size, r->value_head);
-        layout_head(net.channels, net.reduced_policy, HW, net.res_fc_policy, net.n_res_fc_policy, net.action_space, &size,
-                    r->policy_head);
-        if (!tc_heads_fit(r)) {
-            r->tc_capable = r->use_tc = r->split = false;
-            r->heads_off_tc = true;
-        }
-    }
-    // MZ_TC_WIDE=1 (opt-in until measured): the towers of a 128-channel net as x3 tensor-core launches on the dense states
-    // (conv_wide.cu), when the planner accepts the hidden board.  The stems and the heads stay on the CUDA cores.
-    // MZ_TC_WIDE=2: the same, and a board the one-CTA plan refuses (15 x 15, 16 x 16) is split across CTA pairs.
-    const char* wide_env = getenv("MZ_TC_WIDE");
-    if (wide_env && (wide_env[0] == '1' || wide_env[0] == '2') && !tc_off && !(tc_mode && strcmp(tc_mode, "fp16") == 0) &&
-        net.channels == kWideC && !net.downsample) {
-        WideTowerPlan p;
-        const char* why = "";
-        r->wide = wide_tower_plan(max_batch, net.channels, r->hh, r->hw, 1 + 2 * net.blocks, sm_count, &p, &why);
-        std::string reasons = why;
-        if (!r->wide && wide_env[0] == '2') {
-            const char* why_pair = "";
-            r->wide = r->wide_pair = wide_pair_plan(max_batch, net.channels, r->hh, r->hw, 1 + 2 * net.blocks, sm_count, &p, &why_pair);
-            reasons = std::string("one CTA: ") + why + "; CTA pairs: " + why_pair;
-        }
-        if (!r->wide) r->wide_refused = "f32 nets + f64 tree statistics (128-channel towers stay on the CUDA cores: " + reasons + ")";
-    }
+    // the route is known here, so the hidden-state pool and the workspaces are sized for it
+    r->route = choose_route(net, max_batch, sm_count, &r->note);
     const char* no_fuse = getenv("MZ_NO_FUSE");
     r->fuse_small = !(no_fuse && no_fuse[0] == '1');
-    r->state_elems = r->use_tc ? conv_tc_board_elems(r->split) : r->C * r->hh * r->hw;
-    if (r->use_tc) max_elems = std::max(max_elems, (size_t)conv_tc_board_elems(r->split));
+    max_elems = std::max(max_elems, (size_t)state_elems(r));
     r->ws_elems = max_elems * (size_t)max_batch;
     for (int i = 0; i < 3; ++i) {
         if (cudaMalloc(&r->ws[i], r->ws_elems * 4 + 64) != cudaSuccess) { *err = "workspace allocation failed"; resnet_destroy(r); return nullptr; }
         cudaMemset(r->ws[i], 0, r->ws_elems * 4 + 64);      // P64C4 padding positions must read as zero
     }
     if (cudaMalloc(&r->scratch_hidden, (size_t)max_batch * r->C * r->hh * r->hw * 4 + 64) != cudaSuccess ||
-        cudaMalloc(&r->scratch_state, (size_t)max_batch * r->state_elems * 4 + 64) != cudaSuccess) {
+        cudaMalloc(&r->scratch_state, (size_t)max_batch * state_elems(r) * 4 + 64) != cudaSuccess) {
         *err = "workspace allocation failed"; resnet_destroy(r); return nullptr;
     }
-    cudaMemset(r->scratch_state, 0, (size_t)max_batch * r->state_elems * 4 + 64);
+    cudaMemset(r->scratch_state, 0, (size_t)max_batch * state_elems(r) * 4 + 64);
     if (cudaMalloc(&r->d_sat, 64) != cudaSuccess) { *err = "workspace allocation failed"; resnet_destroy(r); return nullptr; }
     cudaMemset(r->d_sat, 0, 64);
     return r;
@@ -664,6 +696,8 @@ float f16_to_float(uint16_t h) {
 }
 
 constexpr int kWideImage = 3;       // pack_conv's `tc` for the x3 image of the wide towers (conv_wide.cu)
+// pack_conv's `tc` for the towers of a route: none on the CUDA cores
+int weight_image(TowerRoute t) { return is_wide(t) ? kWideImage : state_layout(t); }
 
 bool pack_conv(Loader& L, const std::string& conv, const std::string& bn, int cin, int cout, int stride,
                std::vector<float>& blob, std::vector<ConvLayer>& layers, int tc = 0, int H = 0, int W = 0) {
@@ -842,9 +876,9 @@ int resnet_load_weights(ResNetDevice* r, const MzTensor* tensors, int n, std::st
     } else {
         ok = ok && pack_conv(L, rp + ".conv", rp + ".bn", nd.obs_c, C, 1, conv, r->rep_trunk);
     }
-    // the tensor-core images are packed whenever the shape allows them (both the fp16 and the x3 image are cheap), so the
-    // range guard can switch paths without reloading; which one is used is decided per launch
-    const int tc = r->wide ? kWideImage : !r->tc_capable ? 0 : (r->split ? kLayoutSplit : kLayoutF16);
+    // the image of the route's tensor-core towers; the CUDA-core kernels read the fp32 weights, which every route packs,
+    // so the range guard can switch to them without reloading
+    const int tc = weight_image(r->route);
     for (int i = 0; ok && i < nd.blocks; ++i) ok = pack_resblock(L, rp + ".resblocks." + std::to_string(i), C, conv, r->rep_trunk, tc);
     const std::string dp = "dynamics_network.module";
     ok = ok && pack_conv(L, dp + ".conv", dp + ".bn", C + 1, C, 1, conv, r->dyn, tc, r->hh, r->hw);
@@ -871,6 +905,19 @@ int resnet_load_weights(ResNetDevice* r, const MzTensor* tensors, int n, std::st
 struct HeadsPlan { int route = 0, groups = 0, threads = 0, grid = 0; size_t smem = 0; };
 
 namespace {
+// One tower call site of the network: the layers it runs, whether the first of them is a stem conv, and where its input
+// lives.  Every tower family (tower_tc, small_tower, wide_tower, the per-layer convs of site_tower) takes it.
+struct TowerSite {
+    const std::vector<ConvLayer>* layers;
+    size_t first;                  // first layer run; a stem (if any) and then 2 x blocks convs
+    bool stem;
+    int in_channels, H, W;         // the input board's planes (the dynamics stem adds the action plane)
+    const float* in;               // scratch, or in search the hidden-state pool, which stays read only
+    const int32_t* gather_parent;  // in search: game g reads slot gather_parent[g] of pool_stride
+    int pool_stride;
+    const int32_t* action;         // the dynamics stem's action plane
+};
+
 struct Runner {
     ResNetDevice* r; cudaStream_t stream; int64_t* launches; std::string* err; int n;
     int g0 = 0;                // games [g0, g0 + n) of the batch (partitioned replay); buffers are addressed by the global index
@@ -896,11 +943,12 @@ struct Runner {
         static const int dbg = getenv("MZ_TC_DEBUG_SKIP") ? atoi(getenv("MZ_TC_DEBUG_SKIP")) : 0;
         a.debug_skip = dbg;
         a.g0 = g0; a.sat_count = r->d_sat;
+        const bool x3 = r->route == TowerRoute::TcX3;
         kt_begin(KT_TOWER, stream);
-        cudaError_t e = r->split ? launch_conv_tower_x3(a, r->sm_count, stream) : launch_conv_tower_tc(a, r->sm_count, stream);
+        cudaError_t e = x3 ? launch_conv_tower_x3(a, r->sm_count, stream) : launch_conv_tower_tc(a, r->sm_count, stream);
         kt_end(stream);
         if (e != cudaSuccess) return fail("conv_tower_tc launch", e);
-        *launches += r->split ? conv_x3_launches(n, r->sm_count) : 1;
+        *launches += x3 ? conv_x3_launches(n, r->sm_count) : 1;
         return true;
     }
 
@@ -925,20 +973,24 @@ struct Runner {
         return true;
     }
 
-    // [optional stem conv] + `count` residual blocks in as few persistent launches as possible.
-    // ext = tower input (read only, optionally gathered from the hidden pool); ws = three workspaces.
-    // Returns the buffer holding the result (one of ws, or ext if there was nothing to do) or nullptr on error.
-    // `first` = index of the first layer to run; `ext_reusable`: ext is scratch that may be overwritten once read.
-    const float* tower_tc(const std::vector<ConvLayer>& layers, size_t first_layer, bool stem, size_t count, const float* ext,
-                          bool ext_reusable, float* const ws[3], const int32_t* gather_parent, int pool_stride,
-                          const int32_t* action) {
-        if (!r->split && n > conv_tc_max_boards_fused(r->sm_count)) {
+    // The tower of a site in as few persistent launches as possible, its input s.in (in the board layout) followed by
+    // the three workspaces.  Returns the buffer holding the result (one of the workspaces, or s.in if there was nothing
+    // to do) or nullptr on error.
+    const float* tower_tc(const TowerSite& s) {
+        const std::vector<ConvLayer>& layers = *s.layers;
+        float* const* ws = r->ws;
+        const float* ext = s.in;
+        const int32_t *gather_parent = s.gather_parent, *action = s.action;
+        const int pool_stride = s.pool_stride;
+        const bool stem = s.stem;
+        size_t count = r->net.blocks;
+        if (r->route != TowerRoute::TcX3 && n > conv_tc_max_boards_fused(r->sm_count)) {
             // too many tiles per CTA for the fused mode: one launch per conv
             float* free_ws[3]; int nf = 0;
             for (int i = 0; i < 3; ++i) if (ws[i] != ext) free_ws[nf++] = ws[i];
             if (nf < 3) free_ws[nf++] = const_cast<float*>(ext);      // ext is itself a workspace: reusable as the third
             float *cur = free_ws[0], *tmp = free_ws[1], *spare = free_ws[2];
-            size_t first = first_layer;
+            size_t first = s.first;
             // (the result buffer may be ext itself when ext is one of the workspaces: whether any layer ran decides
             // what is returned, not a comparison with ext)
             const bool any = stem || count > 0;
@@ -952,7 +1004,7 @@ struct Runner {
             if (!blocks_tc(layers, first, count, &cur, &tmp, &spare)) return nullptr;
             return any ? cur : ext;
         }
-        size_t li = first_layer, blocks_left = count;
+        size_t li = s.first, blocks_left = count;
         bool stem_left = stem;
         const float* ext_now = ext;                 // buf[0] of the next launch
         const int32_t* gather_now = gather_parent;
@@ -966,9 +1018,9 @@ struct Runner {
             if (nb < 4) a.buf[nb++] = nullptr;      // (only two spare workspaces when the input is one of ws)
             a.gather_parent = gather_now; a.pool_stride = pool_stride; a.action = action;
             int cur = 0, nl = 0;
-            // the input buffer is dead after its last reader: always so for a workspace written by the previous launch,
-            // for the tower's own input only when it is scratch (a gathered pool never is)
-            const bool reuse0 = (ext_reusable || ext_now != ext) && !gather_now;
+            // the input buffer is dead after its last reader: always so for a workspace written by the previous launch and
+            // for the tower's own scratch input, never for a gathered pool
+            const bool reuse0 = !gather_now;
             auto pick = [&](int avoid1, int avoid2) {
                 for (int i = 1; i < 4; ++i) if (i != avoid1 && i != avoid2 && a.buf[i]) return i;
                 if (reuse0 && avoid1 != 0 && avoid2 != 0) return 0;
@@ -997,23 +1049,23 @@ struct Runner {
         return result;
     }
 
-    // The four tower call sites of resnet_inference_tc, each with where its input lives (mz_debug_conv_tower runs the same
-    // helpers).  Representation: the CUDA-core stem (rep_trunk[0]) wrote ws[0].
-    const float* representation_tower() {
-        return tower_tc(r->rep_trunk, 1, false, r->net.blocks, r->ws[0], true, r->ws, nullptr, 0, nullptr);
+    // The four tower call sites of the network (the debug towers run the same descriptions).  Representation: from the
+    // observation planes through the stem or, after_stem, from the stem's output (the tensor-core and wide towers leave
+    // the stem to conv3x3_kernel); the trunk of a downsampled net is blocks only, on the DownSample output.
+    TowerSite representation_site(const float* in, bool after_stem = false) const {
+        if (!r->net.downsample && !after_stem)
+            return TowerSite{&r->rep_trunk, 0, true, r->net.obs_c, r->net.obs_h, r->net.obs_w, in, nullptr, 0, nullptr};
+        return TowerSite{&r->rep_trunk, after_stem ? 1u : 0u, false, r->C, r->hh, r->hw, in, nullptr, 0, nullptr};
     }
-    // Dynamics, plain API call: the dense states were converted into dynamics_staging().
-    float* dynamics_staging() const { return r->ws[2]; }
-    const float* dynamics_tower(const int32_t* action) {
-        return tower_tc(r->dyn, 0, true, r->net.blocks, dynamics_staging(), true, r->ws, nullptr, 0, action);
+    // Dynamics: the stem reads the states and the action plane; in search game g's state is slot gather_parent[g] of
+    // the pool `in`.
+    TowerSite dynamics_site(const float* in, const int32_t* action, const int32_t* gather_parent = nullptr,
+                            int pool_stride = 0) const {
+        return TowerSite{&r->dyn, 0, true, r->C, r->hh, r->hw, in, gather_parent, pool_stride, action};
     }
-    // Dynamics in search: the parents' states are gathered from the pool, which stays read only.
-    const float* dynamics_tower_pool(const float* pool, const int32_t* gather_parent, int pool_stride, const int32_t* action) {
-        return tower_tc(r->dyn, 0, true, r->net.blocks, pool, false, r->ws, gather_parent, pool_stride, action);
-    }
-    // Prediction: the heads wrote the rescaled state into scratch_state.
-    const float* prediction_tower() {
-        return tower_tc(r->pred, 0, false, r->net.blocks, r->scratch_state, true, r->ws, nullptr, 0, nullptr);
+    // Prediction: blocks only, on the rescaled state.
+    TowerSite prediction_site(const float* in) const {
+        return TowerSite{&r->pred, 0, false, r->C, r->hh, r->hw, in, nullptr, 0, nullptr};
     }
 
     bool conv(const ConvLayer& l, const float* in, float* out, const float* residual, bool relu, int Hin, int Win,
@@ -1021,7 +1073,7 @@ struct Runner {
               bool out_p64c4 = false) {
         if (g0 != 0) { *err = "conv3x3: partitioned calls are not supported on the per-layer route"; return false; }
         ConvArgs a{};
-        a.out_p64c4 = out_p64c4 ? (r->split ? kLayoutSplit : kLayoutF16) : 0;
+        a.out_p64c4 = out_p64c4 ? state_layout(r->route) : 0;
         a.in = in; a.out = out; a.residual = residual; a.w = r->d_conv + l.w_off;
         a.bias = l.b_off >= 0 ? r->d_conv + l.b_off : nullptr;
         a.gather_parent = gather_parent; a.pool_stride = pool_stride; a.action = action;
@@ -1068,32 +1120,31 @@ struct Runner {
         return true;
     }
 
-    // [optional stem conv] + `count` residual blocks as ONE fused CUDA-core launch (small_tower.cu).
-    // Returns 1 = launched, 0 = shape not supported (caller falls back to one launch per conv), -1 = error.
-    // arguments of a fused CUDA-core tower; false when the layers are not of the supported kind
-    bool small_tower_args(SmallTowerArgs& a, const std::vector<ConvLayer>& layers, size_t first, bool stem, size_t count, const float* in,
-                          float* out, int in_channels, int H, int W, const int32_t* gather_parent, int pool_stride, const int32_t* action) {
-        const size_t nl = (stem ? 1 : 0) + 2 * count;
+    // arguments of the fused CUDA-core tower of a site writing `out`; false when the layers are not of the supported kind
+    bool small_tower_args(SmallTowerArgs& a, const TowerSite& s, float* out) {
+        const size_t nl = (s.stem ? 1 : 0) + 2 * (size_t)r->net.blocks;
         if (nl == 0 || nl > (size_t)kSmallTowerMaxLayers) return false;
         a = SmallTowerArgs{};
-        a.in = in; a.out = out; a.blob = r->d_conv; a.gather_parent = gather_parent; a.action = action; a.pool_stride = pool_stride;
-        a.n = n; a.g0 = g0; a.C = r->C; a.H = H; a.W = W; a.A = r->net.action_space; a.in_channels = in_channels; a.n_layers = (int)nl;
+        a.in = s.in; a.out = out; a.blob = r->d_conv; a.gather_parent = s.gather_parent; a.action = s.action;
+        a.pool_stride = s.pool_stride;
+        a.n = n; a.g0 = g0; a.C = r->C; a.H = s.H; a.W = s.W; a.A = r->net.action_space; a.in_channels = s.in_channels;
+        a.n_layers = (int)nl;
         for (size_t i = 0; i < nl; ++i) {
-            const ConvLayer& l = layers[first + i];
+            const ConvLayer& l = (*s.layers)[s.first + i];
             if (l.stride != 1 || l.cout != r->C) return false;
             SmallTowerLayer& t = a.layer[i];
             t.w_off = (int)l.w_off; t.b_off = (int)l.b_off; t.cin = l.cin; t.relu = 1;
-            t.residual = (i >= (stem ? 1u : 0u) && ((i - (stem ? 1 : 0)) & 1)) ? 1 : 0;     // second conv of a block
+            t.residual = (i >= (s.stem ? 1u : 0u) && ((i - (s.stem ? 1 : 0)) & 1)) ? 1 : 0;     // second conv of a block
         }
         return true;
     }
 
-    int small_tower(const std::vector<ConvLayer>& layers, size_t first, bool stem, size_t count, const float* in, float* out,
-                    int in_channels, int H, int W, const int32_t* gather_parent = nullptr, int pool_stride = 0,
-                    const int32_t* action = nullptr, bool dry_run = false) {
+    // The tower of a site as ONE fused CUDA-core launch (small_tower.cu).  Returns 1 = launched, 0 = shape not supported
+    // (the caller falls back to one launch per conv), -1 = error.
+    int small_tower(const TowerSite& s, float* out, bool dry_run = false) {
         if (!r->fuse_small) return 0;
         SmallTowerArgs a{};
-        if (!small_tower_args(a, layers, first, stem, count, in, out, in_channels, H, W, gather_parent, pool_stride, action)) return 0;
+        if (!small_tower_args(a, s, out)) return 0;
         if (!small_tower_supported(a)) return 0;
         if (dry_run) return 1;
         kt_begin(KT_SMALL, stream);
@@ -1104,70 +1155,63 @@ struct Runner {
         return 1;
     }
 
-    // The four fused CUDA-core tower call sites of resnet_inference, each with the input it reads (mz_debug_small_tower runs
-    // the same helpers); each returns what small_tower returns.  Representation: stem from the observation planes.
-    int representation_small_tower(const float* obs, float* out) {
-        return small_tower(r->rep_trunk, 0, true, r->net.blocks, obs, out, r->net.obs_c, r->net.obs_h, r->net.obs_w);
-    }
-    // Dynamics, plain API call: dense hidden states plus the action plane.
-    int dynamics_small_tower(const float* states, float* out, const int32_t* action) {
-        return small_tower(r->dyn, 0, true, r->net.blocks, states, out, r->C, r->hh, r->hw, nullptr, 0, action);
-    }
-    // Dynamics in search: the parents' states gathered from the pool, plus the action plane.
-    int dynamics_small_tower_pool(const float* pool, const int32_t* gather_parent, int pool_stride, float* out, const int32_t* action) {
-        return small_tower(r->dyn, 0, true, r->net.blocks, pool, out, r->C, r->hh, r->hw, gather_parent, pool_stride, action);
-    }
-    // Prediction: the rescaled hidden state, no stem (a net without blocks has no prediction tower).
-    int prediction_small_tower(const float* hidden, float* out) {
-        return r->net.blocks > 0 ? small_tower(r->pred, 0, false, r->net.blocks, hidden, out, r->C, r->hh, r->hw) : 0;
-    }
-
-    // [optional stem conv] + `count` residual blocks of a 128-channel net as ONE x3 tensor-core launch (conv_wide.cu), dense
-    // NCHW in and out, one CTA or (r->wide_pair) one CTA pair per board.  Returns what small_tower returns: 1 = launched, 0 = not the wide route, -1 = error.
-    int wide_tower(const std::vector<ConvLayer>& layers, size_t first, bool stem, size_t count, const float* in, float* out,
-                   const int32_t* gather_parent = nullptr, int pool_stride = 0, const int32_t* action = nullptr) {
-        const int nl = (stem ? 1 : 0) + 2 * (int)count;
-        if (!r->wide || nl == 0) return 0;
+    // The tower of a site of a 128-channel net as ONE x3 tensor-core launch (conv_wide.cu), dense NCHW in and out, one CTA
+    // or (WidePair) one CTA pair per board.  Returns what small_tower returns: 1 = launched, 0 = not the wide route, -1 = error.
+    int wide_tower(const TowerSite& s, float* out) {
+        const int nl = (s.stem ? 1 : 0) + 2 * r->net.blocks;
+        if (!is_wide(r->route) || nl == 0) return 0;
+        const bool pair = r->route == TowerRoute::WidePair;
         WideTowerPlan p;
         const char* why = "";
-        if (!(r->wide_pair ? wide_pair_plan : wide_tower_plan)(n, r->C, r->hh, r->hw, nl, r->sm_count, &p, &why)) return 0;
+        if (!(pair ? wide_pair_plan : wide_tower_plan)(n, r->C, r->hh, r->hw, nl, r->sm_count, &p, &why)) return 0;
         WideTowerArgs a{};
-        a.in = in; a.out = out; a.gather_parent = gather_parent; a.pool_stride = pool_stride; a.action = action;
-        a.n = n; a.H = r->hh; a.W = r->hw; a.A = r->net.action_space; a.g0 = g0; a.stem = stem ? 1 : 0; a.n_layers = nl;
+        a.in = s.in; a.out = out; a.gather_parent = s.gather_parent; a.pool_stride = s.pool_stride; a.action = s.action;
+        a.n = n; a.H = r->hh; a.W = r->hw; a.A = r->net.action_space; a.g0 = g0; a.stem = s.stem ? 1 : 0; a.n_layers = nl;
         a.sat_count = r->d_sat;
         for (int i = 0; i < nl; ++i) {
-            const ConvLayer& l = layers[first + i];
+            const ConvLayer& l = (*s.layers)[s.first + i];
             WideLayer& t = a.layer[i];
             t.w = r->d_conv + l.tc_off;
             t.scale = r->d_conv + l.tc_scale_off;
             t.bias = l.b_off >= 0 ? r->d_conv + l.b_off : nullptr;
-            t.action_table = i == 0 && stem && action && l.tc_table_off >= 0 ? r->d_conv + l.tc_table_off : nullptr;
+            t.action_table = i == 0 && s.stem && s.action && l.tc_table_off >= 0 ? r->d_conv + l.tc_table_off : nullptr;
         }
         if (wide_plan_out) *wide_plan_out = p;
         kt_begin(KT_TOWER, stream);
-        cudaError_t e = r->wide_pair ? launch_wide_pair_tower(a, p, stream) : launch_wide_tower(a, p, stream);
+        cudaError_t e = pair ? launch_wide_pair_tower(a, p, stream) : launch_wide_tower(a, p, stream);
         kt_end(stream);
         if (e != cudaSuccess) { fail("wide tower launch", e); return -1; }
         *launches += p.launches;
         return 1;
     }
 
-    // The four wide-tower call sites of resnet_inference (mz_debug_wide_tower runs the same helpers).  Representation: the
-    // blocks after the CUDA-core stem, which wrote `in`.
-    int representation_wide_tower(const float* in, float* out) {
-        return wide_tower(r->rep_trunk, 1, false, r->net.blocks, in, out);
-    }
-    // Dynamics, plain API call: dense hidden states plus the action plane.
-    int dynamics_wide_tower(const float* states, float* out, const int32_t* action) {
-        return wide_tower(r->dyn, 0, true, r->net.blocks, states, out, nullptr, 0, action);
-    }
-    // Dynamics in search: the parents' states gathered from the pool, which stays read only.
-    int dynamics_wide_tower_pool(const float* pool, const int32_t* gather_parent, int pool_stride, float* out, const int32_t* action) {
-        return wide_tower(r->dyn, 0, true, r->net.blocks, pool, out, gather_parent, pool_stride, action);
-    }
-    // Prediction: the rescaled hidden state.
-    int prediction_wide_tower(const float* hidden, float* out) {
-        return wide_tower(r->pred, 0, false, r->net.blocks, hidden, out);
+    // The tower of a site in resnet_inference: the wide launch and then the fused CUDA-core launch, as far as `tries`
+    // names them, else one conv3x3_kernel per conv.  The workspaces *cur, *tmp, *spare rotate: a site with a stem writes
+    // *cur first; one without reads s.in (*cur itself, or the rescaled state, which is never written) and writes *tmp
+    // first.  Returns the buffer holding the result (s.in when the site has no layer), nullptr on error.
+    enum { kTryWide = 1, kTryFused = 2 };
+    const float* site_tower(const TowerSite& s, int tries, float** cur, float** tmp, float** spare) {
+        float* out = s.stem ? *cur : *tmp;
+        int done = (tries & kTryWide) ? wide_tower(s, out) : 0;
+        if (done == 0 && (tries & kTryFused)) done = small_tower(s, out);
+        if (done < 0) return nullptr;
+        if (done) {
+            if (out == *tmp) std::swap(*cur, *tmp);
+            return *cur;
+        }
+        size_t li = s.first;
+        const float* x = s.in;
+        if (s.stem) {
+            if (!conv((*s.layers)[li++], s.in, *cur, nullptr, true, s.H, s.W, s.gather_parent, s.pool_stride, s.action)) return nullptr;
+            x = *cur;
+        }
+        for (int b = 0; b < r->net.blocks; ++b, li += 2) {
+            if (!conv((*s.layers)[li], x, *tmp, nullptr, true, r->hh, r->hw)) return nullptr;
+            if (!conv((*s.layers)[li + 1], *tmp, *spare, x, true, r->hh, r->hw)) return nullptr;
+            std::swap(*cur, *spare);
+            x = *cur;
+        }
+        return x;
     }
 
     // residual tower: layers[2k], layers[2k+1] are one block; x ends up in `*cur`
@@ -1226,35 +1270,20 @@ struct Runner {
         return true;
     }
 
-    // arguments of one heads launch (everything but the launch geometry)
+    // arguments of one heads launch (everything but the launch geometry); x and the states are in the route's layout
     HeadsArgs heads_args(const float* x, int n_heads, const HeadDesc* h0, const HeadDesc* h1, float* l0, float* l1, float* s0, float* s1,
-                         float* rescaled, float* pool_hidden, int pool_stride, int out_slot, bool p64c4 = false, float* state_p64c4 = nullptr) {
+                         float* rescaled, float* pool_hidden, int pool_stride, int out_slot, float* state_p64c4 = nullptr) {
         HeadsArgs a{};
-        a.p64c4 = p64c4 ? (r->split ? kLayoutSplit : kLayoutF16) : 0; a.W = r->hw; a.state_p64c4 = state_p64c4;
+        a.p64c4 = state_layout(r->route); a.W = r->hw; a.state_p64c4 = state_p64c4;
         a.x = x; a.blob = r->d_head; a.n = n; a.g0 = g0; a.C = r->C; a.HW = r->hh * r->hw; a.S = r->net.support_size;
         a.hw_inv = a.HW >= 2 ? (unsigned)((0x100000000ull + (unsigned)a.HW - 1u) / (unsigned)a.HW) : 0u;
         a.n_heads = n_heads;
-        int maxw = 32;
         const HeadDesc* hs[2] = {h0, h1};
-        for (int i = 0; i < n_heads; ++i) {
-            a.head[i] = *hs[i];
-            maxw = std::max(maxw, hs[i]->rc * a.HW + 4);
-            for (int l = 0; l < hs[i]->mlp.n; ++l) maxw = std::max(maxw, hs[i]->mlp.out[l] + 4);
-        }
+        for (int i = 0; i < n_heads; ++i) a.head[i] = *hs[i];
         a.logits[0] = l0; a.logits[1] = l1; a.scalar[0] = s0; a.scalar[1] = s1;
         a.rescaled = rescaled; a.pool_hidden = pool_hidden; a.pool_stride = pool_stride; a.out_slot = out_slot;
-        a.smem_floats = (maxw + 3) & ~3;
-        // blob slice covering the heads of this launch
-        int lo = 1 << 30, hi = 0;
-        for (int i = 0; i < n_heads; ++i) {
-            const HeadDesc& d = *hs[i];
-            lo = std::min(lo, d.w1_off);
-            const int last = d.mlp.n - 1;
-            hi = std::max(hi, d.mlp.b_off[last] + d.mlp.out[last]);
-        }
-        if (n_heads == 0) { lo = 0; hi = 0; }
-        a.w_lo = lo; a.w_floats = ((hi - lo) + 3) & ~3;
-        a.warp_floats = (a.HW * (a.C + 4) + 6 * a.C + 4 * a.smem_floats + 3) & ~3;   // x tile + channel stats + (ping, pong) per head
+        const HeadsFootprint f = heads_footprint(a.C, a.HW, n_heads, hs);
+        a.w_lo = f.w_lo; a.w_floats = f.w_floats; a.smem_floats = f.smem_floats; a.warp_floats = f.warp_floats;
         return a;
     }
 
@@ -1291,8 +1320,8 @@ struct Runner {
     }
 
     bool heads(const float* x, int n_heads, const HeadDesc* h0, const HeadDesc* h1, float* l0, float* l1, float* s0, float* s1,
-               float* rescaled, float* pool_hidden, int pool_stride, int out_slot, bool p64c4 = false, float* state_p64c4 = nullptr) {
-        HeadsArgs a = heads_args(x, n_heads, h0, h1, l0, l1, s0, s1, rescaled, pool_hidden, pool_stride, out_slot, p64c4, state_p64c4);
+               float* rescaled, float* pool_hidden, int pool_stride, int out_slot, float* state_p64c4 = nullptr) {
+        HeadsArgs a = heads_args(x, n_heads, h0, h1, l0, l1, s0, s1, rescaled, pool_hidden, pool_stride, out_slot, state_p64c4);
         const HeadDesc* hs[2] = {h0, h1};
         HeadsPlan plan;
         if (!plan_heads(a, &plan)) return false;
@@ -1323,33 +1352,26 @@ struct Runner {
     // scratch_state, the prediction tower's input.  Representation: rescale only (no heads on the root state).
     bool representation_heads(const float* x, float* hidden, float* pool_hidden, int pool_stride, int out_slot) {
         return heads(x, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, hidden, pool_hidden, pool_stride, out_slot,
-                     r->use_tc, r->use_tc ? r->scratch_state : nullptr);
+                     tc_state());
     }
     // Dynamics (plain API call and in search): reward head on the raw state + rescale.
     bool dynamics_heads(const float* x, float* reward_logits, float* reward, float* hidden, float* pool_hidden, int pool_stride,
                         int out_slot) {
         return heads(x, 1, &r->reward_head, nullptr, reward_logits, nullptr, reward, nullptr, hidden, pool_hidden, pool_stride,
-                     out_slot, r->use_tc, r->use_tc ? r->scratch_state : nullptr);
+                     out_slot, tc_state());
     }
     // Prediction: value and policy heads on the prediction tower's output (a scalar for the value only).
     bool prediction_heads(const float* x, float* value_logits, float* policy_logits, float* value) {
-        return heads(x, 2, &r->value_head, &r->policy_head, value_logits, policy_logits, value, nullptr, nullptr, nullptr, 0, 0, r->use_tc);
+        return heads(x, 2, &r->value_head, &r->policy_head, value_logits, policy_logits, value, nullptr, nullptr, nullptr, 0, 0);
     }
+    float* tc_state() const { return is_tc(r->route) ? r->scratch_state : nullptr; }
 };
 }  // namespace
 
-// every heads launch of resnet_inference_tc (rescale only, reward head, value + policy heads) fits in shared memory with
-// one sample per CTA
-static bool tc_heads_fit(ResNetDevice* r) {
-    std::string err; int64_t launches = 0;
-    Runner R{r, nullptr, &launches, &err, 1, 0};
-    const HeadsArgs calls[3] = {
-        R.heads_args(nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, true),
-        R.heads_args(nullptr, 1, &r->reward_head, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, true),
-        R.heads_args(nullptr, 2, &r->value_head, &r->policy_head, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, true)};
-    for (const HeadsArgs& a : calls)
-        if (((size_t)a.w_floats + a.warp_floats) * 4 > 227 * 1024) return false;
-    return true;
+// Where resnet_inference_tc leaves the input of a tensor-core tower: the representation stem's output, the converted
+// dense states of a plain dynamics call, the rescaled state the heads wrote (in search the dynamics tower reads the pool)
+static float* tc_tower_input(ResNetDevice* r, int site) {
+    return site == MZ_TOWER_REPRESENTATION ? r->ws[0] : site == MZ_TOWER_DYNAMICS ? r->ws[2] : r->scratch_state;
 }
 
 // Tensor-core variant: every C->C conv of the three towers runs in conv_tc.cu on the P64C4 layout; the
@@ -1358,11 +1380,12 @@ static int resnet_inference_tc(ResNetDevice* r, const InferCall& c, cudaStream_t
     const MzNetDesc& nd = r->net;
     const int n = c.n, C = r->C, hh = r->hh, hw = r->hw, F = 2 * nd.support_size + 1;
     Runner R{r, stream, launches, err, n, c.g0};
-    if (c.g0 != 0 && (!r->split || !c.recurrent || !c.gather_parent)) { *err = "resnet: partitioned calls need the x3 towers in pool mode"; return MZ_EINVAL; }
+    if (c.g0 != 0 && (r->route != TowerRoute::TcX3 || !c.recurrent || !c.gather_parent)) { *err = "resnet: partitioned calls need the x3 towers in pool mode"; return MZ_EINVAL; }
     float* state = r->scratch_state;                   // rescaled state, P64C4, input of the prediction tower
     if (!c.recurrent) {
-        if (!R.conv(r->rep_trunk[0], c.in, r->ws[0], nullptr, true, nd.obs_h, nd.obs_w, nullptr, 0, nullptr, true)) return MZ_ECUDA;
-        const float* x = R.representation_tower();
+        float* stem_out = tc_tower_input(r, MZ_TOWER_REPRESENTATION);
+        if (!R.conv(r->rep_trunk[0], c.in, stem_out, nullptr, true, nd.obs_h, nd.obs_w, nullptr, 0, nullptr, true)) return MZ_ECUDA;
+        const float* x = R.tower_tc(R.representation_site(stem_out, true));
         if (!x) return MZ_ECUDA;
         if (!R.representation_heads(x, c.hidden, c.pool_hidden, c.pool_stride, c.out_slot)) return MZ_ECUDA;
         if (c.reward_logits) {
@@ -1376,26 +1399,27 @@ static int resnet_inference_tc(ResNetDevice* r, const InferCall& c, cudaStream_t
     } else {
         const float* x;
         if (c.gather_parent) {
-            x = R.dynamics_tower_pool(c.pool_hidden, c.gather_parent, c.pool_stride, c.action);
+            x = R.tower_tc(R.dynamics_site(c.pool_hidden, c.action, c.gather_parent, c.pool_stride));
         } else {
             // plain API call: dense NCHW hidden states -> P64C4
             const size_t total = (size_t)n * C * hh * hw;
-            nchw_to_p64c4_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(c.in, R.dynamics_staging(), n, C, hh, hw,
-                                                                                       r->split ? 1 : 0);
+            float* staged = tc_tower_input(r, MZ_TOWER_DYNAMICS);
+            nchw_to_p64c4_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(c.in, staged, n, C, hh, hw,
+                                                                                       r->route == TowerRoute::TcX3);
             *launches += 1;
-            x = R.dynamics_tower(c.action);
+            x = R.tower_tc(R.dynamics_site(staged, c.action));
         }
         if (!x) return MZ_ECUDA;
         if (!R.dynamics_heads(x, c.reward_logits, c.reward, c.hidden, c.pool_hidden, c.pool_stride, c.out_slot)) return MZ_ECUDA;
     }
-    const float* x = R.prediction_tower();
+    const float* x = R.tower_tc(R.prediction_site(tc_tower_input(r, MZ_TOWER_PREDICTION)));
     if (!x) return MZ_ECUDA;
     if (!R.prediction_heads(x, c.value_logits, c.policy_logits, c.value)) return MZ_ECUDA;
     return MZ_OK;
 }
 
-int resnet_state_elems(const ResNetDevice* r) { return r->state_elems; }
-bool resnet_uses_tensor_cores(const ResNetDevice* r) { return r->use_tc; }
+int resnet_state_elems(const ResNetDevice* r) { return state_elems(r); }
+bool resnet_uses_tensor_cores(const ResNetDevice* r) { return is_tc(r->route); }
 
 // Partitioned replay (abi.cu) needs every kernel of a recurrent inference to honour a first-game offset: the x3 towers,
 // the fused small towers and heads_kernel do; the per-layer convs, the fp16-mode towers and the generic heads route do not.
@@ -1403,46 +1427,37 @@ static const int32_t kDryRunAction = 0;        // stands for the action array in
 bool resnet_can_partition(const ResNetDevice* r0) {
     ResNetDevice* r = const_cast<ResNetDevice*>(r0);
     if (!r->loaded) return false;
-    if (r->use_tc) return r->split;
+    if (is_tc(r->route)) return r->route == TowerRoute::TcX3;
     std::string err; int64_t launches = 0;
     Runner R{r, nullptr, &launches, &err, r->max_batch, 0};
-    const int nb = r->net.blocks;
-    if (nb < 1) return false;
+    if (r->net.blocks < 1) return false;
     // the wide towers honour g0 (resnet_create accepted the board); otherwise the fused small towers must take both towers
-    if (!r->wide && R.small_tower(r->dyn, 0, true, nb, nullptr, nullptr, r->C, r->hh, r->hw, nullptr, 0, &kDryRunAction, true) != 1) return false;
-    if (!r->wide && R.small_tower(r->pred, 0, false, nb, nullptr, nullptr, r->C, r->hh, r->hw, nullptr, 0, nullptr, true) != 1) return false;
-    // heads_kernel route (not heads_big): the head weights plus one group's tile fit in shared memory
-    const int HW = r->hh * r->hw;
-    int hi = 0, lo = 1 << 30, maxw = 32;
-    for (const HeadDesc* d : {&r->reward_head, &r->value_head, &r->policy_head}) {
-        lo = std::min(lo, d->w1_off);
-        hi = std::max(hi, d->mlp.b_off[d->mlp.n - 1] + d->mlp.out[d->mlp.n - 1]);
-        maxw = std::max(maxw, d->rc * HW + 4);
-        for (int l = 0; l < d->mlp.n; ++l) maxw = std::max(maxw, d->mlp.out[l] + 4);
-    }
-    const size_t warp_floats = (size_t)HW * (r->C + 4) + 6 * r->C + 4 * ((maxw + 3) & ~3);
-    return ((size_t)(hi - lo) + warp_floats) * 4 <= 227 * 1024;
+    if (!is_wide(r->route) && R.small_tower(R.dynamics_site(nullptr, &kDryRunAction), nullptr, true) != 1) return false;
+    if (!is_wide(r->route) && R.small_tower(R.prediction_site(nullptr), nullptr, true) != 1) return false;
+    // heads_kernel route (not heads_big): the weights of all three heads plus one group's tile fit in shared memory
+    const HeadDesc* hs[3] = {&r->reward_head, &r->value_head, &r->policy_head};
+    return heads_fit_one_group(heads_footprint(r->C, r->hh * r->hw, 3, hs));
 }
 const char* resnet_numerics(const ResNetDevice* r) {
-    if (r->wide && r->wide_pair)
+    switch (r->route) {
+    case TowerRoute::WidePair:
         return "f32-grade nets (128-channel towers on the tensor cores, boards split across CTA pairs, split fp16 operands "
                "x = x_h + x_l/2^11, 3 partial products, f32 accumulate; f32 stems and heads) + f64 tree statistics";
-    if (r->wide)
+    case TowerRoute::Wide:
         return "f32-grade nets (128-channel towers on the tensor cores, split fp16 operands x = x_h + x_l/2^11, 3 partial "
                "products, f32 accumulate; f32 stems and heads) + f64 tree statistics";
-    if (r->fell_back == 2) return "f32 nets + f64 tree statistics (128-channel tensor-core towers left after an activation exceeded the fp16 range)";
-    if (!r->wide_refused.empty()) return r->wide_refused.c_str();
-    if (!r->use_tc) return r->heads_off_tc ? "f32 nets + f64 tree statistics (no tensor-core towers: the head weights exceed shared memory)"
-                         : r->fell_back ? "f32 nets + f64 tree statistics (tensor-core towers left after an activation exceeded the fp16 range)"
-                                        : "f32 nets + f64 tree statistics";
-    return r->split ? "f32-grade nets (tensor-core towers on split fp16 operands x = x_h + x_l/2^11, 3 partial products, f32 accumulate; f32 heads) + f64 tree statistics"
-                    : "fp16 operands / f32 accumulate (tensor-core towers), f32 heads, f64 tree statistics";
+    case TowerRoute::TcX3:
+        return "f32-grade nets (tensor-core towers on split fp16 operands x = x_h + x_l/2^11, 3 partial products, f32 accumulate; f32 heads) + f64 tree statistics";
+    case TowerRoute::TcF16: return "fp16 operands / f32 accumulate (tensor-core towers), f32 heads, f64 tree statistics";
+    case TowerRoute::CudaCore: break;
+    }
+    return r->note.empty() ? "f32 nets + f64 tree statistics" : r->note.c_str();
 }
 
 // Range guard of the x3 towers: number of epilogue threads that stored an activation beyond the fp16 range since the
 // last call (synchronises the stream).  resnet_use_strict switches the handle to the fp32 CUDA-core towers for good.
 int resnet_take_saturations(ResNetDevice* r, cudaStream_t stream) {
-    if (!((r->use_tc && r->split) || r->wide) || !r->d_sat) return 0;
+    if (!range_guarded(r->route) || !r->d_sat) return 0;
     int count = 0;
     if (cudaMemcpyAsync(&count, r->d_sat, 4, cudaMemcpyDeviceToHost, stream) != cudaSuccess) return 0;
     if (cudaStreamSynchronize(stream) != cudaSuccess) return 0;
@@ -1450,9 +1465,10 @@ int resnet_take_saturations(ResNetDevice* r, cudaStream_t stream) {
     return count;
 }
 void resnet_use_strict(ResNetDevice* r) {
-    r->fell_back = r->wide ? 2 : 1;
-    r->use_tc = false; r->split = false; r->wide = false; r->wide_pair = false;
-    r->state_elems = r->C * r->hh * r->hw;           // dense NCHW states: smaller than the board layout, the pool fits
+    r->note = is_wide(r->route)
+                  ? "f32 nets + f64 tree statistics (128-channel tensor-core towers left after an activation exceeded the fp16 range)"
+                  : "f32 nets + f64 tree statistics (tensor-core towers left after an activation exceeded the fp16 range)";
+    r->route = TowerRoute::CudaCore;                 // dense NCHW states: smaller than the board layout, the pool fits
 }
 
 // Launch plan of conv3x3_kernel for a shape (host only, behind mz_debug_conv3x3_plan): plan[11] = {P, stride, MAX_ITEMS,
@@ -1463,6 +1479,30 @@ bool resnet_conv_plan(int n, int cin, int cout, int H, int W, int stride, int64_
     const int64_t out[11] = {p.P, p.stride, p.max_items, p.bands, p.band_rows, p.boards, p.cin_chunk,
                              p.grid.x, p.grid.y, p.grid.z, (int64_t)p.smem};
     for (int i = 0; i < 11; ++i) plan[i] = out[i];
+    return true;
+}
+
+// A synthetic net of plain convs for the debug entries: the state_dict "c<i>.weight" of n_convs convs whose OIHW weights
+// follow one another in `w` (conv i reads cin[i] planes), packed as `route` packs its towers, with bias[i] (cout floats
+// each) when biases are given.
+static bool pack_debug_convs(TowerRoute route, int n_convs, const int* cin, int cout, int stride, int H, int W, const float* w,
+                             const float* bias, std::vector<float>& blob, std::vector<ConvLayer>& layers, std::string* err) {
+    std::vector<std::string> names(n_convs);
+    std::vector<MzTensor> tensors(n_convs);
+    size_t w_off = 0;
+    for (int i = 0; i < n_convs; ++i) {
+        names[i] = "c" + std::to_string(i) + ".weight";
+        tensors[i] = MzTensor{names[i].c_str(), w + w_off, (int64_t)cout * cin[i] * 9};
+        w_off += (size_t)cout * cin[i] * 9;
+    }
+    Loader L{tensors.data(), n_convs, err};
+    for (int i = 0; i < n_convs; ++i) {
+        if (!pack_conv(L, "c" + std::to_string(i), "", cin[i], cout, stride, blob, layers, weight_image(route), H, W)) return false;
+        if (bias) {
+            layers.back().b_off = (long)blob.size();
+            blob.insert(blob.end(), bias + (size_t)i * cout, bias + (size_t)(i + 1) * cout);      // (cout % 4 == 0: stays aligned)
+        }
+    }
     return true;
 }
 
@@ -1481,18 +1521,11 @@ int resnet_debug_conv(int n, int cin, int cout, int H, int W, int stride, const 
     nd.kind = MZ_NET_RESNET; nd.channels = C; nd.obs_c = cin; nd.obs_h = H; nd.obs_w = W; nd.action_space = 1;
     ResNetDevice r{};
     r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = Ho; r.hw = Wo;
-    // fake a one-tensor state_dict for pack_conv
-    MzTensor t{"conv.weight", w_oihw, (int64_t)cout * cin * 9};
-    Loader L{&t, 1, err};
+    r.route = use_tc == 2 ? TowerRoute::TcX3 : use_tc ? TowerRoute::TcF16 : TowerRoute::CudaCore;
     std::vector<float> blob;
     std::vector<ConvLayer> layers;
-    r.use_tc = use_tc != 0; r.split = use_tc == 2; r.tc_capable = true;
-    if (!pack_conv(L, "conv", "", cin, cout, stride, blob, layers, use_tc == 2 ? kLayoutSplit : (use_tc ? kLayoutF16 : 0), H, W))
-        return MZ_EINVAL;
-    long bias_off = -1;
-    if (bias) { bias_off = (long)blob.size(); blob.insert(blob.end(), bias, bias + C); while (blob.size() % 4) blob.push_back(0.f); }
-    layers[0].b_off = bias_off;
-    const bool split = use_tc == 2;
+    if (!pack_debug_convs(r.route, 1, &cin, cout, stride, H, W, w_oihw, bias, blob, layers, err)) return MZ_EINVAL;
+    const bool split = r.route == TowerRoute::TcX3;
     const size_t dense_in = (size_t)n * cin * H * W, dense = (size_t)n * C * Ho * Wo, packed = (size_t)n * conv_tc_board_elems(split);
     float *d_blob = nullptr, *d_x = nullptr, *d_res = nullptr, *d_out = nullptr, *d_px = nullptr, *d_pres = nullptr, *d_pout = nullptr;
     auto cleanup = [&]() { for (float* p : {d_blob, d_x, d_res, d_out, d_px, d_pres, d_pout}) if (p) cudaFree(p); };
@@ -1549,135 +1582,6 @@ int resnet_debug_conv(int n, int cin, int cout, int H, int W, int stride, const 
     return good ? MZ_OK : MZ_ECUDA;
 }
 
-// Stand-alone tensor-core tower of one call site of resnet_inference_tc, through the same Runner helpers, on host NCHW
-// data.  The three workspaces, the prediction site's scratch state, the pool and the output start as NaN bytes (0xFF);
-// only the input boards are written, with the zero padding the board layout promises.  So a layer that reads a board or a
-// padding row nobody wrote produces NaN.
-int resnet_debug_tower(int n, int H, int W, int mode, int blocks, int site, int parts, int A, const float* x, const float* w,
-                       const float* bias, const int32_t* action, const int32_t* parent, int pool_stride, float* out,
-                       int64_t* launches, int32_t* saturated, int sm_count, std::string* err) {
-    constexpr int C = 64;
-    const bool stem = site == MZ_TOWER_DYNAMICS || site == MZ_TOWER_DYNAMICS_POOL;
-    const bool in_pool = site == MZ_TOWER_DYNAMICS_POOL;
-    if (n < 1 || blocks < 0 || (!stem && blocks < 1) || site < MZ_TOWER_REPRESENTATION || site > MZ_TOWER_PREDICTION ||
-        (mode != 1 && mode != 2) || !conv_tc_supported(C, H, W)) {
-        *err = "bad shape, site or mode"; return MZ_EINVAL;
-    }
-    if (parts < 1 || parts > 4 || (parts > 1 && (!in_pool || mode != 2))) {
-        *err = "partitions need the x3 towers at the in-search dynamics site, 1 to 4 of them"; return MZ_EINVAL;
-    }
-    if (stem) {
-        if (A < 1 || !action) { *err = "the dynamics sites need actions and A >= 1"; return MZ_EINVAL; }
-        for (int g = 0; g < n; ++g) if (action[g] < 0 || action[g] >= A) { *err = "action out of range"; return MZ_EINVAL; }
-    }
-    if (in_pool) {
-        if (!parent || pool_stride < 1) { *err = "the in-search site needs parents and pool_stride >= 1"; return MZ_EINVAL; }
-        for (int g = 0; g < n; ++g) if (parent[g] < 0 || parent[g] >= pool_stride) { *err = "parent out of range"; return MZ_EINVAL; }
-    }
-    // a state_dict of plain convolutions for pack_conv: "c<i>.weight", the stem [C][C + 1][3][3] first
-    const int n_convs = (stem ? 1 : 0) + 2 * blocks;
-    std::vector<std::string> names(n_convs);
-    std::vector<MzTensor> tensors(n_convs);
-    size_t w_off = 0;
-    for (int i = 0; i < n_convs; ++i) {
-        const int cin = stem && i == 0 ? C + 1 : C;
-        names[i] = "c" + std::to_string(i) + ".weight";
-        tensors[i] = MzTensor{names[i].c_str(), w + w_off, (int64_t)C * cin * 9};
-        w_off += (size_t)C * cin * 9;
-    }
-    MzNetDesc nd{};
-    nd.kind = MZ_NET_RESNET; nd.channels = C; nd.obs_c = C; nd.obs_h = H; nd.obs_w = W; nd.action_space = stem ? A : 1;
-    nd.blocks = blocks;
-    ResNetDevice r{};
-    r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = H; r.hw = W;
-    r.use_tc = r.tc_capable = true; r.split = mode == 2;
-    Loader L{tensors.data(), n_convs, err};
-    std::vector<float> blob;
-    std::vector<ConvLayer> layers;
-    for (int i = 0; i < n_convs; ++i) {
-        const int cin = stem && i == 0 ? C + 1 : C;
-        if (!pack_conv(L, "c" + std::to_string(i), "", cin, C, 1, blob, layers, r.split ? kLayoutSplit : kLayoutF16, H, W))
-            return MZ_EINVAL;
-        if (bias) {
-            layers[i].b_off = (long)blob.size();
-            blob.insert(blob.end(), bias + (size_t)i * C, bias + (size_t)(i + 1) * C);
-        }
-    }
-    if (site == MZ_TOWER_REPRESENTATION) { r.rep_trunk = layers; r.rep_trunk.insert(r.rep_trunk.begin(), ConvLayer{}); }  // [0]: the CUDA-core stem, not run here
-    else if (stem) r.dyn = layers;
-    else r.pred = layers;
-
-    const size_t board = (size_t)conv_tc_board_elems(r.split), packed = (size_t)n * board, dense = (size_t)n * C * H * W;
-    const size_t pool_boards = in_pool ? (size_t)n * pool_stride : 0;
-    float *d_blob = nullptr, *d_x = nullptr, *d_out = nullptr, *d_stage = nullptr, *d_pool = nullptr;
-    int32_t *d_action = nullptr, *d_parent = nullptr;
-    auto cleanup = [&]() {
-        for (void* p : {(void*)d_blob, (void*)d_x, (void*)d_out, (void*)d_stage, (void*)d_pool, (void*)d_action, (void*)d_parent,
-                        (void*)r.ws[0], (void*)r.ws[1], (void*)r.ws[2], (void*)r.scratch_state, (void*)r.d_sat})
-            if (p) cudaFree(p);
-        r.ws[0] = r.ws[1] = r.ws[2] = r.scratch_state = nullptr; r.d_sat = nullptr; r.d_conv = nullptr;
-    };
-    bool ok = cudaMalloc(&d_blob, blob.size() * 4) == cudaSuccess && cudaMalloc(&d_x, dense * 4) == cudaSuccess &&
-              cudaMalloc(&d_out, dense * 4) == cudaSuccess && cudaMalloc(&d_stage, packed * 4) == cudaSuccess &&
-              cudaMalloc(&r.scratch_state, packed * 4) == cudaSuccess && cudaMalloc(&r.d_sat, 64) == cudaSuccess &&
-              cudaMalloc(&d_action, (size_t)n * 4) == cudaSuccess && cudaMalloc(&d_parent, (size_t)n * 4) == cudaSuccess &&
-              (!in_pool || cudaMalloc(&d_pool, pool_boards * board * 4) == cudaSuccess);
-    for (int i = 0; ok && i < 3; ++i) ok = cudaMalloc(&r.ws[i], packed * 4) == cudaSuccess;
-    if (!ok) { cleanup(); *err = "allocation failed"; return MZ_ENOMEM; }
-    r.d_conv = d_blob;
-    cudaMemcpy(d_blob, blob.data(), blob.size() * 4, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_x, x, dense * 4, cudaMemcpyHostToDevice);
-    if (stem) cudaMemcpy(d_action, action, (size_t)n * 4, cudaMemcpyHostToDevice);
-    if (in_pool) cudaMemcpy(d_parent, parent, (size_t)n * 4, cudaMemcpyHostToDevice);
-    for (int i = 0; i < 3; ++i) cudaMemset(r.ws[i], 0xFF, packed * 4);
-    cudaMemset(r.scratch_state, 0xFF, packed * 4);
-    cudaMemset(d_out, 0xFF, dense * 4);
-    cudaMemset(r.d_sat, 0, 64);
-    // the input boards, zero padded, where the stage before the tower leaves them
-    Runner R0{&r, nullptr, launches, err, n};
-    float* input = site == MZ_TOWER_REPRESENTATION ? r.ws[0] : site == MZ_TOWER_DYNAMICS ? R0.dynamics_staging()
-                 : site == MZ_TOWER_PREDICTION ? r.scratch_state : d_stage;
-    const unsigned cblocks = (unsigned)((dense + 255) / 256);
-    cudaMemset(input, 0, packed * 4);
-    nchw_to_p64c4_kernel<<<cblocks, 256>>>(d_x, input, n, C, H, W, r.split ? 1 : 0);
-    if (in_pool) {
-        cudaMemset(d_pool, 0xFF, pool_boards * board * 4);
-        for (int g = 0; g < n; ++g)
-            cudaMemcpy(d_pool + ((size_t)g * pool_stride + parent[g]) * board, d_stage + (size_t)g * board, board * 4,
-                       cudaMemcpyDeviceToDevice);
-    }
-    *launches = 0;
-    const float* result = nullptr;
-    bool good = true;
-    if (site == MZ_TOWER_REPRESENTATION) result = R0.representation_tower();
-    else if (site == MZ_TOWER_DYNAMICS) result = R0.dynamics_tower(d_action);
-    else if (site == MZ_TOWER_PREDICTION) result = R0.prediction_tower();
-    else {
-        // the ranges of the partitioned replay, each through its own Runner; every array stays addressed by the global game
-        const int per = partition_games(n, parts);
-        for (int p = 0; p < parts && good; ++p) {
-            Runner R{&r, nullptr, launches, err, std::min(per, n - p * per), p * per};
-            if (R.n <= 0) continue;
-            const float* res = R.dynamics_tower_pool(d_pool, d_parent, pool_stride, d_action);
-            if (!res || (result && res != result)) { good = false; if (res) *err = "partitions ended in different buffers"; }
-            result = res;
-        }
-    }
-    good = good && result;
-    cudaError_t e = cudaDeviceSynchronize();
-    if (good && e != cudaSuccess) { good = false; *err = std::string("debug tower: ") + cudaGetErrorString(e); }
-    if (good) {
-        p64c4_to_nchw_kernel<<<cblocks, 256>>>(result, d_out, n, C, H, W, r.split ? 1 : 0);
-        e = cudaMemcpy(out, d_out, dense * 4, cudaMemcpyDeviceToHost);
-        int sat = 0;
-        if (e == cudaSuccess) e = cudaMemcpy(&sat, r.d_sat, 4, cudaMemcpyDeviceToHost);
-        if (e != cudaSuccess) { good = false; *err = std::string("debug tower: ") + cudaGetErrorString(e); }
-        if (saturated) *saturated = sat;
-    }
-    cleanup();
-    return good ? MZ_OK : MZ_ECUDA;
-}
-
 // Launch plan of the fused CUDA-core tower (host only, behind mz_debug_small_tower_plan): plan[6] = {P, CO, boards per
 // CTA, threads, grid, shared-memory bytes} of n boards through [a stem conv reading in_channels planes +] `blocks`
 // residual blocks of C channels, from the same Runner::small_tower_args and planner the launch takes.  false with the
@@ -1688,7 +1592,7 @@ bool resnet_small_tower_plan(int n, int in_channels, int C, int H, int W, int bl
     if (!stem && in_channels != C) { *err = "without a stem the tower input has C channels"; return false; }
     if ((stem ? 1 : 0) + 2 * blocks < 1 || (stem ? 1 : 0) + 2 * blocks > kSmallTowerMaxLayers) { *err = "1 to 10 layers"; return false; }
     ResNetDevice r{};
-    r.C = C; r.hh = H; r.hw = W; r.sm_count = sm_count; r.net.action_space = 1;
+    r.C = C; r.hh = H; r.hw = W; r.sm_count = sm_count; r.net.action_space = 1; r.net.blocks = blocks;
     std::vector<ConvLayer> layers((stem ? 1 : 0) + 2 * (size_t)blocks);
     for (size_t i = 0; i < layers.size(); ++i) {
         ConvLayer& l = layers[i];
@@ -1698,7 +1602,7 @@ bool resnet_small_tower_plan(int n, int in_channels, int C, int H, int W, int bl
     int64_t launches = 0;
     Runner R{&r, nullptr, &launches, err, n};
     SmallTowerArgs a{};
-    if (!R.small_tower_args(a, layers, 0, stem, (size_t)blocks, nullptr, nullptr, in_channels, H, W, nullptr, 0, nullptr)) {
+    if (!R.small_tower_args(a, TowerSite{&layers, 0, stem, in_channels, H, W, nullptr, nullptr, 0, nullptr}, nullptr)) {
         *err = "layers the fused tower does not take"; return false;
     }
     SmallTowerPlan p;
@@ -1707,117 +1611,6 @@ bool resnet_small_tower_plan(int n, int in_channels, int C, int H, int W, int bl
     const int64_t out[6] = {p.P, p.CO, p.boards_per_cta, p.threads, p.grid, (int64_t)p.smem};
     for (int i = 0; i < 6; ++i) plan[i] = out[i];
     return true;
-}
-
-// Stand-alone fused CUDA-core tower of one call site of resnet_inference, through the same Runner helpers, on host NCHW
-// data.  The output and the pool's other slots start as NaN bytes (0xFF), so a board the tower does not write, or one read
-// from the wrong slot, produces NaN.
-int resnet_debug_small_tower(int n, int in_channels, int C, int H, int W, int blocks, int site, int parts, int A, const float* x,
-                             const float* w, const float* bias, const int32_t* action, const int32_t* parent, int pool_stride,
-                             float* out, int64_t* plan, int sm_count, std::string* err) {
-    const bool stem = site != MZ_TOWER_PREDICTION;
-    const bool dyn = site == MZ_TOWER_DYNAMICS || site == MZ_TOWER_DYNAMICS_POOL;
-    const bool in_pool = site == MZ_TOWER_DYNAMICS_POOL;
-    if (n < 1 || C < 4 || blocks < 0 || (!stem && blocks < 1) || site < MZ_TOWER_REPRESENTATION || site > MZ_TOWER_PREDICTION ||
-        (site == MZ_TOWER_REPRESENTATION ? in_channels < 1 : in_channels != C)) {
-        *err = "bad shape or site"; return MZ_EINVAL;
-    }
-    if (parts < 1 || parts > 4 || (parts > 1 && !in_pool)) { *err = "partitions need the in-search dynamics site, 1 to 4 of them"; return MZ_EINVAL; }
-    if (dyn) {
-        if (A < 1 || !action) { *err = "the dynamics sites need actions and A >= 1"; return MZ_EINVAL; }
-        for (int g = 0; g < n; ++g) if (action[g] < 0 || action[g] >= A) { *err = "action out of range"; return MZ_EINVAL; }
-    }
-    if (in_pool) {
-        if (!parent || pool_stride < 1) { *err = "the in-search site needs parents and pool_stride >= 1"; return MZ_EINVAL; }
-        for (int g = 0; g < n; ++g) if (parent[g] < 0 || parent[g] >= pool_stride) { *err = "parent out of range"; return MZ_EINVAL; }
-    }
-    // a state_dict of plain convolutions for pack_conv: "c<i>.weight", the stem first
-    const int cin0 = site == MZ_TOWER_REPRESENTATION ? in_channels : dyn ? C + 1 : C;
-    const int n_convs = (stem ? 1 : 0) + 2 * blocks;
-    std::vector<std::string> names(n_convs);
-    std::vector<MzTensor> tensors(n_convs);
-    size_t w_off = 0;
-    for (int i = 0; i < n_convs; ++i) {
-        const int cin = i == 0 ? cin0 : C;
-        names[i] = "c" + std::to_string(i) + ".weight";
-        tensors[i] = MzTensor{names[i].c_str(), w + w_off, (int64_t)C * cin * 9};
-        w_off += (size_t)C * cin * 9;
-    }
-    MzNetDesc nd{};
-    nd.kind = MZ_NET_RESNET; nd.channels = C; nd.obs_c = site == MZ_TOWER_REPRESENTATION ? in_channels : C; nd.obs_h = H; nd.obs_w = W;
-    nd.action_space = dyn ? A : 1; nd.blocks = blocks;
-    ResNetDevice r{};
-    r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = H; r.hw = W;
-    Loader L{tensors.data(), n_convs, err};
-    std::vector<float> blob;
-    std::vector<ConvLayer> layers;
-    for (int i = 0; i < n_convs; ++i) {
-        if (!pack_conv(L, "c" + std::to_string(i), "", i == 0 ? cin0 : C, C, 1, blob, layers)) return MZ_EINVAL;
-        if (bias) {
-            layers[i].b_off = (long)blob.size();
-            blob.insert(blob.end(), bias + (size_t)i * C, bias + (size_t)(i + 1) * C);      // (C % 4 == 0: stays aligned)
-        }
-    }
-    if (site == MZ_TOWER_REPRESENTATION) r.rep_trunk = layers;
-    else if (dyn) r.dyn = layers;
-    else r.pred = layers;
-
-    const size_t in_elems = (size_t)nd.obs_c * H * W, dense = (size_t)n * C * H * W;
-    const size_t in_total = in_pool ? (size_t)n * pool_stride * in_elems : (size_t)n * in_elems;
-    float *d_blob = nullptr, *d_in = nullptr, *d_out = nullptr;
-    int32_t *d_action = nullptr, *d_parent = nullptr;
-    auto cleanup = [&]() { for (void* p : {(void*)d_blob, (void*)d_in, (void*)d_out, (void*)d_action, (void*)d_parent}) if (p) cudaFree(p); };
-    const bool ok = cudaMalloc(&d_blob, blob.size() * 4) == cudaSuccess && cudaMalloc(&d_in, in_total * 4) == cudaSuccess &&
-                    cudaMalloc(&d_out, dense * 4) == cudaSuccess && cudaMalloc(&d_action, (size_t)n * 4) == cudaSuccess &&
-                    cudaMalloc(&d_parent, (size_t)n * 4) == cudaSuccess;
-    if (!ok) { cleanup(); *err = "allocation failed"; return MZ_ENOMEM; }
-    r.d_conv = d_blob;
-    cudaMemcpy(d_blob, blob.data(), blob.size() * 4, cudaMemcpyHostToDevice);
-    if (in_pool) {
-        cudaMemset(d_in, 0xFF, in_total * 4);
-        for (int g = 0; g < n; ++g)
-            cudaMemcpy(d_in + ((size_t)g * pool_stride + parent[g]) * in_elems, x + (size_t)g * in_elems, in_elems * 4,
-                       cudaMemcpyHostToDevice);
-        cudaMemcpy(d_parent, parent, (size_t)n * 4, cudaMemcpyHostToDevice);
-    } else {
-        cudaMemcpy(d_in, x, in_total * 4, cudaMemcpyHostToDevice);
-    }
-    if (dyn) cudaMemcpy(d_action, action, (size_t)n * 4, cudaMemcpyHostToDevice);
-    cudaMemset(d_out, 0xFF, dense * 4);
-    int64_t launches = 0;
-    SmallTowerPlan used{}, first{};
-    int rc = MZ_OK;
-    // the ranges of the partitioned replay, each through its own Runner (one range unless in the pool); every array stays
-    // addressed by the global game.  The plan reported is the first range's.
-    const int per = in_pool ? partition_games(n, parts) : n;
-    for (int p = 0; p * per < n && rc == MZ_OK; ++p) {
-        Runner R{&r, nullptr, &launches, err, std::min(per, n - p * per), p * per};
-        R.small_plan = &used;
-        int fused;
-        if (site == MZ_TOWER_REPRESENTATION) fused = R.representation_small_tower(d_in, d_out);
-        else if (site == MZ_TOWER_DYNAMICS) fused = R.dynamics_small_tower(d_in, d_out, d_action);
-        else if (site == MZ_TOWER_DYNAMICS_POOL) fused = R.dynamics_small_tower_pool(d_in, d_parent, pool_stride, d_out, d_action);
-        else fused = R.prediction_small_tower(d_in, d_out);
-        if (fused == 0) {
-            int64_t unused[6];
-            std::string why = "no fused launch";
-            resnet_small_tower_plan(R.n, cin0, C, H, W, blocks, stem, sm_count, unused, &why);
-            *err = "the fused tower refuses the shape: " + why; rc = MZ_EUNSUPPORTED;
-        }
-        else if (fused < 0) rc = MZ_ECUDA;
-        if (p == 0) first = used;
-    }
-    cudaError_t e = cudaDeviceSynchronize();
-    if (rc == MZ_OK && e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug small tower: ") + cudaGetErrorString(e); }
-    if (rc == MZ_OK) {
-        e = cudaMemcpy(out, d_out, dense * 4, cudaMemcpyDeviceToHost);
-        if (e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug small tower: ") + cudaGetErrorString(e); }
-        const int64_t pl[6] = {first.P, first.CO, first.boards_per_cta, first.threads, first.grid, (int64_t)first.smem};
-        if (plan) for (int i = 0; i < 6; ++i) plan[i] = pl[i];
-    }
-    r.d_conv = nullptr;
-    cleanup();
-    return rc;
 }
 
 // Launch plan of the wide tower (host only, behind mz_debug_wide_tower_plan): plan[9] = {M-tiles, threads, shared-memory bytes,
@@ -1841,20 +1634,32 @@ bool resnet_wide_tower_plan(int n, int C, int H, int W, int blocks, bool stem, i
     return true;
 }
 
-// Stand-alone wide tower of one call site of resnet_inference, through the same Runner helpers and weight packing, on host
-// NCHW data (128 channels); with `pair` always on the CTA-pair kernel.  The output and the pool's other slots start as NaN bytes (0xFF), so a board the tower does not
-// write, or one read from the wrong slot, produces NaN.
-int resnet_debug_wide_tower(int n, int H, int W, int blocks, int site, int parts, int A, const float* x, const float* w,
-                            const float* bias, const int32_t* action, const int32_t* parent, int pool_stride, float* out,
-                            int64_t* launches, int32_t* saturated, int64_t* plan, int sm_count, std::string* err, bool pair) {
-    constexpr int C = kWideC;
-    const bool stem = site == MZ_TOWER_DYNAMICS || site == MZ_TOWER_DYNAMICS_POOL;
+// Stand-alone tower of one call site of the network, through the same site descriptions, Runner helpers and weight
+// packing, on host NCHW data: a 64-channel tensor-core tower of resnet_inference_tc (TcF16 / TcX3, the input staged in
+// the board layout where that function leaves it), the fused CUDA-core tower (CudaCore) or a wide tower (Wide / WidePair)
+// of resnet_inference.  The workspaces, the prediction site's scratch state, the pool and the output start as NaN bytes
+// (0xFF); only the input boards are written, with the zero padding the board layout promises.  So a layer that reads a
+// board, a padding row or a pool slot nobody wrote produces NaN.
+int resnet_debug_tower(TowerRoute route, int n, int in_channels, int C, int H, int W, int blocks, int site, int parts, int A,
+                       const float* x, const float* w, const float* bias, const int32_t* action, const int32_t* parent,
+                       int pool_stride, float* out, int64_t* launches, int32_t* saturated, int64_t* plan, int sm_count,
+                       std::string* err) {
+    const bool tc = is_tc(route), fused = route == TowerRoute::CudaCore, pair = route == TowerRoute::WidePair;
+    const bool dyn = site == MZ_TOWER_DYNAMICS || site == MZ_TOWER_DYNAMICS_POOL;
     const bool in_pool = site == MZ_TOWER_DYNAMICS_POOL;
-    if (n < 1 || blocks < 0 || (!stem && blocks < 1) || site < MZ_TOWER_REPRESENTATION || site > MZ_TOWER_PREDICTION) {
-        *err = "bad shape or site"; return MZ_EINVAL;
+    // only the fused tower takes the representation stem: the others leave it to conv3x3_kernel
+    const bool stem = dyn || (fused && site == MZ_TOWER_REPRESENTATION);
+    if (n < 1 || blocks < 0 || (!stem && blocks < 1) || site < MZ_TOWER_REPRESENTATION || site > MZ_TOWER_PREDICTION ||
+        (fused && (C < 4 || (site == MZ_TOWER_REPRESENTATION ? in_channels < 1 : in_channels != C))) ||
+        (tc && !conv_tc_supported(C, H, W))) {
+        *err = tc ? "bad shape, site or mode" : "bad shape or site"; return MZ_EINVAL;
     }
-    if (parts < 1 || parts > 4 || (parts > 1 && !in_pool)) { *err = "partitions need the in-search dynamics site, 1 to 4 of them"; return MZ_EINVAL; }
-    if (stem) {
+    if (parts < 1 || parts > 4 || (parts > 1 && (!in_pool || route == TowerRoute::TcF16))) {
+        *err = tc ? "partitions need the x3 towers at the in-search dynamics site, 1 to 4 of them"
+                  : "partitions need the in-search dynamics site, 1 to 4 of them";
+        return MZ_EINVAL;
+    }
+    if (dyn) {
         if (A < 1 || !action) { *err = "the dynamics sites need actions and A >= 1"; return MZ_EINVAL; }
         for (int g = 0; g < n; ++g) if (action[g] < 0 || action[g] >= A) { *err = "action out of range"; return MZ_EINVAL; }
     }
@@ -1862,95 +1667,134 @@ int resnet_debug_wide_tower(int n, int H, int W, int blocks, int site, int parts
         if (!parent || pool_stride < 1) { *err = "the in-search site needs parents and pool_stride >= 1"; return MZ_EINVAL; }
         for (int g = 0; g < n; ++g) if (parent[g] < 0 || parent[g] >= pool_stride) { *err = "parent out of range"; return MZ_EINVAL; }
     }
-    {
+    if (is_wide(route)) {
         int64_t unused[9];
         std::string why;
         if (!resnet_wide_tower_plan(n, C, H, W, blocks, stem, sm_count, unused, &why, pair)) {
             *err = std::string(pair ? "the wide pair tower" : "the wide tower") + " refuses the shape: " + why; return MZ_EUNSUPPORTED;
         }
     }
+    // the site's convs, the stem first: [C][in_channels or C + 1][3][3], then two [C][C][3][3] per block
     const int n_convs = (stem ? 1 : 0) + 2 * blocks;
-    std::vector<std::string> names(n_convs);
-    std::vector<MzTensor> tensors(n_convs);
-    size_t w_off = 0;
-    for (int i = 0; i < n_convs; ++i) {
-        const int cin = stem && i == 0 ? C + 1 : C;
-        names[i] = "c" + std::to_string(i) + ".weight";
-        tensors[i] = MzTensor{names[i].c_str(), w + w_off, (int64_t)C * cin * 9};
-        w_off += (size_t)C * cin * 9;
-    }
+    std::vector<int> cin(n_convs, C);
+    if (stem) cin[0] = dyn ? C + 1 : in_channels;
     MzNetDesc nd{};
-    nd.kind = MZ_NET_RESNET; nd.channels = C; nd.obs_c = C; nd.obs_h = H; nd.obs_w = W; nd.action_space = stem ? A : 1;
-    nd.blocks = blocks;
+    nd.kind = MZ_NET_RESNET; nd.channels = C; nd.obs_c = site == MZ_TOWER_REPRESENTATION ? in_channels : C; nd.obs_h = H;
+    nd.obs_w = W; nd.action_space = dyn ? A : 1; nd.blocks = blocks;
     ResNetDevice r{};
-    r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = H; r.hw = W; r.wide = true; r.wide_pair = pair;
-    Loader L{tensors.data(), n_convs, err};
+    r.net = nd; r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = H; r.hw = W; r.route = route;
     std::vector<float> blob;
     std::vector<ConvLayer> layers;
-    for (int i = 0; i < n_convs; ++i) {
-        if (!pack_conv(L, "c" + std::to_string(i), "", stem && i == 0 ? C + 1 : C, C, 1, blob, layers, kWideImage, H, W)) return MZ_EINVAL;
-        if (bias) {
-            layers[i].b_off = (long)blob.size();
-            blob.insert(blob.end(), bias + (size_t)i * C, bias + (size_t)(i + 1) * C);
-        }
+    if (!pack_debug_convs(route, n_convs, cin.data(), C, 1, H, W, w, bias, blob, layers, err)) return MZ_EINVAL;
+    if (site == MZ_TOWER_REPRESENTATION) {
+        r.rep_trunk = layers;
+        if (!stem) r.rep_trunk.insert(r.rep_trunk.begin(), ConvLayer{});      // [0]: the CUDA-core stem, not run here
+    } else if (dyn) {
+        r.dyn = layers;
+    } else {
+        r.pred = layers;
     }
-    if (site == MZ_TOWER_REPRESENTATION) { r.rep_trunk = layers; r.rep_trunk.insert(r.rep_trunk.begin(), ConvLayer{}); }  // [0]: the CUDA-core stem, not run here
-    else if (stem) r.dyn = layers;
-    else r.pred = layers;
 
-    const size_t board = (size_t)C * H * W, dense = (size_t)n * board;
-    const size_t in_total = in_pool ? (size_t)n * pool_stride * board : dense;
-    float *d_blob = nullptr, *d_in = nullptr, *d_out = nullptr;
+    // one stored input board: the tensor-core board layout, or dense planes
+    const size_t in_elems = (size_t)nd.obs_c * H * W, dense = (size_t)n * C * H * W;
+    const size_t board = tc ? (size_t)conv_tc_board_elems(route == TowerRoute::TcX3) : in_elems, boards = (size_t)n * board;
+    const size_t pool_floats = in_pool ? (size_t)n * pool_stride * board : 0;
+    float *d_blob = nullptr, *d_x = nullptr, *d_stage = nullptr, *d_out = nullptr, *d_pool = nullptr;
     int32_t *d_action = nullptr, *d_parent = nullptr;
     auto cleanup = [&]() {
-        for (void* p : {(void*)d_blob, (void*)d_in, (void*)d_out, (void*)d_action, (void*)d_parent, (void*)r.d_sat}) if (p) cudaFree(p);
-        r.d_sat = nullptr; r.d_conv = nullptr;
+        for (void* p : {(void*)d_blob, (void*)d_x, (void*)d_stage, (void*)d_out, (void*)d_pool, (void*)d_action, (void*)d_parent,
+                        (void*)r.ws[0], (void*)r.ws[1], (void*)r.ws[2], (void*)r.scratch_state, (void*)r.d_sat})
+            if (p) cudaFree(p);
+        r.ws[0] = r.ws[1] = r.ws[2] = r.scratch_state = nullptr; r.d_sat = nullptr; r.d_conv = nullptr;
     };
-    const bool ok = cudaMalloc(&d_blob, blob.size() * 4) == cudaSuccess && cudaMalloc(&d_in, in_total * 4) == cudaSuccess &&
-                    cudaMalloc(&d_out, dense * 4) == cudaSuccess && cudaMalloc(&d_action, (size_t)n * 4) == cudaSuccess &&
-                    cudaMalloc(&d_parent, (size_t)n * 4) == cudaSuccess && cudaMalloc(&r.d_sat, 64) == cudaSuccess;
+    bool ok = cudaMalloc(&d_blob, blob.size() * 4) == cudaSuccess && cudaMalloc(&d_x, (size_t)n * in_elems * 4) == cudaSuccess &&
+              cudaMalloc(&d_stage, boards * 4) == cudaSuccess && cudaMalloc(&d_out, dense * 4) == cudaSuccess &&
+              cudaMalloc(&r.scratch_state, boards * 4) == cudaSuccess && cudaMalloc(&r.d_sat, 64) == cudaSuccess &&
+              cudaMalloc(&d_action, (size_t)n * 4) == cudaSuccess && cudaMalloc(&d_parent, (size_t)n * 4) == cudaSuccess &&
+              (!in_pool || cudaMalloc(&d_pool, pool_floats * 4) == cudaSuccess);
+    for (int i = 0; ok && i < 3; ++i) ok = cudaMalloc(&r.ws[i], boards * 4) == cudaSuccess;
     if (!ok) { cleanup(); *err = "allocation failed"; return MZ_ENOMEM; }
     r.d_conv = d_blob;
     cudaMemcpy(d_blob, blob.data(), blob.size() * 4, cudaMemcpyHostToDevice);
-    if (in_pool) {
-        cudaMemset(d_in, 0xFF, in_total * 4);
-        for (int g = 0; g < n; ++g)
-            cudaMemcpy(d_in + ((size_t)g * pool_stride + parent[g]) * board, x + (size_t)g * board, board * 4, cudaMemcpyHostToDevice);
-        cudaMemcpy(d_parent, parent, (size_t)n * 4, cudaMemcpyHostToDevice);
-    } else {
-        cudaMemcpy(d_in, x, dense * 4, cudaMemcpyHostToDevice);
-    }
-    if (stem) cudaMemcpy(d_action, action, (size_t)n * 4, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_x, x, (size_t)n * in_elems * 4, cudaMemcpyHostToDevice);
+    if (dyn) cudaMemcpy(d_action, action, (size_t)n * 4, cudaMemcpyHostToDevice);
+    if (in_pool) cudaMemcpy(d_parent, parent, (size_t)n * 4, cudaMemcpyHostToDevice);
+    for (int i = 0; i < 3; ++i) cudaMemset(r.ws[i], 0xFF, boards * 4);
+    cudaMemset(r.scratch_state, 0xFF, boards * 4);
     cudaMemset(d_out, 0xFF, dense * 4);
     cudaMemset(r.d_sat, 0, 64);
-    *launches = 0;
-    WideTowerPlan used{}, first{};
+    // the input boards, zero padded, where the stage before the tower leaves them
+    const unsigned cblocks = (unsigned)((dense + 255) / 256);
+    const float* stage = d_x;
+    if (tc) {
+        cudaMemset(d_stage, 0, boards * 4);
+        nchw_to_p64c4_kernel<<<cblocks, 256>>>(d_x, d_stage, n, C, H, W, route == TowerRoute::TcX3);
+        stage = d_stage;
+    }
+    const float* in = stage;
+    if (in_pool) {
+        cudaMemset(d_pool, 0xFF, pool_floats * 4);
+        for (int g = 0; g < n; ++g)
+            cudaMemcpy(d_pool + ((size_t)g * pool_stride + parent[g]) * board, stage + (size_t)g * board, board * 4,
+                       cudaMemcpyDeviceToDevice);
+        in = d_pool;
+    } else if (tc) {
+        float* dst = tc_tower_input(&r, site);
+        cudaMemcpy(dst, stage, boards * 4, cudaMemcpyDeviceToDevice);
+        in = dst;
+    }
+    int64_t n_launches = 0;
+    SmallTowerPlan small_used{}, small_first{};
+    WideTowerPlan wide_used{}, wide_first{};
+    const float* result = nullptr;
     int rc = MZ_OK;
     // the ranges of the partitioned replay, each through its own Runner (one range unless in the pool); every array stays
     // addressed by the global game.  The plan reported is the first range's.
     const int per = in_pool ? partition_games(n, parts) : n;
     for (int p = 0; p * per < n && rc == MZ_OK; ++p) {
-        Runner R{&r, nullptr, launches, err, std::min(per, n - p * per), p * per};
-        R.wide_plan_out = &used;
-        int done;
-        if (site == MZ_TOWER_REPRESENTATION) done = R.representation_wide_tower(d_in, d_out);
-        else if (site == MZ_TOWER_DYNAMICS) done = R.dynamics_wide_tower(d_in, d_out, d_action);
-        else if (site == MZ_TOWER_DYNAMICS_POOL) done = R.dynamics_wide_tower_pool(d_in, d_parent, pool_stride, d_out, d_action);
-        else done = R.prediction_wide_tower(d_in, d_out);
-        if (done == 0) { *err = "no wide launch"; rc = MZ_EUNSUPPORTED; }
-        else if (done < 0) rc = MZ_ECUDA;
-        if (p == 0) first = used;
+        Runner R{&r, nullptr, &n_launches, err, std::min(per, n - p * per), p * per};
+        R.small_plan = &small_used; R.wide_plan_out = &wide_used;
+        const TowerSite s = site == MZ_TOWER_REPRESENTATION ? R.representation_site(in, !stem)
+                          : site == MZ_TOWER_PREDICTION     ? R.prediction_site(in)
+                          : R.dynamics_site(in, d_action, in_pool ? d_parent : nullptr, in_pool ? pool_stride : 0);
+        const float* res = d_out;
+        if (tc) {
+            res = R.tower_tc(s);
+            if (!res) rc = MZ_ECUDA;
+        } else {
+            const int done = fused ? R.small_tower(s, d_out) : R.wide_tower(s, d_out);
+            if (done < 0) {
+                rc = MZ_ECUDA;
+            } else if (done == 0 && fused) {
+                int64_t unused[6];
+                std::string why = "no fused launch";
+                resnet_small_tower_plan(R.n, stem ? cin[0] : C, C, H, W, blocks, stem, sm_count, unused, &why);
+                *err = "the fused tower refuses the shape: " + why; rc = MZ_EUNSUPPORTED;
+            } else if (done == 0) {
+                *err = "no wide launch"; rc = MZ_EUNSUPPORTED;
+            }
+        }
+        if (rc == MZ_OK && result && res != result) { *err = "partitions ended in different buffers"; rc = MZ_ECUDA; }
+        result = res;
+        if (p == 0) { small_first = small_used; wide_first = wide_used; }
     }
     cudaError_t e = cudaDeviceSynchronize();
-    if (rc == MZ_OK && e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug wide tower: ") + cudaGetErrorString(e); }
+    if (rc == MZ_OK && e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug tower: ") + cudaGetErrorString(e); }
     if (rc == MZ_OK) {
+        if (tc) p64c4_to_nchw_kernel<<<cblocks, 256>>>(result, d_out, n, C, H, W, route == TowerRoute::TcX3);
         int sat = 0;
         e = cudaMemcpy(out, d_out, dense * 4, cudaMemcpyDeviceToHost);
         if (e == cudaSuccess) e = cudaMemcpy(&sat, r.d_sat, 4, cudaMemcpyDeviceToHost);
-        if (e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug wide tower: ") + cudaGetErrorString(e); }
+        if (e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug tower: ") + cudaGetErrorString(e); }
         if (saturated) *saturated = sat;
-        if (plan) wide_plan_export(first, pair, plan);
+        if (plan && fused) {
+            const SmallTowerPlan& f = small_first;
+            const int64_t pl[6] = {f.P, f.CO, f.boards_per_cta, f.threads, f.grid, (int64_t)f.smem};
+            for (int i = 0; i < 6; ++i) plan[i] = pl[i];
+        }
+        if (plan && is_wide(route)) wide_plan_export(wide_first, pair, plan);
     }
+    if (launches) *launches = n_launches;
     cleanup();
     return rc;
 }
@@ -1970,7 +1814,7 @@ static bool debug_heads_device(ResNetDevice& r, int C, int H, int W, int site, i
     if (*n_heads > 0 && !shapes) { *err = "head shapes missing"; return false; }
     r = ResNetDevice{};
     r.C = C; r.hh = H; r.hw = W; r.sm_count = sm_count; r.max_batch = 0;
-    r.use_tc = layout != kLayoutDense; r.split = layout == kLayoutSplit;
+    r.route = layout == kLayoutSplit ? TowerRoute::TcX3 : layout == kLayoutF16 ? TowerRoute::TcF16 : TowerRoute::CudaCore;
     HeadDesc* dst[2] = {site == MZ_TOWER_PREDICTION ? &r.value_head : &r.reward_head, &r.policy_head};
     size_t size = 0;
     for (int h = 0; h < *n_heads; ++h) {
@@ -1990,7 +1834,7 @@ static HeadsArgs debug_heads_args(Runner& R, int site, int n_heads) {
     ResNetDevice* r = R.r;
     const HeadDesc* h0 = site == MZ_TOWER_PREDICTION ? &r->value_head : &r->reward_head;
     return R.heads_args(nullptr, n_heads, n_heads > 0 ? h0 : nullptr, n_heads > 1 ? &r->policy_head : nullptr, nullptr, nullptr,
-                        nullptr, nullptr, nullptr, nullptr, 0, 0, r->use_tc);
+                        nullptr, nullptr, nullptr, nullptr, 0, 0);
 }
 
 // Launch plan of one heads call (host only, behind mz_debug_heads_plan): plan[5] = {route, groups per CTA, threads, grid,
@@ -2043,7 +1887,7 @@ int resnet_debug_heads(int n, int C, int H, int W, int site, int layout, int rou
         if (!resnet_heads_plan(std::min(per, n - g0), g0, C, H, W, site, layout, route, shapes, sm_count, unused, err)) return MZ_EUNSUPPORTED;
     }
     const size_t dense = (size_t)n * C * H * W;
-    const size_t elems = layout != kLayoutDense ? (size_t)conv_tc_board_elems(r.split) : (size_t)C * H * W;
+    const size_t elems = layout != kLayoutDense ? (size_t)conv_tc_board_elems(layout == kLayoutSplit) : (size_t)C * H * W;
     const int n_out0 = n_heads > 0 ? shapes[1] : 0, n_out1 = n_heads > 1 ? shapes[3 + MZ_MAX_LAYERS + 1] : 0;
     float *d_blob = nullptr, *d_x = nullptr, *d_in = nullptr, *d_l0 = nullptr, *d_l1 = nullptr, *d_sc = nullptr, *d_resc = nullptr,
           *d_pool = nullptr, *d_state = nullptr;
@@ -2061,7 +1905,7 @@ int resnet_debug_heads(int n, int C, int H, int W, int site, int layout, int rou
     cudaMemcpy(d_x, x, dense * 4, cudaMemcpyHostToDevice);
     if (layout != kLayoutDense) {
         cudaMemset(d_in, 0, (size_t)n * elems * 4);                    // padding positions read as zero, as in the workspaces
-        nchw_to_p64c4_kernel<<<(unsigned)((dense + 255) / 256), 256>>>(d_x, d_in, n, C, H, W, r.split ? 1 : 0);
+        nchw_to_p64c4_kernel<<<(unsigned)((dense + 255) / 256), 256>>>(d_x, d_in, n, C, H, W, layout == kLayoutSplit);
     } else {
         cudaMemcpy(d_in, x, dense * 4, cudaMemcpyHostToDevice);
     }
@@ -2098,7 +1942,9 @@ int resnet_debug_heads(int n, int C, int H, int W, int site, int layout, int rou
 // stored hidden states (pool layout) -> dense NCHW, device to device
 int resnet_states_to_nchw(ResNetDevice* r, const float* states, int count, float* out, cudaStream_t stream) {
     const size_t total = (size_t)count * r->C * r->hh * r->hw;
-    if (r->use_tc) p64c4_to_nchw_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(states, out, count, r->C, r->hh, r->hw, r->split ? 1 : 0);
+    if (is_tc(r->route))
+        p64c4_to_nchw_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(states, out, count, r->C, r->hh, r->hw,
+                                                                                   r->route == TowerRoute::TcX3);
     else cudaMemcpyAsync(out, states, total * 4, cudaMemcpyDeviceToDevice, stream);
     return cudaGetLastError() == cudaSuccess ? MZ_OK : MZ_ECUDA;
 }
@@ -2106,9 +1952,10 @@ int resnet_states_to_nchw(ResNetDevice* r, const float* states, int count, float
 // dense NCHW states -> the pool layout, device to device (mz_import_tree)
 int resnet_states_from_nchw(ResNetDevice* r, const float* dense, int count, float* states, cudaStream_t stream) {
     const size_t total = (size_t)count * r->C * r->hh * r->hw;
-    if (r->use_tc) {
-        cudaMemsetAsync(states, 0, (size_t)count * r->state_elems * 4, stream);          // padding positions read as zero
-        nchw_to_p64c4_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(dense, states, count, r->C, r->hh, r->hw, r->split ? 1 : 0);
+    if (is_tc(r->route)) {
+        cudaMemsetAsync(states, 0, (size_t)count * state_elems(r) * 4, stream);          // padding positions read as zero
+        nchw_to_p64c4_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(dense, states, count, r->C, r->hh, r->hw,
+                                                                                   r->route == TowerRoute::TcX3);
     } else {
         cudaMemcpyAsync(states, dense, total * 4, cudaMemcpyDeviceToDevice, stream);
     }
@@ -2120,17 +1967,17 @@ int resnet_states_from_nchw(ResNetDevice* r, const float* dense, int count, floa
 // arguments of the towers and the heads are the ones resnet_inference would launch with, simulation after simulation.
 static bool small_search_build(ResNetDevice* r, const InferCall& c, const TreeStepArgs& tree, int n_sims, SmallSearchArgs* out,
                                int* P, int* CO, int* G, int* threads, size_t* smem) {
-    if (r->use_tc || r->wide || !r->loaded || !r->fuse_small || !c.recurrent || !c.gather_parent || c.hidden || r->net.blocks < 1) return false;
+    if (r->route != TowerRoute::CudaCore || !r->loaded || !r->fuse_small || !c.recurrent || !c.gather_parent || c.hidden || r->net.blocks < 1) return false;
     if (c.value_logits || c.reward_logits) return false;
     std::string err; int64_t launches = 0;
     Runner R{r, nullptr, &launches, &err, c.n, c.g0};
-    const int C = r->C, hh = r->hh, hw = r->hw, nb = r->net.blocks;
+    const int C = r->C, hh = r->hh, hw = r->hw;
     SmallSearchArgs a{};
     float* raw = r->ws[0];                 // dynamics tower output
     float* pred_out = r->ws[1];            // prediction tower output
     float* hidden = r->scratch_hidden;     // rescaled state, dense (input of the prediction tower)
-    if (!R.small_tower_args(a.dyn, r->dyn, 0, true, nb, c.pool_hidden, raw, C, hh, hw, c.gather_parent, c.pool_stride, c.action)) return false;
-    if (!R.small_tower_args(a.pred, r->pred, 0, false, nb, hidden, pred_out, C, hh, hw, nullptr, 0, nullptr)) return false;
+    if (!R.small_tower_args(a.dyn, R.dynamics_site(c.pool_hidden, c.action, c.gather_parent, c.pool_stride), raw)) return false;
+    if (!R.small_tower_args(a.pred, R.prediction_site(hidden), pred_out)) return false;
     if (!small_tower_layout(a.dyn) || !small_tower_layout(a.pred)) return false;
     const int cap = std::max(a.dyn.cap_channels, a.pred.cap_channels);
     a.dyn.cap_channels = a.pred.cap_channels = cap;
@@ -2186,24 +2033,22 @@ int resnet_small_search(ResNetDevice* r, const InferCall& c, const TreeStepArgs&
 int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, int64_t* launches, std::string* err) {
     if (!r->loaded) { *err = "weights not loaded"; return MZ_ESTATE; }
     if (c.g0 < 0 || c.g0 + c.n > r->max_batch) { *err = "batch larger than max_games"; return MZ_EINVAL; }
-    if (r->use_tc) return resnet_inference_tc(r, c, stream, launches, err);
+    if (is_tc(r->route)) return resnet_inference_tc(r, c, stream, launches, err);
     const MzNetDesc& nd = r->net;
-    const int n = c.n, C = r->C, hh = r->hh, hw = r->hw, F = 2 * nd.support_size + 1;
+    const int n = c.n, C = r->C, F = 2 * nd.support_size + 1;
     Runner R{r, stream, launches, err, n, c.g0};
     if (c.g0 != 0 && !c.recurrent) { *err = "resnet: partitioned calls are recurrent only"; return MZ_EINVAL; }
     float *cur = r->ws[0], *tmp = r->ws[1], *spare = r->ws[2];
     float* hidden_out = c.hidden ? c.hidden : r->scratch_hidden;
+    const int kAll = Runner::kTryWide | Runner::kTryFused;
 
     if (!c.recurrent) {
-        int H = nd.obs_h, W = nd.obs_w;
+        const float* x;
         if (nd.downsample == 2) {
             if (!R.cnn_stem(c.in, tmp, cur)) return MZ_ECUDA;
-            H = hh; W = hw;
-            const int fused = R.small_tower(r->rep_trunk, 0, false, nd.blocks, cur, tmp, C, H, W);
-            if (fused < 0) return MZ_ECUDA;
-            if (fused) { float* t = cur; cur = tmp; tmp = t; }
-            else if (!R.blocks(r->rep_trunk, 0, nd.blocks, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
+            x = R.site_tower(R.representation_site(cur), Runner::kTryFused, &cur, &tmp, &spare);
         } else if (nd.downsample) {
+            int H = nd.obs_h, W = nd.obs_w;
             const auto& d = r->rep_down;
             if (!R.conv(d[0], c.in, cur, nullptr, false, H, W)) return MZ_ECUDA;
             H = conv_out(H, 2); W = conv_out(W, 2);
@@ -2221,27 +2066,17 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
                 H = Ho; W = Wo;
                 if (pool == 0 && !R.blocks(d, 12, 3, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
             }
-            const int fused = R.small_tower(r->rep_trunk, 0, false, nd.blocks, cur, tmp, C, H, W);
-            if (fused < 0) return MZ_ECUDA;
-            if (fused) { float* t = cur; cur = tmp; tmp = t; }
-            else if (!R.blocks(r->rep_trunk, 0, nd.blocks, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
-        } else if (r->wide && nd.blocks > 0) {
-            // the stem on the CUDA cores, the blocks as one wide launch
-            if (!R.conv(r->rep_trunk[0], c.in, cur, nullptr, true, H, W)) return MZ_ECUDA;
-            const int wide = R.representation_wide_tower(cur, tmp);
-            if (wide < 0) return MZ_ECUDA;
-            if (wide) { float* t = cur; cur = tmp; tmp = t; }
-            else if (!R.blocks(r->rep_trunk, 1, nd.blocks, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
+            x = R.site_tower(R.representation_site(cur), Runner::kTryFused, &cur, &tmp, &spare);
+        } else if (is_wide(r->route) && nd.blocks > 0) {
+            // the stem on the CUDA cores, the blocks as one wide launch (per layer if the wide launch refuses)
+            if (!R.conv(r->rep_trunk[0], c.in, cur, nullptr, true, nd.obs_h, nd.obs_w)) return MZ_ECUDA;
+            x = R.site_tower(R.representation_site(cur, true), Runner::kTryWide, &cur, &tmp, &spare);
         } else {
-            const int fused = R.representation_small_tower(c.in, cur);
-            if (fused < 0) return MZ_ECUDA;
-            if (!fused) {
-                if (!R.conv(r->rep_trunk[0], c.in, cur, nullptr, true, H, W)) return MZ_ECUDA;
-                if (!R.blocks(r->rep_trunk, 1, nd.blocks, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
-            }
+            x = R.site_tower(R.representation_site(c.in), Runner::kTryFused, &cur, &tmp, &spare);
         }
+        if (!x) return MZ_ECUDA;
         // rescale -> hidden (no heads on the raw state at the root)
-        if (!R.representation_heads(cur, hidden_out, c.pool_hidden, c.pool_stride, c.out_slot)) return MZ_ECUDA;
+        if (!R.representation_heads(x, hidden_out, c.pool_hidden, c.pool_stride, c.out_slot)) return MZ_ECUDA;
         if (c.reward_logits) {
             fill_root_reward_logits_kernel<<<(n * F + 255) / 256, 256, 0, stream>>>(c.reward_logits, n, F, nd.support_size);
             *launches += 1;
@@ -2251,39 +2086,17 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
             *launches += 1;
         }
     } else {
-        const float* in = c.gather_parent ? c.pool_hidden : c.in;
-        int fused = c.gather_parent ? R.dynamics_wide_tower_pool(c.pool_hidden, c.gather_parent, c.pool_stride, cur, c.action)
-                                    : R.dynamics_wide_tower(c.in, cur, c.action);
-        if (fused == 0)
-            fused = c.gather_parent ? R.dynamics_small_tower_pool(c.pool_hidden, c.gather_parent, c.pool_stride, cur, c.action)
-                                    : R.dynamics_small_tower(c.in, cur, c.action);
-        if (fused < 0) return MZ_ECUDA;
-        if (!fused) {
-            if (!R.conv(r->dyn[0], in, cur, nullptr, true, hh, hw, c.gather_parent, c.pool_stride, c.action)) return MZ_ECUDA;
-            if (!R.blocks(r->dyn, 1, nd.blocks, &cur, &tmp, &spare, hh, hw)) return MZ_ECUDA;
-        }
+        const TowerSite s = c.gather_parent ? R.dynamics_site(c.pool_hidden, c.action, c.gather_parent, c.pool_stride)
+                                            : R.dynamics_site(c.in, c.action);
+        const float* x = R.site_tower(s, kAll, &cur, &tmp, &spare);
+        if (!x) return MZ_ECUDA;
         // reward head on the raw state + rescale -> hidden
-        if (!R.dynamics_heads(cur, c.reward_logits, c.reward, hidden_out, c.pool_hidden, c.pool_stride, c.out_slot)) return MZ_ECUDA;
+        if (!R.dynamics_heads(x, c.reward_logits, c.reward, hidden_out, c.pool_hidden, c.pool_stride, c.out_slot)) return MZ_ECUDA;
     }
-    // prediction on the rescaled state
-    {
-        float* x = hidden_out;
-        // the tower must not overwrite the hidden state: first conv reads it, writes workspace
-        float *pc = cur, *pt = tmp, *ps = spare;
-        int fused = R.prediction_wide_tower(x, pt);
-        if (fused == 0) fused = R.prediction_small_tower(x, pt);
-        if (fused < 0) return MZ_ECUDA;
-        if (fused) {
-            x = pt;
-        } else if (nd.blocks > 0) {
-            if (!R.conv(r->pred[0], x, pt, nullptr, true, hh, hw)) return MZ_ECUDA;
-            if (!R.conv(r->pred[1], pt, ps, x, true, hh, hw)) return MZ_ECUDA;
-            { float* t = pc; pc = ps; ps = t; }
-            if (!R.blocks(r->pred, 2, nd.blocks - 1, &pc, &pt, &ps, hh, hw)) return MZ_ECUDA;
-            x = pc;
-        }
-        if (!R.prediction_heads(x, c.value_logits, c.policy_logits, c.value)) return MZ_ECUDA;
-    }
+    // prediction on the rescaled state, which the tower reads and never writes
+    const float* x = R.site_tower(R.prediction_site(hidden_out), kAll, &cur, &tmp, &spare);
+    if (!x) return MZ_ECUDA;
+    if (!R.prediction_heads(x, c.value_logits, c.policy_logits, c.value)) return MZ_ECUDA;
     return MZ_OK;
 }
 

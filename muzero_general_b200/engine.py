@@ -624,6 +624,36 @@ def debug_conv3x3(x, w, bias=None, residual=None, relu=False, tensor_cores=False
 TOWER_SITES = {"representation": 0, "dynamics": 1, "dynamics_pool": 2, "prediction": 3}
 
 
+def _tower_args(x, weights, biases, site, actions, parents, channels=None):
+    """Validates one debug tower call and marshals it for the entry: returns (the tower's channels, its blocks, the arrays
+    x, weights, biases, actions, parents in the entries' order, None where not given).  ``channels``: 64 or 128 for the
+    tensor-core towers, which leave the representation stem to the CUDA cores; None for the fused CUDA-core tower, which
+    takes that stem and any channel count (the first conv's outputs)."""
+    x = numpy.ascontiguousarray(x, numpy.float32)
+    n, cin, H, W = x.shape
+    fused = channels is None
+    dyn = site in ("dynamics", "dynamics_pool")
+    stem = dyn or (fused and site == "representation")
+    ch = numpy.shape(weights[0])[0] if fused else channels
+    if (len(weights) - stem) % 2 != 0 or (cin != ch and not (stem and not dyn)):
+        raise ValueError(f"{cin} input planes / {len(weights)} convs do not make a {ch}-channel tower at site {site}")
+    for i, w in enumerate(weights):
+        want = (ch, (ch + 1 if dyn else cin) if stem and i == 0 else ch, 3, 3)
+        if numpy.shape(w) != want:
+            raise ValueError(f"conv {i}: weights {numpy.shape(w)}, expected {want}")
+    wcat = numpy.ascontiguousarray(numpy.concatenate([numpy.asarray(w, numpy.float32).reshape(-1) for w in weights]))
+    b = None if biases is None else numpy.ascontiguousarray(numpy.stack(biases), numpy.float32)
+    if b is not None and b.shape != (len(weights), ch):
+        raise ValueError(f"biases {b.shape} do not fit {len(weights)} convs")
+    act = None if actions is None else numpy.ascontiguousarray(actions, numpy.int32)
+    par = None if parents is None else numpy.ascontiguousarray(parents, numpy.int32)
+    return ch, (len(weights) - stem) // 2, (x, wcat, b, act, par)
+
+
+def _ptrs(arrays):
+    return [None if a is None else a.ctypes.data for a in arrays]
+
+
 def debug_conv_tower(x, weights, biases=None, mode="x3", site="prediction", actions=None, A=1, parents=None,
                      pool_stride=1, parts=1, device=0):
     """One 64-channel tensor-core tower of a network call site through mz_debug_conv_tower; numpy NCHW in and out.
@@ -632,26 +662,12 @@ def debug_conv_tower(x, weights, biases=None, mode="x3", site="prediction", acti
     (in search: game g's input in pool slot ``parents[g]`` of ``pool_stride``; ``parts`` ranges of the partitioned
     replay) or "prediction".  Returns (out [n, 64, H, W], kernel launches, x3 range-guard count)."""
     lib = _lib.load_library()
-    x = numpy.ascontiguousarray(x, numpy.float32)
-    n, ch, H, W = x.shape
-    stem = site in ("dynamics", "dynamics_pool")
-    if ch != 64 or (len(weights) - stem) % 2 != 0:
-        raise ValueError(f"{ch} channels / {len(weights)} convs do not make a 64-channel tower at site {site}")
-    for i, w in enumerate(weights):
-        if numpy.shape(w) != (64, 65 if stem and i == 0 else 64, 3, 3):
-            raise ValueError(f"conv {i}: weights {numpy.shape(w)}")
-    wcat = numpy.ascontiguousarray(numpy.concatenate([numpy.asarray(w, numpy.float32).reshape(-1) for w in weights]))
-    b = None if biases is None else numpy.ascontiguousarray(numpy.stack(biases), numpy.float32)
-    if b is not None and b.shape != (len(weights), 64):
-        raise ValueError(f"biases {b.shape} do not fit {len(weights)} convs")
-    act = None if actions is None else numpy.ascontiguousarray(actions, numpy.int32)
-    par = None if parents is None else numpy.ascontiguousarray(parents, numpy.int32)
-    out = numpy.empty_like(x)
+    _, blocks, arrays = _tower_args(x, weights, biases, site, actions, parents, 64)
+    n, _, H, W = arrays[0].shape
+    out = numpy.empty_like(arrays[0])
     launches, sat = C.c_int64(0), C.c_int32(0)
-    rc = lib.mz_debug_conv_tower(device, n, H, W, {"fp16": 1, "x3": 2}[mode], (len(weights) - stem) // 2, TOWER_SITES[site],
-                                 parts, A, x.ctypes.data, wcat.ctypes.data, None if b is None else b.ctypes.data,
-                                 None if act is None else act.ctypes.data, None if par is None else par.ctypes.data,
-                                 pool_stride, out.ctypes.data, C.byref(launches), C.byref(sat))
+    rc = lib.mz_debug_conv_tower(device, n, H, W, {"fp16": 1, "x3": 2}[mode], blocks, TOWER_SITES[site], parts, A,
+                                 *_ptrs(arrays), pool_stride, out.ctypes.data, C.byref(launches), C.byref(sat))
     if rc != 0:
         raise _lib.MzError(rc, lib.mz_last_error(None).decode())
     return out, launches.value, sat.value
@@ -678,27 +694,11 @@ def debug_small_tower(x, weights, biases=None, site="prediction", actions=None, 
     recurrent call), "dynamics_pool" (in search: game g's input in pool slot ``parents[g]`` of ``pool_stride``; ``parts``
     ranges of the partitioned replay) or "prediction".  Returns (out [n, C, H, W], the plan of the launch as a dict)."""
     lib = _lib.load_library()
-    x = numpy.ascontiguousarray(x, numpy.float32)
-    n, cin, H, W = x.shape
-    stem = site != "prediction"
-    ch = numpy.shape(weights[0])[0]
-    if (len(weights) - stem) % 2 != 0 or (site != "representation" and cin != ch):
-        raise ValueError(f"{cin} input planes / {len(weights)} convs do not make a {ch}-channel tower at site {site}")
-    for i, w in enumerate(weights):
-        want = (ch, (cin + (site != "representation") if stem else ch) if i == 0 else ch, 3, 3)
-        if numpy.shape(w) != want:
-            raise ValueError(f"conv {i}: weights {numpy.shape(w)}, expected {want}")
-    wcat = numpy.ascontiguousarray(numpy.concatenate([numpy.asarray(w, numpy.float32).reshape(-1) for w in weights]))
-    b = None if biases is None else numpy.ascontiguousarray(numpy.stack(biases), numpy.float32)
-    if b is not None and b.shape != (len(weights), ch):
-        raise ValueError(f"biases {b.shape} do not fit {len(weights)} convs")
-    act = None if actions is None else numpy.ascontiguousarray(actions, numpy.int32)
-    par = None if parents is None else numpy.ascontiguousarray(parents, numpy.int32)
+    ch, blocks, arrays = _tower_args(x, weights, biases, site, actions, parents)
+    n, cin, H, W = arrays[0].shape
     out = numpy.empty((n, ch, H, W), numpy.float32)
     plan = (C.c_int64 * 6)()
-    rc = lib.mz_debug_small_tower(device, n, cin, ch, H, W, (len(weights) - stem) // 2, TOWER_SITES[site], parts, A,
-                                  x.ctypes.data, wcat.ctypes.data, None if b is None else b.ctypes.data,
-                                  None if act is None else act.ctypes.data, None if par is None else par.ctypes.data,
+    rc = lib.mz_debug_small_tower(device, n, cin, ch, H, W, blocks, TOWER_SITES[site], parts, A, *_ptrs(arrays),
                                   pool_stride, out.ctypes.data, plan)
     if rc != 0:
         raise _lib.MzError(rc, lib.mz_last_error(None).decode())
@@ -751,27 +751,13 @@ def debug_wide_pair_tower(x, weights, biases=None, site="prediction", actions=No
 
 def _wide_tower(entry, fields, x, weights, biases, site, actions, A, parents, pool_stride, parts, device):
     lib = _lib.load_library()
-    x = numpy.ascontiguousarray(x, numpy.float32)
-    n, ch, H, W = x.shape
-    stem = site in ("dynamics", "dynamics_pool")
-    if ch != 128 or (len(weights) - stem) % 2 != 0:
-        raise ValueError(f"{ch} channels / {len(weights)} convs do not make a 128-channel tower at site {site}")
-    for i, w in enumerate(weights):
-        if numpy.shape(w) != (128, 129 if stem and i == 0 else 128, 3, 3):
-            raise ValueError(f"conv {i}: weights {numpy.shape(w)}")
-    wcat = numpy.ascontiguousarray(numpy.concatenate([numpy.asarray(w, numpy.float32).reshape(-1) for w in weights]))
-    b = None if biases is None else numpy.ascontiguousarray(numpy.stack(biases), numpy.float32)
-    if b is not None and b.shape != (len(weights), 128):
-        raise ValueError(f"biases {b.shape} do not fit {len(weights)} convs")
-    act = None if actions is None else numpy.ascontiguousarray(actions, numpy.int32)
-    par = None if parents is None else numpy.ascontiguousarray(parents, numpy.int32)
-    out = numpy.empty_like(x)
+    _, blocks, arrays = _tower_args(x, weights, biases, site, actions, parents, 128)
+    n, _, H, W = arrays[0].shape
+    out = numpy.empty_like(arrays[0])
     launches, sat = C.c_int64(0), C.c_int32(0)
     plan = (C.c_int64 * 9)()
-    rc = getattr(lib, entry)(device, n, H, W, (len(weights) - stem) // 2, TOWER_SITES[site], parts, A, x.ctypes.data,
-                             wcat.ctypes.data, None if b is None else b.ctypes.data,
-                             None if act is None else act.ctypes.data, None if par is None else par.ctypes.data,
-                             pool_stride, out.ctypes.data, C.byref(launches), C.byref(sat), plan)
+    rc = getattr(lib, entry)(device, n, H, W, blocks, TOWER_SITES[site], parts, A, *_ptrs(arrays), pool_stride,
+                             out.ctypes.data, C.byref(launches), C.byref(sat), plan)
     if rc != 0:
         raise _lib.MzError(rc, lib.mz_last_error(None).decode())
     return out, launches.value, sat.value, dict(zip(fields, plan))
