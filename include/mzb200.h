@@ -378,6 +378,26 @@ int mz_debug_wide_pair_tower(int device, int32_t n, int32_t H, int32_t W, int32_
                              const float* x, const float* w, const float* bias, const int32_t* action, const int32_t* parent,
                              int32_t pool_stride, float* out, int64_t* launches, int32_t* saturated, int64_t* plan);
 
+/* Launch plan of the 256-channel tower (host only; the route MZ_TC_WIDE=3 opts 256-channel nets such as games/atari.py's
+ * into): n boards of C x H x W through [a stem conv, C + 1 planes with the action plane, if stem] + `blocks` residual blocks
+ * as x3 tensor-core MMAs on clusters of two CTAs, CTA r computing output channels [128 r, 128 r + 128) of `boards` boards
+ * stacked in its M rows and exchanging them through distributed shared memory after every layer.  boards = 0 plans the
+ * largest number of boards per CTA pair that fits, boards > 0 forces that many.  Fills plan[10] = {boards per CTA pair,
+ * M-tiles per CTA, threads per CTA, dynamic shared-memory bytes per CTA, weight ring stages, layers, CTAs per SM, boards per
+ * wave, launches per tower call, registers per thread assumed} and returns 1; returns 0 with the reason in
+ * mz_last_error(NULL) when the tower refuses the shape (C != 256, more than 16 blocks, a board beyond the M-tile or
+ * shared-memory budget). */
+int mz_debug_wide256_tower_plan(int32_t n, int32_t C, int32_t H, int32_t W, int32_t blocks, int32_t stem, int32_t sm_count,
+                                int32_t boards, int64_t* plan);
+
+/* Debug / parity: mz_debug_wide_tower for 256 channels (x [n][256][H][W], w the convs [256][cin][3][3] back to back with
+ * cin = 257 for the dynamics stem, bias [convs][256]) on the 256-channel tower, with `boards` as for
+ * mz_debug_wide256_tower_plan; plan (or NULL) as that entry fills it.  MZ_EUNSUPPORTED when the tower refuses the shape. */
+int mz_debug_wide256_tower(int device, int32_t n, int32_t H, int32_t W, int32_t blocks, int32_t site, int32_t parts, int32_t A,
+                           const float* x, const float* w, const float* bias, const int32_t* action, const int32_t* parent,
+                           int32_t pool_stride, int32_t boards, float* out, int64_t* launches, int32_t* saturated,
+                           int64_t* plan);
+
 /* Routes of the residual heads (route argument of mz_debug_heads_plan and mz_debug_heads, plan[0]).  The network always
  * takes MZ_HEADS_PLANNED: heads_kernel<32> (one warp per sample) when C*H*W <= 1024, heads_kernel<128> (128 threads per
  * sample) otherwise, the generic route (one plain kernel per stage) when the head weights and one sample's tile exceed

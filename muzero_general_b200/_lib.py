@@ -176,6 +176,10 @@ SYMBOLS = [
     ("mz_debug_wide_pair_tower", C.c_int, [C.c_int] + [C.c_int32] * 7 + [C.c_void_p] * 5 + [C.c_int32, C.c_void_p,
                                                                                            C.POINTER(C.c_int64), C.POINTER(C.c_int32),
                                                                                            C.POINTER(C.c_int64)]),
+    ("mz_debug_wide256_tower_plan", C.c_int, [C.c_int32] * 8 + [C.POINTER(C.c_int64)]),
+    ("mz_debug_wide256_tower", C.c_int, [C.c_int] + [C.c_int32] * 7 + [C.c_void_p] * 5 + [C.c_int32, C.c_int32, C.c_void_p,
+                                                                                         C.POINTER(C.c_int64), C.POINTER(C.c_int32),
+                                                                                         C.POINTER(C.c_int64)]),
     ("mz_debug_heads_plan", C.c_int, [C.c_int32] * 8 + [C.c_void_p, C.c_int32, C.POINTER(C.c_int64)]),
     ("mz_debug_heads", C.c_int, [C.c_int] + [C.c_int32] * 8 + [C.c_void_p, C.POINTER(MzTensor), C.c_int32, C.c_void_p,
                                                               C.c_int32, C.c_int32] + [C.c_void_p] * 6 + [C.POINTER(C.c_int64)]),

@@ -1098,6 +1098,31 @@ extern "C" int mz_debug_wide_pair_tower(int device, int32_t n, int32_t H, int32_
     return MZ_OK;
 }
 
+extern "C" int mz_debug_wide256_tower_plan(int32_t n, int32_t C, int32_t H, int32_t W, int32_t blocks, int32_t stem,
+                                           int32_t sm_count, int32_t boards, int64_t* plan) {
+    if (!plan || sm_count < 1) return fail(nullptr, 0, "mz_debug_wide256_tower_plan: bad argument");
+    std::string e;
+    if (!resnet_wide256_tower_plan(n, C, H, W, blocks, stem != 0, sm_count, boards, plan, &e))
+        return fail(nullptr, 0, "mz_debug_wide256_tower_plan: " + e);
+    return 1;
+}
+
+// debug: one 256-channel tower of one call site of the network, the output channels split across a CTA pair
+extern "C" int mz_debug_wide256_tower(int device, int32_t n, int32_t H, int32_t W, int32_t blocks, int32_t site, int32_t parts,
+                                      int32_t A, const float* x, const float* w, const float* bias, const int32_t* action,
+                                      const int32_t* parent, int32_t pool_stride, int32_t boards, float* out, int64_t* launches,
+                                      int32_t* saturated, int64_t* plan) {
+    if (!x || !w || !out || !launches || boards < 0) return fail(nullptr, MZ_EINVAL, "mz_debug_wide256_tower: bad argument");
+    if (cudaSetDevice(device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_wide256_tower: no such device");
+    cudaDeviceProp prop;
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_wide256_tower: device query failed");
+    std::string e;
+    int rc = resnet_debug_tower(TowerRoute::Wide256, n, kWide256C, kWide256C, H, W, blocks, site, parts, A, x, w, bias, action,
+                                parent, pool_stride, out, launches, saturated, plan, prop.multiProcessorCount, &e, boards);
+    if (rc) return fail(nullptr, rc, "mz_debug_wide256_tower: " + e);
+    return MZ_OK;
+}
+
 extern "C" int mz_debug_cnn_stem_plan(int32_t n, int32_t in, int32_t C, int32_t H, int32_t W, int32_t sm_count, int64_t* plan) {
     if (!plan) return fail(nullptr, 0, "mz_debug_cnn_stem_plan: null plan");
     std::string e;

@@ -78,32 +78,6 @@ constexpr int kRegCap = 168;                          // 65536 / 384 rounded dow
 constexpr int kSmemLimit = 232448;
 constexpr float kLoScale = 2048.0f, kLoUnscale = 1.0f / 2048.0f;
 
-MZ_DEVINL void wgmma_wait_one() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
-
-// fp32 -> (x_h, x_l) as the x3 route splits its boards: both halves saturate to the finite fp16 range
-MZ_DEVINL void split_store(unsigned char* hi, unsigned char* lo, float v) {
-    const float s = fminf(fmaxf(v, -65504.0f), 65504.0f);
-    const __half h = __float2half_rn(s);
-    *reinterpret_cast<__half*>(hi) = h;
-    *reinterpret_cast<__half*>(lo) = __float2half_rn(fminf(fmaxf((v - __half2float(h)) * kLoScale, -65504.0f), 65504.0f));
-}
-
-// distributed shared memory of a cluster (the CTA pair)
-MZ_DEVINL uint32_t cluster_rank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-MZ_DEVINL uint32_t map_to_cta(uint32_t addr, uint32_t rank) {     // my shared::cta address -> the same offset in CTA `rank`
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
-MZ_DEVINL void st_cluster_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
-MZ_DEVINL void cluster_barrier() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
 // The board rows [y0, y0 + rows) a CTA owns: all of them on one CTA; on a pair CTA 0 takes ceil(H / 2), CTA 1 the rest.
 // The pair reads its rank with a volatile instruction: the epilogue asks again instead of keeping the geometry live through
 // the MMA loop, whose accumulators fill the register budget.

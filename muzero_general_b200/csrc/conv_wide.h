@@ -55,4 +55,46 @@ cudaError_t launch_wide_tower(WideTowerArgs a, const WideTowerPlan& p, cudaStrea
 bool wide_pair_plan(int n, int C, int H, int W, int layers, int sm_count, WideTowerPlan* p, const char** why);
 cudaError_t launch_wide_pair_tower(WideTowerArgs a, const WideTowerPlan& p, cudaStream_t stream);
 
+// 256-channel towers (conv_wide256.cu, MZ_TC_WIDE=3): the output channels split across a CTA pair, several boards stacked
+// in the M rows of each CTA.  The layers are WideLayers of a 256-channel x3 image: two 128-output-channel halves, each
+// [9 taps][4 K-quarters][256 rows: w_h cout | w_l cout][64 cin] fp16, 128B-swizzled; scale / bias [256]; the dynamics
+// stem's table [H * W][256].
+constexpr int kWide256C = 256;
+constexpr int kWide256MaxLayers = 33;       // a stem + 16 residual blocks (games/atari.py's dynamics tower)
+
+struct Wide256Args {
+    const float* in;              // [n][256][H][W] dense fp32, or the hidden-state pool when gather_parent is set
+    float* out;                   // [n][256][H][W]
+    const int32_t* gather_parent; // board g reads in + (g * pool_stride + gather_parent[g]) * 256 * H * W
+    int pool_stride;
+    const int32_t* action;        // [n] for a stem with an action table
+    int n, H, W, A;
+    int g0;                       // boards [g0, g0 + n): every array is addressed by the global index
+    int stem;                     // layer 0 is a stem; the layers after it are blocks of two convs
+    int n_layers;
+    WideLayer layer[kWide256MaxLayers];
+    int* sat_count;               // bumped when an activation read or stored exceeds the fp16 range
+    // filled by the launcher from the plan
+    int S, boards, interior, plane_bytes, res_off, bar_off;
+};
+
+// Launch plan of one 256-channel tower (host only).  Every per-CTA field describes one CTA of a pair holding `boards`
+// stacked boards and 128 of the output channels.
+struct Wide256Plan {
+    int boards;                   // boards stacked in the M rows of each CTA pair
+    int m_tiles, threads;         // 64-row M-tiles of the (boards (H + 1) - 1) (W + 1) interior rows, one warpgroup each
+    int rows, interior;           // shared-memory rows of one activation plane (multiple of 8); interior rows computed
+    int stages;                   // weight ring stages (one tap x one 64-channel K-quarter x 128 output channels each)
+    size_t smem;                  // dynamic shared-memory bytes per CTA
+    int layers;
+    int ctas_per_sm, wave;        // resident CTAs per SM; boards per wave (ctas_per_sm x SMs / 2 pairs x boards)
+    int launches;                 // kernel launches per tower call
+    int reg_cap;                  // registers per thread the plan assumes (__launch_bounds__ of the kernel)
+};
+
+// false with the reason in *why when the 256-channel tower refuses the shape; force_boards > 0 plans that many boards per
+// CTA pair instead of the largest number that fits
+bool wide256_plan(int n, int C, int H, int W, int layers, int sm_count, int force_boards, Wide256Plan* p, const char** why);
+cudaError_t launch_wide256_tower(Wide256Args a, const Wide256Plan& p, cudaStream_t stream);
+
 }  // namespace mz

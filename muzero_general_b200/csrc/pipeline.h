@@ -88,7 +88,8 @@ cudaError_t launch_tree_adopt_root(const TreeStepArgs& a, cudaStream_t stream); 
 //   TcX3      64-channel tensor-core towers on split operands (default where the board allows), x_h | x_l board states
 //   Wide      128-channel x3 tensor-core towers, one CTA per board (MZ_TC_WIDE=1), dense states
 //   WidePair  the same, each board split across a CTA pair (MZ_TC_WIDE=2), dense states
-enum class TowerRoute { CudaCore, TcF16, TcX3, Wide, WidePair };
+//   Wide256   256-channel x3 tensor-core towers, output channels split across a CTA pair (MZ_TC_WIDE=3), dense states
+enum class TowerRoute { CudaCore, TcF16, TcX3, Wide, WidePair, Wide256 };
 
 struct ResNetDevice;
 ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, std::string* err);
@@ -104,13 +105,14 @@ bool resnet_can_partition(const ResNetDevice* r);
 // games per range of the partitioned replay (the last range may hold fewer): a multiple of 8
 inline int partition_games(int n, int parts) { return ((n + parts - 1) / parts + 7) & ~7; }
 // Debug / parity entry behind mz_debug_conv_tower (route TcF16 / TcX3, C = 64), mz_debug_small_tower (CudaCore: the fused
-// CUDA-core tower), mz_debug_wide_tower (Wide, C = 128) and mz_debug_wide_pair_tower (WidePair): one tower of one call site
-// of the network on host NCHW data (see include/mzb200.h).  `in_channels` is the planes the representation stem reads
-// (CudaCore only; C otherwise); `launches`, `saturated` and `plan` (plan[6] fused, plan[9] wide) may be null.
+// CUDA-core tower), mz_debug_wide_tower (Wide, C = 128), mz_debug_wide_pair_tower (WidePair) and mz_debug_wide256_tower
+// (Wide256, C = 256): one tower of one call site of the network on host NCHW data (see include/mzb200.h).  `in_channels`
+// is the planes the representation stem reads (CudaCore only; C otherwise); `launches`, `saturated` and `plan` (plan[6]
+// fused, plan[9] wide, plan[10] Wide256) may be null; `force_boards` (Wide256 only) forces the boards per CTA pair.
 int resnet_debug_tower(TowerRoute route, int n, int in_channels, int C, int H, int W, int blocks, int site, int parts, int A,
                        const float* x, const float* w, const float* bias, const int32_t* action, const int32_t* parent,
                        int pool_stride, float* out, int64_t* launches, int32_t* saturated, int64_t* plan, int sm_count,
-                       std::string* err);
+                       std::string* err, int force_boards = 0);
 // Host-only plan of the fused CUDA-core tower (plan[6], see include/mzb200.h, mz_debug_small_tower_plan)
 bool resnet_small_tower_plan(int n, int in_channels, int C, int H, int W, int blocks, bool stem, int sm_count, int64_t* plan,
                              std::string* err);
@@ -118,6 +120,9 @@ bool resnet_small_tower_plan(int n, int in_channels, int C, int H, int W, int bl
 // mz_debug_wide_pair_tower_plan), one CTA (a CTA pair) per board
 bool resnet_wide_tower_plan(int n, int C, int H, int W, int blocks, bool stem, int sm_count, int64_t* plan, std::string* err,
                             bool pair = false);
+// Host-only plan of the 256-channel tower (plan[10], see include/mzb200.h, mz_debug_wide256_tower_plan)
+bool resnet_wide256_tower_plan(int n, int C, int H, int W, int blocks, bool stem, int sm_count, int force_boards, int64_t* plan,
+                               std::string* err);
 // Host-only plan of one heads call (plan[5], see include/mzb200.h, mz_debug_heads_plan) and the debug / parity entry behind
 // mz_debug_heads: the heads of one call site of resnet_inference on host NCHW data, in any of the three state layouts
 bool resnet_heads_plan(int n, int g0, int C, int H, int W, int site, int layout, int route, const int32_t* shapes, int sm_count,

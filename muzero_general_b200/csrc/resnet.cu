@@ -392,12 +392,12 @@ struct ResNetDevice {
 };
 
 static bool is_tc(TowerRoute t) { return t == TowerRoute::TcF16 || t == TowerRoute::TcX3; }
-static bool is_wide(TowerRoute t) { return t == TowerRoute::Wide || t == TowerRoute::WidePair; }
+static bool is_wide(TowerRoute t) { return t == TowerRoute::Wide || t == TowerRoute::WidePair || t == TowerRoute::Wide256; }
 // layout of the stored hidden states and of the tensor-core towers' workspaces
 static int state_layout(TowerRoute t) {
     return t == TowerRoute::TcX3 ? kLayoutSplit : t == TowerRoute::TcF16 ? kLayoutF16 : kLayoutDense;
 }
-// the x3 range guard counts saturated activations on these routes (conv_x3.cu, conv_wide.cu)
+// the x3 range guard counts saturated activations on these routes (conv_x3.cu, conv_wide.cu, conv_wide256.cu)
 static bool range_guarded(TowerRoute t) { return t == TowerRoute::TcX3 || is_wide(t); }
 // float slots per stored hidden state: dense C*H*W, or a board of the tensor-core layout (2048 or 4096)
 static int state_elems(const ResNetDevice* r) {
@@ -498,7 +498,7 @@ static bool heads_fit_one_group(const HeadsFootprint& f) { return ((size_t)f.w_f
 
 // The tower route of a net at max_batch boards, from its shape and MZ_TC_MODE / MZ_NO_TC / MZ_TC_WIDE; *note as
 // ResNetDevice::note.  Allocates nothing.
-static TowerRoute choose_route(const MzNetDesc& net, int max_batch, int sm_count, std::string* note) {
+static TowerRoute choose_route(const MzNetDesc& net, int hh, int hw, int max_batch, int sm_count, std::string* note) {
     // MZ_TC_MODE = "off": fp32 CUDA-core towers everywhere; anything else: tensor-core towers where the shape allows
     // (conv_tc.cu).  MZ_NO_TC=1 is the older spelling of "off".
     const char* no_tc = getenv("MZ_NO_TC");
@@ -528,15 +528,25 @@ static TowerRoute choose_route(const MzNetDesc& net, int max_batch, int sm_count
     // MZ_TC_WIDE=1 (opt-in until measured): the towers of a 128-channel net as x3 tensor-core launches on the dense states
     // (conv_wide.cu), when the planner accepts the hidden board.  The stems and the heads stay on the CUDA cores.
     // MZ_TC_WIDE=2: the same, and a board the one-CTA plan refuses (15 x 15, 16 x 16) is split across CTA pairs.
+    // MZ_TC_WIDE=3: as 2, and the towers of a 256-channel net (games/atari.py) on the hidden board hh x hw, with any
+    // representation stem, as x3 tensor-core launches with the output channels split across CTA pairs (conv_wide256.cu).
     const char* wide_env = getenv("MZ_TC_WIDE");
-    if (!wide_env || (wide_env[0] != '1' && wide_env[0] != '2') || fp16 || net.channels != kWideC || net.downsample)
+    if (wide_env && wide_env[0] == '3' && !fp16 && net.channels == kWide256C) {
+        Wide256Plan p;
+        const char* why = "";
+        if (wide256_plan(max_batch, net.channels, hh, hw, 1 + 2 * net.blocks, sm_count, 0, &p, &why)) return TowerRoute::Wide256;
+        *note = std::string("f32 nets + f64 tree statistics (256-channel towers stay on the CUDA cores: ") + why + ")";
+        return TowerRoute::CudaCore;
+    }
+    if (!wide_env || (wide_env[0] != '1' && wide_env[0] != '2' && wide_env[0] != '3') || fp16 || net.channels != kWideC ||
+        net.downsample)
         return TowerRoute::CudaCore;
     const int layers = 1 + 2 * net.blocks;
     WideTowerPlan p;
     const char* why = "";
     if (wide_tower_plan(max_batch, net.channels, net.obs_h, net.obs_w, layers, sm_count, &p, &why)) return TowerRoute::Wide;
     std::string reasons = why;
-    if (wide_env[0] == '2') {
+    if (wide_env[0] != '1') {
         const char* why_pair = "";
         if (wide_pair_plan(max_batch, net.channels, net.obs_h, net.obs_w, layers, sm_count, &p, &why_pair)) return TowerRoute::WidePair;
         reasons = std::string("one CTA: ") + why + "; CTA pairs: " + why_pair;
@@ -613,7 +623,7 @@ ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, s
         }
     }
     // the route is known here, so the hidden-state pool and the workspaces are sized for it
-    r->route = choose_route(net, max_batch, sm_count, &r->note);
+    r->route = choose_route(net, r->hh, r->hw, max_batch, sm_count, &r->note);
     const char* no_fuse = getenv("MZ_NO_FUSE");
     r->fuse_small = !(no_fuse && no_fuse[0] == '1');
     max_elems = std::max(max_elems, (size_t)state_elems(r));
@@ -696,8 +706,11 @@ float f16_to_float(uint16_t h) {
 }
 
 constexpr int kWideImage = 3;       // pack_conv's `tc` for the x3 image of the wide towers (conv_wide.cu)
+constexpr int kWide256Image = 4;    // the same for the 256-channel towers, one image per 128-output-channel half (conv_wide256.cu)
 // pack_conv's `tc` for the towers of a route: none on the CUDA cores
-int weight_image(TowerRoute t) { return is_wide(t) ? kWideImage : state_layout(t); }
+int weight_image(TowerRoute t) {
+    return t == TowerRoute::Wide256 ? kWide256Image : is_wide(t) ? kWideImage : state_layout(t);
+}
 
 bool pack_conv(Loader& L, const std::string& conv, const std::string& bn, int cin, int cout, int stride,
                std::vector<float>& blob, std::vector<ConvLayer>& layers, int tc = 0, int H = 0, int W = 0) {
@@ -732,13 +745,15 @@ bool pack_conv(Loader& L, const std::string& conv, const std::string& bn, int ci
     }
     while (blob.size() % 4) blob.push_back(0.0f);           // keep every layer 16-byte aligned
     l.tc_off = l.tc_table_off = l.tc_scale_off = -1;
-    if (tc == kLayoutSplit || tc == kWideImage) {
+    if (tc == kLayoutSplit || tc == kWideImage || tc == kWide256Image) {
         // x3 image [tap][K-half][2C rows][cin 64]: rows 0..C-1 = w_h of cout 0..C-1, rows C..2C-1 = w_l; w' = w * 2^k with
         // k per output channel such that the row's largest |w'| lies in [1, 2); w_h = fp16(w'), w_l = fp16(w' - w_h).
         // The 16-byte chunks of a row are XOR-ed with row % 8 (wgmma K-major SWIZZLE_128B).  64 channels (conv_x3.cu): one
-        // K-half; 128 (conv_wide.cu): two, each (tap, K-half) one 32 KB stage of the kernel's weight ring.
+        // K-half; 128 (conv_wide.cu): two, each (tap, K-half) one 32 KB stage of the kernel's weight ring.  256
+        // (conv_wide256.cu): per 128-output-channel half [tap][K-quarter][256 rows: w_h | w_l of the half's couts][cin 64],
+        // each (half, tap, K-quarter) one 32 KB stage; the halves follow one another.
         const int C = cout;
-        const bool wide = tc == kWideImage;
+        const bool wide = tc == kWideImage || tc == kWide256Image, halves = tc == kWide256Image;
         l.tc_off = (long)blob.size();
         blob.resize(blob.size() + (size_t)9 * 2 * C * C / 2);
         l.tc_scale_off = (long)blob.size();
@@ -765,6 +780,12 @@ bool pack_conv(Loader& L, const std::string& conv, const std::string& bn, int ci
                     const int cl = ci & 63;
                     const size_t col = (size_t)((((cl >> 3) ^ (co & 7))) << 3) + (cl & 7);
                     const size_t stage = (size_t)tap * (C / 64) + (ci >> 6);
+                    if (halves) {
+                        const size_t at = (((size_t)(co >> 7) * 9 * (C / 64) + stage) * 256 + (co & 127)) * 64 + col;
+                        img[at] = hb;
+                        img[at + 128 * 64] = lb;
+                        continue;
+                    }
                     img[(stage * 2 * C + co) * 64 + col] = hb;
                     img[(stage * 2 * C + C + co) * 64 + col] = lb;
                 }
@@ -925,6 +946,8 @@ struct Runner {
     int heads_route = MZ_HEADS_PLANNED;     // mz_debug_heads only: force a heads route; the network never sets it
     HeadsPlan* heads_plan_out = nullptr;    // when set, heads reports the plan of its launch here (mz_debug_heads)
     WideTowerPlan* wide_plan_out = nullptr; // when set, wide_tower reports the plan of its launch here (mz_debug_wide_tower)
+    Wide256Plan* wide256_plan_out = nullptr; // the same for the 256-channel towers (mz_debug_wide256_tower)
+    int wide256_boards = 0;                 // mz_debug_wide256_tower only: force the boards per CTA pair; 0 = planned
     bool fail(const char* what, cudaError_t e) { *err = std::string(what) + ": " + cudaGetErrorString(e); return false; }
 
     // conv: in -> out. `in` may be gathered from the pool; action adds the constant plane.
@@ -1155,16 +1178,9 @@ struct Runner {
         return 1;
     }
 
-    // The tower of a site of a 128-channel net as ONE x3 tensor-core launch (conv_wide.cu), dense NCHW in and out, one CTA
-    // or (WidePair) one CTA pair per board.  Returns what small_tower returns: 1 = launched, 0 = not the wide route, -1 = error.
-    int wide_tower(const TowerSite& s, float* out) {
-        const int nl = (s.stem ? 1 : 0) + 2 * r->net.blocks;
-        if (!is_wide(r->route) || nl == 0) return 0;
-        const bool pair = r->route == TowerRoute::WidePair;
-        WideTowerPlan p;
-        const char* why = "";
-        if (!(pair ? wide_pair_plan : wide_tower_plan)(n, r->C, r->hh, r->hw, nl, r->sm_count, &p, &why)) return 0;
-        WideTowerArgs a{};
+    // the arguments every wide tower launch shares (WideTowerArgs, Wide256Args) of a site with nl layers writing `out`
+    template <typename Args>
+    void wide_args(Args& a, const TowerSite& s, float* out, int nl) {
         a.in = s.in; a.out = out; a.gather_parent = s.gather_parent; a.pool_stride = s.pool_stride; a.action = s.action;
         a.n = n; a.H = r->hh; a.W = r->hw; a.A = r->net.action_space; a.g0 = g0; a.stem = s.stem ? 1 : 0; a.n_layers = nl;
         a.sat_count = r->d_sat;
@@ -1176,6 +1192,34 @@ struct Runner {
             t.bias = l.b_off >= 0 ? r->d_conv + l.b_off : nullptr;
             t.action_table = i == 0 && s.stem && s.action && l.tc_table_off >= 0 ? r->d_conv + l.tc_table_off : nullptr;
         }
+    }
+
+    // The tower of a site of a 128-channel net as ONE x3 tensor-core launch (conv_wide.cu), dense NCHW in and out, one CTA
+    // or (WidePair) one CTA pair per board; of a 256-channel net (Wide256, conv_wide256.cu) one CTA pair per group of
+    // boards, each CTA computing half the output channels.  Returns what small_tower returns: 1 = launched, 0 = not the
+    // wide route, -1 = error.
+    int wide_tower(const TowerSite& s, float* out) {
+        const int nl = (s.stem ? 1 : 0) + 2 * r->net.blocks;
+        if (!is_wide(r->route) || nl == 0) return 0;
+        const char* why = "";
+        if (r->route == TowerRoute::Wide256) {
+            Wide256Plan p;
+            if (!wide256_plan(n, r->C, r->hh, r->hw, nl, r->sm_count, wide256_boards, &p, &why)) return 0;
+            Wide256Args a{};
+            wide_args(a, s, out, nl);
+            if (wide256_plan_out) *wide256_plan_out = p;
+            kt_begin(KT_TOWER, stream);
+            cudaError_t e = launch_wide256_tower(a, p, stream);
+            kt_end(stream);
+            if (e != cudaSuccess) { fail("wide256 tower launch", e); return -1; }
+            *launches += p.launches;
+            return 1;
+        }
+        const bool pair = r->route == TowerRoute::WidePair;
+        WideTowerPlan p;
+        if (!(pair ? wide_pair_plan : wide_tower_plan)(n, r->C, r->hh, r->hw, nl, r->sm_count, &p, &why)) return 0;
+        WideTowerArgs a{};
+        wide_args(a, s, out, nl);
         if (wide_plan_out) *wide_plan_out = p;
         kt_begin(KT_TOWER, stream);
         cudaError_t e = pair ? launch_wide_pair_tower(a, p, stream) : launch_wide_tower(a, p, stream);
@@ -1440,6 +1484,9 @@ bool resnet_can_partition(const ResNetDevice* r0) {
 }
 const char* resnet_numerics(const ResNetDevice* r) {
     switch (r->route) {
+    case TowerRoute::Wide256:
+        return "f32-grade nets (256-channel towers on the tensor cores, output channels split across CTA pairs, split fp16 "
+               "operands x = x_h + x_l/2^11, 3 partial products, f32 accumulate; f32 stems and heads) + f64 tree statistics";
     case TowerRoute::WidePair:
         return "f32-grade nets (128-channel towers on the tensor cores, boards split across CTA pairs, split fp16 operands "
                "x = x_h + x_l/2^11, 3 partial products, f32 accumulate; f32 stems and heads) + f64 tree statistics";
@@ -1465,7 +1512,9 @@ int resnet_take_saturations(ResNetDevice* r, cudaStream_t stream) {
     return count;
 }
 void resnet_use_strict(ResNetDevice* r) {
-    r->note = is_wide(r->route)
+    r->note = r->route == TowerRoute::Wide256
+                  ? "f32 nets + f64 tree statistics (256-channel tensor-core towers left after an activation exceeded the fp16 range)"
+              : is_wide(r->route)
                   ? "f32 nets + f64 tree statistics (128-channel tensor-core towers left after an activation exceeded the fp16 range)"
                   : "f32 nets + f64 tree statistics (tensor-core towers left after an activation exceeded the fp16 range)";
     r->route = TowerRoute::CudaCore;                 // dense NCHW states: smaller than the board layout, the pool fits
@@ -1634,6 +1683,24 @@ bool resnet_wide_tower_plan(int n, int C, int H, int W, int blocks, bool stem, i
     return true;
 }
 
+// Launch plan of the 256-channel tower (host only, behind mz_debug_wide256_tower_plan): plan[10] = {boards per CTA pair,
+// M-tiles per CTA, threads per CTA, shared-memory bytes per CTA, weight ring stages, layers, CTAs per SM, boards per wave,
+// launches, registers per thread assumed}.  force_boards > 0 plans that many boards per CTA pair.
+static void wide256_plan_export(const Wide256Plan& p, int64_t* plan) {
+    const int64_t v[10] = {p.boards, p.m_tiles, p.threads, (int64_t)p.smem, p.stages, p.layers, p.ctas_per_sm, p.wave,
+                           p.launches, p.reg_cap};
+    for (int i = 0; i < 10; ++i) plan[i] = v[i];
+}
+bool resnet_wide256_tower_plan(int n, int C, int H, int W, int blocks, bool stem, int sm_count, int force_boards, int64_t* plan,
+                               std::string* err) {
+    if (blocks < 0) { *err = "bad shape"; return false; }
+    Wide256Plan p;
+    const char* why = "";
+    if (!wide256_plan(n, C, H, W, (stem ? 1 : 0) + 2 * blocks, sm_count, force_boards, &p, &why)) { *err = why; return false; }
+    wide256_plan_export(p, plan);
+    return true;
+}
+
 // Stand-alone tower of one call site of the network, through the same site descriptions, Runner helpers and weight
 // packing, on host NCHW data: a 64-channel tensor-core tower of resnet_inference_tc (TcF16 / TcX3, the input staged in
 // the board layout where that function leaves it), the fused CUDA-core tower (CudaCore) or a wide tower (Wide / WidePair)
@@ -1643,8 +1710,9 @@ bool resnet_wide_tower_plan(int n, int C, int H, int W, int blocks, bool stem, i
 int resnet_debug_tower(TowerRoute route, int n, int in_channels, int C, int H, int W, int blocks, int site, int parts, int A,
                        const float* x, const float* w, const float* bias, const int32_t* action, const int32_t* parent,
                        int pool_stride, float* out, int64_t* launches, int32_t* saturated, int64_t* plan, int sm_count,
-                       std::string* err) {
+                       std::string* err, int force_boards) {
     const bool tc = is_tc(route), fused = route == TowerRoute::CudaCore, pair = route == TowerRoute::WidePair;
+    const bool w256 = route == TowerRoute::Wide256;
     const bool dyn = site == MZ_TOWER_DYNAMICS || site == MZ_TOWER_DYNAMICS_POOL;
     const bool in_pool = site == MZ_TOWER_DYNAMICS_POOL;
     // only the fused tower takes the representation stem: the others leave it to conv3x3_kernel
@@ -1667,7 +1735,13 @@ int resnet_debug_tower(TowerRoute route, int n, int in_channels, int C, int H, i
         if (!parent || pool_stride < 1) { *err = "the in-search site needs parents and pool_stride >= 1"; return MZ_EINVAL; }
         for (int g = 0; g < n; ++g) if (parent[g] < 0 || parent[g] >= pool_stride) { *err = "parent out of range"; return MZ_EINVAL; }
     }
-    if (is_wide(route)) {
+    if (w256) {
+        int64_t unused[10];
+        std::string why;
+        if (!resnet_wide256_tower_plan(n, C, H, W, blocks, stem, sm_count, force_boards, unused, &why)) {
+            *err = "the 256-channel tower refuses the shape: " + why; return MZ_EUNSUPPORTED;
+        }
+    } else if (is_wide(route)) {
         int64_t unused[9];
         std::string why;
         if (!resnet_wide_tower_plan(n, C, H, W, blocks, stem, sm_count, unused, &why, pair)) {
@@ -1746,6 +1820,7 @@ int resnet_debug_tower(TowerRoute route, int n, int in_channels, int C, int H, i
     int64_t n_launches = 0;
     SmallTowerPlan small_used{}, small_first{};
     WideTowerPlan wide_used{}, wide_first{};
+    Wide256Plan w256_used{}, w256_first{};
     const float* result = nullptr;
     int rc = MZ_OK;
     // the ranges of the partitioned replay, each through its own Runner (one range unless in the pool); every array stays
@@ -1753,7 +1828,8 @@ int resnet_debug_tower(TowerRoute route, int n, int in_channels, int C, int H, i
     const int per = in_pool ? partition_games(n, parts) : n;
     for (int p = 0; p * per < n && rc == MZ_OK; ++p) {
         Runner R{&r, nullptr, &n_launches, err, std::min(per, n - p * per), p * per};
-        R.small_plan = &small_used; R.wide_plan_out = &wide_used;
+        R.small_plan = &small_used; R.wide_plan_out = &wide_used; R.wide256_plan_out = &w256_used;
+        R.wide256_boards = force_boards;
         const TowerSite s = site == MZ_TOWER_REPRESENTATION ? R.representation_site(in, !stem)
                           : site == MZ_TOWER_PREDICTION     ? R.prediction_site(in)
                           : R.dynamics_site(in, d_action, in_pool ? d_parent : nullptr, in_pool ? pool_stride : 0);
@@ -1776,7 +1852,7 @@ int resnet_debug_tower(TowerRoute route, int n, int in_channels, int C, int H, i
         }
         if (rc == MZ_OK && result && res != result) { *err = "partitions ended in different buffers"; rc = MZ_ECUDA; }
         result = res;
-        if (p == 0) { small_first = small_used; wide_first = wide_used; }
+        if (p == 0) { small_first = small_used; wide_first = wide_used; w256_first = w256_used; }
     }
     cudaError_t e = cudaDeviceSynchronize();
     if (rc == MZ_OK && e != cudaSuccess) { rc = MZ_ECUDA; *err = std::string("debug tower: ") + cudaGetErrorString(e); }
@@ -1792,7 +1868,8 @@ int resnet_debug_tower(TowerRoute route, int n, int in_channels, int C, int H, i
             const int64_t pl[6] = {f.P, f.CO, f.boards_per_cta, f.threads, f.grid, (int64_t)f.smem};
             for (int i = 0; i < 6; ++i) plan[i] = pl[i];
         }
-        if (plan && is_wide(route)) wide_plan_export(wide_first, pair, plan);
+        if (plan && w256) wide256_plan_export(w256_first, plan);
+        else if (plan && is_wide(route)) wide_plan_export(wide_first, pair, plan);
     }
     if (launches) *launches = n_launches;
     cleanup();
@@ -2046,7 +2123,7 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
         const float* x;
         if (nd.downsample == 2) {
             if (!R.cnn_stem(c.in, tmp, cur)) return MZ_ECUDA;
-            x = R.site_tower(R.representation_site(cur), Runner::kTryFused, &cur, &tmp, &spare);
+            x = R.site_tower(R.representation_site(cur), kAll, &cur, &tmp, &spare);
         } else if (nd.downsample) {
             int H = nd.obs_h, W = nd.obs_w;
             const auto& d = r->rep_down;
@@ -2066,7 +2143,9 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
                 H = Ho; W = Wo;
                 if (pool == 0 && !R.blocks(d, 12, 3, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
             }
-            x = R.site_tower(R.representation_site(cur), Runner::kTryFused, &cur, &tmp, &spare);
+            // the stems stay on the CUDA cores; the trunk's blocks take the wide launch on the Wide256 route (the only
+            // wide route that accepts a downsampled net)
+            x = R.site_tower(R.representation_site(cur), kAll, &cur, &tmp, &spare);
         } else if (is_wide(r->route) && nd.blocks > 0) {
             // the stem on the CUDA cores, the blocks as one wide launch (per layer if the wide launch refuses)
             if (!R.conv(r->rep_trunk[0], c.in, cur, nullptr, true, nd.obs_h, nd.obs_w)) return MZ_ECUDA;

@@ -1,5 +1,6 @@
-// Device helpers shared by the tensor-core tower kernels (conv_tc.cu, conv_x3.cu): mbarriers, bulk copies (TMA unit),
-// warpgroup MMAs (wgmma) with shared-memory matrix descriptors, fp16 packing.
+// Device helpers shared by the tensor-core tower kernels (conv_tc.cu, conv_x3.cu, conv_wide.cu, conv_wide256.cu):
+// mbarriers, bulk copies (TMA unit), warpgroup MMAs (wgmma) with shared-memory matrix descriptors, fp16 packing and
+// splitting, distributed shared memory of a cluster.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
@@ -77,6 +78,33 @@ MZ_DEVINL void wgmma_m64n64k16(float* d, uint32_t a_lo, uint32_t b_lo, uint32_t 
 
 // barrier over the 128 threads of warpgroup wg (named barrier 1 + wg; 0 is __syncthreads)
 MZ_DEVINL void warpgroup_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+
+MZ_DEVINL void wgmma_wait_one() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+
+// fp32 -> (x_h, x_l = (v - x_h) 2^11) as the x3 towers on dense boards split their inputs (conv_wide.cu,
+// conv_wide256.cu): both halves saturate to the finite fp16 range
+MZ_DEVINL void split_store(unsigned char* hi, unsigned char* lo, float v) {
+    const float s = fminf(fmaxf(v, -65504.0f), 65504.0f);
+    const __half h = __float2half_rn(s);
+    *reinterpret_cast<__half*>(hi) = h;
+    *reinterpret_cast<__half*>(lo) = __float2half_rn(fminf(fmaxf((v - __half2float(h)) * 2048.0f, -65504.0f), 65504.0f));
+}
+
+// distributed shared memory of a cluster (the CTA pairs of conv_wide.cu and conv_wide256.cu)
+MZ_DEVINL uint32_t cluster_rank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+MZ_DEVINL uint32_t map_to_cta(uint32_t addr, uint32_t rank) {     // my shared::cta address -> the same offset in CTA `rank`
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+    return r;
+}
+MZ_DEVINL void st_cluster_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+MZ_DEVINL void cluster_barrier() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
 
 // two fp32 -> packed fp16x2, round to nearest even, saturating to the finite range
 MZ_DEVINL uint32_t pack_f16x2(float lo, float hi) {

@@ -749,18 +749,44 @@ def debug_wide_pair_tower(x, weights, biases=None, site="prediction", actions=No
                        pool_stride, parts, device)
 
 
-def _wide_tower(entry, fields, x, weights, biases, site, actions, A, parents, pool_stride, parts, device):
+def _wide_tower(entry, fields, x, weights, biases, site, actions, A, parents, pool_stride, parts, device, channels=128,
+                extra=()):
+    """The wide debug towers' marshalling: ``extra`` are the entry's int32 arguments after pool_stride (the 256-channel
+    entry's forced boards per CTA pair); the plan has len(fields) entries."""
     lib = _lib.load_library()
-    _, blocks, arrays = _tower_args(x, weights, biases, site, actions, parents, 128)
+    _, blocks, arrays = _tower_args(x, weights, biases, site, actions, parents, channels)
     n, _, H, W = arrays[0].shape
     out = numpy.empty_like(arrays[0])
     launches, sat = C.c_int64(0), C.c_int32(0)
-    plan = (C.c_int64 * 9)()
-    rc = getattr(lib, entry)(device, n, H, W, blocks, TOWER_SITES[site], parts, A, *_ptrs(arrays), pool_stride,
+    plan = (C.c_int64 * len(fields))()
+    rc = getattr(lib, entry)(device, n, H, W, blocks, TOWER_SITES[site], parts, A, *_ptrs(arrays), pool_stride, *extra,
                              out.ctypes.data, C.byref(launches), C.byref(sat), plan)
     if rc != 0:
         raise _lib.MzError(rc, lib.mz_last_error(None).decode())
     return out, launches.value, sat.value, dict(zip(fields, plan))
+
+
+WIDE256_TOWER_PLAN = ("boards", "m_tiles", "threads", "smem", "stages", "layers", "ctas_per_sm", "wave", "launches", "reg_cap")
+
+
+def debug_wide256_tower_plan(n, channels, H, W, blocks, stem, sm_count, boards=0):
+    """Launch plan of the 256-channel x3 tensor-core tower, output channels split across a CTA pair and ``boards`` boards
+    per pair (0: the largest number that fits) stacked in M (mz_debug_wide256_tower_plan, host only): (a dict of
+    WIDE256_TOWER_PLAN, per-CTA figures except ``wave``, the boards per wave), "") or (None, the reason)."""
+    lib = _lib.load_library()
+    out = (C.c_int64 * 10)()
+    if not lib.mz_debug_wide256_tower_plan(n, channels, H, W, blocks, int(stem), sm_count, boards, out):
+        return None, lib.mz_last_error(None).decode()
+    return dict(zip(WIDE256_TOWER_PLAN, out)), ""
+
+
+def debug_wide256_tower(x, weights, biases=None, site="prediction", actions=None, A=1, parents=None, pool_stride=1, parts=1,
+                        boards=0, device=0):
+    """debug_wide_tower for 256 channels (mz_debug_wide256_tower): x is [n, 256, H, W], ``weights`` [256, 257, 3, 3] for a
+    dynamics stem and [256, 256, 3, 3] per block conv; ``boards`` forces the boards per CTA pair (0: planned).  Returns
+    (out, kernel launches, range-guard count, the plan of the launch as a dict of WIDE256_TOWER_PLAN)."""
+    return _wide_tower("mz_debug_wide256_tower", WIDE256_TOWER_PLAN, x, weights, biases, site, actions, A, parents,
+                       pool_stride, parts, device, channels=256, extra=(boards,))
 
 
 HEADS_ROUTES = {"planned": 0, "warp": 1, "wide": 2, "generic": 3}
