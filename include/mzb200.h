@@ -472,6 +472,8 @@ const char* mz_numerics(const MzHandle* h);
  * H x W; the records and the staged blocks hold the environment's own C * H * W observation. */
 enum { MZ_ENV_CARTPOLE = 0, MZ_ENV_TICTACTOE = 1, MZ_ENV_CONNECT4 = 2, MZ_ENV_GOMOKU = 3, MZ_ENV_TWENTYONE = 4,
        MZ_ENV_SIMPLE_GRID = 5 };
+/* not an environment of the library: any game, stepped by the caller (mz_selfplay_begin_host) */
+#define MZ_ENV_HOST 6
 
 typedef struct MzSelfPlayDesc {
     int32_t env;                  /* MZ_ENV_*: games/cartpole.py:131-174 (restated cart-pole physics),
@@ -575,6 +577,40 @@ int mz_selfplay_wait(MzHandle* h, MzSelfPlayStats* stats);
  * {byte offset of the game's block, (slot << 32) | length}, so a consumer can address any game without walking. */
 int mz_selfplay_drain(MzHandle* h, const void** data, uint64_t* bytes, int32_t* n_games, const uint64_t** index);
 int mz_selfplay_peek(MzHandle* h, const MzSelfPlayPeek* out);
+
+/* Host-stepped games (env = MZ_ENV_HOST): the device loop for a game whose environment only the caller can step (any
+ * game plug-in).  Search, the action sample (the same Philox stream), the per-move records, stacked observations, PER
+ * priorities and the packed hand-over stay on the device; each move is
+ *   mz_selfplay_host_act      one batched search and the action of every playing slot, -1 for a slot that is not
+ *                             playing (its finished game is parked: the staging area was full); do not step those
+ *   [the caller steps the environments of the slots with action >= 0]
+ *   mz_selfplay_host_observe  the step's rows for the whole batch (rows of slots that did not play are ignored):
+ *                             obs [n][C*H*W], reward [n] (the game's reward rounded once to float), done [n],
+ *                             legal [n][A], to_play [n] after the move.  finished [n] receives 1 for the slots whose game
+ *                             ended (done, or max_moves reached) and was packed: reset their environments
+ *   mz_selfplay_host_restart  the first rows of the next game of the slots of `which` (a subset of those reported
+ *                             finished); that game's id is the slot's previous id + game_id_stride
+ * A game that ended but did not fit into the staging area is reported finished by a later observe, after a drain.
+ * Every slot reported finished must be restarted before the next act; calls out of this order fail with MZ_ESTATE, and
+ * so do mz_selfplay_moves / _enqueue on a host-stepped loop.  mz_selfplay_drain and mz_selfplay_peek work as above. */
+typedef struct MzHostEnvDesc {
+    int32_t obs_channels;         /* the environment's observation is obs_channels x obs_h x obs_w floats; the stack's */
+    int32_t obs_h;                /* action planes are obs_h x obs_w (GameHistory.get_stacked_observations) */
+    int32_t obs_w;
+} MzHostEnvDesc;
+
+/* Starts games first_game_id + g from the caller's first rows (obs [n][C*H*W], legal [n][A], to_play [n]).  Refused
+ * with MZ_EINVAL: desc->env other than MZ_ENV_HOST, an observation that with stacked_observations does not give the
+ * handle's obs_elems, a row without a legal action, a to_play outside the players (mz_selfplay_begin_vs refuses
+ * MZ_ENV_HOST with an opponent other than MZ_OPPONENT_SELF: test-mode games need a device environment).  MZ_ENOMEM, with
+ * the bytes per slot, when the records ([max_games][max_moves + 1] observations) do not fit on the device. */
+int mz_selfplay_begin_host(MzHandle* h, const MzSelfPlayDesc* desc, const MzHostEnvDesc* env, const float* obs,
+                           const uint8_t* legal, const int32_t* to_play);
+int mz_selfplay_host_act(MzHandle* h, double temperature, const MzSelfPlayInject* inject, int32_t* actions);
+int mz_selfplay_host_observe(MzHandle* h, const float* obs, const float* reward, const uint8_t* done, const uint8_t* legal,
+                             const int32_t* to_play, uint8_t* finished, MzSelfPlayStats* stats);
+int mz_selfplay_host_restart(MzHandle* h, const uint8_t* which, const float* obs, const uint8_t* legal,
+                             const int32_t* to_play);
 
 /* Debug / parity: the device opponent (MZ_OPPONENT_EXPERT or MZ_OPPONENT_RANDOM) of env (MZ_ENV_TICTACTOE,
  * MZ_ENV_CONNECT4, or MZ_ENV_GOMOKU with MZ_OPPONENT_RANDOM only, on its default 11 x 11 board: this call has no handle

@@ -114,12 +114,17 @@ class MzSelfPlayStats(C.Structure):
                 ("staging_capacity", C.c_int64)]
 
 
+class MzHostEnvDesc(C.Structure):
+    _fields_ = [("obs_channels", C.c_int32), ("obs_h", C.c_int32), ("obs_w", C.c_int32)]
+
+
 class MzSelfPlayPeek(C.Structure):
     _fields_ = [("obs", C.c_void_p), ("legal_mask", C.c_void_p), ("to_play", C.c_void_p), ("game_id", C.c_void_p),
                 ("move_index", C.c_void_p), ("last_action", C.c_void_p)]
 
 
 MZ_ENV_CARTPOLE, MZ_ENV_TICTACTOE, MZ_ENV_CONNECT4, MZ_ENV_GOMOKU, MZ_ENV_TWENTYONE, MZ_ENV_SIMPLE_GRID = 0, 1, 2, 3, 4, 5
+MZ_ENV_HOST = 6
 MZ_OPPONENT_SELF, MZ_OPPONENT_EXPERT, MZ_OPPONENT_RANDOM = 0, 1, 2
 MZ_STAGED_HEADER_BYTES = 32
 
@@ -156,6 +161,11 @@ SYMBOLS = [
     ("mz_selfplay_drain", C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_int32),
                                     C.POINTER(C.c_void_p)]),
     ("mz_selfplay_peek", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayPeek)]),
+    ("mz_selfplay_begin_host", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayDesc), C.POINTER(MzHostEnvDesc), C.c_void_p,
+                                         C.c_void_p, C.c_void_p]),
+    ("mz_selfplay_host_act", C.c_int, [C.c_void_p, C.c_double, C.POINTER(MzSelfPlayInject), C.c_void_p]),
+    ("mz_selfplay_host_observe", C.c_int, [C.c_void_p] + [C.c_void_p] * 6 + [C.POINTER(MzSelfPlayStats)]),
+    ("mz_selfplay_host_restart", C.c_int, [C.c_void_p] * 5),
     ("mz_debug_opponent_action", C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p]),
     ("mz_debug_small_search_plan", C.c_int, [C.c_int32] * 10 + [C.POINTER(C.c_int64)]),

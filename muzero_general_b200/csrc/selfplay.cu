@@ -33,6 +33,16 @@
 // Stacked observations (config.stacked_observations = s > 0): the search input of a slot is [B][O_in] with
 // O_in = O + s * (O + plane), the current observation (O floats) followed by the tail that stack_fill builds from the
 // slot's records.  Records, staged blocks and rec_obs keep the environment's own O.
+//
+// Host-stepped environments (MZ_ENV_HOST, mz_selfplay_begin_host): any game plug-in, its step left to the host.  A move
+// is two device halves with the host's step between them:
+//   act       [batched MCTS.run] -> host_act_kernel: the action sample and the search records of move t (choose_action +
+//             record_search, slot_act's first half); the actions go to the host, -1 for a slot not playing
+//   observe   the host's rows (observation, reward, done, legal mask, to_play) -> host_observe_kernel: the rest of
+//             record_move, fin, packing (pack_game, the step kernel's code), the stacked tail
+//   restart   the next game's first rows of the slots observe packed -> host_start_kernel
+// A finished game that does not fit into the staging area stays parked in its slot (fin > 0, action -1) and every
+// observe pass tries again; the slot reports "finished" (its environment is reset, then restarted) once it is packed.
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -81,8 +91,10 @@ struct SpDev {
     int32_t* rec_to_play;      // [B][T]   (after the move)
     float* rec_obs;            // [B][T+1][O]
     int32_t* first_to_play;    // [B]
-    int32_t* fin;              // [B] 0 = playing, T > 0 = finished after T moves, waiting to be packed
+    int32_t* fin;              // [B] 0 = playing, T > 0 = finished after T moves, waiting to be packed,
+                               //     -1 = MZ_ENV_HOST: packed, waiting for the next game's first rows
     int32_t* last_action;      // [B]
+    int32_t* host_action;      // [B] MZ_ENV_HOST: the action of the move in flight, -1 for a slot not playing it
     // counters: [0] env_steps, [1] games_finished, [2] staging cursor (may run past the capacity), [3] staged games,
     //           [4] park events of this call, [5] end of the valid staged bytes
     unsigned long long* counters;
@@ -337,13 +349,19 @@ MZ_DEVINL int opponent_action(const SpDev& s, int g, double u, int dflt = -1) {
     return s.opponent == MZ_OPPONENT_EXPERT ? expert_action(s, g, d) : d;
 }
 
-// record of move t of slot g, then the slot's search inputs for the next move (store_search_statistics uses the
-// pre-step root, self_play.py:169-175); root NaN and visits nullptr (all zero) mark a move no search chose
-MZ_DEVINL void record_move(const SpDev& s, int g, int t, int action, float reward, double root, const int32_t* visits) {
+// the search's part of the record of move t of slot g (store_search_statistics uses the pre-step root,
+// self_play.py:169-175); root NaN and visits nullptr (all zero) mark a move no search chose
+MZ_DEVINL void record_search(const SpDev& s, int g, int t, int action, double root, const int32_t* visits) {
     const size_t r = (size_t)g * s.max_moves + t;
     s.rec_root[r] = root;
     for (int k = 0; k < s.A; ++k) s.rec_visits[r * s.A + k] = visits ? visits[k] : 0;
     s.rec_action[r] = action;
+}
+
+// record of move t of slot g, then the slot's search inputs for the next move
+MZ_DEVINL void record_move(const SpDev& s, int g, int t, int action, float reward, double root, const int32_t* visits) {
+    const size_t r = (size_t)g * s.max_moves + t;
+    record_search(s, g, t, action, root, visits);
     s.rec_reward[r] = reward;
     publish(s, g);
     s.rec_to_play[r] = s.to_play[g];
@@ -453,18 +471,25 @@ MZ_DEVINL int sample_action(const SpDev& s, int g, double temperature, double u)
     return pick;
 }
 
+// the action of move t in slot g: the injected one, else select_action's sample on the Philox uniform of (game, t)
+// with the temperature threshold applied
+template <int kMaxA>
+MZ_DEVINL int choose_action(const SpDev& s, int g, int t) {
+    int action = s.forced_action ? s.forced_action[g] : -1;
+    if (action < 0) {
+        const double T = (s.threshold == 0 || t + 1 < s.threshold) ? s.temperature : 0.0;
+        const double u = s.uniform ? s.uniform[g] : philox_uniform53(s.seed, s.game_id[g], t, 0u, kTagAction);
+        action = sample_action<kMaxA>(s, g, T, u);
+    }
+    return action;
+}
+
 // select_action + Game.step + record for slot g (one thread), then the opponent's reply in a test-mode game; returns
 // the moves played
 template <int kMaxA>
 MZ_DEVINL int slot_act(const SpDev& s, int g) {
     const int t = s.move[g];
-    const int64_t gid = s.game_id[g];
-    int action = s.forced_action ? s.forced_action[g] : -1;
-    if (action < 0) {
-        const double T = (s.threshold == 0 || t + 1 < s.threshold) ? s.temperature : 0.0;
-        const double u = s.uniform ? s.uniform[g] : philox_uniform53(s.seed, gid, t, 0u, kTagAction);
-        action = sample_action<kMaxA>(s, g, T, u);
-    }
+    const int action = choose_action<kMaxA>(s, g, t);
     float reward;
     bool done;
     if (s.env == MZ_ENV_CARTPOLE) {
@@ -525,14 +550,73 @@ MZ_DEVINL float initial_priority(const SpDev& s, int g, int T, int i) {
     return (float)(s.per_alpha == 1.0 ? d : __dsqrt_rn(d));
 }
 
+// Copies the finished game of slot g (T moves) into the staging area with the 32 lanes of one warp; returns false when
+// it does not fit (the game stays parked in its slot, packed by a later pass after the host has drained).  Staging space
+// is reserved with ONE atomicAdd per finished game (a compare-and-swap loop serialises hundreds of finishing warps per
+// move): the cursor may run past the capacity, reservations that end beyond it are void, and since the cursor only
+// grows the valid reservations are a contiguous prefix whose end is tracked in counters[5].
+MZ_DEVINL bool pack_game(const SpDev& s, int g, int T, int lane) {
+    const unsigned long long bytes = staged_block_bytes(T, s.A, s.O);
+    unsigned long long off = 0;
+    int ok = 0;
+    if (lane == 0) {
+        off = atomicAdd(&s.counters[2], bytes);
+        ok = off + bytes <= s.staging_cap;
+        if (ok) {
+            atomicMax(&s.counters[5], off + bytes);
+            atomicAdd(&s.counters[1], 1ull);
+            const unsigned long long i = atomicAdd(&s.counters[3], 1ull);
+            s.index[2 * i] = off;
+            s.index[2 * i + 1] = ((unsigned long long)(unsigned)g << 32) | (unsigned)T;
+        } else {
+            atomicAdd(&s.counters[4], 1ull);
+        }
+    }
+    ok = __shfl_sync(0xffffffffu, ok, 0);
+    if (!ok) return false;
+    off = ((unsigned long long)__shfl_sync(0xffffffffu, (unsigned)(off >> 32), 0) << 32) | __shfl_sync(0xffffffffu, (unsigned)off, 0);
+    unsigned char* dst = s.staging + off;
+    if (lane == 0) {
+        *reinterpret_cast<int64_t*>(dst) = s.game_id[g];
+        int32_t* hd = reinterpret_cast<int32_t*>(dst + 8);
+        hd[0] = g; hd[1] = T; hd[2] = s.first_to_play[g]; hd[3] = s.O; hd[4] = s.A; hd[5] = (int32_t)bytes;
+    }
+    unsigned char* p = dst + MZ_STAGED_HEADER_BYTES;
+    const size_t r = (size_t)g * s.max_moves;
+    {
+        double* d = reinterpret_cast<double*>(p);
+        for (int i = lane; i < T; i += 32) d[i] = s.rec_root[r + i];
+        p += (size_t)T * 8;
+    }
+    {
+        int32_t* d = reinterpret_cast<int32_t*>(p);
+        for (int i = lane; i < T * s.A; i += 32) d[i] = s.rec_visits[r * s.A + i];
+        p += (size_t)T * s.A * 4;
+        d = reinterpret_cast<int32_t*>(p);
+        for (int i = lane; i < T; i += 32) d[i] = s.rec_action[r + i];
+        p += (size_t)T * 4;
+        float* f = reinterpret_cast<float*>(p);
+        for (int i = lane; i < T; i += 32) f[i] = s.rec_reward[r + i];
+        p += (size_t)T * 4;
+        d = reinterpret_cast<int32_t*>(p);
+        for (int i = lane; i < T; i += 32) d[i] = s.rec_to_play[r + i];
+        p += (size_t)T * 4;
+        f = reinterpret_cast<float*>(p);
+        for (int i = lane; i < T; i += 32) f[i] = s.td_steps > 0 ? initial_priority(s, g, T, i) : 0.0f;
+        p += (size_t)T * 4;
+        f = reinterpret_cast<float*>(p);
+        const float* src = s.rec_obs + (size_t)g * (s.max_moves + 1) * s.O;
+        for (int i = lane; i < (T + 1) * s.O; i += 32) f[i] = src[i];
+    }
+    __syncwarp();
+    return true;
+}
+
 // One warp per slot, 32 slots per CTA.  act != 0: lane 0 plays the slot's move (sampling, environment step, record)
 // unless the slot is parked; then, whatever `act`, a finished game is copied into the staging area by the whole warp and
-// the slot starts its next game (act == 0 is the drain-only pass that re-packs games parked by an earlier call).
-// Staging space is reserved with ONE atomicAdd per finished game (a compare-and-swap loop serialises hundreds of
-// finishing warps per move): the cursor may run
-// past the capacity, reservations that end beyond it are void (the game stays parked), and since the cursor only grows
-// the valid reservations are a contiguous prefix whose end is tracked in counters[5].  With stacked observations, a
-// slot whose move was played or whose game restarted then rebuilds its stacked tail with the whole warp.
+// the slot starts its next game (act == 0 is the drain-only pass that re-packs games parked by an earlier call).  With
+// stacked observations, a slot whose move was played or whose game restarted then rebuilds its stacked tail with the
+// whole warp.
 // kMaxA (128 or 256, the least that holds |A|) sizes the sampler's stack array, so the configurations of up to 128
 // actions keep their stack frame.
 constexpr int kStepThreads = 1024;
@@ -558,66 +642,12 @@ __global__ void __launch_bounds__(kStepThreads) selfplay_step_kernel(const SpDev
         T = __shfl_sync(0xffffffffu, T, 0);
         __syncwarp();
     }
-    if (T != 0) {
-        const unsigned long long bytes = staged_block_bytes(T, s.A, s.O);
-        unsigned long long off = 0;
-        int ok = 0;
+    if (T != 0 && pack_game(s, g, T, lane)) {
         if (lane == 0) {
-            off = atomicAdd(&s.counters[2], bytes);
-            ok = off + bytes <= s.staging_cap;
-            if (ok) {
-                atomicMax(&s.counters[5], off + bytes);
-                atomicAdd(&s.counters[1], 1ull);
-                const unsigned long long i = atomicAdd(&s.counters[3], 1ull);
-                s.index[2 * i] = off;
-                s.index[2 * i + 1] = ((unsigned long long)(unsigned)g << 32) | (unsigned)T;
-            } else {
-                atomicAdd(&s.counters[4], 1ull);
-            }
+            const int played = start_game(s, g, s.game_id[g] + s.id_stride);
+            if (played) atomicAdd(&s_active, played);
         }
-        ok = __shfl_sync(0xffffffffu, ok, 0);
-        if (ok) {                                     // else parked: packed by a later call, after the host has drained
-            off = ((unsigned long long)__shfl_sync(0xffffffffu, (unsigned)(off >> 32), 0) << 32) | __shfl_sync(0xffffffffu, (unsigned)off, 0);
-            unsigned char* dst = s.staging + off;
-            if (lane == 0) {
-                *reinterpret_cast<int64_t*>(dst) = s.game_id[g];
-                int32_t* hd = reinterpret_cast<int32_t*>(dst + 8);
-                hd[0] = g; hd[1] = T; hd[2] = s.first_to_play[g]; hd[3] = s.O; hd[4] = s.A; hd[5] = (int32_t)bytes;
-            }
-            unsigned char* p = dst + MZ_STAGED_HEADER_BYTES;
-            const size_t r = (size_t)g * s.max_moves;
-            {
-                double* d = reinterpret_cast<double*>(p);
-                for (int i = lane; i < T; i += 32) d[i] = s.rec_root[r + i];
-                p += (size_t)T * 8;
-            }
-            {
-                int32_t* d = reinterpret_cast<int32_t*>(p);
-                for (int i = lane; i < T * s.A; i += 32) d[i] = s.rec_visits[r * s.A + i];
-                p += (size_t)T * s.A * 4;
-                d = reinterpret_cast<int32_t*>(p);
-                for (int i = lane; i < T; i += 32) d[i] = s.rec_action[r + i];
-                p += (size_t)T * 4;
-                float* f = reinterpret_cast<float*>(p);
-                for (int i = lane; i < T; i += 32) f[i] = s.rec_reward[r + i];
-                p += (size_t)T * 4;
-                d = reinterpret_cast<int32_t*>(p);
-                for (int i = lane; i < T; i += 32) d[i] = s.rec_to_play[r + i];
-                p += (size_t)T * 4;
-                f = reinterpret_cast<float*>(p);
-                for (int i = lane; i < T; i += 32) f[i] = s.td_steps > 0 ? initial_priority(s, g, T, i) : 0.0f;
-                p += (size_t)T * 4;
-                f = reinterpret_cast<float*>(p);
-                const float* src = s.rec_obs + (size_t)g * (s.max_moves + 1) * s.O;
-                for (int i = lane; i < (T + 1) * s.O; i += 32) f[i] = src[i];
-            }
-            __syncwarp();
-            if (lane == 0) {
-                const int played = start_game(s, g, s.game_id[g] + s.id_stride);
-                if (played) atomicAdd(&s_active, played);
-            }
-            changed = 1;
-        }
+        changed = 1;
     }
     if (s.stack && g < s.B && __any_sync(0xffffffffu, changed)) {
         __syncwarp();                                 // lane 0's records and move count, visible to the warp
@@ -631,6 +661,116 @@ static void launch_selfplay_step(const SpDev& s, int act, cudaStream_t stream) {
     const int grid = (s.B * 32 + kStepThreads - 1) / kStepThreads;
     if (s.A <= 128) selfplay_step_kernel<128><<<grid, kStepThreads, 0, stream>>>(s, act);
     else selfplay_step_kernel<256><<<grid, kStepThreads, 0, stream>>>(s, act);
+}
+
+// ------------------------------------------------------------------------------------------
+// MZ_ENV_HOST: the environment step is the host's
+// ------------------------------------------------------------------------------------------
+// device copies of what the host uploads for the whole batch
+struct HostRows {
+    float* obs;                // [B][O]
+    float* reward;             // [B]
+    uint8_t* done;             // [B]
+    uint8_t* legal;            // [B][A]
+    int32_t* to_play;          // [B]
+};
+
+// publish() of a host-stepped slot: its observation row becomes the current observation (the first O floats of the
+// search input) and rec_obs[t], its legal-mask row the slot's mask.  Threads tid, tid + nt, ... share the copies.
+MZ_DEVINL void take_rows(const SpDev& s, const HostRows& h, int g, int t, int tid, int nt) {
+    const float* src = h.obs + (size_t)g * s.O;
+    float* o = s.obs + (size_t)g * s.O_in;
+    float* ro = s.rec_obs + ((size_t)g * (s.max_moves + 1) + t) * s.O;
+    for (int i = tid; i < s.O; i += nt) {
+        const float v = src[i];
+        o[i] = v;
+        ro[i] = v;
+    }
+    for (int k = tid; k < s.A; k += nt) s.legal[(size_t)g * s.A + k] = h.legal[(size_t)g * s.A + k];
+}
+
+// threads per slot of the observe / restart kernels (one CTA per slot): a warp for small observations, more for image
+// frames and deep stacks, whose copies would otherwise run on a few SMs
+static int host_slot_threads(const SpDev& s) { return s.O_in + s.A > 4096 ? 256 : 32; }
+
+// one thread per slot: the action of every playing slot (fin == 0) and its search records; -1 for the others
+constexpr int kActThreads = 128;
+
+template <int kMaxA>
+__global__ void __launch_bounds__(kActThreads) host_act_kernel(const SpDev s) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    bool playing = false;
+    if (g < s.B) {
+        int action = -1;
+        if (s.fin[g] == 0) {
+            const int t = s.move[g];
+            action = choose_action<kMaxA>(s, g, t);
+            record_search(s, g, t, action, s.root_value[g], s.visits + (size_t)g * s.A);
+            playing = true;
+        }
+        s.host_action[g] = action;
+    }
+    const unsigned n = __popc(__ballot_sync(0xffffffffu, playing));
+    if ((threadIdx.x & 31) == 0 && n) atomicAdd(&s.counters[0], (unsigned long long)n);
+}
+
+// One CTA per slot.  A slot that played finishes its move t with the host's rows (record_move's second half) and is
+// finished when done or at max_moves; then every finished slot, parked ones included, is packed by warp 0.
+// finished[g] = 1: the slot's game was packed in this pass and the slot waits for the next game's first rows (fin = -1).
+__global__ void host_observe_kernel(const SpDev s, const HostRows h, uint8_t* finished) {
+    __shared__ int s_T;
+    const int g = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+    const int a = s.host_action[g];
+    const int t = s.move[g];
+    if (tid == 0) s_T = s.fin[g];
+    __syncthreads();                                  // every thread has read the slot's state before it changes
+    if (a >= 0) {
+        take_rows(s, h, g, t + 1, tid, nt);
+        if (tid == 0) {
+            const size_t r = (size_t)g * s.max_moves + t;
+            s.rec_reward[r] = h.reward[g];
+            s.to_play[g] = h.to_play[g];
+            s.rec_to_play[r] = h.to_play[g];
+            s.move[g] = t + 1;
+            s.last_action[g] = a;
+            s_T = (h.done[g] || t + 1 >= s.max_moves) ? t + 1 : 0;
+            s.fin[g] = s_T;
+        }
+    }
+    __syncthreads();                                  // the records of move t, visible to the packing warp
+    const int T = s_T;
+    if (T > 0) {
+        if (tid < 32) {
+            const bool packed = pack_game(s, g, T, tid);
+            if (tid == 0) {
+                if (packed) s.fin[g] = -1;
+                finished[g] = packed;
+            }
+        }
+        return;
+    }
+    if (tid == 0) finished[g] = 0;
+    if (a >= 0 && s.stack) stack_fill(s, g, tid, nt);
+}
+
+// One CTA per slot of `which` (all slots when nullptr, with the ids first_game_id + g): the slot starts a game from the
+// host's first rows, as start_game does for the device environments.  A slot of `which` must be waiting (fin == -1).
+__global__ void host_start_kernel(const SpDev s, const HostRows h, const uint8_t* which, int64_t first_game_id) {
+    const int g = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+    if (which && !(which[g] && s.fin[g] == -1)) return;
+    const int64_t gid = which ? s.game_id[g] + s.id_stride : first_game_id + g;
+    __syncthreads();                                  // every thread has read the slot's state before it changes
+    take_rows(s, h, g, 0, tid, nt);
+    if (tid == 0) {
+        s.game_id[g] = gid;
+        s.move[g] = 0;
+        s.fin[g] = 0;
+        s.last_action[g] = -1;
+        s.to_play[g] = h.to_play[g];
+        s.first_to_play[g] = h.to_play[g];
+    }
+    __syncthreads();
+    if (s.stack) stack_fill(s, g, tid, nt);
 }
 
 }  // namespace mz
@@ -656,6 +796,16 @@ struct MzSelfPlay {
     int32_t* d_first = nullptr;
     uint64_t drained_bytes = 0;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
+    // MZ_ENV_HOST
+    bool host = false;
+    bool observe_due = false;                  // an act waits for its observe
+    std::vector<int32_t> actions;              // the actions of the last act
+    std::vector<uint8_t> awaiting;             // slots whose game was packed, waiting for mz_selfplay_host_restart
+    int n_awaiting = 0;
+    HostRows rows{};                           // device buffers of the host's uploads
+    uint8_t* d_which = nullptr;
+    uint8_t* d_finished = nullptr;
+    float act_ms = 0.0f;
 };
 
 void mz_selfplay_destroy(MzHandle* h) {
@@ -683,14 +833,50 @@ static bool sp_alloc(MzSelfPlay* sp, T** p, size_t count) {
     return true;
 }
 
+// The host's rows of a host-stepped batch: every row of `which` (all rows when nullptr) whose game goes on (`done` nullptr
+// or 0) has a legal action, and every to_play names a player.  Returns MZ_OK or fails with the first bad row.
+static int check_host_rows(MzHandle* h, const char* who, const uint8_t* which, const uint8_t* legal, const int32_t* to_play,
+                           const uint8_t* done) {
+    const int B = h->search.max_games, A = h->net.action_space, P = h->search.num_players;
+    for (int g = 0; g < B; ++g) {
+        if (which && !which[g]) continue;
+        if (to_play[g] < 0 || to_play[g] >= P)
+            return fail(h, MZ_EINVAL, std::string(who) + ": row " + std::to_string(g) + " has to_play " + std::to_string(to_play[g]) +
+                                      ", outside the " + std::to_string(P) + " players");
+        if (done && done[g]) continue;
+        bool any = false;
+        for (int k = 0; k < A && !any; ++k) any = legal[(size_t)g * A + k] != 0;
+        if (!any) return fail(h, MZ_EINVAL, std::string(who) + ": row " + std::to_string(g) + " has no legal action");
+    }
+    return MZ_OK;
+}
+
+static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int32_t muzero_player, const MzHostEnvDesc* e,
+                    const float* obs, const uint8_t* legal, const int32_t* to_play);
+
 extern "C" int mz_selfplay_begin(MzHandle* h, const MzSelfPlayDesc* d) {
     return mz_selfplay_begin_vs(h, d, MZ_OPPONENT_SELF, 0);
 }
 
 extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int32_t muzero_player) {
+    return sp_begin(h, d, opponent, muzero_player, nullptr, nullptr, nullptr, nullptr);
+}
+
+extern "C" int mz_selfplay_begin_host(MzHandle* h, const MzSelfPlayDesc* d, const MzHostEnvDesc* e, const float* obs,
+                                      const uint8_t* legal, const int32_t* to_play) {
+    if (!h || !d || !e || !obs || !legal || !to_play) return fail(h, MZ_EINVAL, "mz_selfplay_begin_host: null argument");
+    if (d->env != MZ_ENV_HOST) return fail(h, MZ_EINVAL, "mz_selfplay_begin_host: desc->env must be MZ_ENV_HOST");
+    return sp_begin(h, d, MZ_OPPONENT_SELF, 0, e, obs, legal, to_play);
+}
+
+static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int32_t muzero_player, const MzHostEnvDesc* e,
+                    const float* obs, const uint8_t* legal, const int32_t* to_play) {
     if (!h || !d) return fail(h, MZ_EINVAL, "mz_selfplay_begin: null argument");
     if (opponent != MZ_OPPONENT_SELF && opponent != MZ_OPPONENT_EXPERT && opponent != MZ_OPPONENT_RANDOM)
         return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin_vs: unknown opponent " + std::to_string(opponent));
+    if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_HOST)
+        return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: host-stepped games play against themselves only (test-mode games "
+                                  "against an opponent need a device environment)");
     if (muzero_player != 0 && muzero_player != 1)
         return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: muzero_player must be 0 or 1, got " + std::to_string(muzero_player));
     if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_CARTPOLE)
@@ -727,6 +913,15 @@ extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_
         }
         case MZ_ENV_TWENTYONE: name = "Twenty-One"; C = 3; ph = 3; pw = 3; A_env = 2; break;
         case MZ_ENV_SIMPLE_GRID: name = "Simple Grid"; C = 1; ph = 1; pw = 9; A_env = 2; break;
+        case MZ_ENV_HOST: {
+            if (!e) return fail(h, MZ_EINVAL, "mz_selfplay_begin: host-stepped games (MZ_ENV_HOST) start with mz_selfplay_begin_host");
+            if (e->obs_channels < 1 || e->obs_h < 1 || e->obs_w < 1)
+                return fail(h, MZ_EINVAL, "mz_selfplay_begin_host: the observation's channels, height and width must be >= 1");
+            int rc = check_host_rows(h, "mz_selfplay_begin_host", nullptr, legal, to_play, nullptr);
+            if (rc) return rc;
+            name = "the host-stepped environment"; C = e->obs_channels; ph = e->obs_h; pw = e->obs_w; A_env = A;
+            break;
+        }
         default: return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin: unknown environment");
     }
     // the network input: the observation and, per stacked step, an earlier observation and its action plane
@@ -739,6 +934,19 @@ extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_
                                   " actions and " + std::to_string(h->obs_elems) + " input values");
     const int O = C * ph * pw;
     if (d->max_moves < 1) return fail(h, MZ_EINVAL, "mz_selfplay_begin: max_moves < 1");
+    {
+        // device memory per slot: the search input and outputs, the records of a maximum-length game ([max_moves + 1][O]
+        // observations) and the host's upload rows
+        const unsigned long long Tm = (unsigned long long)d->max_moves;
+        const unsigned long long per_slot = (unsigned long long)h->obs_elems * 4 + (Tm + 1) * O * 4 + Tm * (8 + 4ull * A + 12) +
+                                            (d->env == MZ_ENV_HOST ? (unsigned long long)O * 4 + A + 16 : 0) + 24ull * A + 64;
+        size_t free_bytes = 0, total_bytes = 0;
+        if (cudaMemGetInfo(&free_bytes, &total_bytes) == cudaSuccess && per_slot * B > free_bytes)
+            return fail(h, MZ_ENOMEM, "mz_selfplay_begin: the records of " + std::to_string(B) + " slots do not fit on the device: " +
+                                      std::to_string(per_slot) + " bytes per slot (" + std::to_string(d->max_moves + 1) +
+                                      " observations of " + std::to_string(O) + " floats for max_moves = " +
+                                      std::to_string(d->max_moves) + "), " + std::to_string(free_bytes) + " bytes free");
+    }
     MzSelfPlay* sp = new (std::nothrow) MzSelfPlay();
     if (!sp) return fail(h, MZ_ENOMEM, "mz_selfplay_begin: out of host memory");
     h->sp = sp;
@@ -770,7 +978,19 @@ extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_
               sp_alloc(sp, &s.rec_to_play, B * T) && sp_alloc(sp, &s.rec_obs, B * (T + 1) * O) && sp_alloc(sp, &s.first_to_play, B) &&
               sp_alloc(sp, &s.fin, B) && sp_alloc(sp, &s.last_action, B) && sp_alloc(sp, &s.counters, 8) &&
               sp_alloc(sp, &sp->d_forced, B) && sp_alloc(sp, &sp->d_uniform, B) && sp_alloc(sp, &sp->d_noise, (size_t)B * A) &&
-              sp_alloc(sp, &sp->d_first, B);
+              sp_alloc(sp, &sp->d_first, B) && sp_alloc(sp, &s.host_action, B);
+    if (ok && d->env == MZ_ENV_HOST) {
+        float *r_obs = nullptr, *r_reward = nullptr;
+        uint8_t *r_done = nullptr, *r_legal = nullptr;
+        int32_t* r_to_play = nullptr;
+        ok = sp_alloc(sp, &r_obs, (size_t)B * O) && sp_alloc(sp, &r_reward, B) && sp_alloc(sp, &r_done, B) &&
+             sp_alloc(sp, &r_legal, (size_t)B * A) && sp_alloc(sp, &r_to_play, B) && sp_alloc(sp, &sp->d_which, B) &&
+             sp_alloc(sp, &sp->d_finished, B);
+        sp->rows = HostRows{r_obs, r_reward, r_done, r_legal, r_to_play};
+        sp->host = true;
+        sp->actions.assign(B, -1);
+        sp->awaiting.assign(B, 0);
+    }
     if (!ok) { mz_selfplay_destroy(h); return fail(h, MZ_ENOMEM, "mz_selfplay_begin: out of device memory"); }
     // staging (two areas of this size): by default 4x the room for every slot finishing a maximum-length game at once,
     // within [16, 64] MiB;
@@ -806,7 +1026,14 @@ extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_
     s.index = sp->d_index[0];
     s.staging_cap = cap;
     cudaEventCreate(&sp->e0); cudaEventCreate(&sp->e1);
-    selfplay_reset_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(s, d->first_game_id);
+    if (sp->host) {
+        MZ_CUDA(h, cudaMemcpyAsync(sp->rows.obs, obs, (size_t)B * O * 4, cudaMemcpyHostToDevice, h->stream));
+        MZ_CUDA(h, cudaMemcpyAsync(sp->rows.legal, legal, (size_t)B * A, cudaMemcpyHostToDevice, h->stream));
+        MZ_CUDA(h, cudaMemcpyAsync(sp->rows.to_play, to_play, (size_t)B * 4, cudaMemcpyHostToDevice, h->stream));
+        host_start_kernel<<<B, host_slot_threads(s), 0, h->stream>>>(s, sp->rows, nullptr, d->first_game_id);
+    } else {
+        selfplay_reset_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(s, d->first_game_id);
+    }
     h->launches += 1;
     MZ_CUDA(h, cudaGetLastError());
     MZ_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -829,21 +1056,12 @@ static int sp_read_counters(MzHandle* h, MzSelfPlayStats* stats, float ms) {
     return MZ_OK;
 }
 
-static int sp_enqueue(MzHandle* h, int32_t n_moves, double temperature, const MzSelfPlayInject* inj, const char* who) {
-    if (!h || !h->sp) return fail(h, MZ_ESTATE, std::string(who) + ": call mz_selfplay_begin first");
-    if (!h->weights_loaded) return fail(h, MZ_ESTATE, std::string(who) + ": weights not loaded");
-    if (n_moves < 0) return fail(h, MZ_EINVAL, std::string(who) + ": n_moves < 0");
-    if (inj && n_moves > 1 && (inj->forced_action || inj->uniform || inj->noise || inj->first_index))
-        return fail(h, MZ_EINVAL, std::string(who) + ": per-move overrides need n_moves == 1");
-    if (!(temperature >= 0.0)) return fail(h, MZ_EINVAL, std::string(who) + ": temperature must be >= 0");
+// The kernel arguments of a move (the staging area in use, the temperature, the injected overrides copied to the
+// device) and the search call on the slots' device-side inputs.
+static int sp_move_setup(MzHandle* h, double temperature, const MzSelfPlayInject* inj, SpDev* out, SearchCall* call) {
     MzSelfPlay* sp = h->sp;
-    if (inj && inj->uniform)
-        for (int g = 0; g < sp->dev.B; ++g)
-            if (!(inj->uniform[g] >= 0.0 && inj->uniform[g] < 1.0))
-                return fail(h, MZ_EINVAL, std::string(who) + ": injected uniforms must lie in [0, 1)");
-    if (sp->in_flight) return fail(h, MZ_ESTATE, std::string(who) + ": moves already enqueued, call mz_selfplay_wait first");
-    MZ_CUDA(h, cudaSetDevice(h->device));
-    SpDev s = sp->dev;
+    SpDev& s = *out;
+    s = sp->dev;
     s.staging = sp->d_staging[sp->cur];
     s.index = sp->d_index[sp->cur];
     const int B = s.B, A = s.A;
@@ -857,6 +1075,34 @@ static int sp_enqueue(MzHandle* h, int32_t n_moves, double temperature, const Mz
         if (inj->noise) { MZ_CUDA(h, cudaMemcpyAsync(sp->d_noise, inj->noise, (size_t)B * A * 8, cudaMemcpyHostToDevice, h->stream)); noise = sp->d_noise; }
         if (inj->first_index) { MZ_CUDA(h, cudaMemcpyAsync(sp->d_first, inj->first_index, (size_t)B * 4, cudaMemcpyHostToDevice, h->stream)); first = sp->d_first; }
     }
+    *call = SearchCall{};
+    call->n = B;
+    call->obs = s.obs; call->legal_mask = s.legal; call->to_play = s.to_play;
+    call->add_noise = 1; call->noise = noise; call->first_index = first;
+    call->game_id = s.game_id; call->move_index = s.move;
+    call->visit_counts = s.visits; call->root_value = s.root_value;
+    return MZ_OK;
+}
+
+static int sp_enqueue(MzHandle* h, int32_t n_moves, double temperature, const MzSelfPlayInject* inj, const char* who) {
+    if (!h || !h->sp) return fail(h, MZ_ESTATE, std::string(who) + ": call mz_selfplay_begin first");
+    if (!h->weights_loaded) return fail(h, MZ_ESTATE, std::string(who) + ": weights not loaded");
+    if (n_moves < 0) return fail(h, MZ_EINVAL, std::string(who) + ": n_moves < 0");
+    if (inj && n_moves > 1 && (inj->forced_action || inj->uniform || inj->noise || inj->first_index))
+        return fail(h, MZ_EINVAL, std::string(who) + ": per-move overrides need n_moves == 1");
+    if (!(temperature >= 0.0)) return fail(h, MZ_EINVAL, std::string(who) + ": temperature must be >= 0");
+    MzSelfPlay* sp = h->sp;
+    if (sp->host) return fail(h, MZ_ESTATE, std::string(who) + ": host-stepped games move with mz_selfplay_host_act / _observe / _restart");
+    if (inj && inj->uniform)
+        for (int g = 0; g < sp->dev.B; ++g)
+            if (!(inj->uniform[g] >= 0.0 && inj->uniform[g] < 1.0))
+                return fail(h, MZ_EINVAL, std::string(who) + ": injected uniforms must lie in [0, 1)");
+    if (sp->in_flight) return fail(h, MZ_ESTATE, std::string(who) + ": moves already enqueued, call mz_selfplay_wait first");
+    MZ_CUDA(h, cudaSetDevice(h->device));
+    SpDev s;
+    SearchCall call{};
+    int rc = sp_move_setup(h, temperature, inj, &s, &call);
+    if (rc) return rc;
     if (sp->drained_bytes) {
         // the host has taken the staged games (and the areas were swapped): rewind the cursor; parked games are packed
         // by the first pass below
@@ -864,12 +1110,6 @@ static int sp_enqueue(MzHandle* h, int32_t n_moves, double temperature, const Mz
         MZ_CUDA(h, cudaMemsetAsync(s.counters + 5, 0, 8, h->stream));
         sp->drained_bytes = 0;
     }
-    SearchCall call{};
-    call.n = B;
-    call.obs = s.obs; call.legal_mask = s.legal; call.to_play = s.to_play;
-    call.add_noise = 1; call.noise = noise; call.first_index = first;
-    call.game_id = s.game_id; call.move_index = s.move;
-    call.visit_counts = s.visits; call.root_value = s.root_value;
     MZ_CUDA(h, cudaEventRecord(sp->e0, h->stream));
     if (sp->h_counters[4]) {                           // games parked by the previous call first, so their slots play again
         launch_selfplay_step(s, 0, h->stream);
@@ -920,11 +1160,142 @@ extern "C" int mz_selfplay_wait(MzHandle* h, MzSelfPlayStats* stats) {
     return sp_wait(h, stats);
 }
 
+static int host_loop(MzHandle* h, const char* who) {
+    if (!h || !h->sp || !h->sp->host) return fail(h, MZ_ESTATE, std::string(who) + ": call mz_selfplay_begin_host first");
+    return MZ_OK;
+}
+
+extern "C" int mz_selfplay_host_act(MzHandle* h, double temperature, const MzSelfPlayInject* inj, int32_t* actions) {
+    const char* who = "mz_selfplay_host_act";
+    int rc = host_loop(h, who);
+    if (rc) return rc;
+    MzSelfPlay* sp = h->sp;
+    if (!actions) return fail(h, MZ_EINVAL, std::string(who) + ": null actions");
+    if (!h->weights_loaded) return fail(h, MZ_ESTATE, std::string(who) + ": weights not loaded");
+    if (!(temperature >= 0.0)) return fail(h, MZ_EINVAL, std::string(who) + ": temperature must be >= 0");
+    if (sp->observe_due) return fail(h, MZ_ESTATE, std::string(who) + ": the last act waits for mz_selfplay_host_observe");
+    if (sp->n_awaiting)
+        return fail(h, MZ_ESTATE, std::string(who) + ": " + std::to_string(sp->n_awaiting) +
+                                  " finished slots wait for mz_selfplay_host_restart");
+    const int B = sp->dev.B;
+    if (inj && inj->uniform)
+        for (int g = 0; g < B; ++g)
+            if (!(inj->uniform[g] >= 0.0 && inj->uniform[g] < 1.0))
+                return fail(h, MZ_EINVAL, std::string(who) + ": injected uniforms must lie in [0, 1)");
+    MZ_CUDA(h, cudaSetDevice(h->device));
+    SpDev s;
+    SearchCall call{};
+    rc = sp_move_setup(h, temperature, inj, &s, &call);
+    if (rc) return rc;
+    MZ_CUDA(h, cudaEventRecord(sp->e0, h->stream));
+    rc = mz_dispatch_search(h, call, false, false, 0);
+    if (rc) return rc;
+    if (s.A <= 128) host_act_kernel<128><<<(B + kActThreads - 1) / kActThreads, kActThreads, 0, h->stream>>>(s);
+    else host_act_kernel<256><<<(B + kActThreads - 1) / kActThreads, kActThreads, 0, h->stream>>>(s);
+    h->launches += 1;
+    MZ_CUDA(h, cudaGetLastError());
+    MZ_CUDA(h, cudaEventRecord(sp->e1, h->stream));
+    MZ_CUDA(h, cudaMemcpyAsync(sp->actions.data(), s.host_action, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));
+    MZ_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (h->res && resnet_take_saturations(h->res, h->stream) > 0) mz_switch_to_strict(h);    // as sp_wait
+    sp->act_ms = 0.0f;
+    cudaEventElapsedTime(&sp->act_ms, sp->e0, sp->e1);
+    memcpy(actions, sp->actions.data(), (size_t)B * 4);
+    sp->observe_due = true;
+    return MZ_OK;
+}
+
+extern "C" int mz_selfplay_host_observe(MzHandle* h, const float* obs, const float* reward, const uint8_t* done,
+                                        const uint8_t* legal, const int32_t* to_play, uint8_t* finished,
+                                        MzSelfPlayStats* stats) {
+    const char* who = "mz_selfplay_host_observe";
+    int rc = host_loop(h, who);
+    if (rc) return rc;
+    MzSelfPlay* sp = h->sp;
+    if (!obs || !reward || !done || !legal || !to_play || !finished) return fail(h, MZ_EINVAL, std::string(who) + ": null argument");
+    if (!sp->observe_due) return fail(h, MZ_ESTATE, std::string(who) + ": no move in flight, call mz_selfplay_host_act first");
+    const int B = sp->dev.B, A = sp->dev.A, O = sp->dev.O;
+    std::vector<uint8_t> played(B);
+    for (int g = 0; g < B; ++g) played[g] = sp->actions[g] >= 0;
+    rc = check_host_rows(h, who, played.data(), legal, to_play, done);
+    if (rc) return rc;
+    MZ_CUDA(h, cudaSetDevice(h->device));
+    const HostRows& r = sp->rows;
+    MZ_CUDA(h, cudaMemcpyAsync(r.obs, obs, (size_t)B * O * 4, cudaMemcpyHostToDevice, h->stream));
+    MZ_CUDA(h, cudaMemcpyAsync(r.reward, reward, (size_t)B * 4, cudaMemcpyHostToDevice, h->stream));
+    MZ_CUDA(h, cudaMemcpyAsync(r.done, done, (size_t)B, cudaMemcpyHostToDevice, h->stream));
+    MZ_CUDA(h, cudaMemcpyAsync(r.legal, legal, (size_t)B * A, cudaMemcpyHostToDevice, h->stream));
+    MZ_CUDA(h, cudaMemcpyAsync(r.to_play, to_play, (size_t)B * 4, cudaMemcpyHostToDevice, h->stream));
+    SpDev s = sp->dev;
+    s.staging = sp->d_staging[sp->cur];
+    s.index = sp->d_index[sp->cur];
+    if (sp->drained_bytes) {                       // as sp_enqueue: the host has taken the staged games
+        MZ_CUDA(h, cudaMemsetAsync(s.counters + 2, 0, 16, h->stream));
+        MZ_CUDA(h, cudaMemsetAsync(s.counters + 5, 0, 8, h->stream));
+        sp->drained_bytes = 0;
+    }
+    MZ_CUDA(h, cudaMemsetAsync(s.counters + 4, 0, 8, h->stream));      // [4] = park events of THIS pass
+    MZ_CUDA(h, cudaEventRecord(sp->e0, h->stream));
+    host_observe_kernel<<<B, host_slot_threads(s), 0, h->stream>>>(s, r, sp->d_finished);
+    h->launches += 1;
+    MZ_CUDA(h, cudaGetLastError());
+    MZ_CUDA(h, cudaEventRecord(sp->e1, h->stream));
+    MZ_CUDA(h, cudaMemcpyAsync(finished, sp->d_finished, (size_t)B, cudaMemcpyDeviceToHost, h->stream));
+    rc = sp_read_counters(h, stats, 0.0f);         // synchronises
+    if (rc) return rc;
+    float ms = 0.0f;
+    cudaEventElapsedTime(&ms, sp->e0, sp->e1);
+    if (stats) stats->device_ms = sp->act_ms + ms;
+    for (int g = 0; g < B; ++g)
+        if (finished[g]) { sp->awaiting[g] = 1; ++sp->n_awaiting; }
+    sp->observe_due = false;
+    return MZ_OK;
+}
+
+extern "C" int mz_selfplay_host_restart(MzHandle* h, const uint8_t* which, const float* obs, const uint8_t* legal,
+                                        const int32_t* to_play) {
+    const char* who = "mz_selfplay_host_restart";
+    int rc = host_loop(h, who);
+    if (rc) return rc;
+    MzSelfPlay* sp = h->sp;
+    if (!which || !obs || !legal || !to_play) return fail(h, MZ_EINVAL, std::string(who) + ": null argument");
+    if (sp->observe_due) return fail(h, MZ_ESTATE, std::string(who) + ": the last act waits for mz_selfplay_host_observe");
+    const int B = sp->dev.B, A = sp->dev.A, O = sp->dev.O;
+    for (int g = 0; g < B; ++g)
+        if (which[g] && !sp->awaiting[g])
+            return fail(h, MZ_ESTATE, std::string(who) + ": slot " + std::to_string(g) +
+                                      " has no packed game waiting for a restart (observe reports them as finished)");
+    rc = check_host_rows(h, who, which, legal, to_play, nullptr);
+    if (rc) return rc;
+    MZ_CUDA(h, cudaSetDevice(h->device));
+    const HostRows& r = sp->rows;
+    MZ_CUDA(h, cudaMemcpyAsync(r.obs, obs, (size_t)B * O * 4, cudaMemcpyHostToDevice, h->stream));
+    MZ_CUDA(h, cudaMemcpyAsync(r.legal, legal, (size_t)B * A, cudaMemcpyHostToDevice, h->stream));
+    MZ_CUDA(h, cudaMemcpyAsync(r.to_play, to_play, (size_t)B * 4, cudaMemcpyHostToDevice, h->stream));
+    MZ_CUDA(h, cudaMemcpyAsync(sp->d_which, which, (size_t)B, cudaMemcpyHostToDevice, h->stream));
+    host_start_kernel<<<B, host_slot_threads(sp->dev), 0, h->stream>>>(sp->dev, r, sp->d_which, 0);
+    h->launches += 1;
+    MZ_CUDA(h, cudaGetLastError());
+    MZ_CUDA(h, cudaStreamSynchronize(h->stream));
+    for (int g = 0; g < B; ++g)
+        if (which[g]) { sp->awaiting[g] = 0; --sp->n_awaiting; }
+    return MZ_OK;
+}
+
 extern "C" int mz_selfplay_drain(MzHandle* h, const void** data, uint64_t* bytes, int32_t* n_games, const uint64_t** index) {
     if (!h || !h->sp || !data || !bytes || !n_games) return fail(h, MZ_EINVAL, "mz_selfplay_drain: bad argument");
     MzSelfPlay* sp = h->sp;
     if (sp->in_flight) return fail(h, MZ_ESTATE, "mz_selfplay_drain: moves in flight, call mz_selfplay_wait first");
     MZ_CUDA(h, cudaSetDevice(h->device));
+    if (sp->drained_bytes) {
+        // drained already, and no move since has rewound the device's cursor: its counters still describe the games
+        // returned then, from the other area
+        *data = sp->staging[sp->cur];
+        if (index) *index = reinterpret_cast<const uint64_t*>(sp->index[sp->cur]);
+        *bytes = 0;
+        *n_games = 0;
+        return MZ_OK;
+    }
     int rc = sp_read_counters(h, nullptr, 0.0f);
     if (rc) return rc;
     *data = sp->staging[sp->cur];

@@ -461,8 +461,20 @@ class DeviceSelfPlayLoop:
             raise NotImplementedError(f"no device opponent {opponent!r} (expected one of {sorted(self.OPPONENTS)})")
         self.engine = engine
         self.opponent, self.muzero_player = opponent, int(muzero_player)
+        d = self._desc(self.ENVS[env], max_moves, temperature_threshold, reward_scale, first_game_id, staging_bytes,
+                       game_id_stride, td_steps, per_alpha, discount, stacked_observations)
+        try:
+            engine._check(engine.lib.mz_selfplay_begin_vs(engine._h, C.byref(d), self.OPPONENTS[opponent], self.muzero_player))
+        except _lib.MzError as e:
+            if e.code == _lib.MZ_EUNSUPPORTED:
+                raise NotImplementedError(str(e)) from e
+            raise
+        self.stats = _lib.MzSelfPlayStats()
+
+    def _desc(self, env, max_moves, temperature_threshold, reward_scale, first_game_id, staging_bytes, game_id_stride,
+              td_steps, per_alpha, discount, stacked_observations):
         d = _lib.MzSelfPlayDesc()
-        d.env = self.ENVS[env]
+        d.env = env
         d.max_moves = int(max_moves)
         d.temperature_threshold = int(temperature_threshold or 0)
         d.reward_scale = int(reward_scale)
@@ -476,24 +488,25 @@ class DeviceSelfPlayLoop:
             d.discount_pow = C.cast(self._discount_pow, C.c_void_p)
         self.with_priorities = bool(d.td_steps)
         d.staging_bytes = int(staging_bytes)
-        try:
-            engine._check(engine.lib.mz_selfplay_begin_vs(engine._h, C.byref(d), self.OPPONENTS[opponent], self.muzero_player))
-        except _lib.MzError as e:
-            if e.code == _lib.MZ_EUNSUPPORTED:
-                raise NotImplementedError(str(e)) from e
-            raise
-        self.stats = _lib.MzSelfPlayStats()
+        return d
+
+    def _inject(self, keep, forced_action, uniform, noise, first_index):
+        """MzSelfPlayInject of the given overrides, or None when there are none."""
+        if forced_action is None and uniform is None and noise is None and first_index is None:
+            return None
+        eng = self.engine
+        inj = _lib.MzSelfPlayInject()
+        inj.forced_action = eng._ptr(forced_action, numpy.int32, keep)
+        inj.uniform = eng._ptr(uniform, numpy.float64, keep)
+        inj.noise = eng._ptr(noise, numpy.float64, keep)
+        inj.first_index = eng._ptr(first_index, numpy.int32, keep)
+        return inj
 
     def moves(self, n_moves: int, temperature: float, forced_action=None, uniform=None, noise=None, first_index=None):
         """Play ``n_moves`` lockstep moves; returns the stats struct (env_steps, games_finished, staged_*, device_ms)."""
         eng = self.engine
-        inj, keep = None, []
-        if forced_action is not None or uniform is not None or noise is not None or first_index is not None:
-            inj = _lib.MzSelfPlayInject()
-            inj.forced_action = eng._ptr(forced_action, numpy.int32, keep)
-            inj.uniform = eng._ptr(uniform, numpy.float64, keep)
-            inj.noise = eng._ptr(noise, numpy.float64, keep)
-            inj.first_index = eng._ptr(first_index, numpy.int32, keep)
+        keep = []
+        inj = self._inject(keep, forced_action, uniform, noise, first_index)
         eng._check(eng.lib.mz_selfplay_moves(eng._h, int(n_moves), float(temperature),
                                             C.byref(inj) if inj is not None else None, C.byref(self.stats)))
         return self.stats
@@ -541,6 +554,69 @@ class DeviceSelfPlayLoop:
             setattr(pk, k, v.ctypes.data)
         eng._check(eng.lib.mz_selfplay_peek(eng._h, C.byref(pk)))
         return out
+
+
+class HostEnvSelfPlayLoop(DeviceSelfPlayLoop):
+    """Python face of mz_selfplay_begin_host / _host_act / _host_observe / _host_restart: the device loop for a game
+    whose environment the caller steps.  Each move is ``act`` -> [step the environments of the slots whose action is
+    >= 0] -> ``observe`` -> [reset the environments of the slots it reports finished] -> ``restart``; ``drain`` and
+    ``peek`` are the device loop's.  Rows are ``[max_games, ...]`` arrays (or sequences of per-game arrays)."""
+
+    def __init__(self, engine: SearchEngine, obs_shape, max_moves: int, obs, legal_mask, to_play,
+                 temperature_threshold=None, first_game_id: int = 0, staging_bytes: int = 0, game_id_stride: int = 0,
+                 td_steps: int = 0, per_alpha: float = 1.0, discount: float = 1.0, stacked_observations: int = 0):
+        """``obs_shape`` is the environment's (C, H, W); ``obs``, ``legal_mask`` and ``to_play`` the first rows of the
+        games ``first_game_id + g``."""
+        self.engine = engine
+        self.opponent, self.muzero_player = "self", 0
+        B = engine.max_games
+        self.O = int(numpy.prod(obs_shape))
+        d = self._desc(_lib.MZ_ENV_HOST, max_moves, temperature_threshold, 0, first_game_id, staging_bytes, game_id_stride,
+                       td_steps, per_alpha, discount, stacked_observations)
+        e = _lib.MzHostEnvDesc(*(int(x) for x in obs_shape))
+        o, lg, tp = self._rows(obs, legal_mask, to_play)
+        engine._check(engine.lib.mz_selfplay_begin_host(engine._h, C.byref(d), C.byref(e), o.ctypes.data, lg.ctypes.data,
+                                                        tp.ctypes.data))
+        self.stats = _lib.MzSelfPlayStats()
+        self.actions = numpy.empty(B, numpy.int32)
+        self.finished = numpy.empty(B, numpy.uint8)
+
+    def _rows(self, obs, legal_mask, to_play):
+        B = self.engine.max_games
+        if not isinstance(obs, numpy.ndarray):
+            obs = numpy.stack([numpy.asarray(x) for x in obs])
+        return (numpy.ascontiguousarray(obs, numpy.float32).reshape(B, self.O),
+                numpy.ascontiguousarray(legal_mask, numpy.uint8).reshape(B, self.engine.A),
+                numpy.ascontiguousarray(to_play, numpy.int32).reshape(B))
+
+    def act(self, temperature: float, forced_action=None, uniform=None, noise=None, first_index=None):
+        """One batched search and the action of every slot: an int32 ``[max_games]`` array (reused by the next call),
+        -1 for a slot that is not playing this move (its finished game waits for staging space)."""
+        eng = self.engine
+        keep = []
+        inj = self._inject(keep, forced_action, uniform, noise, first_index)
+        eng._check(eng.lib.mz_selfplay_host_act(eng._h, float(temperature), C.byref(inj) if inj is not None else None,
+                                               self.actions.ctypes.data))
+        return self.actions
+
+    def observe(self, obs, reward, done, legal_mask, to_play):
+        """The step's rows for the whole batch (rows of slots that did not play are ignored); ``reward`` is rounded once to
+        float32.  Returns the bool ``[max_games]`` mask of the slots whose game ended and was packed (reset them, then
+        ``restart``); the stats struct is ``self.stats``."""
+        eng = self.engine
+        o, lg, tp = self._rows(obs, legal_mask, to_play)
+        r = numpy.ascontiguousarray(numpy.asarray(reward, numpy.float64).astype(numpy.float32).reshape(-1))
+        dn = numpy.ascontiguousarray(numpy.asarray(done).astype(numpy.uint8).reshape(-1))
+        eng._check(eng.lib.mz_selfplay_host_observe(eng._h, o.ctypes.data, r.ctypes.data, dn.ctypes.data, lg.ctypes.data,
+                                                   tp.ctypes.data, self.finished.ctypes.data, C.byref(self.stats)))
+        return self.finished.astype(bool)
+
+    def restart(self, which, obs, legal_mask, to_play):
+        """The first rows of the next games of the slots of ``which`` (the mask ``observe`` returned, or part of it)."""
+        eng = self.engine
+        w = numpy.ascontiguousarray(numpy.asarray(which).astype(numpy.uint8).reshape(-1))
+        o, lg, tp = self._rows(obs, legal_mask, to_play)
+        eng._check(eng.lib.mz_selfplay_host_restart(eng._h, w.ctypes.data, o.ctypes.data, lg.ctypes.data, tp.ctypes.data))
 
 
 def parse_staged_game(buf: bytes, off: int):

@@ -26,7 +26,7 @@ from collections import deque
 
 import numpy
 
-from .engine import DeviceSelfPlayLoop, SearchEngine, parse_staged_game
+from .engine import DeviceSelfPlayLoop, HostEnvSelfPlayLoop, SearchEngine, parse_staged_game
 
 
 # ----------------------------------------------------------------------------------------
@@ -443,7 +443,7 @@ class SelfPlay:
                     trained_steps=_call(shared_storage, "get_info", "training_step"))
                 if self.num_parallel_games > 1:
                     # the lockstep batch advances between two weight refreshes; every finished game goes to the buffer
-                    if self.loop_path == "device":
+                    if self.loop_path in ("device", "device-host-env"):
                         games = self.play_moves(int(getattr(cfg, "moves_per_weight_refresh", 8)), temperature,
                                                 cfg.temperature_threshold)
                     else:
@@ -606,10 +606,19 @@ class SelfPlay:
             return None
         return name
 
+    def _host_env_device_loop(self):
+        """True when the game's own (host) environment plays on the device loop: ``config.host_env_device_loop``, philox
+        draws, and no device-resident environment in use."""
+        return (bool(getattr(self.config, "host_env_device_loop", False)) and self.rng_mode == "philox"
+                and not self._device_env_name())
+
     @property
     def loop_path(self):
-        """"device": environments, sampling and records on the GPU (mz_selfplay_*); "host": numpy environments."""
-        return "device" if self._device_env_name() else "host"
+        """"device": environments, sampling and records on the GPU (mz_selfplay_*); "device-host-env": the same with the
+        game's own environment stepped on the host (mz_selfplay_host_*); "host": the host loop."""
+        if self._device_env_name():
+            return "device"
+        return "device-host-env" if self._host_env_device_loop() else "host"
 
     @property
     def env_steps(self):
@@ -624,11 +633,14 @@ class SelfPlay:
         With ``rng_mode="philox"`` and a game that has a device-resident environment (CartPole, TicTacToe, Connect4,
         Gomoku, Twenty-One, Simple Grid)
         the whole loop - observation, search, visit-count sampling, environment step, history records - runs on the
-        GPU (``mz_selfplay_moves``) and only finished games cross to the host, as ``PackedGameHistory`` objects.
-        Otherwise the host loop (``BatchedSelfPlay.move``) is used."""
-        if self._device_env_name():
+        GPU (``mz_selfplay_moves``) and only finished games cross to the host, as ``PackedGameHistory`` objects.  With
+        ``rng_mode="philox"``, ``config.host_env_device_loop`` and no device environment in use, the same loop runs
+        with the game's own environment stepped on the host (``DeviceHostEnvSelfPlay``).  Otherwise the host loop
+        (``BatchedSelfPlay.move``) is used."""
+        if self.loop_path != "host":
             if getattr(self, "_device_loop", None) is None:
-                self._device_loop = DeviceBatchedSelfPlay(self, temperature_threshold)
+                self._device_loop = (DeviceBatchedSelfPlay if self.loop_path == "device" else DeviceHostEnvSelfPlay)(
+                    self, temperature_threshold)
             games = self._device_loop.moves(n_moves, temperature)
             self.played_games += len(games)
             self.played_steps += games.total_moves
@@ -724,9 +736,14 @@ class _ObjectVector:
     def observations(self):
         return self._obs
 
-    def step(self, actions):
+    def step(self, actions, which=None):
+        """Steps every game, or the games of the bool mask ``which`` (the others report reward 0, not done)."""
         rewards, dones = [], []
         for g, game in enumerate(self.games):
+            if which is not None and not which[g]:
+                rewards.append(0)
+                dones.append(False)
+                continue
             o, r, d = game.step(actions[g])
             self._obs[g] = numpy.asarray(o)
             rewards.append(r)
@@ -820,6 +837,81 @@ class DeviceBatchedSelfPlay:
             if st.staged_bytes > 0:
                 grow = min(grow, int(0.5 * st.staging_capacity * k / st.staged_bytes))
             self.chunk = max(1, grow)
+
+
+class DeviceHostEnvSelfPlay:
+    """Lockstep self-play of a game without a device environment (``config.host_env_device_loop``): the device loop of
+    ``DeviceBatchedSelfPlay`` with only the environment step on the host.  The environments are ``Game.vector(B,
+    seed)`` when the game has one, else ``B`` ``Game`` objects; per move: ``act`` (search, sampling and records on the
+    device) -> step the environments of the slots with an action -> ``observe`` (records, stacking, priorities, packing)
+    -> reset the environments of the games it packed -> ``restart``.  Slot g plays the global games ``first_game_id + g
+    + k * stride`` with the Philox draws of the device loop, so a game's history is the device loop's wherever both
+    can play it."""
+
+    DRAIN_FILL = 0.5        # drain when the staging area is fuller than this, or holds parked games
+
+    def __init__(self, worker, temperature_threshold=None):
+        cfg, Game = worker.config, worker.Game
+        self.B, self.A = worker.num_parallel_games, len(cfg.action_space)
+        self.env = Game.vector(self.B, worker.seed) if hasattr(Game, "vector") else \
+            _ObjectVector(Game, self.B, worker.seed, self.A)
+        vec = getattr(Game, "VECTOR", None)
+        self.obs_shape = tuple(cfg.observation_shape)
+        self.obs_dtype = getattr(vec, "OBS_DTYPE", numpy.float32)
+        self.reward_type = int if vec is not None else float
+        priorities = getattr(cfg, "PER", False) and getattr(cfg, "device_priorities", True)
+        obs = self.env.reset()
+        self.loop = HostEnvSelfPlayLoop(worker.model.engine, self.obs_shape, cfg.max_moves, obs, self.env.legal_mask(),
+                                        self.env.to_play(), temperature_threshold=temperature_threshold,
+                                        first_game_id=worker.first_game_id, game_id_stride=worker.game_id_stride,
+                                        td_steps=int(cfg.td_steps) if priorities else 0, per_alpha=cfg.PER_alpha,
+                                        discount=cfg.discount,
+                                        staging_bytes=int(getattr(cfg, "selfplay_staging_bytes", 0) or 0),
+                                        stacked_observations=int(cfg.stacked_observations))
+        self.device_s = 0.0       # host clock in the library calls (they end in a device synchronisation), so far
+        self.env_s = 0.0          # host clock in the environments' step / reset / legal_mask / to_play, so far
+        self.parked_events = 0    # finished games that had to wait for a drain (staging area full), so far
+
+    def _step(self, actions):
+        playing = actions >= 0
+        actions = actions.astype(numpy.int64)
+        if playing.all():
+            return self.env.step(actions)
+        if isinstance(self.env, _ObjectVector):
+            return self.env.step(actions, playing)
+        # a VectorGame steps all its games: a slot that is not playing (its finished game waits for staging space) takes
+        # action 0 and its results are ignored; its environment is reset before its next game
+        return self.env.step(numpy.where(playing, actions, 0))
+
+    def moves(self, n_moves, temperature, **inject):
+        """``n_moves`` lockstep moves -> ``PackedGames`` of the games that finished (and were packed) meanwhile."""
+        out = PackedGames(self.obs_shape, self.obs_dtype, self.reward_type, self.loop.with_priorities)
+        env, loop = self.env, self.loop
+        clock = time.perf_counter
+        for _ in range(int(n_moves)):
+            t0 = clock()
+            actions = loop.act(temperature, **inject)
+            t1 = clock()
+            obs, reward, done = self._step(actions)
+            legal, to_play = env.legal_mask(), env.to_play()
+            t2 = clock()
+            finished = loop.observe(obs, reward, done, legal, to_play)
+            t3 = clock()
+            self.device_s += (t1 - t0) + (t3 - t2)
+            self.env_s += t2 - t1
+            if finished.any():
+                obs = env.reset(finished)
+                legal, to_play = env.legal_mask(), env.to_play()
+                t4 = clock()
+                loop.restart(finished, obs, legal, to_play)
+                self.env_s += t4 - t3
+                self.device_s += clock() - t4
+            st = loop.stats
+            self.parked_events += int(st.parked_slots)
+            if st.parked_slots or st.staged_bytes > self.DRAIN_FILL * st.staging_capacity:
+                out.add(*loop.drain())
+        out.add(*loop.drain())
+        return out
 
 
 class PackedGames:
