@@ -541,6 +541,7 @@ typedef struct MzSelfPlayPeek {
  *   int64 game_id; int32 slot; int32 length T; int32 first_to_play; int32 obs_elems O; int32 actions A; int32 bytes;
  *   double root_value[T]; int32 visit_counts[T][A]; int32 action[T]; float reward[T]; int32 to_play[T] (after the move);
  *   float priority[T] (zeros unless td_steps > 0); float observation[T+1][O] (index 0 = reset observation); padding to 8.
+ * Loops begun with mz_selfplay_begin_host_window stage O = 0 and no observations: the caller kept them.
  * = the fields of GameHistory (self_play.py:479-511) minus the dummy first entries.
  * In test-mode games (mz_selfplay_begin_vs with an opponent) a move the opponent played has root_value NaN and all
  * visit counts 0 (store_search_statistics(None), self_play.py:496-511: root_values holds None there and child_visits
@@ -606,6 +607,13 @@ typedef struct MzHostEnvDesc {
  * the bytes per slot, when the records ([max_games][max_moves + 1] observations) do not fit on the device. */
 int mz_selfplay_begin_host(MzHandle* h, const MzSelfPlayDesc* desc, const MzHostEnvDesc* env, const float* obs,
                            const uint8_t* legal, const int32_t* to_play);
+/* mz_selfplay_begin_host, but the caller keeps each game's observations: the device holds a window of the last
+ * stacked_observations + 1 observations per slot, and staged blocks carry obs_elems = 0 and no observation section.
+ * For image games with long episodes (games/atari.py: 27000 moves of 3 x 96 x 96 frames, 2.99 GB per slot with the whole
+ * game on the device, 3.65 MB with the window of 33).  The stacked inputs, records, priorities and every other call are
+ * those of mz_selfplay_begin_host, and so are its refusals; MZ_ENOMEM counts the window's observations per slot. */
+int mz_selfplay_begin_host_window(MzHandle* h, const MzSelfPlayDesc* desc, const MzHostEnvDesc* env, const float* obs,
+                                  const uint8_t* legal, const int32_t* to_play);
 int mz_selfplay_host_act(MzHandle* h, double temperature, const MzSelfPlayInject* inject, int32_t* actions);
 int mz_selfplay_host_observe(MzHandle* h, const float* obs, const float* reward, const uint8_t* done, const uint8_t* legal,
                              const int32_t* to_play, uint8_t* finished, MzSelfPlayStats* stats);

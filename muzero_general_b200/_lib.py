@@ -13,7 +13,7 @@ MZ_MAX_LAYERS = 8
 MZ_MAX_ACTIONS = 256
 MZ_MEM_HOST, MZ_MEM_DEVICE = 0, 1
 MZ_FLAG_KEEP_TREE, MZ_FLAG_STEPWISE, MZ_FLAG_CONTINUE = 1, 2, 4
-MZ_EUNSUPPORTED, MZ_ESTATE = -3, -4
+MZ_EUNSUPPORTED, MZ_ESTATE, MZ_ENOMEM = -3, -4, -5
 
 _L = C.c_int32 * MZ_MAX_LAYERS
 
@@ -163,6 +163,8 @@ SYMBOLS = [
     ("mz_selfplay_peek", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayPeek)]),
     ("mz_selfplay_begin_host", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayDesc), C.POINTER(MzHostEnvDesc), C.c_void_p,
                                          C.c_void_p, C.c_void_p]),
+    ("mz_selfplay_begin_host_window", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayDesc), C.POINTER(MzHostEnvDesc),
+                                                C.c_void_p, C.c_void_p, C.c_void_p]),
     ("mz_selfplay_host_act", C.c_int, [C.c_void_p, C.c_double, C.POINTER(MzSelfPlayInject), C.c_void_p]),
     ("mz_selfplay_host_observe", C.c_int, [C.c_void_p] + [C.c_void_p] * 6 + [C.POINTER(MzSelfPlayStats)]),
     ("mz_selfplay_host_restart", C.c_int, [C.c_void_p] * 5),

@@ -43,6 +43,8 @@
 //   restart   the next game's first rows of the slots observe packed -> host_start_kernel
 // A finished game that does not fit into the staging area stays parked in its slot (fin > 0, action -1) and every
 // observe pass tries again; the slot reports "finished" (its environment is reset, then restarted) once it is packed.
+// mz_selfplay_begin_host_window: the caller keeps each game's observations.  rec_obs then holds a window of stack + 1
+// rows per slot (observation p in row p % rows: all stack_fill reads) and the staged blocks carry none (O_staged = 0).
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -62,6 +64,9 @@ struct SpDev {
     int O_in;                  // floats of a slot's search input: O, plus stack * (O + plane) stacked floats
     int stack;                 // config.stacked_observations
     int plane;                 // floats of one observation plane (the action plane of the stack has this size)
+    int rows;                  // observations rec_obs keeps per slot: observation p of a game is row p % rows, with
+                               // rows = max_moves + 1 (the whole game) or stack + 1 (a window: the caller keeps the game's)
+    int O_staged;              // floats per observation in a staged block: O, or 0 for a window
     int opponent;              // MZ_OPPONENT_*
     int muzero_player;         // to_play of MuZero's side when opponent != MZ_OPPONENT_SELF
     uint64_t seed;
@@ -89,7 +94,7 @@ struct SpDev {
     int32_t* rec_action;       // [B][T]
     float* rec_reward;         // [B][T]
     int32_t* rec_to_play;      // [B][T]   (after the move)
-    float* rec_obs;            // [B][T+1][O]
+    float* rec_obs;            // [B][rows][O]
     int32_t* first_to_play;    // [B]
     int32_t* fin;              // [B] 0 = playing, T > 0 = finished after T moves, waiting to be packed,
                                //     -1 = MZ_ENV_HOST: packed, waiting for the next game's first rows
@@ -366,7 +371,7 @@ MZ_DEVINL void record_move(const SpDev& s, int g, int t, int action, float rewar
     publish(s, g);
     s.rec_to_play[r] = s.to_play[g];
     const float* o = s.obs + (size_t)g * s.O_in;
-    float* ro = s.rec_obs + ((size_t)g * (s.max_moves + 1) + t + 1) * s.O;
+    float* ro = s.rec_obs + ((size_t)g * s.rows + (t + 1) % s.rows) * s.O;
     for (int i = 0; i < s.O; ++i) ro[i] = o[i];
     s.move[g] = t + 1;
     s.last_action[g] = action;
@@ -396,7 +401,7 @@ MZ_DEVINL int start_game(const SpDev& s, int g, int64_t gid) {
     publish(s, g);
     s.first_to_play[g] = s.to_play[g];
     const float* o = s.obs + (size_t)g * s.O_in;
-    float* r0 = s.rec_obs + (size_t)g * (s.max_moves + 1) * s.O;
+    float* r0 = s.rec_obs + (size_t)g * s.rows * s.O;
     for (int i = 0; i < s.O; ++i) r0[i] = o[i];
     if (s.opponent == MZ_OPPONENT_SELF || s.to_play[g] == s.muzero_player) return 0;
     const bool done = opponent_move(s, g);
@@ -406,19 +411,19 @@ MZ_DEVINL int start_game(const SpDev& s, int g, int64_t gid) {
 
 // The stacked tail of slot g's search input, after its current observation (GameHistory.get_stacked_observations(-1),
 // self_play.py:513-550): for k = 1 .. stack, p = t - k with t the moves played, the observation after move p
-// (rec_obs[p]) and a plane of action_history[p + 1] / A = rec_action[p] / A, or O + plane zeros when p < 0.  The
+// (rec_obs row p % rows) and a plane of action_history[p + 1] / A = rec_action[p] / A, or O + plane zeros when p < 0.  The
 // action plane is the fp64 quotient rounded once to fp32, what the reference's float64 plane becomes after .float().
 // Threads lane, lane + step, ... share the floats; the slot's records must be visible to all of them.
 MZ_DEVINL void stack_fill(const SpDev& s, int g, int lane, int step) {
     const int t = s.move[g];
     const int block = s.O + s.plane;
     float* tail = s.obs + (size_t)g * s.O_in + s.O;
-    const float* rec = s.rec_obs + (size_t)g * (s.max_moves + 1) * s.O;
+    const float* rec = s.rec_obs + (size_t)g * s.rows * s.O;
     const int32_t* act = s.rec_action + (size_t)g * s.max_moves;
     for (int i = lane; i < s.stack * block; i += step) {
         const int k = i / block, j = i - k * block, p = t - 1 - k;
         float v = 0.0f;
-        if (p >= 0) v = j < s.O ? rec[(size_t)p * s.O + j] : __double2float_rn(__ddiv_rn((double)act[p], (double)s.A));
+        if (p >= 0) v = j < s.O ? rec[(size_t)(p % s.rows) * s.O + j] : __double2float_rn(__ddiv_rn((double)act[p], (double)s.A));
         tail[i] = v;
     }
 }
@@ -556,7 +561,7 @@ MZ_DEVINL float initial_priority(const SpDev& s, int g, int T, int i) {
 // move): the cursor may run past the capacity, reservations that end beyond it are void, and since the cursor only
 // grows the valid reservations are a contiguous prefix whose end is tracked in counters[5].
 MZ_DEVINL bool pack_game(const SpDev& s, int g, int T, int lane) {
-    const unsigned long long bytes = staged_block_bytes(T, s.A, s.O);
+    const unsigned long long bytes = staged_block_bytes(T, s.A, s.O_staged);
     unsigned long long off = 0;
     int ok = 0;
     if (lane == 0) {
@@ -579,7 +584,7 @@ MZ_DEVINL bool pack_game(const SpDev& s, int g, int T, int lane) {
     if (lane == 0) {
         *reinterpret_cast<int64_t*>(dst) = s.game_id[g];
         int32_t* hd = reinterpret_cast<int32_t*>(dst + 8);
-        hd[0] = g; hd[1] = T; hd[2] = s.first_to_play[g]; hd[3] = s.O; hd[4] = s.A; hd[5] = (int32_t)bytes;
+        hd[0] = g; hd[1] = T; hd[2] = s.first_to_play[g]; hd[3] = s.O_staged; hd[4] = s.A; hd[5] = (int32_t)bytes;
     }
     unsigned char* p = dst + MZ_STAGED_HEADER_BYTES;
     const size_t r = (size_t)g * s.max_moves;
@@ -605,8 +610,8 @@ MZ_DEVINL bool pack_game(const SpDev& s, int g, int T, int lane) {
         for (int i = lane; i < T; i += 32) f[i] = s.td_steps > 0 ? initial_priority(s, g, T, i) : 0.0f;
         p += (size_t)T * 4;
         f = reinterpret_cast<float*>(p);
-        const float* src = s.rec_obs + (size_t)g * (s.max_moves + 1) * s.O;
-        for (int i = lane; i < (T + 1) * s.O; i += 32) f[i] = src[i];
+        const float* src = s.rec_obs + (size_t)g * s.rows * s.O;       // the whole game when O_staged > 0
+        for (int i = lane; i < (T + 1) * s.O_staged; i += 32) f[i] = src[i];
     }
     __syncwarp();
     return true;
@@ -676,11 +681,11 @@ struct HostRows {
 };
 
 // publish() of a host-stepped slot: its observation row becomes the current observation (the first O floats of the
-// search input) and rec_obs[t], its legal-mask row the slot's mask.  Threads tid, tid + nt, ... share the copies.
+// search input) and rec_obs row t % rows, its legal-mask row the slot's mask.  Threads tid, tid + nt, ... share the copies.
 MZ_DEVINL void take_rows(const SpDev& s, const HostRows& h, int g, int t, int tid, int nt) {
     const float* src = h.obs + (size_t)g * s.O;
     float* o = s.obs + (size_t)g * s.O_in;
-    float* ro = s.rec_obs + ((size_t)g * (s.max_moves + 1) + t) * s.O;
+    float* ro = s.rec_obs + ((size_t)g * s.rows + t % s.rows) * s.O;
     for (int i = tid; i < s.O; i += nt) {
         const float v = src[i];
         o[i] = v;
@@ -852,25 +857,34 @@ static int check_host_rows(MzHandle* h, const char* who, const uint8_t* which, c
 }
 
 static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int32_t muzero_player, const MzHostEnvDesc* e,
-                    const float* obs, const uint8_t* legal, const int32_t* to_play);
+                    const float* obs, const uint8_t* legal, const int32_t* to_play, bool window);
 
 extern "C" int mz_selfplay_begin(MzHandle* h, const MzSelfPlayDesc* d) {
     return mz_selfplay_begin_vs(h, d, MZ_OPPONENT_SELF, 0);
 }
 
 extern "C" int mz_selfplay_begin_vs(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int32_t muzero_player) {
-    return sp_begin(h, d, opponent, muzero_player, nullptr, nullptr, nullptr, nullptr);
+    return sp_begin(h, d, opponent, muzero_player, nullptr, nullptr, nullptr, nullptr, false);
 }
 
 extern "C" int mz_selfplay_begin_host(MzHandle* h, const MzSelfPlayDesc* d, const MzHostEnvDesc* e, const float* obs,
                                       const uint8_t* legal, const int32_t* to_play) {
     if (!h || !d || !e || !obs || !legal || !to_play) return fail(h, MZ_EINVAL, "mz_selfplay_begin_host: null argument");
     if (d->env != MZ_ENV_HOST) return fail(h, MZ_EINVAL, "mz_selfplay_begin_host: desc->env must be MZ_ENV_HOST");
-    return sp_begin(h, d, MZ_OPPONENT_SELF, 0, e, obs, legal, to_play);
+    return sp_begin(h, d, MZ_OPPONENT_SELF, 0, e, obs, legal, to_play, false);
 }
 
+extern "C" int mz_selfplay_begin_host_window(MzHandle* h, const MzSelfPlayDesc* d, const MzHostEnvDesc* e, const float* obs,
+                                             const uint8_t* legal, const int32_t* to_play) {
+    if (!h || !d || !e || !obs || !legal || !to_play) return fail(h, MZ_EINVAL, "mz_selfplay_begin_host_window: null argument");
+    if (d->env != MZ_ENV_HOST) return fail(h, MZ_EINVAL, "mz_selfplay_begin_host_window: desc->env must be MZ_ENV_HOST");
+    return sp_begin(h, d, MZ_OPPONENT_SELF, 0, e, obs, legal, to_play, true);
+}
+
+// window: rec_obs keeps the last stacked_observations + 1 observations of a slot's game and the staged blocks none
+// (mz_selfplay_begin_host_window); otherwise the whole game's
 static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int32_t muzero_player, const MzHostEnvDesc* e,
-                    const float* obs, const uint8_t* legal, const int32_t* to_play) {
+                    const float* obs, const uint8_t* legal, const int32_t* to_play, bool window) {
     if (!h || !d) return fail(h, MZ_EINVAL, "mz_selfplay_begin: null argument");
     if (opponent != MZ_OPPONENT_SELF && opponent != MZ_OPPONENT_EXPERT && opponent != MZ_OPPONENT_RANDOM)
         return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin_vs: unknown opponent " + std::to_string(opponent));
@@ -917,7 +931,8 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
             if (!e) return fail(h, MZ_EINVAL, "mz_selfplay_begin: host-stepped games (MZ_ENV_HOST) start with mz_selfplay_begin_host");
             if (e->obs_channels < 1 || e->obs_h < 1 || e->obs_w < 1)
                 return fail(h, MZ_EINVAL, "mz_selfplay_begin_host: the observation's channels, height and width must be >= 1");
-            int rc = check_host_rows(h, "mz_selfplay_begin_host", nullptr, legal, to_play, nullptr);
+            int rc = check_host_rows(h, window ? "mz_selfplay_begin_host_window" : "mz_selfplay_begin_host", nullptr, legal,
+                                     to_play, nullptr);
             if (rc) return rc;
             name = "the host-stepped environment"; C = e->obs_channels; ph = e->obs_h; pw = e->obs_w; A_env = A;
             break;
@@ -934,17 +949,20 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
                                   " actions and " + std::to_string(h->obs_elems) + " input values");
     const int O = C * ph * pw;
     if (d->max_moves < 1) return fail(h, MZ_EINVAL, "mz_selfplay_begin: max_moves < 1");
+    // observations rec_obs keeps per slot, and the floats of each staged observation
+    const int rows = window ? (int)stack + 1 : d->max_moves + 1, O_staged = window ? 0 : O;
     {
-        // device memory per slot: the search input and outputs, the records of a maximum-length game ([max_moves + 1][O]
+        // device memory per slot: the search input and outputs, the records of a maximum-length game (with `rows`
         // observations) and the host's upload rows
         const unsigned long long Tm = (unsigned long long)d->max_moves;
-        const unsigned long long per_slot = (unsigned long long)h->obs_elems * 4 + (Tm + 1) * O * 4 + Tm * (8 + 4ull * A + 12) +
+        const unsigned long long per_slot = (unsigned long long)h->obs_elems * 4 + (unsigned long long)rows * O * 4 +
+                                            Tm * (8 + 4ull * A + 12) +
                                             (d->env == MZ_ENV_HOST ? (unsigned long long)O * 4 + A + 16 : 0) + 24ull * A + 64;
         size_t free_bytes = 0, total_bytes = 0;
         if (cudaMemGetInfo(&free_bytes, &total_bytes) == cudaSuccess && per_slot * B > free_bytes)
             return fail(h, MZ_ENOMEM, "mz_selfplay_begin: the records of " + std::to_string(B) + " slots do not fit on the device: " +
-                                      std::to_string(per_slot) + " bytes per slot (" + std::to_string(d->max_moves + 1) +
-                                      " observations of " + std::to_string(O) + " floats for max_moves = " +
+                                      std::to_string(per_slot) + " bytes per slot (" + (window ? "a window of " : "") +
+                                      std::to_string(rows) + " observations of " + std::to_string(O) + " floats for max_moves = " +
                                       std::to_string(d->max_moves) + "), " + std::to_string(free_bytes) + " bytes free");
     }
     MzSelfPlay* sp = new (std::nothrow) MzSelfPlay();
@@ -953,7 +971,7 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
     sp->desc = *d;
     SpDev& s = sp->dev;
     s.env = d->env; s.B = B; s.A = A; s.O = O; s.H = H; s.W = W; s.K = K; s.max_moves = d->max_moves;
-    s.O_in = (int)h->obs_elems; s.stack = (int)stack; s.plane = ph * pw;
+    s.O_in = (int)h->obs_elems; s.stack = (int)stack; s.plane = ph * pw; s.rows = rows; s.O_staged = O_staged;
     s.threshold = d->temperature_threshold; s.reward_scale = d->reward_scale; s.seed = h->search.seed;
     s.opponent = opponent; s.muzero_player = muzero_player;
     s.id_stride = d->game_id_stride > 0 ? d->game_id_stride : B;
@@ -975,7 +993,7 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
               sp_alloc(sp, &s.to_play, B) && sp_alloc(sp, &s.game_id, B) && sp_alloc(sp, &s.move, B) &&
               sp_alloc(sp, &s.visits, (size_t)B * A) && sp_alloc(sp, &s.root_value, B) && sp_alloc(sp, &s.rec_root, B * T) &&
               sp_alloc(sp, &s.rec_visits, B * T * A) && sp_alloc(sp, &s.rec_action, B * T) && sp_alloc(sp, &s.rec_reward, B * T) &&
-              sp_alloc(sp, &s.rec_to_play, B * T) && sp_alloc(sp, &s.rec_obs, B * (T + 1) * O) && sp_alloc(sp, &s.first_to_play, B) &&
+              sp_alloc(sp, &s.rec_to_play, B * T) && sp_alloc(sp, &s.rec_obs, B * (size_t)rows * O) && sp_alloc(sp, &s.first_to_play, B) &&
               sp_alloc(sp, &s.fin, B) && sp_alloc(sp, &s.last_action, B) && sp_alloc(sp, &s.counters, 8) &&
               sp_alloc(sp, &sp->d_forced, B) && sp_alloc(sp, &sp->d_uniform, B) && sp_alloc(sp, &sp->d_noise, (size_t)B * A) &&
               sp_alloc(sp, &sp->d_first, B) && sp_alloc(sp, &s.host_action, B);
@@ -996,15 +1014,15 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
     // within [16, 64] MiB;
     // whatever the size, games that do not fit wait in their slots (parked) - nothing is dropped
     unsigned long long cap = d->staging_bytes;
-    const unsigned long long worst = staged_block_bytes(d->max_moves, A, O) * (unsigned long long)B;
+    const unsigned long long game_bytes = staged_block_bytes(d->max_moves, A, O_staged);
     if (cap == 0) {
-        cap = 4 * worst;
+        cap = 4 * game_bytes * (unsigned long long)B;
         if (cap < (16ull << 20)) cap = 16ull << 20;
         if (cap > (64ull << 20)) cap = 64ull << 20;
-        if (cap < staged_block_bytes(d->max_moves, A, O)) cap = staged_block_bytes(d->max_moves, A, O);
+        if (cap < game_bytes) cap = game_bytes;
     }
-    if (cap < staged_block_bytes(d->max_moves, A, O)) { mz_selfplay_destroy(h); return fail(h, MZ_EINVAL, "mz_selfplay_begin: staging_bytes smaller than one game"); }
-    const unsigned long long index_entries = cap / staged_block_bytes(1, A, O) + 1;
+    if (cap < game_bytes) { mz_selfplay_destroy(h); return fail(h, MZ_EINVAL, "mz_selfplay_begin: staging_bytes smaller than one game"); }
+    const unsigned long long index_entries = cap / staged_block_bytes(1, A, O_staged) + 1;
     bool pinned = cudaHostAlloc(reinterpret_cast<void**>(&sp->h_counters), 64, cudaHostAllocDefault) == cudaSuccess;
     for (int i = 0; i < 2 && pinned; ++i)
         pinned = cudaHostAlloc(reinterpret_cast<void**>(&sp->staging[i]), cap, cudaHostAllocMapped) == cudaSuccess &&

@@ -562,11 +562,19 @@ class HostEnvSelfPlayLoop(DeviceSelfPlayLoop):
     >= 0] -> ``observe`` -> [reset the environments of the slots it reports finished] -> ``restart``; ``drain`` and
     ``peek`` are the device loop's.  Rows are ``[max_games, ...]`` arrays (or sequences of per-game arrays)."""
 
+    OBS_HISTORIES = ("device", "host")
+
     def __init__(self, engine: SearchEngine, obs_shape, max_moves: int, obs, legal_mask, to_play,
                  temperature_threshold=None, first_game_id: int = 0, staging_bytes: int = 0, game_id_stride: int = 0,
-                 td_steps: int = 0, per_alpha: float = 1.0, discount: float = 1.0, stacked_observations: int = 0):
+                 td_steps: int = 0, per_alpha: float = 1.0, discount: float = 1.0, stacked_observations: int = 0,
+                 obs_history: str = "device"):
         """``obs_shape`` is the environment's (C, H, W); ``obs``, ``legal_mask`` and ``to_play`` the first rows of the
-        games ``first_game_id + g``."""
+        games ``first_game_id + g``.  ``obs_history`` says who keeps each game's observations: "device" (the staged
+        blocks carry them, mz_selfplay_begin_host) or "host" (the device keeps the last stacked_observations + 1 per
+        slot, mz_selfplay_begin_host_window, and this object keeps a float32 copy of every row it passes on for the
+        game in flight; ``drain`` hands them over with the blocks)."""
+        if obs_history not in self.OBS_HISTORIES:
+            raise ValueError(f"obs_history must be one of {self.OBS_HISTORIES}, got {obs_history!r}")
         self.engine = engine
         self.opponent, self.muzero_player = "self", 0
         B = engine.max_games
@@ -575,11 +583,19 @@ class HostEnvSelfPlayLoop(DeviceSelfPlayLoop):
                        td_steps, per_alpha, discount, stacked_observations)
         e = _lib.MzHostEnvDesc(*(int(x) for x in obs_shape))
         o, lg, tp = self._rows(obs, legal_mask, to_play)
-        engine._check(engine.lib.mz_selfplay_begin_host(engine._h, C.byref(d), C.byref(e), o.ctypes.data, lg.ctypes.data,
-                                                        tp.ctypes.data))
+        begin = engine.lib.mz_selfplay_begin_host if obs_history == "device" else engine.lib.mz_selfplay_begin_host_window
+        engine._check(begin(engine._h, C.byref(d), C.byref(e), o.ctypes.data, lg.ctypes.data, tp.ctypes.data))
+        self.obs_history = obs_history
         self.stats = _lib.MzSelfPlayStats()
         self.actions = numpy.empty(B, numpy.int32)
         self.finished = numpy.empty(B, numpy.uint8)
+        if obs_history == "host":
+            # per slot: its game's id (the library's: first + g, then + stride per restart) and rows so far; the rows of
+            # games observe reported finished wait here, by game id, for the drain that returns their blocks
+            self._game_id = [int(first_game_id) + g for g in range(B)]
+            self._stride = int(game_id_stride) if int(game_id_stride) > 0 else B
+            self._rows_of = [[o[g].copy()] for g in range(B)]
+            self._finished_rows = {}
 
     def _rows(self, obs, legal_mask, to_play):
         B = self.engine.max_games
@@ -609,7 +625,14 @@ class HostEnvSelfPlayLoop(DeviceSelfPlayLoop):
         dn = numpy.ascontiguousarray(numpy.asarray(done).astype(numpy.uint8).reshape(-1))
         eng._check(eng.lib.mz_selfplay_host_observe(eng._h, o.ctypes.data, r.ctypes.data, dn.ctypes.data, lg.ctypes.data,
                                                    tp.ctypes.data, self.finished.ctypes.data, C.byref(self.stats)))
-        return self.finished.astype(bool)
+        finished = self.finished.astype(bool)
+        if self.obs_history == "host":
+            for g in numpy.nonzero(self.actions >= 0)[0]:        # a parked slot's row is not its game's
+                self._rows_of[g].append(o[g].copy())
+            for g in numpy.nonzero(finished)[0]:
+                self._finished_rows[self._game_id[g]] = numpy.stack(self._rows_of[g])
+                self._rows_of[g] = None
+        return finished
 
     def restart(self, which, obs, legal_mask, to_play):
         """The first rows of the next games of the slots of ``which`` (the mask ``observe`` returned, or part of it)."""
@@ -617,6 +640,19 @@ class HostEnvSelfPlayLoop(DeviceSelfPlayLoop):
         w = numpy.ascontiguousarray(numpy.asarray(which).astype(numpy.uint8).reshape(-1))
         o, lg, tp = self._rows(obs, legal_mask, to_play)
         eng._check(eng.lib.mz_selfplay_host_restart(eng._h, w.ctypes.data, o.ctypes.data, lg.ctypes.data, tp.ctypes.data))
+        if self.obs_history == "host":
+            for g in numpy.nonzero(w)[0]:
+                self._game_id[g] += self._stride
+                self._rows_of[g] = [o[g].copy()]
+
+    def drain(self):
+        """(bytes, index) of the staged finished games, as ``DeviceSelfPlayLoop.drain``; with ``obs_history="host"``
+        also ``{game id: [T + 1, O] float32}``, the observations of those games (their blocks carry none)."""
+        buf, index = super().drain()
+        if self.obs_history == "device":
+            return buf, index
+        ids = [int(numpy.frombuffer(buf, numpy.int64, 1, int(off))[0]) for off in index[:, 0]]
+        return buf, index, {gid: self._finished_rows.pop(gid) for gid in ids}
 
 
 def parse_staged_game(buf: bytes, off: int):

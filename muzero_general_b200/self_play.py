@@ -26,6 +26,7 @@ from collections import deque
 
 import numpy
 
+from . import _lib
 from .engine import DeviceSelfPlayLoop, HostEnvSelfPlayLoop, SearchEngine, parse_staged_game
 
 
@@ -846,7 +847,9 @@ class DeviceHostEnvSelfPlay:
     device) -> step the environments of the slots with an action -> ``observe`` (records, stacking, priorities, packing)
     -> reset the environments of the games it packed -> ``restart``.  Slot g plays the global games ``first_game_id + g
     + k * stride`` with the Philox draws of the device loop, so a game's history is the device loop's wherever both
-    can play it."""
+    can play it.  The device keeps each game's observations when they fit in its memory; otherwise (games/atari.py's
+    27000 moves of 96 x 96 frames) it keeps the stack's window and the host keeps the games' observations, as the
+    reference's ``GameHistory`` does."""
 
     DRAIN_FILL = 0.5        # drain when the staging area is fuller than this, or holds parked games
 
@@ -861,13 +864,18 @@ class DeviceHostEnvSelfPlay:
         self.reward_type = int if vec is not None else float
         priorities = getattr(cfg, "PER", False) and getattr(cfg, "device_priorities", True)
         obs = self.env.reset()
-        self.loop = HostEnvSelfPlayLoop(worker.model.engine, self.obs_shape, cfg.max_moves, obs, self.env.legal_mask(),
-                                        self.env.to_play(), temperature_threshold=temperature_threshold,
-                                        first_game_id=worker.first_game_id, game_id_stride=worker.game_id_stride,
-                                        td_steps=int(cfg.td_steps) if priorities else 0, per_alpha=cfg.PER_alpha,
-                                        discount=cfg.discount,
-                                        staging_bytes=int(getattr(cfg, "selfplay_staging_bytes", 0) or 0),
-                                        stacked_observations=int(cfg.stacked_observations))
+        args = (worker.model.engine, self.obs_shape, cfg.max_moves, obs, self.env.legal_mask(), self.env.to_play())
+        kw = dict(temperature_threshold=temperature_threshold, first_game_id=worker.first_game_id,
+                  game_id_stride=worker.game_id_stride, td_steps=int(cfg.td_steps) if priorities else 0,
+                  per_alpha=cfg.PER_alpha, discount=cfg.discount,
+                  staging_bytes=int(getattr(cfg, "selfplay_staging_bytes", 0) or 0),
+                  stacked_observations=int(cfg.stacked_observations))
+        try:
+            self.loop = HostEnvSelfPlayLoop(*args, obs_history="device", **kw)
+        except _lib.MzError as e:
+            if e.code != _lib.MZ_ENOMEM:
+                raise
+            self.loop = HostEnvSelfPlayLoop(*args, obs_history="host", **kw)
         self.device_s = 0.0       # host clock in the library calls (they end in a device synchronisation), so far
         self.env_s = 0.0          # host clock in the environments' step / reset / legal_mask / to_play, so far
         self.parked_events = 0    # finished games that had to wait for a drain (staging area full), so far
@@ -923,14 +931,19 @@ class PackedGames:
     def __init__(self, obs_shape, obs_dtype, reward_type, with_priorities=False):
         self._args = (obs_shape, obs_dtype, reward_type, with_priorities)
         self._chunks = []            # (bytes, index[n, 2])
+        self._obs = {}               # game id -> [T + 1, O] float32, for blocks without observations (obs_elems = 0)
         self._n = 0
         self.total_moves = 0
 
-    def add(self, buf, index):
+    def add(self, buf, index, obs=None):
+        """One drain's games; ``obs`` the host-kept observations of its games (``HostEnvSelfPlayLoop`` with
+        ``obs_history="host"``) by game id."""
         if len(index):
             self._chunks.append((buf, index))
             self._n += len(index)
             self.total_moves += int((index[:, 1] & numpy.uint64(0xFFFFFFFF)).sum())
+        if obs:
+            self._obs.update(obs)
 
     def __len__(self):
         return self._n
@@ -944,7 +957,10 @@ class PackedGames:
             if self._chunks else numpy.zeros(0, numpy.int64)
 
     def _make(self, buf, off):
-        return PackedGameHistory(parse_staged_game(buf, int(off)), *self._args)
+        g = parse_staged_game(buf, int(off))
+        if g["obs"].shape[1] == 0:          # the host kept this game's observations
+            g["obs"] = self._obs[g["game_id"]]
+        return PackedGameHistory(g, *self._args)
 
     def __iter__(self):
         for buf, index in self._chunks:
