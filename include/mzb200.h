@@ -543,7 +543,7 @@ typedef struct MzSelfPlayPeek {
  *   float priority[T] (zeros unless td_steps > 0); float observation[T+1][O] (index 0 = reset observation); padding to 8.
  * Loops begun with mz_selfplay_begin_host_window stage O = 0 and no observations: the caller kept them.
  * = the fields of GameHistory (self_play.py:479-511) minus the dummy first entries.
- * In test-mode games (mz_selfplay_begin_vs with an opponent) a move the opponent played has root_value NaN and all
+ * In test-mode games (mz_selfplay_begin_vs or mz_selfplay_begin_host_vs with an opponent) a move the opponent played has root_value NaN and all
  * visit counts 0 (store_search_statistics(None), self_play.py:496-511: root_values holds None there and child_visits
  * has no row); its action, reward, to_play and observation are recorded like MuZero's. */
 #define MZ_STAGED_HEADER_BYTES 32
@@ -603,8 +603,9 @@ typedef struct MzHostEnvDesc {
 /* Starts games first_game_id + g from the caller's first rows (obs [n][C*H*W], legal [n][A], to_play [n]).  Refused
  * with MZ_EINVAL: desc->env other than MZ_ENV_HOST, an observation that with stacked_observations does not give the
  * handle's obs_elems, a row without a legal action, a to_play outside the players (mz_selfplay_begin_vs refuses
- * MZ_ENV_HOST with an opponent other than MZ_OPPONENT_SELF: test-mode games need a device environment).  MZ_ENOMEM, with
- * the bytes per slot, when the records ([max_games][max_moves + 1] observations) do not fit on the device. */
+ * MZ_ENV_HOST with an opponent other than MZ_OPPONENT_SELF: test-mode games of host-stepped games begin with
+ * mz_selfplay_begin_host_vs).  MZ_ENOMEM, with the bytes per slot, when the records ([max_games][max_moves + 1]
+ * observations) do not fit on the device. */
 int mz_selfplay_begin_host(MzHandle* h, const MzSelfPlayDesc* desc, const MzHostEnvDesc* env, const float* obs,
                            const uint8_t* legal, const int32_t* to_play);
 /* mz_selfplay_begin_host, but the caller keeps each game's observations: the device holds a window of the last
@@ -619,6 +620,32 @@ int mz_selfplay_host_observe(MzHandle* h, const float* obs, const float* reward,
                              const int32_t* to_play, uint8_t* finished, MzSelfPlayStats* stats);
 int mz_selfplay_host_restart(MzHandle* h, const uint8_t* which, const float* obs, const uint8_t* legal,
                              const int32_t* to_play);
+
+/* Test-mode games of host-stepped games: play_game(temperature, threshold, False, opponent, muzero_player) as
+ * mz_selfplay_begin_vs plays them, with the opponent's moves stepped by the caller.  window = 0 begins like
+ * mz_selfplay_begin_host, 1 like mz_selfplay_begin_host_window; with MZ_OPPONENT_SELF and muzero_player 0 the call IS
+ * that entry point.  Refused: those entry points' refusals and mz_selfplay_begin_vs's (an unknown opponent:
+ * MZ_EUNSUPPORTED; muzero_player outside {0, 1}, td_steps > 0 with an opponent: MZ_EINVAL), an opponent on a handle of
+ * one player and window outside {0, 1} (MZ_EINVAL).
+ * With an opponent, every begin, observe and restart is followed by the opponent phase, repeated while moves are due:
+ *   mz_selfplay_host_opponent_turn  defaults [n] receives, for every slot whose game is in play and whose to_play is not
+ *                                   muzero_player, the random default of MZ_OPPONENT_RANDOM (the same Philox draw as
+ *                                   the device opponent's, on the slot's published legal mask), -1 for the others.
+ *                                   Returns the number of such slots; 0 ends the phase and MuZero moves next
+ *   mz_selfplay_host_opponent_act   the opponent's move of every such slot: actions[g] (the caller's EXPERT, which may
+ *                                   fall back to the default), or the default when actions is NULL (the RANDOM
+ *                                   opponent).  played [n] receives the moves, -1 for a slot without one; the move is
+ *                                   recorded with root_value NaN and zero visit counts and counts in env_steps
+ *   [the caller steps the environments of the slots with played >= 0]
+ *   mz_selfplay_host_observe        as above; it may finish games, reported and restarted as usual
+ * max_moves counts both sides' moves.  mz_selfplay_host_act answers MZ_ESTATE until a turn returned 0, and so do the
+ * opponent calls out of this order or on a loop without an opponent.  MZ_EINVAL: NULL actions with the EXPERT opponent,
+ * an action that is not legal in its slot's published mask (nothing is recorded; the call can be made again). */
+int mz_selfplay_begin_host_vs(MzHandle* h, const MzSelfPlayDesc* desc, const MzHostEnvDesc* env, int32_t opponent,
+                              int32_t muzero_player, int32_t window, const float* obs, const uint8_t* legal,
+                              const int32_t* to_play);
+int mz_selfplay_host_opponent_turn(MzHandle* h, int32_t* defaults);
+int mz_selfplay_host_opponent_act(MzHandle* h, const int32_t* actions, int32_t* played);
 
 /* Debug / parity: the device opponent (MZ_OPPONENT_EXPERT or MZ_OPPONENT_RANDOM) of env (MZ_ENV_TICTACTOE,
  * MZ_ENV_CONNECT4, or MZ_ENV_GOMOKU with MZ_OPPONENT_RANDOM only, on its default 11 x 11 board: this call has no handle

@@ -168,6 +168,10 @@ SYMBOLS = [
     ("mz_selfplay_host_act", C.c_int, [C.c_void_p, C.c_double, C.POINTER(MzSelfPlayInject), C.c_void_p]),
     ("mz_selfplay_host_observe", C.c_int, [C.c_void_p] + [C.c_void_p] * 6 + [C.POINTER(MzSelfPlayStats)]),
     ("mz_selfplay_host_restart", C.c_int, [C.c_void_p] * 5),
+    ("mz_selfplay_begin_host_vs", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayDesc), C.POINTER(MzHostEnvDesc), C.c_int32,
+                                            C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("mz_selfplay_host_opponent_turn", C.c_int, [C.c_void_p, C.c_void_p]),
+    ("mz_selfplay_host_opponent_act", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     ("mz_debug_opponent_action", C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p]),
     ("mz_debug_small_search_plan", C.c_int, [C.c_int32] * 10 + [C.POINTER(C.c_int64)]),

@@ -45,6 +45,10 @@
 // observe pass tries again; the slot reports "finished" (its environment is reset, then restarted) once it is packed.
 // mz_selfplay_begin_host_window: the caller keeps each game's observations.  rec_obs then holds a window of stack + 1
 // rows per slot (observation p in row p % rows: all stack_fill reads) and the staged blocks carry none (O_staged = 0).
+// Their test-mode games (mz_selfplay_begin_host_vs): after begin, observe and restart, the slots whose side to move is
+// the opponent's play the opponent's move as a move of its own: opponent_turn (host_opponent_turn_kernel, the random
+// default of opponent_move's draw) -> opponent_act (host_opponent_act_kernel: the host's or the default move, recorded
+// with a NaN root and no visits) -> the host's step -> observe, which completes it as it completes MuZero's.
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -707,7 +711,7 @@ __global__ void __launch_bounds__(kActThreads) host_act_kernel(const SpDev s) {
     bool playing = false;
     if (g < s.B) {
         int action = -1;
-        if (s.fin[g] == 0) {
+        if (s.fin[g] == 0 && (s.opponent == MZ_OPPONENT_SELF || s.to_play[g] == s.muzero_player)) {
             const int t = s.move[g];
             action = choose_action<kMaxA>(s, g, t);
             record_search(s, g, t, action, s.root_value[g], s.visits + (size_t)g * s.A);
@@ -778,6 +782,51 @@ __global__ void host_start_kernel(const SpDev s, const HostRows h, const uint8_t
     if (s.stack) stack_fill(s, g, tid, nt);
 }
 
+// Test-mode games of host-stepped environments (mz_selfplay_begin_host_vs): the opponent's move is a move of its own,
+// stepped by the host between opponent_act and observe like MuZero's.  A slot's opponent move is due when its game is
+// in play and the side to move is not MuZero's.
+MZ_DEVINL bool opponent_due(const SpDev& s, int g) {
+    return s.opponent != MZ_OPPONENT_SELF && s.fin[g] == 0 && s.to_play[g] != s.muzero_player;
+}
+
+// one thread per slot: the random default of every slot whose opponent move is due (opponent_move's draw on the
+// published legal mask), -1 for the others
+__global__ void __launch_bounds__(kActThreads) host_opponent_turn_kernel(const SpDev s, int32_t* defaults) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= s.B) return;
+    int d = -1;
+    if (opponent_due(s, g)) {
+        const double u = philox_uniform53(s.seed, s.game_id[g], s.move[g], 0u, kTagOpponent);
+        d = uniform_legal_pick(s.legal + (size_t)g * s.A, s.A, u);
+    }
+    defaults[g] = d;
+}
+
+// One thread per slot; `defaults` is the turn's (>= 0: the slot's opponent move is due), the move actions[g] or, when
+// actions is nullptr, the default.  kCheck: count the due slots whose move is not legal in counters[6].  Otherwise, and
+// only when that count is 0: record the move as opponent_move does (root NaN, no visit row), hand it to the host's step
+// in host_action (-1 for the slots without one) and count it in env_steps.
+template <bool kCheck>
+__global__ void __launch_bounds__(kActThreads) host_opponent_act_kernel(const SpDev s, const int32_t* defaults,
+                                                                        const int32_t* actions) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    bool moved = false;
+    if (g < s.B) {
+        const int d = defaults[g];
+        const int a = d >= 0 && actions ? actions[g] : d;
+        if (kCheck) {
+            if (d >= 0 && (a < 0 || a >= s.A || !s.legal[(size_t)g * s.A + a])) atomicAdd(&s.counters[6], 1ull);
+        } else if (s.counters[6] == 0) {
+            if (d >= 0) record_search(s, g, s.move[g], a, __longlong_as_double(0x7FF8000000000000ll), nullptr);
+            s.host_action[g] = a;
+            moved = d >= 0;
+        }
+    }
+    if (kCheck) return;
+    const unsigned n = __popc(__ballot_sync(0xffffffffu, moved));
+    if ((threadIdx.x & 31) == 0 && n) atomicAdd(&s.counters[0], (unsigned long long)n);
+}
+
 }  // namespace mz
 
 using namespace mz;
@@ -811,6 +860,11 @@ struct MzSelfPlay {
     uint8_t* d_which = nullptr;
     uint8_t* d_finished = nullptr;
     float act_ms = 0.0f;
+    // MZ_ENV_HOST test-mode games: 1 = begin, observe or restart ran and mz_selfplay_host_opponent_turn must look for
+    // due opponent moves, 2 = it found some and they wait for mz_selfplay_host_opponent_act, 0 = MuZero moves next
+    int opp_phase = 0;
+    int32_t* d_defaults = nullptr;             // [B] the turn's random defaults, -1 for a slot without an opponent move
+    int32_t* d_opp_actions = nullptr;          // [B] the host's opponent moves
 };
 
 void mz_selfplay_destroy(MzHandle* h) {
@@ -881,6 +935,18 @@ extern "C" int mz_selfplay_begin_host_window(MzHandle* h, const MzSelfPlayDesc* 
     return sp_begin(h, d, MZ_OPPONENT_SELF, 0, e, obs, legal, to_play, true);
 }
 
+extern "C" int mz_selfplay_begin_host_vs(MzHandle* h, const MzSelfPlayDesc* d, const MzHostEnvDesc* e, int32_t opponent,
+                                         int32_t muzero_player, int32_t window, const float* obs, const uint8_t* legal,
+                                         const int32_t* to_play) {
+    if (window != 0 && window != 1)
+        return fail(h, MZ_EINVAL, "mz_selfplay_begin_host_vs: window must be 0 or 1, got " + std::to_string(window));
+    if (opponent == MZ_OPPONENT_SELF && muzero_player == 0)
+        return (window ? mz_selfplay_begin_host_window : mz_selfplay_begin_host)(h, d, e, obs, legal, to_play);
+    if (!h || !d || !e || !obs || !legal || !to_play) return fail(h, MZ_EINVAL, "mz_selfplay_begin_host_vs: null argument");
+    if (d->env != MZ_ENV_HOST) return fail(h, MZ_EINVAL, "mz_selfplay_begin_host_vs: desc->env must be MZ_ENV_HOST");
+    return sp_begin(h, d, opponent, muzero_player, e, obs, legal, to_play, window == 1);
+}
+
 // window: rec_obs keeps the last stacked_observations + 1 observations of a slot's game and the staged blocks none
 // (mz_selfplay_begin_host_window); otherwise the whole game's
 static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int32_t muzero_player, const MzHostEnvDesc* e,
@@ -888,9 +954,11 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
     if (!h || !d) return fail(h, MZ_EINVAL, "mz_selfplay_begin: null argument");
     if (opponent != MZ_OPPONENT_SELF && opponent != MZ_OPPONENT_EXPERT && opponent != MZ_OPPONENT_RANDOM)
         return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin_vs: unknown opponent " + std::to_string(opponent));
-    if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_HOST)
+    if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_HOST && !e)
         return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: host-stepped games play against themselves only (test-mode games "
-                                  "against an opponent need a device environment)");
+                                  "of host-stepped games begin with mz_selfplay_begin_host_vs)");
+    if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_HOST && h->search.num_players < 2)
+        return fail(h, MZ_EINVAL, "mz_selfplay_begin_host_vs: the handle's game has one player, its opponent is \"self\"");
     if (muzero_player != 0 && muzero_player != 1)
         return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: muzero_player must be 0 or 1, got " + std::to_string(muzero_player));
     if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_CARTPOLE)
@@ -1003,9 +1071,10 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
         int32_t* r_to_play = nullptr;
         ok = sp_alloc(sp, &r_obs, (size_t)B * O) && sp_alloc(sp, &r_reward, B) && sp_alloc(sp, &r_done, B) &&
              sp_alloc(sp, &r_legal, (size_t)B * A) && sp_alloc(sp, &r_to_play, B) && sp_alloc(sp, &sp->d_which, B) &&
-             sp_alloc(sp, &sp->d_finished, B);
+             sp_alloc(sp, &sp->d_finished, B) && sp_alloc(sp, &sp->d_defaults, B) && sp_alloc(sp, &sp->d_opp_actions, B);
         sp->rows = HostRows{r_obs, r_reward, r_done, r_legal, r_to_play};
         sp->host = true;
+        sp->opp_phase = opponent != MZ_OPPONENT_SELF;
         sp->actions.assign(B, -1);
         sp->awaiting.assign(B, 0);
     }
@@ -1195,6 +1264,10 @@ extern "C" int mz_selfplay_host_act(MzHandle* h, double temperature, const MzSel
     if (sp->n_awaiting)
         return fail(h, MZ_ESTATE, std::string(who) + ": " + std::to_string(sp->n_awaiting) +
                                   " finished slots wait for mz_selfplay_host_restart");
+    if (sp->opp_phase == 1)
+        return fail(h, MZ_ESTATE, std::string(who) + ": opponent moves may be due, call mz_selfplay_host_opponent_turn first");
+    if (sp->opp_phase == 2)
+        return fail(h, MZ_ESTATE, std::string(who) + ": opponent moves are due, call mz_selfplay_host_opponent_act first");
     const int B = sp->dev.B;
     if (inj && inj->uniform)
         for (int g = 0; g < B; ++g)
@@ -1267,6 +1340,7 @@ extern "C" int mz_selfplay_host_observe(MzHandle* h, const float* obs, const flo
     for (int g = 0; g < B; ++g)
         if (finished[g]) { sp->awaiting[g] = 1; ++sp->n_awaiting; }
     sp->observe_due = false;
+    sp->opp_phase = sp->dev.opponent != MZ_OPPONENT_SELF;
     return MZ_OK;
 }
 
@@ -1297,6 +1371,77 @@ extern "C" int mz_selfplay_host_restart(MzHandle* h, const uint8_t* which, const
     MZ_CUDA(h, cudaStreamSynchronize(h->stream));
     for (int g = 0; g < B; ++g)
         if (which[g]) { sp->awaiting[g] = 0; --sp->n_awaiting; }
+    sp->opp_phase = sp->dev.opponent != MZ_OPPONENT_SELF;
+    return MZ_OK;
+}
+
+// the opponent calls of a loop begun with mz_selfplay_begin_host_vs: MZ_ESTATE unless the loop has an opponent and is
+// in the call's `phase` (opp_phase)
+static int host_opponent_loop(MzHandle* h, const char* who, int phase) {
+    int rc = host_loop(h, who);
+    if (rc) return rc;
+    MzSelfPlay* sp = h->sp;
+    if (sp->dev.opponent == MZ_OPPONENT_SELF)
+        return fail(h, MZ_ESTATE, std::string(who) + ": the loop plays against itself (begin it with mz_selfplay_begin_host_vs "
+                                  "and an opponent)");
+    if (sp->observe_due) return fail(h, MZ_ESTATE, std::string(who) + ": the last move waits for mz_selfplay_host_observe");
+    if (sp->n_awaiting)
+        return fail(h, MZ_ESTATE, std::string(who) + ": " + std::to_string(sp->n_awaiting) +
+                                  " finished slots wait for mz_selfplay_host_restart");
+    if (sp->opp_phase != phase)
+        return fail(h, MZ_ESTATE, std::string(who) + (sp->opp_phase == 0 ? ": no opponent move is due, MuZero moves next (mz_selfplay_host_act)"
+                                                      : sp->opp_phase == 1 ? ": call mz_selfplay_host_opponent_turn first"
+                                                                           : ": opponent moves are due, call mz_selfplay_host_opponent_act"));
+    MZ_CUDA(h, cudaSetDevice(h->device));
+    return MZ_OK;
+}
+
+extern "C" int mz_selfplay_host_opponent_turn(MzHandle* h, int32_t* defaults) {
+    const char* who = "mz_selfplay_host_opponent_turn";
+    int rc = host_opponent_loop(h, who, 1);
+    if (rc) return rc;
+    if (!defaults) return fail(h, MZ_EINVAL, std::string(who) + ": null defaults");
+    MzSelfPlay* sp = h->sp;
+    const int B = sp->dev.B;
+    host_opponent_turn_kernel<<<(B + kActThreads - 1) / kActThreads, kActThreads, 0, h->stream>>>(sp->dev, sp->d_defaults);
+    h->launches += 1;
+    MZ_CUDA(h, cudaGetLastError());
+    MZ_CUDA(h, cudaMemcpyAsync(defaults, sp->d_defaults, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));
+    MZ_CUDA(h, cudaStreamSynchronize(h->stream));
+    int due = 0;
+    for (int g = 0; g < B; ++g) due += defaults[g] >= 0;
+    sp->opp_phase = due ? 2 : 0;
+    return due;
+}
+
+extern "C" int mz_selfplay_host_opponent_act(MzHandle* h, const int32_t* actions, int32_t* played) {
+    const char* who = "mz_selfplay_host_opponent_act";
+    int rc = host_opponent_loop(h, who, 2);
+    if (rc) return rc;
+    MzSelfPlay* sp = h->sp;
+    if (!played) return fail(h, MZ_EINVAL, std::string(who) + ": null played");
+    if (!actions && sp->dev.opponent == MZ_OPPONENT_EXPERT)
+        return fail(h, MZ_EINVAL, std::string(who) + ": the EXPERT opponent's moves come from the host, actions is null");
+    const int B = sp->dev.B;
+    const SpDev& s = sp->dev;
+    const int grid = (B + kActThreads - 1) / kActThreads;
+    if (actions) MZ_CUDA(h, cudaMemcpyAsync(sp->d_opp_actions, actions, (size_t)B * 4, cudaMemcpyHostToDevice, h->stream));
+    const int32_t* d_actions = actions ? sp->d_opp_actions : nullptr;
+    MZ_CUDA(h, cudaMemsetAsync(s.counters + 6, 0, 8, h->stream));
+    host_opponent_act_kernel<true><<<grid, kActThreads, 0, h->stream>>>(s, sp->d_defaults, d_actions);
+    host_opponent_act_kernel<false><<<grid, kActThreads, 0, h->stream>>>(s, sp->d_defaults, d_actions);
+    h->launches += 2;
+    MZ_CUDA(h, cudaGetLastError());
+    MZ_CUDA(h, cudaMemcpyAsync(sp->h_counters + 6, s.counters + 6, 8, cudaMemcpyDeviceToHost, h->stream));
+    MZ_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (sp->h_counters[6])                         // nothing was recorded: the opponent's moves can be given again
+        return fail(h, MZ_EINVAL, std::string(who) + ": " + std::to_string(sp->h_counters[6]) +
+                                  " opponent moves are not legal in their slot's published mask");
+    MZ_CUDA(h, cudaMemcpy(sp->actions.data(), s.host_action, (size_t)B * 4, cudaMemcpyDeviceToHost));
+    memcpy(played, sp->actions.data(), (size_t)B * 4);
+    sp->act_ms = 0.0f;
+    sp->opp_phase = 0;
+    sp->observe_due = true;
     return MZ_OK;
 }
 

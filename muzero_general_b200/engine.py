@@ -567,28 +567,41 @@ class HostEnvSelfPlayLoop(DeviceSelfPlayLoop):
     def __init__(self, engine: SearchEngine, obs_shape, max_moves: int, obs, legal_mask, to_play,
                  temperature_threshold=None, first_game_id: int = 0, staging_bytes: int = 0, game_id_stride: int = 0,
                  td_steps: int = 0, per_alpha: float = 1.0, discount: float = 1.0, stacked_observations: int = 0,
-                 obs_history: str = "device"):
+                 obs_history: str = "device", opponent: str = "self", muzero_player: int = 0):
         """``obs_shape`` is the environment's (C, H, W); ``obs``, ``legal_mask`` and ``to_play`` the first rows of the
         games ``first_game_id + g``.  ``obs_history`` says who keeps each game's observations: "device" (the staged
         blocks carry them, mz_selfplay_begin_host) or "host" (the device keeps the last stacked_observations + 1 per
         slot, mz_selfplay_begin_host_window, and this object keeps a float32 copy of every row it passes on for the
-        game in flight; ``drain`` hands them over with the blocks)."""
+        game in flight; ``drain`` hands them over with the blocks).  ``opponent`` "expert" or "random" plays test-mode
+        games (mz_selfplay_begin_host_vs): after begin, ``observe`` and ``restart``, run the opponent phase
+        (``opponent_turn`` / ``opponent_act`` / [step] / ``observe``) until ``opponent_turn`` returns None."""
         if obs_history not in self.OBS_HISTORIES:
             raise ValueError(f"obs_history must be one of {self.OBS_HISTORIES}, got {obs_history!r}")
+        if opponent not in self.OPPONENTS:
+            raise NotImplementedError(f"no device opponent {opponent!r} (expected one of {sorted(self.OPPONENTS)})")
         self.engine = engine
-        self.opponent, self.muzero_player = "self", 0
+        self.opponent, self.muzero_player = opponent, int(muzero_player)
         B = engine.max_games
         self.O = int(numpy.prod(obs_shape))
         d = self._desc(_lib.MZ_ENV_HOST, max_moves, temperature_threshold, 0, first_game_id, staging_bytes, game_id_stride,
                        td_steps, per_alpha, discount, stacked_observations)
         e = _lib.MzHostEnvDesc(*(int(x) for x in obs_shape))
         o, lg, tp = self._rows(obs, legal_mask, to_play)
-        begin = engine.lib.mz_selfplay_begin_host if obs_history == "device" else engine.lib.mz_selfplay_begin_host_window
-        engine._check(begin(engine._h, C.byref(d), C.byref(e), o.ctypes.data, lg.ctypes.data, tp.ctypes.data))
+        if opponent == "self" and self.muzero_player == 0:
+            begin = engine.lib.mz_selfplay_begin_host if obs_history == "device" else engine.lib.mz_selfplay_begin_host_window
+            engine._check(begin(engine._h, C.byref(d), C.byref(e), o.ctypes.data, lg.ctypes.data, tp.ctypes.data))
+        else:
+            rc = engine.lib.mz_selfplay_begin_host_vs(engine._h, C.byref(d), C.byref(e), self.OPPONENTS[opponent],
+                                                      self.muzero_player, int(obs_history == "host"), o.ctypes.data,
+                                                      lg.ctypes.data, tp.ctypes.data)
+            if rc == _lib.MZ_EUNSUPPORTED:
+                raise NotImplementedError(engine.lib.mz_last_error(engine._h).decode())
+            engine._check(rc)
         self.obs_history = obs_history
         self.stats = _lib.MzSelfPlayStats()
         self.actions = numpy.empty(B, numpy.int32)
         self.finished = numpy.empty(B, numpy.uint8)
+        self.defaults = numpy.empty(B, numpy.int32)
         if obs_history == "host":
             # per slot: its game's id (the library's: first + g, then + stride per restart) and rows so far; the rows of
             # games observe reported finished wait here, by game id, for the drain that returns their blocks
@@ -613,6 +626,24 @@ class HostEnvSelfPlayLoop(DeviceSelfPlayLoop):
         inj = self._inject(keep, forced_action, uniform, noise, first_index)
         eng._check(eng.lib.mz_selfplay_host_act(eng._h, float(temperature), C.byref(inj) if inj is not None else None,
                                                self.actions.ctypes.data))
+        return self.actions
+
+    def opponent_turn(self):
+        """The random default of every slot whose opponent move is due, -1 for the others: an int32 ``[max_games]``
+        array (reused by the next call), or None when no opponent move is due and MuZero moves next."""
+        eng = self.engine
+        n = eng.lib.mz_selfplay_host_opponent_turn(eng._h, self.defaults.ctypes.data)
+        eng._check(min(n, 0))
+        return self.defaults if n > 0 else None
+
+    def opponent_act(self, actions=None):
+        """The opponent's moves of the slots ``opponent_turn`` found: ``actions`` (an int array ``[max_games]``, read at
+        those slots) or, when None, their random defaults.  Returns the moves as ``act`` does, -1 for the slots without
+        one: step those with a move, then ``observe``."""
+        eng = self.engine
+        a = None if actions is None else numpy.ascontiguousarray(actions, numpy.int32).reshape(-1)
+        eng._check(eng.lib.mz_selfplay_host_opponent_act(eng._h, None if a is None else a.ctypes.data,
+                                                        self.actions.ctypes.data))
         return self.actions
 
     def observe(self, obs, reward, done, legal_mask, to_play):

@@ -7,6 +7,8 @@ player +1 moves first and is ``to_play() == 0``; the mover gets reward 1 on comp
 line, the game also ends when the board is full.  Winning lines are precomputed as index
 tables, so a whole batch is checked with one gather.
 """
+import copy
+
 import numpy
 
 from .abstract_game import VectorGame
@@ -63,7 +65,22 @@ class BoardVector(VectorGame):
             return (top == 0).astype(numpy.uint8)
         return (self.board == 0).astype(numpy.uint8)
 
-    def step(self, actions):
+    def step(self, actions, which=None):
+        """Steps every game, or the games of the bool mask ``which`` (the others keep their state and report reward 0,
+        not done)."""
+        if which is not None:
+            g = numpy.nonzero(which)[0]
+            sub = copy.copy(self)
+            sub.num_games, sub.board, sub.player = len(g), self.board[g], self.player[g]
+            r, d = sub._step_all(numpy.asarray(actions, dtype=numpy.int64)[g])
+            self.board[g], self.player[g] = sub.board, sub.player
+            reward, done = numpy.zeros(self.num_games, r.dtype), numpy.zeros(self.num_games, bool)
+            reward[g], done[g] = r, d
+            return self.observations(), reward, done
+        reward, done = self._step_all(actions)
+        return self.observations(), reward, done
+
+    def _step_all(self, actions):
         actions = numpy.asarray(actions, dtype=numpy.int64)
         g = numpy.arange(self.num_games)
         if self.GRAVITY:
@@ -80,7 +97,21 @@ class BoardVector(VectorGame):
         full = ~(self.legal_mask().any(axis=1))
         reward = numpy.where(won | full if self.REWARD_WHEN_FULL else won, 1, 0) * self.REWARD_SCALE
         self.player = -self.player
-        return self.observations(), reward, won | full
+        return reward, won | full
+
+    @staticmethod
+    def expert_windows(board):
+        """The windows of the game's hard-coded opponent for ``_threat_scan``, in the reference's scan order."""
+        raise NotImplementedError("this game has no expert opponent (the reference's Game has no expert_agent)")
+
+    def expert_actions(self, defaults, which):
+        """``BoardGame.expert_agent`` of the games of the bool mask ``which``, each with the random fallback
+        ``defaults[g]`` in place of its ``numpy.random.choice`` draw; -1 for the others."""
+        out = numpy.full(self.num_games, -1, numpy.int32)
+        boards = self.board.reshape(self.num_games, self.H, self.W)
+        for g in numpy.nonzero(which)[0]:
+            out[g] = _threat_scan(boards[g], int(self.player[g]), self.expert_windows(boards[g]), int(defaults[g]))
+        return out
 
 
 def _threat_scan(board, player, windows, default):
@@ -149,4 +180,4 @@ class BoardGame:
         return _threat_scan(board, player, self._expert_windows(board), default)
 
     def _expert_windows(self, board):
-        raise NotImplementedError
+        return self.VECTOR.expert_windows(board)

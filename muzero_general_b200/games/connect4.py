@@ -30,21 +30,8 @@ class Connect4Vector(BoardVector):
     OBS_DTYPE = numpy.float64
     REWARD_SCALE = 10          # games/connect4.py:144
 
-
-class Game(BoardGame, AbstractGame):
-    DEVICE_ENV = "connect4"        # csrc/selfplay.cu restates these rules on the device
-    VECTOR = Connect4Vector
-
-    def action_to_string(self, action_number):
-        return f"Play column {action_number + 1}"
-
-    def human_to_action(self):
-        choice = input(f"Enter the column to play for the player {self.to_play()}: ")
-        while choice not in [str(action) for action in self.legal_actions()]:
-            choice = input("Enter another column : ")
-        return int(choice)
-
-    def _expert_windows(self, board):
+    @staticmethod
+    def expert_windows(board):
         """Scan order of games/connect4.py:310-346: 4x4 sub-boards (k = 0..2 rows up, l = 0..3 columns right); inside
         one: for i = 0..3 the i-th row then the i-th column, then the diagonal, then the anti-diagonal.  A gap counts
         only when it is the next free cell of its column; the vertical check plays its column unconditionally."""
@@ -64,3 +51,20 @@ class Game(BoardGame, AbstractGame):
                 out.append(([(k + j, l + j) for j in range(4)], 3, ok, None))
                 out.append(([(k + j, l + 3 - j) for j in range(4)], 3, ok, None))
         return out
+
+
+class Game(BoardGame, AbstractGame):
+    DEVICE_ENV = "connect4"        # csrc/selfplay.cu restates these rules on the device
+    VECTOR = Connect4Vector
+
+    def action_to_string(self, action_number):
+        return f"Play column {action_number + 1}"
+
+    def human_to_action(self):
+        choice = input(f"Enter the column to play for the player {self.to_play()}: ")
+        while choice not in [str(action) for action in self.legal_actions()]:
+            choice = input("Enter another column : ")
+        return int(choice)
+
+    def _expert_windows(self, board):
+        return Connect4Vector.expert_windows(board)

@@ -28,15 +28,8 @@ class TicTacToeVector(BoardVector):
     OBS_DTYPE = numpy.int32
     REWARD_SCALE = 20          # games/tictactoe.py:144
 
-
-class Game(BoardGame, AbstractGame):
-    DEVICE_ENV = "tictactoe"        # csrc/selfplay.cu restates these rules on the device
-    VECTOR = TicTacToeVector
-
-    def action_to_string(self, action_number):
-        return f"Play row {action_number // 3 + 1}, column {action_number % 3 + 1}"
-
-    def _expert_windows(self, board):
+    @staticmethod
+    def expert_windows(board):
         """Scan order of games/tictactoe.py:313-347: row i then column i for i = 0..2, diagonal, anti-diagonal."""
         class Any:
             def __call__(self, y, x): return True
@@ -50,6 +43,17 @@ class Game(BoardGame, AbstractGame):
         out.append(([(0, 0), (1, 1), (2, 2)], 2, ok, None))
         out.append(([(0, 2), (1, 1), (2, 0)], 2, ok, None))      # numpy.fliplr(board).diagonal(): index j <-> (j, 2 - j)
         return out
+
+
+class Game(BoardGame, AbstractGame):
+    DEVICE_ENV = "tictactoe"        # csrc/selfplay.cu restates these rules on the device
+    VECTOR = TicTacToeVector
+
+    def action_to_string(self, action_number):
+        return f"Play row {action_number // 3 + 1}, column {action_number % 3 + 1}"
+
+    def _expert_windows(self, board):
+        return TicTacToeVector.expert_windows(board)
 
     def human_to_action(self):
         while True:

@@ -656,8 +656,10 @@ class SelfPlay:
     def play_test_games(self, n_games, opponent=None, muzero_player=None, temperature=0):
         """``n_games`` games of the reference's test worker (self_play.py:54-90), played as one device batch:
         ``play_game(temperature, config.temperature_threshold, False, opponent, muzero_player)`` with the opponent
-        ("expert", "random" or "self") moving on the GPU.  ``opponent`` and ``muzero_player`` default to the config's,
-        like the test worker ("self" for one-player games).  Returns ``(PackedGames, summary)``: the games have the
+        ("expert", "random" or "self") moving on the GPU - or, for a game whose environment the host steps
+        (``loop_path == "device-host-env"``), the opponent's moves stepped on the host like MuZero's, the "expert" from
+        the vector game's ``expert_actions`` or the plug-in's ``expert_agent``.  ``opponent`` and ``muzero_player``
+        default to the config's, like the test worker ("self" for one-player games).  Returns ``(PackedGames, summary)``: the games have the
         reference's test-mode shape (``root_values`` is None at opponent moves, ``child_visits`` has rows for MuZero's
         moves only), and ``summary`` holds the means over the games of what the test worker reports
         (``episode_length``, ``total_reward``, ``mean_value``; ``muzero_reward`` and ``opponent_reward`` for two
@@ -669,11 +671,11 @@ class SelfPlay:
         calls give the same games.  The device loop replaces the handle's self-play loop: with one running, call
         ``reset_stream()`` first."""
         cfg = self.config
-        if self._device_env_name() is None:
+        if self.loop_path == "host":
             raise NotImplementedError(
-                "test games on the device need a device environment (CartPole, TicTacToe, Connect4, Gomoku, Twenty-One "
-                "or Simple Grid with rng_mode='philox' and device_envs on); play them one at a time with "
-                "play_game(0, config.temperature_threshold, False, opponent, muzero_player)")
+                "test games on the device need rng_mode='philox' and a device environment (CartPole, TicTacToe, "
+                "Connect4, Gomoku, Twenty-One or Simple Grid with device_envs on) or config.host_env_device_loop; play "
+                "them one at a time with play_game(0, config.temperature_threshold, False, opponent, muzero_player)")
         if self._device_loop is not None:
             raise RuntimeError("this worker's device self-play loop has games in flight, and starting test games on the "
                                "same handle would drop them; call reset_stream() first")
@@ -687,17 +689,20 @@ class SelfPlay:
         B, stride, first = self.num_parallel_games, self.game_id_stride, self._next_test_game_id
         i = numpy.arange(n_games)
         wanted = first + (i // B) * stride + i % B
-        dev = DeviceBatchedSelfPlay(self, cfg.temperature_threshold, opponent, muzero_player, first_game_id=first)
+        Loop = DeviceBatchedSelfPlay if self.loop_path == "device" else DeviceHostEnvSelfPlay
+        dev = Loop(self, cfg.temperature_threshold, opponent, muzero_player, first_game_id=first)
         games = PackedGames(dev.obs_shape, dev.obs_dtype, dev.reward_type)
         missing = n_games
         while missing:
             # a few moves per call: every move past the last wanted game's end is searched for the whole batch
-            for buf, index in dev.moves(min(dev.chunk, 4), temperature)._chunks:
+            out = dev.moves(min(getattr(dev, "chunk", 4), 4), temperature)
+            for buf, index in out._chunks:
                 ids = numpy.array([int(numpy.frombuffer(buf, numpy.int64, 1, int(off))[0]) for off in index[:, 0]])
                 keep = numpy.isin(ids, wanted)
                 # in game-id order: the games of one drain are staged in the order their warps reserved space, and
                 # the summary's float means must not depend on it
-                games.add(buf, index[keep][numpy.argsort(ids[keep], kind="stable")])
+                games.add(buf, index[keep][numpy.argsort(ids[keep], kind="stable")],
+                          {int(gid): out._obs[int(gid)] for gid in ids[keep] if int(gid) in out._obs})
                 missing -= int(keep.sum())
         # the next call starts past every id this one began
         started = int(dev.loop.peek()["game_id"].max())
@@ -759,6 +764,14 @@ class _ObjectVector:
 
     def to_play(self):
         return numpy.array([game.to_play() for game in self.games], dtype=numpy.int32)
+
+    def expert_actions(self, defaults, which):
+        """``Game.expert_agent()`` of the games of the bool mask ``which``, as the reference's test worker calls it (the
+        plug-in draws its own fallback, so ``defaults`` is not used); -1 for the others."""
+        out = numpy.full(self.num_games, -1, numpy.int32)
+        for g in numpy.nonzero(which)[0]:
+            out[g] = int(self.games[g].expert_agent())
+        return out
 
 
 class DeviceBatchedSelfPlay:
@@ -849,11 +862,16 @@ class DeviceHostEnvSelfPlay:
     + k * stride`` with the Philox draws of the device loop, so a game's history is the device loop's wherever both
     can play it.  The device keeps each game's observations when they fit in its memory; otherwise (games/atari.py's
     27000 moves of 96 x 96 frames) it keeps the stack's window and the host keeps the games' observations, as the
-    reference's ``GameHistory`` does."""
+    reference's ``GameHistory`` does.
+
+    ``opponent`` "expert" or "random" plays test-mode games (``play_game(..., opponent, muzero_player)``): after the
+    begin and after every observe and restart, the slots whose side to move is the opponent's play its move - the
+    library's random default, or for "expert" ``env.expert_actions(defaults, due)`` (``BoardVector``'s threat scan, or
+    ``Game.expert_agent()`` per game for plug-ins without a vector game) - and only those environments are stepped."""
 
     DRAIN_FILL = 0.5        # drain when the staging area is fuller than this, or holds parked games
 
-    def __init__(self, worker, temperature_threshold=None):
+    def __init__(self, worker, temperature_threshold=None, opponent="self", muzero_player=0, first_game_id=None):
         cfg, Game = worker.config, worker.Game
         self.B, self.A = worker.num_parallel_games, len(cfg.action_space)
         self.env = Game.vector(self.B, worker.seed) if hasattr(Game, "vector") else \
@@ -862,14 +880,21 @@ class DeviceHostEnvSelfPlay:
         self.obs_shape = tuple(cfg.observation_shape)
         self.obs_dtype = getattr(vec, "OBS_DTYPE", numpy.float32)
         self.reward_type = int if vec is not None else float
-        priorities = getattr(cfg, "PER", False) and getattr(cfg, "device_priorities", True)
+        if opponent == "expert" and not hasattr(self.env, "expert_actions"):
+            raise NotImplementedError(f"{type(self.env).__name__} has no expert_actions(defaults, which): no expert opponent")
+        self.opponent = opponent
+        # test-mode games never reach a replay buffer (self_play.py:54-66): no priorities against an opponent
+        priorities = opponent == "self" and getattr(cfg, "PER", False) and getattr(cfg, "device_priorities", True)
         obs = self.env.reset()
         args = (worker.model.engine, self.obs_shape, cfg.max_moves, obs, self.env.legal_mask(), self.env.to_play())
-        kw = dict(temperature_threshold=temperature_threshold, first_game_id=worker.first_game_id,
+        kw = dict(temperature_threshold=temperature_threshold,
+                  first_game_id=worker.first_game_id if first_game_id is None else first_game_id,
                   game_id_stride=worker.game_id_stride, td_steps=int(cfg.td_steps) if priorities else 0,
                   per_alpha=cfg.PER_alpha, discount=cfg.discount,
                   staging_bytes=int(getattr(cfg, "selfplay_staging_bytes", 0) or 0),
                   stacked_observations=int(cfg.stacked_observations))
+        if opponent != "self" or muzero_player != 0:
+            kw.update(opponent=opponent, muzero_player=muzero_player)
         try:
             self.loop = HostEnvSelfPlayLoop(*args, obs_history="device", **kw)
         except _lib.MzError as e:
@@ -879,47 +904,72 @@ class DeviceHostEnvSelfPlay:
         self.device_s = 0.0       # host clock in the library calls (they end in a device synchronisation), so far
         self.env_s = 0.0          # host clock in the environments' step / reset / legal_mask / to_play, so far
         self.parked_events = 0    # finished games that had to wait for a drain (staging area full), so far
+        self._staged = PackedGames(self.obs_shape, self.obs_dtype, self.reward_type, self.loop.with_priorities)
+        self._opponent_phase(self._staged)        # the opponent opens the games where it moves first
 
-    def _step(self, actions):
+    def _step(self, actions, only_playing=False):
+        """Steps the environments of the slots with an action >= 0.  ``only_playing``: the others are in a game and must
+        keep their state (the opponent's moves), so a vector game is stepped with ``which`` too."""
         playing = actions >= 0
         actions = actions.astype(numpy.int64)
         if playing.all():
             return self.env.step(actions)
-        if isinstance(self.env, _ObjectVector):
-            return self.env.step(actions, playing)
+        if only_playing or isinstance(self.env, _ObjectVector):
+            return self.env.step(numpy.where(playing, actions, 0), playing)
         # a VectorGame steps all its games: a slot that is not playing (its finished game waits for staging space) takes
         # action 0 and its results are ignored; its environment is reset before its next game
         return self.env.step(numpy.where(playing, actions, 0))
 
     def moves(self, n_moves, temperature, **inject):
-        """``n_moves`` lockstep moves -> ``PackedGames`` of the games that finished (and were packed) meanwhile."""
-        out = PackedGames(self.obs_shape, self.obs_dtype, self.reward_type, self.loop.with_priorities)
-        env, loop = self.env, self.loop
+        """``n_moves`` lockstep moves -> ``PackedGames`` of the games that finished (and were packed) meanwhile.  Against
+        an opponent a move is MuZero's move and the opponent's replies."""
+        out, self._staged = self._staged, PackedGames(self.obs_shape, self.obs_dtype, self.reward_type,
+                                                      self.loop.with_priorities)
         clock = time.perf_counter
         for _ in range(int(n_moves)):
             t0 = clock()
-            actions = loop.act(temperature, **inject)
-            t1 = clock()
-            obs, reward, done = self._step(actions)
-            legal, to_play = env.legal_mask(), env.to_play()
-            t2 = clock()
-            finished = loop.observe(obs, reward, done, legal, to_play)
-            t3 = clock()
-            self.device_s += (t1 - t0) + (t3 - t2)
-            self.env_s += t2 - t1
-            if finished.any():
-                obs = env.reset(finished)
-                legal, to_play = env.legal_mask(), env.to_play()
-                t4 = clock()
-                loop.restart(finished, obs, legal, to_play)
-                self.env_s += t4 - t3
-                self.device_s += clock() - t4
-            st = loop.stats
-            self.parked_events += int(st.parked_slots)
-            if st.parked_slots or st.staged_bytes > self.DRAIN_FILL * st.staging_capacity:
-                out.add(*loop.drain())
-        out.add(*loop.drain())
+            actions = self.loop.act(temperature, **inject)
+            self.device_s += clock() - t0
+            self._advance(actions, out)
+            self._opponent_phase(out)
+        out.add(*self.loop.drain())
         return out
+
+    def _advance(self, actions, out, only_playing=False):
+        """Steps the slots of ``actions`` and observes them; resets and restarts the games observe packed, and drains
+        into ``out`` when the staging area fills."""
+        env, loop = self.env, self.loop
+        clock = time.perf_counter
+        t1 = clock()
+        obs, reward, done = self._step(actions, only_playing)
+        legal, to_play = env.legal_mask(), env.to_play()
+        t2 = clock()
+        finished = loop.observe(obs, reward, done, legal, to_play)
+        t3 = clock()
+        self.device_s += t3 - t2
+        self.env_s += t2 - t1
+        if finished.any():
+            obs = env.reset(finished)
+            legal, to_play = env.legal_mask(), env.to_play()
+            t4 = clock()
+            loop.restart(finished, obs, legal, to_play)
+            self.env_s += t4 - t3
+            self.device_s += clock() - t4
+        st = loop.stats
+        self.parked_events += int(st.parked_slots)
+        if st.parked_slots or st.staged_bytes > self.DRAIN_FILL * st.staging_capacity:
+            out.add(*loop.drain())
+
+    def _opponent_phase(self, out):
+        """The opponent's moves, until MuZero is to move in every slot whose game is in play."""
+        if self.opponent == "self":
+            return
+        while True:
+            defaults = self.loop.opponent_turn()
+            if defaults is None:
+                return
+            actions = self.env.expert_actions(defaults, defaults >= 0) if self.opponent == "expert" else None
+            self._advance(self.loop.opponent_act(actions), out, only_playing=True)
 
 
 class PackedGames:
