@@ -225,6 +225,45 @@ int mz_initial_inference(MzHandle* h, int32_t n, int32_t mem, const float* obs, 
 int mz_recurrent_inference(MzHandle* h, int32_t n, int32_t mem, const float* hidden, const int32_t* action,
                            const MzInferenceOut* out);
 
+/* Arguments of mz_reanalyse_values: the fresh root values of every position of n games (Reanalyse, replay_buffer.py:
+ * 345-366).  `mem` says where frames, actions and values live; the offsets and positions are HOST arrays (the library
+ * plans its chunks from them).  Game g owns frame rows [frame_offsets[g], frame_offsets[g + 1]) (its observation_history)
+ * and entries [action_offsets[g], action_offsets[g + 1]) of actions (its action_history, leading 0 included); its
+ * positions are i = 0 .. positions[g] - 1 (len(root_values)).  The stack depth s is the handle's: obs_elems =
+ * O + s * (O + H * W) with O = frame_elems and H x W the handle's obs_h x obs_w. */
+typedef struct MzReanalyseIO {
+    int32_t n_games;
+    int32_t mem;                  /* MZ_MEM_HOST or MZ_MEM_DEVICE for frames, actions and values */
+    int32_t stacked_observations; /* the caller's s: must be the handle's */
+    int32_t reserved;
+    int64_t frame_elems;          /* O: floats per frame (the environment's C x H x W observation) */
+    const float* frames;          /* [F][O] fp32, every game's observation_history back to back */
+    const int64_t* frame_offsets; /* [n + 1] host, non-negative, non-decreasing */
+    const int32_t* actions;       /* [action_offsets[n]] every game's action_history back to back, each in [0, A) */
+    const int64_t* action_offsets;/* [n + 1] host, non-negative, non-decreasing */
+    const int64_t* positions;     /* [n] host: T_g, 0 <= T_g <= frames of game g, and T_g <= actions of game g */
+    float* values;                /* [sum T_g] out: support_to_scalar(initial_inference(stacked input)[0]), game order */
+} MzReanalyseIO;
+
+/* replaces the stacked-observation gathering and model.initial_inference of Reanalyse (replay_buffer.py:345-366) for a
+ * batch of games: the positions, in game order, are cut into chunks of at most max_games (a chunk may span many games
+ * or cut through one); per chunk a kernel builds each position's stacked input, GameHistory.get_stacked_observations(
+ * i, s, A) (self_play.py:304-315), in the representation's input workspace and the network of mz_initial_inference
+ * runs on it (its route, its range guard).  With host memory each chunk's frame rows (the positions' rows and the s
+ * before the first) are staged through two pinned buffers, the next chunk's upload overlapping the current chunk's
+ * network; device memory is read in place.  The staging buffers are allocated by the first call and kept with the
+ * handle (a larger frame_elems or s grows them).  Beyond mz_create's allocations the call takes at most
+ * 2 x ((max_games + s) x (O + 1) x 4 + max_games x 20) bytes of device memory (and as much pinned host memory with host
+ * frames), whatever the games' lengths.  Refused with MZ_EINVAL, before anything is written: stacked_observations other
+ * than the handle's, a frame_elems that with it does not give obs_elems (the message names the s the handle implies for
+ * that O), negative or decreasing offsets, a T_g outside [0, frames of g] or above the game's actions, an action outside
+ * [0, A). */
+int mz_reanalyse_values(MzHandle* h, const MzReanalyseIO* io);
+/* Debug / parity: the stacked inputs chunk `chunk` of mz_reanalyse_values(h, io) builds, without the network: out (HOST)
+ * receives [n_c][obs_elems] floats, n_c = the chunk's positions; io->values is not used.  The refusals of
+ * mz_reanalyse_values, and MZ_EINVAL for a chunk beyond the call's. */
+int mz_debug_reanalyse_stack(MzHandle* h, const MzReanalyseIO* io, int32_t chunk, float* out);
+
 /* Node graph access for callers that walk the tree (self_play.py:229-232,499-509; diagnose_model.py:164,222-255) */
 int mz_export_tree(MzHandle* h, int32_t game, MzTreeExport* out);
 /* The inverse: seed game `game`'s tree in the pool from host arrays in the same layout (n_expansions, root_visit,

@@ -97,6 +97,12 @@ class MzInferenceOut(C.Structure):
                 ("hidden", C.c_void_p), ("value", C.c_void_p), ("reward", C.c_void_p)]
 
 
+class MzReanalyseIO(C.Structure):
+    _fields_ = [("n_games", C.c_int32), ("mem", C.c_int32), ("stacked_observations", C.c_int32), ("reserved", C.c_int32),
+                ("frame_elems", C.c_int64), ("frames", C.c_void_p), ("frame_offsets", C.c_void_p), ("actions", C.c_void_p),
+                ("action_offsets", C.c_void_p), ("positions", C.c_void_p), ("values", C.c_void_p)]
+
+
 class MzSelfPlayDesc(C.Structure):
     _fields_ = [("env", C.c_int32), ("max_moves", C.c_int32), ("temperature_threshold", C.c_int32),
                 ("reward_scale", C.c_int32), ("first_game_id", C.c_int64), ("game_id_stride", C.c_int64),
@@ -140,6 +146,8 @@ SYMBOLS = [
     ("mz_search_device_wait", C.c_int, [C.c_void_p, C.POINTER(MzDeviceSearchIO)]),
     ("mz_initial_inference", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(MzInferenceOut)]),
     ("mz_recurrent_inference", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(MzInferenceOut)]),
+    ("mz_reanalyse_values", C.c_int, [C.c_void_p, C.POINTER(MzReanalyseIO)]),
+    ("mz_debug_reanalyse_stack", C.c_int, [C.c_void_p, C.POINTER(MzReanalyseIO), C.c_int32, C.c_void_p]),
     ("mz_export_tree", C.c_int, [C.c_void_p, C.c_int32, C.POINTER(MzTreeExport)]),
     ("mz_import_tree", C.c_int, [C.c_void_p, C.c_int32, C.POINTER(MzTreeExport)]),
     ("mz_hidden_elems", C.c_int64, [C.c_void_p]),

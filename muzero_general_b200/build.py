@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmzb200.so")
-SOURCES = ["abi.cu", "ktimer.cu", "fc_search.cu", "fc_infer.cu", "tree_kernels.cu", "tree_wide.cu", "pipeline.cu", "resnet.cu", "conv_tc.cu", "conv_x3.cu", "small_tower.cu", "small_search.cu", "selfplay.cu", "cnn_stem.cu", "conv_wide.cu", "conv_wide256.cu"]
+SOURCES = ["abi.cu", "ktimer.cu", "fc_search.cu", "fc_infer.cu", "tree_kernels.cu", "tree_wide.cu", "pipeline.cu", "resnet.cu", "conv_tc.cu", "conv_x3.cu", "small_tower.cu", "small_search.cu", "selfplay.cu", "cnn_stem.cu", "conv_wide.cu", "conv_wide256.cu", "reanalyse.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

@@ -203,6 +203,7 @@ extern "C" int mz_destroy(MzHandle* h) {
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     mz_selfplay_destroy(h);
+    mz_reanalyse_destroy(h);
     NodePool& p = h->pool;
     void* ptrs[] = {p.visit, p.vsum, p.mval, p.reward, p.prior, p.expansion, p.root_prior, p.hidden, p.root_visit, p.root_vsum,
                     p.root_reward, p.range, p.n_expanded, p.ties, p.max_depth, p.legal, p.path, p.path_reward, p.leaf_depth,
@@ -773,6 +774,28 @@ extern "C" int mz_debug_host_split(const MzHandle* h, int64_t* out) {
 // ------------------------------------------------------------------------------------------
 // network entry points
 // ------------------------------------------------------------------------------------------
+int mz_network_enqueue(MzHandle* h, const InferCall& c) {
+    if (h->net.kind == MZ_NET_FC) {
+        FcInferArgs a{};
+        a.n = c.n; a.recurrent = c.recurrent; a.net = h->fc; a.blob = h->d_fc_blob; a.in = c.in; a.action = c.action;
+        a.value_logits = c.value_logits; a.reward_logits = c.reward_logits; a.policy_logits = c.policy_logits;
+        a.hidden = c.hidden; a.value = c.value; a.reward = c.reward;
+        cudaError_t e = launch_fc_inference(a, h->fc_group, h->sm_count, h->stream);
+        if (e != cudaSuccess) return fail(h, MZ_ECUDA, std::string("fc_inference launch: ") + cudaGetErrorString(e));
+        h->launches += 1;
+        return MZ_OK;
+    }
+    std::string e;
+    const int rc = resnet_inference(h->res, c, h->stream, &h->launches, &e);
+    return rc ? fail(h, rc, "resnet_inference: " + e) : MZ_OK;
+}
+
+int mz_network_guard(MzHandle* h, const InferCall& c) {
+    if (!h->res || resnet_take_saturations(h->res, h->stream) == 0) return MZ_OK;
+    mz_switch_to_strict(h);
+    return mz_network_enqueue(h, c);
+}
+
 static int run_inference(MzHandle* h, int n, int mem, const float* in, const int32_t* action, const MzInferenceOut* out,
                          bool recurrent) {
     if (!h || !in || !out) return fail(h, MZ_EINVAL, "inference: null argument");
@@ -794,25 +817,8 @@ static int run_inference(MzHandle* h, int n, int mem, const float* in, const int
     if ((rc = debug_out(h, "i.h", out->hidden, (size_t)n * h->hidden_elems, mem, &c.hidden, outs))) return rc;
     if ((rc = debug_out(h, "i.v", out->value, n, mem, &c.value, outs))) return rc;
     if ((rc = debug_out(h, "i.r", out->reward, n, mem, &c.reward, outs))) return rc;
-    if (h->net.kind == MZ_NET_FC) {
-        FcInferArgs a{};
-        a.n = n; a.recurrent = recurrent; a.net = h->fc; a.blob = h->d_fc_blob; a.in = c.in; a.action = c.action;
-        a.value_logits = c.value_logits; a.reward_logits = c.reward_logits; a.policy_logits = c.policy_logits;
-        a.hidden = c.hidden; a.value = c.value; a.reward = c.reward;
-        cudaError_t e = launch_fc_inference(a, h->fc_group, h->sm_count, h->stream);
-        if (e != cudaSuccess) return fail(h, MZ_ECUDA, std::string("fc_inference launch: ") + cudaGetErrorString(e));
-        h->launches += 1;
-    } else {
-        std::string e;
-        rc = resnet_inference(h->res, c, h->stream, &h->launches, &e);
-        if (rc) return fail(h, rc, "resnet_inference: " + e);
-    }
-    if (h->res && resnet_take_saturations(h->res, h->stream) > 0) {
-        mz_switch_to_strict(h);
-        std::string e;
-        rc = resnet_inference(h->res, c, h->stream, &h->launches, &e);
-        if (rc) return fail(h, rc, "resnet_inference: " + e);
-    }
+    if ((rc = mz_network_enqueue(h, c))) return rc;
+    if ((rc = mz_network_guard(h, c))) return rc;
     for (const DebugOut& d : outs)
         MZ_CUDA(h, cudaMemcpyAsync(d.user, d.dev, d.bytes, cudaMemcpyDeviceToHost, h->stream));
     MZ_CUDA(h, cudaStreamSynchronize(h->stream));

@@ -1,4 +1,4 @@
-// The library handle and the helpers shared by the entry-point files (abi.cu, selfplay.cu).
+// The library handle and the helpers shared by the entry-point files (abi.cu, selfplay.cu, reanalyse.cu).
 #pragma once
 #include <time.h>
 
@@ -11,6 +11,7 @@
 #include "ktimer.h"
 
 struct MzSelfPlay;                     // device-resident self-play state (selfplay.cu)
+struct MzReanalyse;                    // Reanalyse's staging buffers and copy stream (reanalyse.cu)
 using namespace mz;
 
 struct MzHandle {
@@ -69,6 +70,7 @@ struct MzHandle {
     std::vector<void*> debug_allocs;
     std::map<std::string, std::pair<void*, size_t>> named;
     MzSelfPlay* sp = nullptr;          // mz_selfplay_begin
+    MzReanalyse* ra = nullptr;         // mz_reanalyse_values, on first use
     int pool_n = 0;                    // layout "N" of the node pool and tables: num_simulations + extra_expansions
     int imported_expansions = 0;       // expansions of the tree mz_import_tree seeded last (MZ_FLAG_CONTINUE)
     int range_fallbacks = 0;           // times the x3 range guard switched this handle to the fp32 towers (0 or 1)
@@ -100,6 +102,12 @@ static inline int fail(MzHandle* h, int code, const std::string& msg) { return m
 // One batched search on device buffers, enqueued on h->stream without synchronising: the fused FC kernel or the
 // step-wise pipeline (eager for the first two calls with a given argument set, then a CUDA-graph replay).
 int mz_dispatch_search(MzHandle* h, const mz::SearchCall& call, bool teacher, bool trace, int flags);
+// One batched network call (mz_initial_inference / mz_recurrent_inference's): the FC kernel or resnet_inference, enqueued
+// on h->stream.  mz_network_guard then synchronises; when the x3 towers' range guard fired it switches the handle to the
+// fp32 towers and enqueues the call again.
+int mz_network_enqueue(MzHandle* h, const mz::InferCall& c);
+int mz_network_guard(MzHandle* h, const mz::InferCall& c);
+void mz_reanalyse_destroy(MzHandle* h);
 void mz_selfplay_destroy(MzHandle* h);
 void mz_switch_to_strict(MzHandle* h);
 void mz_drop_graphs(MzHandle* h);             // captured graphs refer to buffers or kernels that are about to change

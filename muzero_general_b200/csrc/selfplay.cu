@@ -55,6 +55,7 @@
 
 #include "handle.h"
 #include "common.cuh"
+#include "stack.cuh"
 
 namespace mz {
 
@@ -414,22 +415,18 @@ MZ_DEVINL int start_game(const SpDev& s, int g, int64_t gid) {
 }
 
 // The stacked tail of slot g's search input, after its current observation (GameHistory.get_stacked_observations(-1),
-// self_play.py:513-550): for k = 1 .. stack, p = t - k with t the moves played, the observation after move p
-// (rec_obs row p % rows) and a plane of action_history[p + 1] / A = rec_action[p] / A, or O + plane zeros when p < 0.  The
-// action plane is the fp64 quotient rounded once to fp32, what the reference's float64 plane becomes after .float().
+// self_play.py:513-550), by stack_tail_element (stack.cuh) with t the moves played: observation p is rec_obs row
+// p % rows and action_history[p + 1] is rec_action[p].
 // Threads lane, lane + step, ... share the floats; the slot's records must be visible to all of them.
 MZ_DEVINL void stack_fill(const SpDev& s, int g, int lane, int step) {
     const int t = s.move[g];
-    const int block = s.O + s.plane;
     float* tail = s.obs + (size_t)g * s.O_in + s.O;
     const float* rec = s.rec_obs + (size_t)g * s.rows * s.O;
     const int32_t* act = s.rec_action + (size_t)g * s.max_moves;
-    for (int i = lane; i < s.stack * block; i += step) {
-        const int k = i / block, j = i - k * block, p = t - 1 - k;
-        float v = 0.0f;
-        if (p >= 0) v = j < s.O ? rec[(size_t)(p % s.rows) * s.O + j] : __double2float_rn(__ddiv_rn((double)act[p], (double)s.A));
-        tail[i] = v;
-    }
+    const auto frame = [&](int p) { return rec + (size_t)(p % s.rows) * s.O; };
+    const auto action = [&](int p) { return act[p]; };
+    for (int i = lane; i < s.stack * (s.O + s.plane); i += step)
+        tail[i] = stack_tail_element(i, t, s.O, s.plane, s.A, frame, action);
 }
 
 __global__ void selfplay_reset_kernel(const SpDev s, int64_t first_game_id) {

@@ -394,6 +394,57 @@ class SearchEngine:
         hidden = numpy.asarray(hidden, dtype=numpy.float32)
         return self._inference(self.lib.mz_recurrent_inference, hidden.shape[0], hidden, action)
 
+    # ------------------------------------------------------------------ Reanalyse
+    def _reanalyse_io(self, frames, frame_offsets, actions, action_offsets, positions, stacked_observations, keep):
+        """MzReanalyseIO over numpy arrays (host) or CUDA torch tensors (device) of frames [F][O] and actions."""
+        device_mem = _is_torch(frames)
+        if not device_mem:
+            frames = numpy.asarray(frames, dtype=numpy.float32)
+        O = int(frames.shape[1]) if frames.ndim == 2 else int(numpy.prod(tuple(frames.shape[1:]), dtype=numpy.int64))
+        io = _lib.MzReanalyseIO()
+        positions = numpy.ascontiguousarray(positions, dtype=numpy.int64)
+        io.n_games = len(positions)
+        io.mem = _lib.MZ_MEM_DEVICE if device_mem else _lib.MZ_MEM_HOST
+        io.stacked_observations = int(self.config.stacked_observations if stacked_observations is None
+                                      else stacked_observations)
+        io.frame_elems = O
+        io.frames = self._ptr(frames, numpy.float32, keep)
+        io.actions = self._ptr(actions, numpy.int32, keep)
+        io.frame_offsets = self._ptr(numpy.asarray(frame_offsets, dtype=numpy.int64), numpy.int64, keep)
+        io.action_offsets = self._ptr(numpy.asarray(action_offsets, dtype=numpy.int64), numpy.int64, keep)
+        io.positions = self._ptr(positions, numpy.int64, keep)
+        return io, int(positions.sum()), device_mem
+
+    def reanalyse_values(self, frames, frame_offsets, actions, action_offsets, positions, stacked_observations=None):
+        """Fresh root values of every position of a batch of games (mz_reanalyse_values): game g's frames are rows
+        [frame_offsets[g], frame_offsets[g + 1]) of ``frames`` ([F][O] float32), its action history (leading 0
+        included) entries [action_offsets[g], action_offsets[g + 1]) of ``actions``, its positions 0 .. positions[g] - 1.
+        Returns float32 [sum positions] in game order: a numpy array for host frames, a CUDA tensor for CUDA frames and
+        actions."""
+        keep = []
+        io, total, device_mem = self._reanalyse_io(frames, frame_offsets, actions, action_offsets, positions,
+                                                   stacked_observations, keep)
+        if device_mem:
+            import torch
+            values = torch.empty(total, dtype=torch.float32, device=frames.device)
+            io.values = values.data_ptr() if total else None
+        else:
+            values = numpy.empty(total, numpy.float32)
+            io.values = values.ctypes.data if total else None
+        self._check(self.lib.mz_reanalyse_values(self._h, C.byref(io)))
+        return values
+
+    def debug_reanalyse_stack(self, chunk, frames, frame_offsets, actions, action_offsets, positions,
+                              stacked_observations=None):
+        """The stacked inputs [n_c][obs_elems] chunk ``chunk`` of reanalyse_values builds (mz_debug_reanalyse_stack)."""
+        keep = []
+        io, total, _ = self._reanalyse_io(frames, frame_offsets, actions, action_offsets, positions, stacked_observations,
+                                          keep)
+        n = max(0, min(self.max_games, total - int(chunk) * self.max_games))
+        out = numpy.empty((n, self.obs_elems), numpy.float32)
+        self._check(self.lib.mz_debug_reanalyse_stack(self._h, C.byref(io), int(chunk), out.ctypes.data if n else None))
+        return out
+
     # ------------------------------------------------------------------ tree
     def export_tree(self, game: int, with_hidden: bool = False):
         S = (self.pool_n + 1) * self.A

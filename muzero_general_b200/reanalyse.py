@@ -1,9 +1,10 @@
 """The callers either side of the self-play path, in bulk (SURVEY.md 8f-2 / 8f-3).
 
 * ``Reanalyse`` - same constructor and ``reanalyse(replay_buffer, shared_storage)`` loop as the reference actor
-  (``replay_buffer.py:307-373``), but the fresh root values of MANY games come from ONE batched
-  ``mz_initial_inference`` per call (the representation + prediction kernels of the search path, with
-  ``support_to_scalar`` fused behind the value head) instead of one game per RPC on the CPU.
+  (``replay_buffer.py:307-373``), but the fresh root values of MANY games come from ONE call per batch (the
+  representation + prediction kernels of the search path, with ``support_to_scalar`` fused behind the value head)
+  instead of one game per RPC on the CPU: ``mz_reanalyse_values``, which stacks the observations on the GPU, for
+  configs with stacked observations, chunked ``mz_initial_inference`` otherwise.
 * ``initial_priorities`` / ``save_games`` - the prioritised-replay priorities ``ReplayBuffer.save_game`` computes one
   position at a time in Python (``replay_buffer.py:33-51`` calling ``compute_target_value``, ``:230-262``), evaluated
   for a whole game with array arithmetic in the reference's operation order (bit-identical float32 priorities), and
@@ -14,6 +15,7 @@ Nothing here imports torch; the engine does the arithmetic on the GPU.
 """
 from __future__ import annotations
 
+import itertools
 import time
 
 import numpy
@@ -32,6 +34,49 @@ def _call(obj, method, *args, **kw):
 def _fire(obj, method, *args):
     fn = getattr(obj, method)
     return fn.remote(*args) if hasattr(fn, "remote") else fn(*args)
+
+
+def _frame_source(gh):
+    """(frame rows, action history, positions T) of a game without building anything per position: a
+    ``PackedGameHistory`` whose lists were never built gives its block's contiguous ``obs`` [T + 1][O] float32 and
+    ``action`` sections, any other history its ``observation_history`` list (rows converted when read) and
+    ``action_history``."""
+    d = getattr(gh, "__dict__", {})
+    if "_packed" in d and "observation_history" not in d:
+        g = d["_packed"][0]
+        T = int(g["length"])
+        actions = numpy.empty(T + 1, numpy.int32)
+        actions[0] = 0
+        actions[1:] = g["action"]
+        return numpy.asarray(g["obs"], dtype=numpy.float32).reshape(T + 1, -1), actions, T
+    return gh.observation_history, gh.action_history, len(gh.root_values)
+
+
+def _row(rows, i):
+    """Frame i of a source as float32 [O]: ``numpy.asarray(get_stacked_observations(i, 0, A), float32)`` flattened."""
+    return numpy.asarray(rows[i], dtype=numpy.float32).reshape(-1)
+
+
+def pack_frames(sources):
+    """The arguments of ``SearchEngine.reanalyse_values`` for ``_frame_source`` tuples: every game's frames once as
+    float32 [sum (T + 1)][O] (O(T * O) host memory, no stack) and its action history as int32, back to back, with the
+    per-game offsets and positions."""
+    O = next(_row(rows, 0).size for rows, _, T in sources if T)
+    frame_off = numpy.zeros(len(sources) + 1, numpy.int64)
+    action_off = numpy.zeros(len(sources) + 1, numpy.int64)
+    for g, (rows, actions, _) in enumerate(sources):
+        frame_off[g + 1] = frame_off[g] + len(rows)
+        action_off[g + 1] = action_off[g] + len(actions)
+    frames = numpy.empty((int(frame_off[-1]), O), numpy.float32)
+    for g, (rows, _, _) in enumerate(sources):
+        if isinstance(rows, numpy.ndarray):
+            frames[frame_off[g]:frame_off[g + 1]] = rows.reshape(len(rows), O)
+        else:                                            # one row at a time: no second copy of the game
+            for k in range(len(rows)):
+                frames[frame_off[g] + k] = _row(rows, k)
+    actions = numpy.concatenate([numpy.asarray(a, dtype=numpy.int32).reshape(-1) for _, a, _ in sources])
+    positions = numpy.array([T for _, _, T in sources], numpy.int64)
+    return dict(frames=frames, frame_offsets=frame_off, actions=actions, action_offsets=action_off, positions=positions)
 
 
 class Reanalyse:
@@ -57,28 +102,42 @@ class Reanalyse:
     def fresh_root_values(self, game_histories):
         """``models.support_to_scalar(model.initial_inference(observations)[0])`` (replay_buffer.py:345-366) for every
         position of every game, batched over games; returns one float32 array per game (``torch.squeeze`` shape:
-        ``[T]``, or 0-d for a one-position game)."""
-        cfg = self.config
-        A = len(cfg.action_space)
-        obs, counts = [], []
-        for gh in game_histories:
-            T = len(gh.root_values)
-            counts.append(T)
-            for i in range(T):
-                obs.append(numpy.asarray(gh.get_stacked_observations(i, cfg.stacked_observations, A), dtype=numpy.float32))
-        if not obs:
+        ``[T]``, or 0-d for a one-position game).
+
+        With ``stacked_observations`` s > 0 the host hands each game's frames over once and the stacked inputs are built
+        on the GPU (``SearchEngine.reanalyse_values``); with s = 0 the observations are gathered one chunk of
+        ``max_positions`` at a time for ``initial_inference``.  Either way no per-position stack is built on the host."""
+        sources = [_frame_source(gh) for gh in game_histories]
+        counts = [src[2] for src in sources]
+        total = sum(counts)
+        if not total:
             return [numpy.zeros(0, numpy.float32) for _ in game_histories]
-        obs = numpy.stack(obs).reshape(len(obs), -1)
-        values = numpy.empty(len(obs), numpy.float32)
-        for lo in range(0, len(obs), self.max_positions):
-            hi = min(len(obs), lo + self.max_positions)
-            values[lo:hi] = self.engine.initial_inference(obs[lo:hi])["value"]
+        if int(self.config.stacked_observations) > 0:
+            values = self._stacked_values(sources)
+        else:
+            values = self._plain_values(sources, total)
         out, off = [], 0
         for T in counts:
             v = values[off:off + T].copy()
             out.append(v.reshape(()) if T == 1 else v)
             off += T
         return out
+
+    def _stacked_values(self, sources):
+        """One mz_reanalyse_values over every game."""
+        p = pack_frames(sources)
+        return self.engine.reanalyse_values(p["frames"], p["frame_offsets"], p["actions"], p["action_offsets"],
+                                            p["positions"])
+
+    def _plain_values(self, sources, total):
+        """s = 0: the observation of each position is its frame; one initial_inference per max_positions positions."""
+        values = numpy.empty(total, numpy.float32)
+        flat = ((rows, i) for rows, _, T in sources for i in range(T))
+        for lo in range(0, total, self.max_positions):
+            hi = min(total, lo + self.max_positions)
+            obs = numpy.stack([_row(rows, i) for rows, i in itertools.islice(flat, hi - lo)])
+            values[lo:hi] = self.engine.initial_inference(obs)["value"]
+        return values
 
     def reanalyse_games(self, game_histories):
         """Set ``reanalysed_predicted_root_values`` on every history (one batched inference); returns the histories."""
