@@ -476,6 +476,41 @@ int mz_debug_heads(int device, int32_t n, int32_t C, int32_t H, int32_t W, int32
                    int32_t pool_stride, int32_t out_slot, float* logits0, float* logits1, float* scalar, float* rescaled,
                    float* pool, float* state, int64_t* plan);
 
+/* Routes of the fully-connected networks (route argument of mz_debug_fc_net_plan and mz_debug_fc_net): fc_inference_kernel
+ * as mz_initial_inference, mz_recurrent_inference and the step-wise search's pool call run it, and the two network calls of
+ * the fused search kernel (its root evaluation and one simulation's recurrent inference).  Paths (plan[0]): */
+#define MZ_FC_INFER_INITIAL 0
+#define MZ_FC_INFER_RECURRENT 1
+#define MZ_FC_INFER_POOL 2          /* parents gathered from and the new state written to a [n][pool_stride][E] pool */
+#define MZ_FC_SEARCH_ROOT 3
+#define MZ_FC_SEARCH_SIM 4
+#define MZ_FC_PATH_INFER 0          /* fc_inference_kernel<G> */
+#define MZ_FC_PATH_FIXED 1          /* the search's unrolled network of games/cartpole.py's shape (G = 16 or 32) */
+#define MZ_FC_PATH_FUSED 2          /* the search's descriptors walk, the three heads side by side (equal depth) */
+#define MZ_FC_PATH_SPLIT 3          /* the search's descriptors walk, the heads one after the other */
+
+/* Launch plan (host only) of one FC network route for n samples with G lanes per sample (4, 8, 16 or 32) on sm_count SMs with
+ * smem_cap bytes of shared memory per block.  `net` gives the shape (kind, encoding, action_space, support_size, layer lists)
+ * and obs_elems the observation floats.  force_split (search routes) walks the layer descriptors with the heads one after
+ * the other, even for the unrolled shape or heads of equal depth; the network never does.  Fills plan[5] = {path (MZ_FC_PATH_*), G, threads per CTA, grid, dynamic shared-memory
+ * bytes} and returns 1; returns 0 with the reason in mz_last_error(NULL) when the shape is refused (it does not fit in
+ * shared memory, or a search route with action_space > G). */
+int mz_debug_fc_net_plan(const MzNetDesc* net, int32_t obs_elems, int32_t G, int32_t route, int32_t force_split, int32_t n,
+                         int32_t sm_count, int64_t smem_cap, int64_t* plan);
+
+/* Debug / parity: one FC network route for n samples, weights packed from `tensors` named as in the reference state_dict.
+ * in: observations [n][obs_elems] (MZ_FC_INFER_INITIAL, MZ_FC_SEARCH_ROOT) or parent states [n][E]; action [n] on the
+ * recurrent routes; on MZ_FC_INFER_POOL parent [n] is each sample's pool slot, where the entry puts its parent state, and
+ * out_slot the slot the kernel writes (pool: [n][pool_stride][E] back).  Outputs (NULL: not copied back), each filled with
+ * NaN bytes before the launch: raw [n][E] the state before the rescale (search routes), hidden [n][E] after it, reward /
+ * value logits [n][2S+1], policy logits [n][A] (the unrolled path keeps its logits in registers and writes none), prior
+ * [n][A] (search routes), value [n] and reward [n] (the search's root has none; the initial inference writes the value
+ * transform of 0).  plan gets the plan of the launch.  MZ_EUNSUPPORTED when the plan is refused. */
+int mz_debug_fc_net(int device, const MzNetDesc* net, int32_t obs_elems, const MzTensor* tensors, int32_t n_tensors, int32_t G,
+                    int32_t route, int32_t force_split, int32_t n, const float* in, const int32_t* action, const int32_t* parent,
+                    int32_t pool_stride, int32_t out_slot, float* raw, float* hidden, float* reward_logits, float* value_logits,
+                    float* policy_logits, float* prior, float* value, float* reward, float* pool, int64_t* plan);
+
 /* Launch plan of the DownsampleCNN stem (downsample = 2, models.py:278-297; host only) for n boards of `in` planes of H x W
  * and C channels on sm_count SMs.  Fills plan[36] = {h, w (hidden board, ceil(H / 16) x ceil(W / 16)), mid (conv1's
  * channels, (in + C) / 2)}, then per stage (conv1 + pool1 at plan[3], conv2 + pool2 + average at plan[19]) {kernel, stride,

@@ -207,6 +207,9 @@ SYMBOLS = [
     ("mz_debug_heads_plan", C.c_int, [C.c_int32] * 8 + [C.c_void_p, C.c_int32, C.POINTER(C.c_int64)]),
     ("mz_debug_heads", C.c_int, [C.c_int] + [C.c_int32] * 8 + [C.c_void_p, C.POINTER(MzTensor), C.c_int32, C.c_void_p,
                                                               C.c_int32, C.c_int32] + [C.c_void_p] * 6 + [C.POINTER(C.c_int64)]),
+    ("mz_debug_fc_net_plan", C.c_int, [C.POINTER(MzNetDesc)] + [C.c_int32] * 6 + [C.c_int64, C.POINTER(C.c_int64)]),
+    ("mz_debug_fc_net", C.c_int, [C.c_int, C.POINTER(MzNetDesc), C.c_int32, C.POINTER(MzTensor)] + [C.c_int32] * 5
+     + [C.c_void_p] * 3 + [C.c_int32, C.c_int32] + [C.c_void_p] * 9 + [C.POINTER(C.c_int64)]),
     ("mz_debug_cnn_stem_plan", C.c_int, [C.c_int32] * 6 + [C.POINTER(C.c_int64)]),
     ("mz_debug_cnn_stem", C.c_int, [C.c_int] + [C.c_int32] * 5 + [C.c_void_p] * 6 + [C.POINTER(C.c_int64)]),
 ]

@@ -262,17 +262,17 @@ static const MzTensor* find_tensor(const MzTensor* t, int n, const std::string& 
 }
 
 // Appends one mlp (models.py:630-642) to the blob: per Linear the weights packed [i/4][out][i%4]
-// (zero padded), the bias, and - for the first dynamics layer - the one-hot rows [A][out].
-static int pack_mlp(MzHandle* h, const MzTensor* t, int n, const std::string& prefix, const std::vector<int>& sizes,
-                    MlpDesc& d, std::vector<float>& blob, int onehot_rows) {
+// (zero padded), the bias, and - for the first dynamics layer - the one-hot rows [A][out].  t == nullptr packs zeros
+// (the shapes alone, for the host-only plans).
+static bool pack_mlp(const MzTensor* t, int n, const std::string& prefix, const std::vector<int>& sizes, MlpDesc& d,
+                     std::vector<float>& blob, int onehot_rows, std::string* err) {
     d.n = (int)sizes.size() - 1;
     for (int l = 0; l < d.n; ++l) {
         const int in = sizes[l], out = sizes[l + 1];
-        const MzTensor* w = find_tensor(t, n, prefix + "." + std::to_string(2 * l) + ".weight");
-        const MzTensor* b = find_tensor(t, n, prefix + "." + std::to_string(2 * l) + ".bias");
-        if (!w || !b) return fail(h, MZ_EINVAL, "mz_load_weights: missing tensor " + prefix + "." + std::to_string(2 * l));
-        if (w->numel != (int64_t)in * out || b->numel != out)
-            return fail(h, MZ_EINVAL, "mz_load_weights: shape mismatch for " + prefix + "." + std::to_string(2 * l));
+        const MzTensor* w = t ? find_tensor(t, n, prefix + "." + std::to_string(2 * l) + ".weight") : nullptr;
+        const MzTensor* b = t ? find_tensor(t, n, prefix + "." + std::to_string(2 * l) + ".bias") : nullptr;
+        if (t && (!w || !b)) { *err = "missing tensor " + prefix + "." + std::to_string(2 * l); return false; }
+        if (t && (w->numel != (int64_t)in * out || b->numel != out)) { *err = "shape mismatch for " + prefix + "." + std::to_string(2 * l); return false; }
         const int extra = (l == 0) ? onehot_rows : 0;
         const int dense = in - extra, in4 = (dense + 3) / 4;
         d.in[l] = in; d.out[l] = out; d.in_dense[l] = dense;
@@ -280,47 +280,70 @@ static int pack_mlp(MzHandle* h, const MzTensor* t, int n, const std::string& pr
         d.w_off[l] = (int)blob.size();
         blob.resize(blob.size() + (size_t)in4 * out * 4, 0.0f);
         float* dst = blob.data() + d.w_off[l];
-        for (int o = 0; o < out; ++o)
-            for (int i = 0; i < dense; ++i)
-                dst[((size_t)(i / 4) * out + o) * 4 + (i % 4)] = w->data[(size_t)o * in + i];     // torch Linear: [out][in]
+        if (t)
+            for (int o = 0; o < out; ++o)
+                for (int i = 0; i < dense; ++i)
+                    dst[((size_t)(i / 4) * out + o) * 4 + (i % 4)] = w->data[(size_t)o * in + i];     // torch Linear: [out][in]
         d.b_off[l] = (int)blob.size();
-        blob.insert(blob.end(), b->data, b->data + out);
+        if (t) blob.insert(blob.end(), b->data, b->data + out);
+        else blob.resize(blob.size() + out, 0.0f);
         d.x_off[l] = -1;
         if (extra > 0) {
             d.x_off[l] = (int)blob.size();
             for (int a = 0; a < extra; ++a)
-                for (int o = 0; o < out; ++o) blob.push_back(w->data[(size_t)o * in + dense + a]);
+                for (int o = 0; o < out; ++o) blob.push_back(t ? w->data[(size_t)o * in + dense + a] : 0.0f);
         }
     }
-    return MZ_OK;
+    return true;
 }
 
-static int load_fc_weights(MzHandle* h, const MzTensor* t, int n) {
-    const MzNetDesc& nd = h->net;
+// The descriptors and the shared-memory blob of an FC network (nd's shape, obs_elems inputs) from torch-layout tensors, or
+// of zeros when t == nullptr.
+static bool fc_build_net(const MzNetDesc& nd, int obs_elems, const MzTensor* t, int n, FcNet* out, std::vector<float>* blob_out,
+                  std::string* err) {
     const int E = nd.encoding, A = nd.action_space, F = 2 * nd.support_size + 1;
+    if (E < 1 || A < 1 || nd.support_size < 0 || obs_elems < 1) { *err = "bad network shape"; return false; }
     FcNet fc{};
-    std::vector<float> blob;
+    std::vector<float>& blob = *blob_out;
+    blob.clear();
     std::vector<int> sz;
-    int rc;
-    if (mlp_dims(nd.fc_representation, nd.n_fc_representation, (int)h->obs_elems, E, sz)) return fail(h, MZ_EINVAL, "bad layers");
-    if ((rc = pack_mlp(h, t, n, "representation_network.module", sz, fc.rep, blob, 0))) return rc;
-    if (mlp_dims(nd.fc_dynamics, nd.n_fc_dynamics, E + A, E, sz)) return fail(h, MZ_EINVAL, "bad layers");
-    if ((rc = pack_mlp(h, t, n, "dynamics_encoded_state_network.module", sz, fc.dyn, blob, A))) return rc;
-    if (mlp_dims(nd.fc_reward, nd.n_fc_reward, E, F, sz)) return fail(h, MZ_EINVAL, "bad layers");
-    if ((rc = pack_mlp(h, t, n, "dynamics_reward_network.module", sz, fc.rew, blob, 0))) return rc;
-    if (mlp_dims(nd.fc_value, nd.n_fc_value, E, F, sz)) return fail(h, MZ_EINVAL, "bad layers");
-    if ((rc = pack_mlp(h, t, n, "prediction_value_network.module", sz, fc.val, blob, 0))) return rc;
-    if (mlp_dims(nd.fc_policy, nd.n_fc_policy, E, A, sz)) return fail(h, MZ_EINVAL, "bad layers");
-    if ((rc = pack_mlp(h, t, n, "prediction_policy_network.module", sz, fc.pol, blob, 0))) return rc;
+    const struct { const int32_t* hidden; int n_hidden; const char* prefix; int in, out, onehot; MlpDesc* d; } mlps[] = {
+        {nd.fc_representation, nd.n_fc_representation, "representation_network.module", obs_elems, E, 0, &fc.rep},
+        {nd.fc_dynamics, nd.n_fc_dynamics, "dynamics_encoded_state_network.module", E + A, E, A, &fc.dyn},
+        {nd.fc_reward, nd.n_fc_reward, "dynamics_reward_network.module", E, F, 0, &fc.rew},
+        {nd.fc_value, nd.n_fc_value, "prediction_value_network.module", E, F, 0, &fc.val},
+        {nd.fc_policy, nd.n_fc_policy, "prediction_policy_network.module", E, A, 0, &fc.pol}};
+    for (const auto& m : mlps) {
+        if (mlp_dims(m.hidden, m.n_hidden, m.in, m.out, sz)) { *err = "bad layers"; return false; }
+        for (int w : sz) if (w < 1) { *err = "bad layers"; return false; }
+        if (!pack_mlp(t, n, m.prefix, sz, *m.d, blob, m.onehot, err)) return false;
+    }
     fc.blob_floats = (int)blob.size();
-    fc.obs_elems = (int)h->obs_elems; fc.E = E; fc.A = A; fc.S = nd.support_size; fc.F = F;
+    fc.obs_elems = obs_elems; fc.E = E; fc.A = A; fc.S = nd.support_size; fc.F = F;
     int maxw = E > F ? E : F;
     if (A > maxw) maxw = A;
-    if ((int)h->obs_elems > maxw) maxw = (int)h->obs_elems;
+    if (obs_elems > maxw) maxw = obs_elems;
     while (blob.size() % 4) blob.push_back(0.0f);
     const MlpDesc* all[] = {&fc.rep, &fc.dyn, &fc.rew, &fc.val, &fc.pol};
     for (const MlpDesc* d : all) for (int l = 0; l < d->n; ++l) if (d->out[l] > maxw) maxw = d->out[l];
     fc.maxw = (maxw + 3) & ~3;
+    *out = fc;
+    return true;
+}
+
+static int load_fc_weights(MzHandle* h, const MzTensor* t, int n) {
+    FcNet fc;
+    std::vector<float> blob;
+    std::string e;
+    if (!fc_build_net(h->net, (int)h->obs_elems, t, n, &fc, &blob, &e)) return fail(h, MZ_EINVAL, "mz_load_weights: " + e);
+    // every inference and every search needs the blob and at least one warp's lane groups in one CTA's shared memory
+    FcInferPlan ip;
+    if (!fc_infer_plan(fc.blob_floats, fc.maxw, h->fc_group, 1, h->sm_count, h->fc_launch.smem_cap, &ip))
+        return fail(h, MZ_EUNSUPPORTED, "mz_load_weights: the FC network needs " +
+                                            std::to_string(fc_infer_smem(fc.blob_floats, fc.maxw, 32 / h->fc_group)) +
+                                            " bytes of shared memory per CTA (" + std::to_string(fc.blob_floats * 4) +
+                                            " of weights and the scratch of " + std::to_string(32 / h->fc_group) +
+                                            " lane groups), the device allows " + std::to_string(h->fc_launch.smem_cap));
     if (h->d_fc_blob) cudaFree(h->d_fc_blob);
     h->d_fc_blob = nullptr;
     MZ_CUDA(h, dev_alloc(&h->d_fc_blob, blob.size()));
@@ -461,7 +484,7 @@ int mz_dispatch_search(MzHandle* h, const SearchCall& call, bool teacher, bool t
             // the tree does not fit in shared memory next to the weights: use the HBM node pool
             (void)cudaGetLastError();
             rc = run_stepwise_search(h->net, h->search, h->pool_n, h->pool, h->d_pbc, h->d_sqrt, h->d_ucb, h->fc, h->d_fc_blob, h->res, call_,
-                                     h->fc_group, h->sm_count, h->stream, &h->launches, &h->err);
+                                     h->fc_group, h->sm_count, h->fc_launch.smem_cap, h->stream, &h->launches, &h->err);
             if (rc) return rc;
         } else if (e != cudaSuccess) {
             return fail(h, MZ_ECUDA, std::string("fc_search launch: ") + cudaGetErrorString(e));
@@ -509,7 +532,7 @@ int mz_dispatch_search(MzHandle* h, const SearchCall& call, bool teacher, bool t
         mix((uint64_t)n); mix((uint64_t)call.add_noise); mix((uint64_t)call.keep_tree); mix((uint64_t)call_.continue_from);
         auto run = [&](const SearchCall& sc, cudaStream_t st) {
             return run_stepwise_search(h->net, h->search, h->pool_n, h->pool, h->d_pbc, h->d_sqrt, h->d_ucb, h->fc, h->d_fc_blob, h->res, sc,
-                                       h->fc_group, h->sm_count, st, &h->launches, &h->err);
+                                       h->fc_group, h->sm_count, h->fc_launch.smem_cap, st, &h->launches, &h->err);
         };
         auto eager = [&]() { return run(call_, h->stream); };
         // Partitioned replay.  A simulation is a chain of dependent kernels (tower -> heads -> tower -> heads -> tree step) and
@@ -780,7 +803,7 @@ int mz_network_enqueue(MzHandle* h, const InferCall& c) {
         a.n = c.n; a.recurrent = c.recurrent; a.net = h->fc; a.blob = h->d_fc_blob; a.in = c.in; a.action = c.action;
         a.value_logits = c.value_logits; a.reward_logits = c.reward_logits; a.policy_logits = c.policy_logits;
         a.hidden = c.hidden; a.value = c.value; a.reward = c.reward;
-        cudaError_t e = launch_fc_inference(a, h->fc_group, h->sm_count, h->stream);
+        cudaError_t e = launch_fc_inference(a, h->fc_group, h->sm_count, h->fc_launch.smem_cap, h->stream);
         if (e != cudaSuccess) return fail(h, MZ_ECUDA, std::string("fc_inference launch: ") + cudaGetErrorString(e));
         h->launches += 1;
         return MZ_OK;
@@ -1172,5 +1195,106 @@ extern "C" int mz_debug_heads(int device, int32_t n, int32_t C, int32_t H, int32
     int rc = resnet_debug_heads(n, C, H, W, site, layout, route, parts, shapes, tensors, n_tensors, x, pool_stride, out_slot, logits0,
                                 logits1, scalar, rescaled, pool, state, plan, prop.multiProcessorCount, &e);
     if (rc) return fail(nullptr, rc, "mz_debug_heads: " + e);
+    return MZ_OK;
+}
+
+extern "C" int mz_debug_fc_net_plan(const MzNetDesc* net, int32_t obs_elems, int32_t G, int32_t route, int32_t force_split, int32_t n,
+                                    int32_t sm_count, int64_t smem_cap, int64_t* plan) {
+    if (!net || !plan || smem_cap < 0) return fail(nullptr, 0, "mz_debug_fc_net_plan: bad argument");
+    FcNet fc;
+    std::vector<float> blob;
+    std::string e;
+    if (!fc_build_net(*net, obs_elems, nullptr, 0, &fc, &blob, &e) ||
+        !fc_debug_plan(fc, G, route, force_split != 0, n, sm_count, (size_t)smem_cap, plan, &e))
+        return fail(nullptr, 0, "mz_debug_fc_net_plan: " + e);
+    return 1;
+}
+
+// debug: one FC network route (host data in, every output back)
+extern "C" int mz_debug_fc_net(int device, const MzNetDesc* net, int32_t obs_elems, const MzTensor* tensors, int32_t n_tensors, int32_t G,
+                               int32_t route, int32_t force_split, int32_t n, const float* in, const int32_t* action, const int32_t* parent,
+                               int32_t pool_stride, int32_t out_slot, float* raw, float* hidden, float* reward_logits, float* value_logits,
+                               float* policy_logits, float* prior, float* value, float* reward, float* pool, int64_t* plan) {
+    if (!net || !in || !tensors || n_tensors < 1 || !plan || n < 1) return fail(nullptr, MZ_EINVAL, "mz_debug_fc_net: bad argument");
+    const bool recurrent = route == MZ_FC_INFER_RECURRENT || route == MZ_FC_INFER_POOL || route == MZ_FC_SEARCH_SIM;
+    if (recurrent && !action) return fail(nullptr, MZ_EINVAL, "mz_debug_fc_net: action is null");
+    if (route == MZ_FC_INFER_POOL && (!parent || !pool || pool_stride < 1 || out_slot < 0 || out_slot >= pool_stride))
+        return fail(nullptr, MZ_EINVAL, "mz_debug_fc_net: bad pool arguments");
+    if (cudaSetDevice(device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_fc_net: no such device");
+    cudaDeviceProp prop;
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_fc_net: device query failed");
+    FcNet fc;
+    std::vector<float> blob;
+    std::string e;
+    if (!fc_build_net(*net, obs_elems, tensors, n_tensors, &fc, &blob, &e)) return fail(nullptr, MZ_EINVAL, "mz_debug_fc_net: " + e);
+    if (!fc_debug_plan(fc, G, route, force_split != 0, n, prop.multiProcessorCount, prop.sharedMemPerBlockOptin, plan, &e))
+        return fail(nullptr, MZ_EUNSUPPORTED, "mz_debug_fc_net: " + e);
+    const int E = fc.E, A = fc.A, F = fc.F;
+    const size_t in_elems = (size_t)n * (recurrent ? E : obs_elems);
+    std::vector<void*> bufs;
+    cudaError_t err = cudaSuccess;
+    // device copy of host data (src) or a buffer of NaN bytes (src == nullptr); nullptr when host is null
+    auto dev = [&](const void* host, const void* src, size_t bytes) -> void* {
+        if (!host || err != cudaSuccess) return nullptr;
+        void* d = nullptr;
+        err = cudaMalloc(&d, bytes);
+        if (err != cudaSuccess) return nullptr;
+        bufs.push_back(d);
+        err = src ? cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice) : cudaMemset(d, 0xFF, bytes);
+        return d;
+    };
+    const float* d_blob = (const float*)dev(blob.data(), blob.data(), blob.size() * 4);
+    const float* d_in = (const float*)dev(in, route == MZ_FC_INFER_POOL ? nullptr : in, in_elems * 4);
+    const int32_t* d_action = (const int32_t*)dev(recurrent ? action : nullptr, action, (size_t)n * 4);
+    float* d_raw = (float*)dev(raw, nullptr, (size_t)n * E * 4);
+    float* d_hidden = (float*)dev(hidden, nullptr, (size_t)n * E * 4);
+    float* d_rl = (float*)dev(reward_logits, nullptr, (size_t)n * F * 4);
+    float* d_vl = (float*)dev(value_logits, nullptr, (size_t)n * F * 4);
+    float* d_pl = (float*)dev(policy_logits, nullptr, (size_t)n * A * 4);
+    float* d_prior = (float*)dev(prior, nullptr, (size_t)n * A * 4);
+    float* d_value = (float*)dev(value, nullptr, (size_t)n * 4);
+    float* d_reward = (float*)dev(reward, nullptr, (size_t)n * 4);
+    const size_t pool_floats = (size_t)n * pool_stride * E;
+    std::vector<float> h_pool;
+    if (route == MZ_FC_INFER_POOL) {              // NaN bytes everywhere but each sample's parent slot
+        h_pool.assign(pool_floats, 0.0f);
+        memset(h_pool.data(), 0xFF, pool_floats * 4);
+        for (int g = 0; g < n; ++g) {
+            if (parent[g] < 0 || parent[g] >= pool_stride) { err = cudaErrorInvalidValue; break; }
+            memcpy(h_pool.data() + ((size_t)g * pool_stride + parent[g]) * E, in + (size_t)g * E, (size_t)E * 4);
+        }
+    }
+    float* d_pool = (float*)dev(route == MZ_FC_INFER_POOL ? pool : nullptr, h_pool.data(), pool_floats * 4);
+    const int32_t* d_parent = (const int32_t*)dev(route == MZ_FC_INFER_POOL ? parent : nullptr, parent, (size_t)n * 4);
+    if (err == cudaSuccess) {
+        if (route == MZ_FC_SEARCH_ROOT || route == MZ_FC_SEARCH_SIM) {
+            FcDebugArgs a{};
+            a.n = n; a.route = route; a.force_split = force_split != 0; a.net = fc; a.blob = d_blob; a.in = d_in; a.action = d_action;
+            a.raw = d_raw; a.hidden = d_hidden; a.reward_logits = d_rl; a.value_logits = d_vl; a.policy_logits = d_pl;
+            a.prior = d_prior; a.value = d_value; a.reward = d_reward;
+            err = launch_fc_debug_net(a, G, plan, 0);
+        } else if (route == MZ_FC_INFER_POOL) {
+            InferCall c{};
+            c.n = n; c.recurrent = 1; c.action = d_action; c.gather_parent = d_parent; c.pool_hidden = d_pool;
+            c.pool_stride = pool_stride; c.out_slot = out_slot; c.value_logits = d_vl; c.reward_logits = d_rl;
+            c.policy_logits = d_pl; c.hidden = d_hidden; c.value = d_value; c.reward = d_reward;
+            err = launch_fc_inference_pool(fc, d_blob, c, G, prop.multiProcessorCount, prop.sharedMemPerBlockOptin, 0);
+        } else {
+            FcInferArgs a{};
+            a.n = n; a.recurrent = recurrent; a.net = fc; a.blob = d_blob; a.in = d_in; a.action = d_action;
+            a.value_logits = d_vl; a.reward_logits = d_rl; a.policy_logits = d_pl; a.hidden = d_hidden; a.value = d_value;
+            a.reward = d_reward;
+            err = launch_fc_inference(a, G, prop.multiProcessorCount, prop.sharedMemPerBlockOptin, 0);
+        }
+    }
+    if (err == cudaSuccess) err = cudaDeviceSynchronize();
+    const struct { void* host; const void* d; size_t bytes; } back[] = {
+        {raw, d_raw, (size_t)n * E * 4}, {hidden, d_hidden, (size_t)n * E * 4}, {reward_logits, d_rl, (size_t)n * F * 4},
+        {value_logits, d_vl, (size_t)n * F * 4}, {policy_logits, d_pl, (size_t)n * A * 4}, {prior, d_prior, (size_t)n * A * 4},
+        {value, d_value, (size_t)n * 4}, {reward, d_reward, (size_t)n * 4}, {pool, d_pool, pool_floats * 4}};
+    for (const auto& b : back)
+        if (err == cudaSuccess && b.host && b.d) err = cudaMemcpy(b.host, b.d, b.bytes, cudaMemcpyDeviceToHost);
+    for (void* d : bufs) cudaFree(d);
+    if (err != cudaSuccess) return fail(nullptr, MZ_ECUDA, std::string("mz_debug_fc_net: ") + cudaGetErrorString(err));
     return MZ_OK;
 }

@@ -65,43 +65,57 @@ __global__ void __launch_bounds__(kFcThreads) fc_inference_kernel(const __grid_c
     }
 }
 
+// Threads of a CTA of fc_inference_kernel<G>: the most of 128, 96, 64, 32 whose groups' scratch fits next to the weight blob
+// in `smem_cap` bytes of shared memory (the device's opt-in limit per block).  Host arithmetic only.
+bool fc_infer_plan(int blob_floats, int maxw, int G, int n, int sm_count, size_t smem_cap, FcInferPlan* p) {
+    if (G < 1 || G > 32 || 32 % G || n < 1 || sm_count < 1 || blob_floats < 0 || maxw < 1) return false;
+    for (int t = kFcThreads; t >= 32; t -= 32) {
+        const size_t smem = fc_infer_smem(blob_floats, maxw, t / G);
+        if (smem > smem_cap) continue;
+        const int groups = t / G;
+        int grid = (n + groups - 1) / groups;
+        if (grid > sm_count * 8) grid = sm_count * 8;
+        *p = FcInferPlan{t, groups, grid, smem};
+        return true;
+    }
+    return false;
+}
+
 template <int G>
-static cudaError_t launch_infer(const FcInferArgs& a, int sm_count, cudaStream_t stream) {
-    const int groups = kFcThreads / G;
-    const size_t smem = (((size_t)a.net.blob_floats + 3) & ~(size_t)3) * 4 + (size_t)groups * (4 * a.net.maxw + 4) * 4;
+static cudaError_t launch_infer(const FcInferArgs& a, int sm_count, size_t smem_cap, cudaStream_t stream) {
+    FcInferPlan p;
+    if (!fc_infer_plan(a.net.blob_floats, a.net.maxw, G, a.n, sm_count, smem_cap, &p)) return cudaErrorInvalidConfiguration;
     auto kern = fc_inference_kernel<G>;
     static size_t attr_smem = 0;
-    if (attr_smem < smem) {
-        cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (attr_smem < p.smem) {
+        const cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem);
         if (err != cudaSuccess) return err;
-        attr_smem = smem;
+        attr_smem = p.smem;
     }
-    int grid = (a.n + groups - 1) / groups;
-    if (grid > sm_count * 8) grid = sm_count * 8;
-    if (grid < 1) grid = 1;
-    kern<<<grid, kFcThreads, smem, stream>>>(a);
+    kern<<<p.grid, p.threads, p.smem, stream>>>(a);
     return cudaGetLastError();
 }
 
 // The lane-group width must equal the fused search kernel's: the fp32 reductions (softmax and
 // support sums) are shuffle trees over G lanes, so the same G gives bit-identical outputs.
-cudaError_t launch_fc_inference(const FcInferArgs& a, int group, int sm_count, cudaStream_t stream) {
+cudaError_t launch_fc_inference(const FcInferArgs& a, int group, int sm_count, size_t smem_cap, cudaStream_t stream) {
     switch (group) {
-        case 4: return launch_infer<4>(a, sm_count, stream);
-        case 8: return launch_infer<8>(a, sm_count, stream);
-        case 16: return launch_infer<16>(a, sm_count, stream);
-        case 32: return launch_infer<32>(a, sm_count, stream);
+        case 4: return launch_infer<4>(a, sm_count, smem_cap, stream);
+        case 8: return launch_infer<8>(a, sm_count, smem_cap, stream);
+        case 16: return launch_infer<16>(a, sm_count, smem_cap, stream);
+        case 32: return launch_infer<32>(a, sm_count, smem_cap, stream);
     }
     return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_fc_inference_pool(const FcNet& net, const float* blob, const InferCall& c, int group, int sm_count, cudaStream_t stream) {
+cudaError_t launch_fc_inference_pool(const FcNet& net, const float* blob, const InferCall& c, int group, int sm_count, size_t smem_cap,
+                                     cudaStream_t stream) {
     FcInferArgs a{};
     a.n = c.n; a.recurrent = c.recurrent; a.net = net; a.blob = blob; a.in = c.in; a.action = c.action;
     a.gather_parent = c.gather_parent; a.pool_hidden = c.pool_hidden; a.pool_stride = c.pool_stride; a.out_slot = c.out_slot;
     a.value_logits = c.value_logits; a.reward_logits = c.reward_logits; a.policy_logits = c.policy_logits;
     a.hidden = c.hidden; a.value = c.value; a.reward = c.reward;
-    return launch_fc_inference(a, group, sm_count, stream);
+    return launch_fc_inference(a, group, sm_count, smem_cap, stream);
 }
 
 }  // namespace mz

@@ -88,6 +88,80 @@ struct PhaseClock {
 };
 #endif
 
+// ---- the search's two network calls (fc_search_kernel and fc_debug_net_kernel run these)
+// A tap sees each intermediate vector of a call while it is still in shared memory - tap(what, v, n), v[0..n) - and may only
+// read it: the next write to that scratch follows a group barrier.  The search passes NoTap; mz_debug_fc_net copies them out.
+enum { kTapRaw, kTapReward, kTapPolicy, kTapValue };
+struct NoTap { MZ_DEVINL void operator()(int, const float*, int) const {} };
+
+// Root: representation (models.py:133-145) of obs into hidden (rescaled, zero padded to a multiple of 4), then prediction
+// (models.py:128-131): this lane's policy logit (0 in lanes >= A) and the scalarised value.  s0, s1, s2: scratch of maxw.
+// E and S are the kernel's net.E and net.S, read once per launch: re-reading them through `net` here changes the search
+// kernel's code (fc_search_kernel's SASS is the same as with these blocks written inline).
+template <int G, typename Tap>
+MZ_DEVINL void fc_root_inference(const FcNet& net, const float* blob, const float* obs, float* hidden, float* s0, float* s1,
+                                 float* s2, int E, int S, int A, float& logit, float& value, Tap&& tap) {
+    const int lane = LaneGroup<G>::lane();
+    load_vector<G>(obs, s1, net.obs_elems);
+    float* raw = mlp_forward<G>(net.rep, blob, s1, s0, s1, s2);
+    tap(kTapRaw, raw, E);
+    rescale_unit_range<G>(raw, hidden, E);
+    float* pol = mlp_forward<G>(net.pol, blob, hidden, s0, s1, s2);
+    logit = (lane < A) ? pol[lane] : 0.0f;
+    tap(kTapPolicy, pol, A);
+    LaneGroup<G>::sync();
+    float* val = mlp_forward<G>(net.val, blob, hidden, s0, s1, s2);
+    value = support_to_scalar_group<G>(val, S);
+    tap(kTapValue, val, 2 * S + 1);
+    LaneGroup<G>::sync();
+}
+
+// One simulation's recurrent inference (models.py:147-170, 128-131): dynamics of (h, action) into hn (rescaled, zero padded),
+// this lane's prior (softmax over the first A lanes), the scalarised value and reward.  SH = FcFixedShape runs the unrolled
+// fc_recurrent_fixed; otherwise the descriptors walk, with the three heads side by side (mlp_forward_multi) when they have
+// equal depth (fused_heads) and one after the other when not.  hb: the heads' ping-pong vectors, 3 x 2 of maxw.
+template <int G, typename SH, typename Tap>
+MZ_DEVINL void fc_sim_inference(const FcNet& net, const float* blob, const float* h, int action, float* hn, float* s0, float* s1,
+                                float* s2, float* const (&hb)[3][2], bool fused_heads, int E, int S, int A, float& logit,
+                                float& prior, float& value, float& reward, Tap&& tap) {
+    const int lane = LaneGroup<G>::lane();
+    const int F = 2 * S + 1;
+    if constexpr (SH::kEnabled) {
+        fc_recurrent_fixed<G, SH>(net, blob, h, action, hn, s0, s1, hb[0][0], hb[1][0], hb[2][0], prior, value, reward);
+        tap(kTapRaw, s1, E);                            // the logits stay in registers
+    } else {
+        float* raw = mlp_forward<G>(net.dyn, blob, h, s0, s1, s2, action);
+        if (fused_heads) {
+            // rescale first, then reward (raw state), policy and value (rescaled state) side by side
+            rescale_unit_range<G>(raw, hn, E);
+            const MlpDesc* const ds[3] = {&net.rew, &net.pol, &net.val};
+            const float* const xs[3] = {raw, hn, hn};
+            float* outs[3];
+            mlp_forward_multi<G, 3>(ds, blob, xs, hb, outs);
+            logit = (lane < A) ? outs[1][lane] : 0.0f;
+            support_to_scalar_group2<G>(outs[2], outs[0], S, value, reward);
+            tap(kTapRaw, raw, E); tap(kTapReward, outs[0], F); tap(kTapPolicy, outs[1], A); tap(kTapValue, outs[2], F);
+            LaneGroup<G>::sync();
+        } else {
+            // reward head reads the un-normalised next state
+            float* rl = mlp_forward<G>(net.rew, blob, raw, s0, s1, nullptr);
+            reward = support_to_scalar_group<G>(rl, S);
+            tap(kTapRaw, raw, E); tap(kTapReward, rl, F);
+            LaneGroup<G>::sync();
+            rescale_unit_range<G>(raw, hn, E);
+            float* pol = mlp_forward<G>(net.pol, blob, hn, s0, s1, s2);
+            logit = (lane < A) ? pol[lane] : 0.0f;
+            tap(kTapPolicy, pol, A);
+            LaneGroup<G>::sync();
+            float* vl = mlp_forward<G>(net.val, blob, hn, s0, s1, s2);
+            value = support_to_scalar_group<G>(vl, S);
+            tap(kTapValue, vl, F);
+            LaneGroup<G>::sync();
+        }
+        prior = group_softmax_masked<G>(logit, lane < A);
+    }
+}
+
 template <typename SH>
 constexpr int fixed_actions() {
     if constexpr (SH::kEnabled) return SH::A;
@@ -134,7 +208,7 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
     t.path_reward = reinterpret_cast<float*>(mine + L.path_reward);
     float* s_hidden = reinterpret_cast<float*>(mine + L.hidden);
     float* s_act = reinterpret_cast<float*>(mine + L.act);
-    const int E = a.net.E, F = a.net.F, S = a.net.S, maxw = a.net.maxw;
+    const int E = a.net.E, S = a.net.S, maxw = a.net.maxw;
     const int Epad = (E + 3) & ~3;
     float* s0 = s_act;
     float* s1 = s_act + maxw;
@@ -170,17 +244,8 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
             root_value = a.teacher.root_value[g];
             root_reward = a.teacher.root_reward[g];
         } else {
-            // representation (models.py:133-145) -> hidden[0]
-            load_vector<G>(a.obs + (size_t)g * a.net.obs_elems, s1, a.net.obs_elems);
-            float* raw = mlp_forward<G>(a.net.rep, s_blob, s1, s0, s1, s2);
-            rescale_unit_range<G>(raw, s_hidden, E);
-            // prediction (models.py:128-131)
-            float* pol = mlp_forward<G>(a.net.pol, s_blob, s_hidden, s0, s1, s2);
-            logit = (lane < A) ? pol[lane] : 0.0f;
-            LaneGroup<G>::sync();
-            float* val = mlp_forward<G>(a.net.val, s_blob, s_hidden, s0, s1, s2);
-            root_value = support_to_scalar_group<G>(val, S);
-            LaneGroup<G>::sync();
+            fc_root_inference<G>(a.net, s_blob, a.obs + (size_t)g * a.net.obs_elems, s_hidden, s0, s1, s2, E, S, A, logit, root_value,
+                                 NoTap{});
             root_reward = inverse_value_transform(0.0f);     // log(one-hot centre), models.py:176-183
         }
         float prior;
@@ -207,38 +272,9 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
                 reward = a.teacher.reward[(size_t)g * N + sim];
                 prior = (lane < A) ? a.teacher.priors[((size_t)g * N + sim) * A + lane] : 0.0f;
             } else {
-                // dynamics (models.py:147-170)
-                const float* h = s_hidden + (size_t)leaf.parent_exp * Epad;
-                float* hn = s_hidden + (size_t)t.n_expanded * Epad;
-                if constexpr (SH::kEnabled) {
-                    fc_recurrent_fixed<G, SH>(a.net, s_blob, h, leaf.action, hn, s0, s1, hb[0][0], hb[1][0], hb[2][0], prior, value, reward);
-                } else {
-                float* raw = mlp_forward<G>(a.net.dyn, s_blob, h, s0, s1, s2, leaf.action);
-                if (fused_heads) {
-                    // rescale first, then reward (raw state), policy and value (rescaled state) side by side
-                    rescale_unit_range<G>(raw, hn, E);
-                    const MlpDesc* const ds[3] = {&a.net.rew, &a.net.pol, &a.net.val};
-                    const float* const xs[3] = {raw, hn, hn};
-                    float* outs[3];
-                    mlp_forward_multi<G, 3>(ds, s_blob, xs, hb, outs);
-                    logit = (lane < A) ? outs[1][lane] : 0.0f;
-                    support_to_scalar_group2<G>(outs[2], outs[0], S, value, reward);
-                    LaneGroup<G>::sync();
-                } else {
-                    // reward head reads the un-normalised next state
-                    float* rl = mlp_forward<G>(a.net.rew, s_blob, raw, s0, s1, nullptr);
-                    reward = support_to_scalar_group<G>(rl, S);
-                    LaneGroup<G>::sync();
-                    rescale_unit_range<G>(raw, hn, E);
-                    float* pol = mlp_forward<G>(a.net.pol, s_blob, hn, s0, s1, s2);
-                    logit = (lane < A) ? pol[lane] : 0.0f;
-                    LaneGroup<G>::sync();
-                    float* vl = mlp_forward<G>(a.net.val, s_blob, hn, s0, s1, s2);
-                    value = support_to_scalar_group<G>(vl, S);
-                    LaneGroup<G>::sync();
-                }
-                }
-                if constexpr (!SH::kEnabled) prior = group_softmax_masked<G>(logit, lane < A);
+                fc_sim_inference<G, SH>(a.net, s_blob, s_hidden + (size_t)leaf.parent_exp * Epad, leaf.action,
+                                        s_hidden + (size_t)t.n_expanded * Epad, s0, s1, s2, hb, fused_heads, E, S, A, logit, prior, value, reward,
+                                        NoTap{});
             }
             ph.mark(kPhNet);
             if (a.trace.depth && own) {
@@ -292,7 +328,6 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
         ph.finish();
         LaneGroup<G>::sync();
     }
-    (void)F;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -381,9 +416,12 @@ static cudaError_t prepare_one(const FcSearchArgs& a, bool one_level, int sm_cou
 // shapes with a fully unrolled network path: games/cartpole.py (encoding 8, hidden 16, support 10, 2 actions)
 using CartPoleShape = FcFixedShape<8, 16, 10, 2>;
 
+// Does the search run the unrolled network of CartPoleShape at this lane-group width?
+static bool fc_uses_fixed(const FcNet& net, int G) { return (G == 16 || G == 32) && fc_matches_fixed<CartPoleShape>(net); }
+
 static cudaError_t prepare_fc_search(const FcSearchArgs& a, int group, bool teacher, bool generic, bool one_level,
                                      int sm_count, FcLaunchState* st, FcPrepared* p) {
-    if (!teacher && !generic && fc_matches_fixed<CartPoleShape>(a.net)) {
+    if (!teacher && !generic && fc_uses_fixed(a.net, group)) {
         // (a single player: the backup's value recurrence and its signs simplify)
         if (group == 16 && a.P == 1) return prepare_one<16, false, CartPoleShape, 1>(a, one_level, sm_count, st, p);
         if (group == 16) return prepare_one<16, false, CartPoleShape>(a, one_level, sm_count, st, p);
@@ -428,6 +466,138 @@ cudaError_t launch_fc_search(const FcSearchArgs& a_in, int group, bool teacher, 
         st->last = p.info;
     }
     return err;
+}
+
+// ------------------------------------------------------------------------------------------
+// mz_debug_fc_net: the network calls of the search and of fc_inference_kernel on their own
+// ------------------------------------------------------------------------------------------
+// Copies each tapped vector of the group's sample to global memory (the rows of samples past the last one stay untouched).
+struct CopyTap {
+    const FcDebugArgs* a;
+    int g, lane, step;
+    bool own;
+    MZ_DEVINL void operator()(int what, const float* v, int n) const {
+        float* dst = what == kTapRaw ? a->raw : what == kTapReward ? a->reward_logits : what == kTapPolicy ? a->policy_logits : a->value_logits;
+        if (!dst || !own) return;
+        for (int i = lane; i < n; i += step) dst[(size_t)g * n + i] = v[i];
+    }
+};
+
+// The search's root evaluation or one simulation's network call for each of a.n samples, with the shared-memory layout of
+// fc_search_kernel (the blob, then per game the region of game_smem_layout, here for a one-simulation tree), every game's
+// region overwritten with NaN bytes before the first layer.  One warp per CTA; the groups stride over the samples as in the
+// search.  force_split walks the descriptors with the heads one after the other even for the fixed shape or heads of equal
+// depth (the network never does).
+template <int G, typename SH>
+__global__ void __launch_bounds__(32) fc_debug_net_kernel(const __grid_constant__ FcDebugArgs a) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    float* s_blob = reinterpret_cast<float*>(smem);
+    for (int i = threadIdx.x; i < a.net.blob_floats; i += blockDim.x) s_blob[i] = a.blob[i];
+    __syncthreads();
+    const int E = a.net.E, A = a.net.A, maxw = a.net.maxw, Epad = (E + 3) & ~3;
+    const GameSmem L = game_smem_layout(1, A, E, maxw, true);
+    const int groups_per_cta = blockDim.x / G;
+    const int gi = threadIdx.x / G;
+    const int lane = LaneGroup<G>::lane();
+    unsigned char* mine = smem + ((a.net.blob_floats * 4 + 15) & ~15) + (size_t)gi * L.bytes;
+    float* s_hidden = reinterpret_cast<float*>(mine + L.hidden);
+    float* s_act = reinterpret_cast<float*>(mine + L.act);
+    float* s0 = s_act;
+    float* s1 = s_act + maxw;
+    float* s2 = s_act + 2 * maxw;
+    float* const hb[3][2] = {{s_act + 3 * maxw, s_act + 4 * maxw}, {s_act + 5 * maxw, s_act + 6 * maxw},
+                             {s_act + 7 * maxw, s_act + 8 * maxw}};
+    const bool fused_heads = (a.net.rew.n == a.net.pol.n) && (a.net.pol.n == a.net.val.n) && !a.force_split;
+    const int warp_first = (int)blockIdx.x * groups_per_cta + (int)(threadIdx.x & ~31u) / G;
+    for (int g0 = warp_first; g0 < a.n; g0 += gridDim.x * groups_per_cta) {
+        const int g_own = g0 + gi - (int)(threadIdx.x & ~31u) / G;
+        const bool own = g_own < a.n;
+        const int g = own ? g_own : a.n - 1;
+        for (int i = lane; i < L.bytes / 4; i += G) reinterpret_cast<unsigned*>(mine)[i] = 0xFFFFFFFFu;
+        LaneGroup<G>::sync();
+        const CopyTap tap{&a, g, lane, G, own};
+        float logit = 0.0f, prior, value, reward = 0.0f;
+        float* hn = s_hidden;
+        if (a.route == MZ_FC_SEARCH_ROOT) {
+            fc_root_inference<G>(a.net, s_blob, a.in + (size_t)g * a.net.obs_elems, s_hidden, s0, s1, s2, E, a.net.S, A, logit, value,
+                                 tap);
+            prior = group_softmax_masked<G>(logit, lane < A);
+        } else {
+            load_vector<G>(a.in + (size_t)g * E, s_hidden, E);
+            hn = s_hidden + Epad;
+            fc_sim_inference<G, SH>(a.net, s_blob, s_hidden, a.action[g], hn, s0, s1, s2, hb, fused_heads, E, a.net.S, A, logit, prior, value,
+                                    reward, tap);
+        }
+        if (own) {
+            if (a.hidden) for (int i = lane; i < E; i += G) a.hidden[(size_t)g * E + i] = hn[i];
+            if (a.prior && lane < A) a.prior[(size_t)g * A + lane] = prior;
+            if (lane == 0) {
+                if (a.value) a.value[g] = value;
+                if (a.reward && a.route == MZ_FC_SEARCH_SIM) a.reward[g] = reward;
+            }
+        }
+        LaneGroup<G>::sync();
+    }
+}
+
+bool fc_debug_plan(const FcNet& net, int G, int route, bool force_split, int n, int sm_count, size_t smem_cap, int64_t* plan,
+                   std::string* err) {
+    if (G != 4 && G != 8 && G != 16 && G != 32) { *err = "the lane group must be 4, 8, 16 or 32"; return false; }
+    if (n < 1 || sm_count < 1) { *err = "bad batch or SM count"; return false; }
+    if (route == MZ_FC_INFER_INITIAL || route == MZ_FC_INFER_RECURRENT || route == MZ_FC_INFER_POOL) {
+        FcInferPlan p;
+        if (!fc_infer_plan(net.blob_floats, net.maxw, G, n, sm_count, smem_cap, &p)) {
+            *err = "fc_inference_kernel needs " + std::to_string(fc_infer_smem(net.blob_floats, net.maxw, 32 / G)) +
+                   " bytes of shared memory for one warp, the device allows " + std::to_string(smem_cap);
+            return false;
+        }
+        const int64_t out[5] = {MZ_FC_PATH_INFER, G, p.threads, p.grid, (int64_t)p.smem};
+        for (int i = 0; i < 5; ++i) plan[i] = out[i];
+        return true;
+    }
+    if (route != MZ_FC_SEARCH_ROOT && route != MZ_FC_SEARCH_SIM) { *err = "unknown route"; return false; }
+    if (net.A > G) { *err = "the search needs one lane per action (action_space <= lane group)"; return false; }
+    const bool fixed = fc_uses_fixed(net, G) && !force_split;
+    const bool fused = net.rew.n == net.pol.n && net.pol.n == net.val.n && !force_split;
+    const GameSmem L = game_smem_layout(1, net.A, net.E, net.maxw, true);
+    const size_t smem = (size_t)((net.blob_floats * 4 + 15) & ~15) + (size_t)(32 / G) * L.bytes;
+    if (smem > smem_cap) {
+        *err = "the search's network call needs " + std::to_string(smem) + " bytes of shared memory, the device allows " +
+               std::to_string(smem_cap);
+        return false;
+    }
+    const int groups = 32 / G;
+    const int grid = std::min((n + groups - 1) / groups, 8 * sm_count);
+    const int64_t out[5] = {fixed ? MZ_FC_PATH_FIXED : fused ? MZ_FC_PATH_FUSED : MZ_FC_PATH_SPLIT, G, 32, grid, (int64_t)smem};
+    for (int i = 0; i < 5; ++i) plan[i] = out[i];
+    return true;
+}
+
+template <int G, typename SH>
+static cudaError_t launch_debug(const FcDebugArgs& a, int grid, size_t smem, cudaStream_t stream) {
+    auto kern = fc_debug_net_kernel<G, SH>;
+    cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (err != cudaSuccess) return err;
+    kern<<<grid, 32, smem, stream>>>(a);
+    return cudaGetLastError();
+}
+
+// the search routes of mz_debug_fc_net (plan from fc_debug_plan)
+cudaError_t launch_fc_debug_net(const FcDebugArgs& a, int G, const int64_t* plan, cudaStream_t stream) {
+    const int grid = (int)plan[3];
+    const size_t smem = (size_t)plan[4];
+    if (plan[0] == MZ_FC_PATH_FIXED) {
+        if (G == 16) return launch_debug<16, CartPoleShape>(a, grid, smem, stream);
+        if (G == 32) return launch_debug<32, CartPoleShape>(a, grid, smem, stream);
+        return cudaErrorInvalidValue;
+    }
+    switch (G) {
+        case 4: return launch_debug<4, FcGenericShape>(a, grid, smem, stream);
+        case 8: return launch_debug<8, FcGenericShape>(a, grid, smem, stream);
+        case 16: return launch_debug<16, FcGenericShape>(a, grid, smem, stream);
+        case 32: return launch_debug<32, FcGenericShape>(a, grid, smem, stream);
+    }
+    return cudaErrorInvalidValue;
 }
 
 #ifdef MZ_FC_PHASES

@@ -4,6 +4,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <string>
 #include <vector>
 
 #include "../../include/mzb200.h"
@@ -100,7 +101,34 @@ struct FcInferArgs {
     int pool_stride, out_slot;
     float *value_logits, *reward_logits, *policy_logits, *hidden, *value, *reward;
 };
-cudaError_t launch_fc_inference(const FcInferArgs& a, int group, int sm_count, cudaStream_t stream);
+// smem_cap: the device's shared memory per block (opt-in), which the CTA is sized to (fc_infer_plan)
+cudaError_t launch_fc_inference(const FcInferArgs& a, int group, int sm_count, size_t smem_cap, cudaStream_t stream);
+
+// Launch of fc_inference_kernel<G> over n samples: `threads` per CTA of `groups` samples, `grid` CTAs (at most 8 per SM; the
+// CTAs stride over the rest), `smem` bytes: the weight blob, then 4 maxw + 4 floats of scratch per group.
+struct FcInferPlan { int threads, groups, grid; size_t smem; };
+inline size_t fc_infer_smem(int blob_floats, int maxw, int groups) {
+    return (((size_t)blob_floats + 3) & ~(size_t)3) * 4 + (size_t)groups * (4 * (size_t)maxw + 4) * 4;
+}
+// False when not even one warp's groups fit next to the blob in smem_cap bytes (mz_load_weights refuses such a net).
+bool fc_infer_plan(int blob_floats, int maxw, int G, int n, int sm_count, size_t smem_cap, FcInferPlan* plan);
+
+// mz_debug_fc_net: one network call of the search (routes MZ_FC_SEARCH_*) for each of n samples.  Output rows of n x E
+// (raw: the next or initial state before the rescale; hidden: after it), n x F / n x A logits, n x A priors and n scalars;
+// a null pointer is not written.
+struct FcDebugArgs {
+    int n, route;
+    bool force_split;
+    FcNet net;
+    const float* blob;
+    const float* in;            // obs [n, obs_elems] (root) or parent states [n, E] (simulation)
+    const int32_t* action;      // [n] (simulation)
+    float *raw, *hidden, *reward_logits, *value_logits, *policy_logits, *prior, *value, *reward;
+};
+// plan[5] = {path (MZ_FC_PATH_*), G, threads, grid, smem} of a route, or false and the reason
+bool fc_debug_plan(const FcNet& net, int G, int route, bool force_split, int n, int sm_count, size_t smem_cap, int64_t* plan,
+                   std::string* err);
+cudaError_t launch_fc_debug_net(const FcDebugArgs& a, int G, const int64_t* plan, cudaStream_t stream);
 
 struct FcLaunchInfo { int grid, block, ctas_per_sm, group; size_t smem; };
 

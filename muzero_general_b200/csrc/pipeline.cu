@@ -7,7 +7,8 @@ namespace mz {
 
 int run_stepwise_search(const MzNetDesc& net, const MzSearchDesc& search, int pool_n, const NodePool& pool, const double* d_pbc,
                         const double* d_sqrt, const double* d_ucb, const FcNet& fc, const float* d_fc_blob, ResNetDevice* res,
-                        const SearchCall& call, int fc_group, int sm_count, cudaStream_t stream, int64_t* launches, std::string* err) {
+                        const SearchCall& call, int fc_group, int sm_count, size_t smem_cap, cudaStream_t stream, int64_t* launches,
+                        std::string* err) {
     // N = simulations of this call; NP = the layout size of the pool / tables (N + extra_expansions)
     const int n = call.n, N = search.num_simulations, NP = pool_n, A = net.action_space;
     const bool teacher = call.teacher.root_value != nullptr;
@@ -19,7 +20,7 @@ int run_stepwise_search(const MzNetDesc& net, const MzSearchDesc& search, int po
     auto infer = [&](const InferCall& c) -> int {
         if (net.kind == MZ_NET_FC) {
             kt_begin(KT_OTHER, stream);
-            cudaError_t e = launch_fc_inference_pool(fc, d_fc_blob, c, fc_group, sm_count, stream);
+            cudaError_t e = launch_fc_inference_pool(fc, d_fc_blob, c, fc_group, sm_count, smem_cap, stream);
             kt_end(stream);
             if (e != cudaSuccess) return cuda_fail("fc_inference", e);
             *launches += 1;

@@ -140,12 +140,14 @@ void resnet_use_strict(ResNetDevice* r);                // fp32 CUDA-core towers
 int resnet_state_elems(const ResNetDevice* r);        // floats per stored hidden state in the pool
 int resnet_states_to_nchw(ResNetDevice* r, const float* states, int count, float* out, cudaStream_t stream);
 
-cudaError_t launch_fc_inference_pool(const FcNet& net, const float* blob, const InferCall& c, int group, int sm_count, cudaStream_t stream);
+cudaError_t launch_fc_inference_pool(const FcNet& net, const float* blob, const InferCall& c, int group, int sm_count, size_t smem_cap,
+                                     cudaStream_t stream);
 
 int resnet_states_from_nchw(ResNetDevice* r, const float* dense, int count, float* states, cudaStream_t stream);
 
 int run_stepwise_search(const MzNetDesc& net, const MzSearchDesc& search, int pool_n, const NodePool& pool, const double* d_pbc,
                         const double* d_sqrt, const double* d_ucb, const FcNet& fc, const float* d_fc_blob, ResNetDevice* res,
-                        const SearchCall& call, int fc_group, int sm_count, cudaStream_t stream, int64_t* launches, std::string* err);
+                        const SearchCall& call, int fc_group, int sm_count, size_t smem_cap, cudaStream_t stream, int64_t* launches,
+                        std::string* err);
 
 }  // namespace mz

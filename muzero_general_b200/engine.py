@@ -1067,3 +1067,63 @@ def debug_heads(x, heads, site, layout="dense", route="planned", parts=1, pool_s
     if state is not None:
         out["state"] = state
     return out
+
+
+FC_ROUTES = {"infer_initial": 0, "infer_recurrent": 1, "infer_pool": 2, "search_root": 3, "search_sim": 4}
+FC_PATH_NAMES = {0: "infer", 1: "fixed", 2: "fused", 3: "split"}
+FC_NET_PLAN = ("path", "G", "threads", "grid", "smem")
+H100_SMEM_OPTIN = 232448            # cudaDevAttrMaxSharedMemoryPerBlockOptin of an H100 (227 KB)
+
+
+def debug_fc_net_plan(spec, G, route, n, force_split=False, sm_count=132, smem_cap=H100_SMEM_OPTIN):
+    """Launch plan of one fully-connected network route (mz_debug_fc_net_plan, host only) for n samples with G lanes each:
+    (a dict of FC_NET_PLAN, path "infer" = fc_inference_kernel<G>, "fixed" / "fused" / "split" = the search's network call,
+    "") or (None, the reason) when the shape is refused.  ``spec`` is an FC NetSpec; ``force_split`` makes the search routes
+    walk the layer descriptors with the heads one after the other (the network never does)."""
+    lib = _lib.load_library()
+    out = (C.c_int64 * 5)()
+    if not lib.mz_debug_fc_net_plan(C.byref(net_desc(spec)), spec.obs_elems, G, FC_ROUTES[route], int(force_split), n, sm_count,
+                                    smem_cap, out):
+        return None, lib.mz_last_error(None).decode()
+    plan = dict(zip(FC_NET_PLAN, out))
+    plan["path"] = FC_PATH_NAMES[plan["path"]]
+    return plan, ""
+
+
+def debug_fc_net(spec, weights, G, route, x, actions=None, parents=None, pool_stride=1, out_slot=0, force_split=False, device=0):
+    """One fully-connected network route through mz_debug_fc_net; numpy in and out.  ``weights``: the five MLPs' tensors named
+    as in the reference state_dict.  ``x``: observations [n, obs_elems] (infer_initial, search_root) or parent states [n, E];
+    ``actions`` [n] on the recurrent routes; on infer_pool ``parents`` [n] is the pool slot each parent is put in and
+    ``out_slot`` the slot the kernel writes.  Returns a dict of "raw" (the state before the rescale, search routes), "hidden",
+    "reward_logits", "value_logits", "policy_logits", "prior", "value", "reward", "pool" (infer_pool, [n, pool_stride, E])
+    and "plan" as debug_fc_net_plan gives it.  Every output starts as NaN bytes; what a route does not write keeps them."""
+    lib = _lib.load_library()
+    x = numpy.ascontiguousarray(x, numpy.float32)
+    n = x.shape[0]
+    E, A, F = spec.encoding, spec.action_space, spec.full_support
+    keep, arr = [], (_lib.MzTensor * len(weights))()
+    for i, (name, a) in enumerate(weights.items()):
+        a = numpy.ascontiguousarray(a, numpy.float32)
+        keep.append((name.encode(), a))
+        arr[i].name, arr[i].data, arr[i].numel = keep[-1][0], a.ctypes.data, a.size
+    out = {"raw": numpy.empty((n, E), numpy.float32), "hidden": numpy.empty((n, E), numpy.float32),
+           "reward_logits": numpy.empty((n, F), numpy.float32), "value_logits": numpy.empty((n, F), numpy.float32),
+           "policy_logits": numpy.empty((n, A), numpy.float32), "prior": numpy.empty((n, A), numpy.float32),
+           "value": numpy.empty(n, numpy.float32), "reward": numpy.empty(n, numpy.float32)}
+    pool = numpy.empty((n, pool_stride, E), numpy.float32) if route == "infer_pool" else None
+    act = None if actions is None else numpy.ascontiguousarray(actions, numpy.int32)
+    par = None if parents is None else numpy.ascontiguousarray(parents, numpy.int32)
+    plan = (C.c_int64 * 5)()
+    ptr = lambda a: None if a is None else a.ctypes.data        # noqa: E731
+    rc = lib.mz_debug_fc_net(device, C.byref(net_desc(spec)), spec.obs_elems, arr, len(weights), G, FC_ROUTES[route],
+                             int(force_split), n, x.ctypes.data, ptr(act), ptr(par), pool_stride, out_slot,
+                             *[out[k].ctypes.data for k in ("raw", "hidden", "reward_logits", "value_logits", "policy_logits",
+                                                             "prior", "value", "reward")], ptr(pool), plan)
+    if rc != 0:
+        raise _lib.MzError(rc, lib.mz_last_error(None).decode())
+    p = dict(zip(FC_NET_PLAN, plan))
+    p["path"] = FC_PATH_NAMES[p["path"]]
+    out["plan"] = p
+    if pool is not None:
+        out["pool"] = pool
+    return out
