@@ -548,6 +548,8 @@ enum { MZ_ENV_CARTPOLE = 0, MZ_ENV_TICTACTOE = 1, MZ_ENV_CONNECT4 = 2, MZ_ENV_GO
        MZ_ENV_SIMPLE_GRID = 5 };
 /* not an environment of the library: any game, stepped by the caller (mz_selfplay_begin_host) */
 #define MZ_ENV_HOST 6
+/* Gridworld (games/gridworld.py), a device environment numbered after MZ_ENV_HOST */
+#define MZ_ENV_GRIDWORLD 7
 
 typedef struct MzSelfPlayDesc {
     int32_t env;                  /* MZ_ENV_*: games/cartpole.py:131-174 (restated cart-pole physics),
@@ -560,7 +562,14 @@ typedef struct MzSelfPlayDesc {
                                      stream tag 0x7169E006 at counter (game id, draw k, 0, game id >> 32): card =
                                      1 + floor(12 u), value min(card, 10); draw 0 = the player's first card, 1 = the
                                      dealer's, then hits and the dealer's draws in the reference's order),
-                                     games/simple_grid.py:125-229 (one player; 3x3 grid, one-hot observation of 9) */
+                                     games/simple_grid.py:125-229 (one player; 3x3 grid, one-hot observation of 9),
+                                     MZ_ENV_GRIDWORLD: games/gridworld.py's restatement of gym_minigrid's
+                                     MiniGrid-Empty-Random-6x6-v0 behind ImgObsWrapper (one player; 3 actions; the
+                                     7x7x3 view [x'][y'][c] as 7 planes of 7x3; reward 1 - 0.9 * step_count / 144 in
+                                     fp64 on reaching the goal, rounded to float; reward_scale unused; placement
+                                     from the Philox stream tag 0x7169E007 at counter (game id, draw k, 0, game id
+                                     >> 32): draw 0 gives the floor(15 u)-th free cell, x = 1 + i % 4,
+                                     y = 1 + i / 4, draw 1 the direction floor(4 u)) */
     int32_t max_moves;            /* config.max_moves */
     int32_t temperature_threshold;/* config.temperature_threshold, 0 = None (self_play.py:153-156) */
     int32_t reward_scale;         /* board games: reward of the winning move (tictactoe.py:144: 20, connect4.py:144: 10,
@@ -637,7 +646,7 @@ enum { MZ_OPPONENT_SELF = 0, MZ_OPPONENT_EXPERT = 1, MZ_OPPONENT_RANDOM = 2 };
  * mz_selfplay_begin with the opponent playing every move whose to_play is not muzero_player, in the same step, so
  * every search is at MuZero's turn (the opponent opens a game when muzero_player is 1).  max_moves counts both sides'
  * moves, and so does MzSelfPlayStats.env_steps.  mz_selfplay_begin(h, d) is mz_selfplay_begin_vs(h, d, MZ_OPPONENT_SELF, 0).
- * Refused: an opponent on a one-player game (CartPole, Twenty-One, Simple Grid), muzero_player outside {0, 1}, td_steps > 0
+ * Refused: an opponent on a one-player game (CartPole, Twenty-One, Simple Grid, Gridworld), muzero_player outside {0, 1}, td_steps > 0
  * with an opponent, stacked_observations < 0, a handle whose action space or obs_elems does not fit the environment and
  * stacked_observations (MZ_EINVAL); an unknown opponent, EXPERT on Gomoku (MZ_EUNSUPPORTED).  The opponent's moves are
  * part of the stacked history like MuZero's. */

@@ -131,6 +131,7 @@ class MzSelfPlayPeek(C.Structure):
 
 MZ_ENV_CARTPOLE, MZ_ENV_TICTACTOE, MZ_ENV_CONNECT4, MZ_ENV_GOMOKU, MZ_ENV_TWENTYONE, MZ_ENV_SIMPLE_GRID = 0, 1, 2, 3, 4, 5
 MZ_ENV_HOST = 6
+MZ_ENV_GRIDWORLD = 7
 MZ_OPPONENT_SELF, MZ_OPPONENT_EXPERT, MZ_OPPONENT_RANDOM = 0, 1, 2
 MZ_STAGED_HEADER_BYTES = 32
 

@@ -18,13 +18,17 @@
 //              reward_scale * get_reward (Game.step's x10)
 //   SimpleGrid games/simple_grid.py:125-229: 3x3 grid from (0, 0), action 0 = row + 1, 1 = column + 1, a move off the
 //              edge changes nothing; one-hot observation of 9; reward_scale and done on reaching (2, 2)
+//   Gridworld  games/gridworld.py's restatement of gym_minigrid's MiniGrid-Empty-Random-6x6-v0 + ImgObsWrapper (the
+//              rules are written down there): 6x6 room, goal (4, 4), turn left / turn right / forward; reward
+//              1 - 0.9 * step_count / 144 on reaching the goal, done there or at 144 steps; 7x7x3 egocentric view
 // State per slot lives in HBM (a few dozen bytes); per-move records go to per-slot struct-of-arrays buffers
 // [B][max_moves] and leave the device only when the game ends, as one packed block written by a warp straight into
 // mapped pinned host memory (no per-move D2H, no host-side bookkeeping per move).
 //
 // Random draws: Philox4x32-10 keyed by (seed, global game id, move): root noise and first-simulation ties inside the
 // search (tree.cuh), the action sample here (tag kTagAction), CartPole's reset state (tag kTagReset), the opponent's
-// random default move in test-mode games (tag kTagOpponent), Twenty-One's cards (tag kTagCard, counter (game, draw k)).
+// random default move in test-mode games (tag kTagOpponent), Twenty-One's cards (tag kTagCard, counter (game, draw k)),
+// Gridworld's placement (tag kTagPlace, counter (game, draw k)).
 //
 // Test-mode games (mz_selfplay_begin_vs, the reference's play_game(0, ..., opponent, muzero_player),
 // self_play.py:110-183): the opponent's move is played by the thread that played MuZero's, right after it (or by
@@ -62,6 +66,7 @@ namespace mz {
 constexpr uint32_t kTagReset = 0x7169E004u;
 constexpr uint32_t kTagOpponent = 0x7169E005u;
 constexpr uint32_t kTagCard = 0x7169E006u;
+constexpr uint32_t kTagPlace = 0x7169E007u;
 constexpr int kMaxCells = 256;             // board cells per slot (Gomoku: up to 16 x 16)
 
 struct SpDev {
@@ -84,7 +89,8 @@ struct SpDev {
     int* cart_steps;           // [B]
     int8_t* board;             // [B][kMaxCells], +1 / -1 / 0
     int8_t* player;            // [B] side to move, +1 / -1
-    int32_t* ints;             // [B][4] Twenty-One: player's hand, dealer's hand, cards drawn; Simple Grid: row, column
+    int32_t* ints;             // [B][4] Twenty-One: player's hand, dealer's hand, cards drawn; Simple Grid: row, column;
+                               //        Gridworld: x, y, dir, step_count
     // search inputs / outputs (device)
     float* obs;                // [B][O_in]
     uint8_t* legal;            // [B][A]
@@ -200,6 +206,58 @@ MZ_DEVINL bool grid_step(const SpDev& s, int g, int action) {
     return st[0] == 2 && st[1] == 2;
 }
 
+// Gridworld (games/gridworld.py): the agent on the floor(15 u0)-th free cell, x = 1 + i % 4, y = 1 + i / 4 (the goal
+// would be i = 15; 15 u < 15 for every u < 1), facing floor(4 u1); u_k from draw k of the game's placement stream
+MZ_DEVINL void gridworld_reset(const SpDev& s, int g, int64_t gid) {
+    int32_t* st = s.ints + (size_t)g * 4;
+    const int i = (int)(15.0 * philox_uniform53(s.seed, gid, 0, 0u, kTagPlace));
+    st[0] = 1 + i % 4;
+    st[1] = 1 + i / 4;
+    st[2] = (int)(4.0 * philox_uniform53(s.seed, gid, 1, 0u, kTagPlace));
+    st[3] = 0;
+}
+
+// the view [x'][y'][c]: view cell (x', y') lies 6 - y' cells ahead of the agent and x' - 3 cells to its right (the
+// rules' window rotated dir + 1 times); cells outside the room read as walls, the agent's own cell (3, 6) as empty
+MZ_DEVINL void gridworld_observe(const SpDev& s, int g, float* out) {
+    const int32_t* st = s.ints + (size_t)g * 4;
+    const int d = st[2];
+    const int fx = d == 0 ? 1 : (d == 2 ? -1 : 0), fy = d == 1 ? 1 : (d == 3 ? -1 : 0);   // ahead; right = (-fy, fx)
+#pragma unroll 1
+    for (int xv = 0; xv < 7; ++xv)
+#pragma unroll 1
+        for (int yv = 0; yv < 7; ++yv) {
+            const int ahead = 6 - yv, right = xv - 3;
+            const int x = st[0] + ahead * fx - right * fy, y = st[1] + ahead * fy + right * fx;
+            const bool own = xv == 3 && yv == 6;
+            const bool wall = !own && (x <= 0 || x >= 5 || y <= 0 || y >= 5);
+            const bool goal = !own && x == 4 && y == 4;
+            float* c = out + (xv * 7 + yv) * 3;
+            c[0] = wall ? 2.0f : (goal ? 8.0f : 1.0f);          // empty (1, 0, 0), wall (2, 5, 0), goal (8, 1, 0)
+            c[1] = wall ? 5.0f : (goal ? 1.0f : 0.0f);
+            c[2] = 0.0f;
+        }
+}
+
+// returns done; *reward = 1 - 0.9 * (step_count / 144) in fp64 on entering the goal, rounded once to fp32
+MZ_DEVINL bool gridworld_step(const SpDev& s, int g, int action, float* reward) {
+    int32_t* st = s.ints + (size_t)g * 4;
+    const int steps = ++st[3];
+    const int d = st[2];
+    bool goal = false;
+    if (action == 0) {
+        st[2] = (d + 3) & 3;
+    } else if (action == 1) {
+        st[2] = (d + 1) & 3;
+    } else if (action == 2) {
+        const int x = st[0] + (d == 0) - (d == 2), y = st[1] + (d == 1) - (d == 3);
+        if (x >= 1 && x <= 4 && y >= 1 && y <= 4) { st[0] = x; st[1] = y; }
+        goal = x == 4 && y == 4;
+    }
+    *reward = goal ? (float)(1.0 - 0.9 * ((double)steps / 144.0)) : 0.0f;
+    return goal || steps >= 144;
+}
+
 MZ_DEVINL void board_reset(const SpDev& s, int g) {
     int8_t* b = s.board + (size_t)g * kMaxCells;
     for (int i = 0; i < kMaxCells; ++i) b[i] = 0;
@@ -266,10 +324,12 @@ MZ_DEVINL void board_step(const SpDev& s, int g, int action, bool* paid, bool* d
 MZ_DEVINL void publish(const SpDev& s, int g) {
     float* o = s.obs + (size_t)g * s.O_in;
     uint8_t* lg = s.legal + (size_t)g * s.A;
-    if (s.env == MZ_ENV_CARTPOLE || s.env == MZ_ENV_TWENTYONE || s.env == MZ_ENV_SIMPLE_GRID) {
+    if (s.env == MZ_ENV_CARTPOLE || s.env == MZ_ENV_TWENTYONE || s.env == MZ_ENV_SIMPLE_GRID || s.env == MZ_ENV_GRIDWORLD) {
         const int32_t* st = s.ints + (size_t)g * 4;
         if (s.env == MZ_ENV_CARTPOLE) {
             cartpole_observe(s, g, o);
+        } else if (s.env == MZ_ENV_GRIDWORLD) {
+            gridworld_observe(s, g, o);
         } else if (s.env == MZ_ENV_TWENTYONE) {
             for (int i = 0; i < 9; ++i) { o[i] = (float)st[0]; o[9 + i] = (float)st[1]; o[18 + i] = 0.0f; }
         } else {
@@ -402,6 +462,7 @@ MZ_DEVINL int start_game(const SpDev& s, int g, int64_t gid) {
     if (s.env == MZ_ENV_CARTPOLE) cartpole_reset(s, g, gid);
     else if (s.env == MZ_ENV_TWENTYONE) twentyone_reset(s, g);
     else if (s.env == MZ_ENV_SIMPLE_GRID) { s.ints[(size_t)g * 4] = 0; s.ints[(size_t)g * 4 + 1] = 0; }
+    else if (s.env == MZ_ENV_GRIDWORLD) gridworld_reset(s, g, gid);
     else board_reset(s, g);
     publish(s, g);
     s.first_to_play[g] = s.to_play[g];
@@ -506,6 +567,8 @@ MZ_DEVINL int slot_act(const SpDev& s, int g) {
     } else if (s.env == MZ_ENV_SIMPLE_GRID) {
         done = grid_step(s, g, action);
         reward = done ? (float)s.reward_scale : 0.0f;
+    } else if (s.env == MZ_ENV_GRIDWORLD) {
+        done = gridworld_step(s, g, action, &reward);
     } else {
         bool paid;
         board_step(s, g, action, &paid, &done);
@@ -962,6 +1025,8 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
         return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: CartPole has one player, its opponent is \"self\"");
     if (opponent != MZ_OPPONENT_SELF && (d->env == MZ_ENV_TWENTYONE || d->env == MZ_ENV_SIMPLE_GRID))
         return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: Twenty-One and Simple Grid have one player, their opponent is \"self\"");
+    if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_GRIDWORLD)
+        return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: Gridworld has one player, its opponent is \"self\"");
     if (opponent == MZ_OPPONENT_EXPERT && d->env == MZ_ENV_GOMOKU)
         return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin_vs: Gomoku has no expert opponent (the reference's Game has no expert_agent)");
     if (opponent != MZ_OPPONENT_SELF && d->td_steps > 0)
@@ -992,6 +1057,8 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
         }
         case MZ_ENV_TWENTYONE: name = "Twenty-One"; C = 3; ph = 3; pw = 3; A_env = 2; break;
         case MZ_ENV_SIMPLE_GRID: name = "Simple Grid"; C = 1; ph = 1; pw = 9; A_env = 2; break;
+        // the reference's observation_shape (7, 7, 3): 7 planes of 7 x 3, the stack's planes too
+        case MZ_ENV_GRIDWORLD: name = "Gridworld"; C = 7; ph = 7; pw = 3; A_env = 3; break;
         case MZ_ENV_HOST: {
             if (!e) return fail(h, MZ_EINVAL, "mz_selfplay_begin: host-stepped games (MZ_ENV_HOST) start with mz_selfplay_begin_host");
             if (e->obs_channels < 1 || e->obs_h < 1 || e->obs_w < 1)

@@ -494,7 +494,8 @@ class DeviceSelfPlayLoop:
     finished games handed back as packed struct-of-arrays blocks (SURVEY.md 8f-1, include/mzb200.h)."""
 
     ENVS = {"cartpole": _lib.MZ_ENV_CARTPOLE, "tictactoe": _lib.MZ_ENV_TICTACTOE, "connect4": _lib.MZ_ENV_CONNECT4,
-            "gomoku": _lib.MZ_ENV_GOMOKU, "twentyone": _lib.MZ_ENV_TWENTYONE, "simple_grid": _lib.MZ_ENV_SIMPLE_GRID}
+            "gomoku": _lib.MZ_ENV_GOMOKU, "twentyone": _lib.MZ_ENV_TWENTYONE, "simple_grid": _lib.MZ_ENV_SIMPLE_GRID,
+            "gridworld": _lib.MZ_ENV_GRIDWORLD}
     OPPONENTS = {"self": _lib.MZ_OPPONENT_SELF, "expert": _lib.MZ_OPPONENT_EXPERT, "random": _lib.MZ_OPPONENT_RANDOM}
 
     def __init__(self, engine: SearchEngine, env: str, max_moves: int, temperature_threshold=None, reward_scale: int = 1,

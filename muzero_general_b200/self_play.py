@@ -632,7 +632,7 @@ class SelfPlay:
         """Advance every game of the lockstep batch by ``n_moves`` moves; returns the games that finished.
 
         With ``rng_mode="philox"`` and a game that has a device-resident environment (CartPole, TicTacToe, Connect4,
-        Gomoku, Twenty-One, Simple Grid)
+        Gomoku, Twenty-One, Simple Grid, Gridworld)
         the whole loop - observation, search, visit-count sampling, environment step, history records - runs on the
         GPU (``mz_selfplay_moves``) and only finished games cross to the host, as ``PackedGameHistory`` objects.  With
         ``rng_mode="philox"``, ``config.host_env_device_loop`` and no device environment in use, the same loop runs
@@ -674,7 +674,8 @@ class SelfPlay:
         if self.loop_path == "host":
             raise NotImplementedError(
                 "test games on the device need rng_mode='philox' and a device environment (CartPole, TicTacToe, "
-                "Connect4, Gomoku, Twenty-One or Simple Grid with device_envs on) or config.host_env_device_loop; play "
+                "Connect4, Gomoku, Twenty-One, Simple Grid or Gridworld with device_envs on) or "
+                "config.host_env_device_loop; play "
                 "them one at a time with play_game(0, config.temperature_threshold, False, opponent, muzero_player)")
         if self._device_loop is not None:
             raise RuntimeError("this worker's device self-play loop has games in flight, and starting test games on the "
@@ -786,7 +787,7 @@ class DeviceBatchedSelfPlay:
         vec = getattr(Game, "VECTOR", None)
         self.obs_shape = tuple(cfg.observation_shape)
         self.obs_dtype = getattr(vec, "OBS_DTYPE", numpy.float32)
-        self.reward_type = int if vec is not None else float
+        self.reward_type = getattr(vec, "REWARD_TYPE", int) if vec is not None else float
         # test-mode games never reach a replay buffer (self_play.py:54-66): no priorities against an opponent
         priorities = opponent == "self" and getattr(cfg, "PER", False) and getattr(cfg, "device_priorities", True)
         self.loop = DeviceSelfPlayLoop(worker.model.engine, Game.DEVICE_ENV, cfg.max_moves,
@@ -879,7 +880,7 @@ class DeviceHostEnvSelfPlay:
         vec = getattr(Game, "VECTOR", None)
         self.obs_shape = tuple(cfg.observation_shape)
         self.obs_dtype = getattr(vec, "OBS_DTYPE", numpy.float32)
-        self.reward_type = int if vec is not None else float
+        self.reward_type = getattr(vec, "REWARD_TYPE", int) if vec is not None else float
         if opponent == "expert" and not hasattr(self.env, "expert_actions"):
             raise NotImplementedError(f"{type(self.env).__name__} has no expert_actions(defaults, which): no expert opponent")
         self.opponent = opponent
