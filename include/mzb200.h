@@ -264,6 +264,35 @@ int mz_reanalyse_values(MzHandle* h, const MzReanalyseIO* io);
  * mz_reanalyse_values, and MZ_EINVAL for a chunk beyond the call's. */
 int mz_debug_reanalyse_stack(MzHandle* h, const MzReanalyseIO* io, int32_t chunk, float* out);
 
+/* Arguments of mz_reanalyse_search: the self-play search re-run at every position of n games (the MuZero paper's
+ * Reanalyze).  The positions are games' as in mz_reanalyse_values (games->values is not used); `games->mem` also says
+ * where legal_mask, to_play and the outputs live.  Position i of game g is searched as MCTS.run(model,
+ * get_stacked_observations(i, s, A), legal actions, to_play, add_exploration_noise) with the Philox streams keyed by
+ * (seed, game_id[g], move index i), so a position searched with its self-play game id reproduces that move's search. */
+typedef struct MzReanalyseSearchIO {
+    const MzReanalyseIO* games;   /* frames, actions, offsets, positions, mem, s and O, as mz_reanalyse_values takes them */
+    const uint8_t* legal_mask;    /* [sum T_g][A] non-zero = legal, game order; NULL = all legal */
+    const int32_t* to_play;       /* [sum T_g] to_play_history[i], each in [0, num_players); NULL = 0 */
+    const int64_t* game_id;       /* [n] HOST: the Philox game id of each game; NULL = 0 .. n - 1 */
+    int32_t add_exploration_noise;/* self_play.py:310-314 (the root noise is drawn on the device) */
+    int32_t reserved;
+    int32_t* visit_counts;        /* [sum T_g][A] out: child.visit_count by action id, 0 if illegal, game order */
+    double* root_value;           /* [sum T_g] out: root.value(), game order; may be NULL */
+} MzReanalyseSearchIO;
+
+/* Fresh policy targets for Reanalyse: per chunk of at most max_games positions, the stack of mz_reanalyse_values, then a
+ * kernel writes each position's legal row, to_play, game id and move index into the search's input arena and the search
+ * of mz_search runs on them (the same route: fused FC, fused small search, step-wise towers, the x3 range guard).  With
+ * host memory the legal rows and to_play travel with the chunk's frames through the two pinned staging buffers, and the
+ * results come back through the handle's pinned output arena while the next chunk searches; device memory is read and
+ * written in place.  Beyond mz_create's allocations the call takes at most 2 x ((max_games + s) x (O + 1) x 4 +
+ * max_games x (32 + A)) bytes of device memory (and as much pinned host memory with host memory), plus 256-byte
+ * alignment per staged array, whatever the games' lengths.  With device memory the checks below read the legal masks
+and to_play on the host: sum T_g x (A + 4) bytes of host memory for the duration of the call.  Refused with MZ_EINVAL, before anything is written: every
+ * refusal of mz_reanalyse_values, visit_counts NULL with positions to search, a position without a legal action, a to_play
+ * outside [0, num_players).  MZ_ESTATE: a handle created with num_simulations = 0. */
+int mz_reanalyse_search(MzHandle* h, const MzReanalyseSearchIO* io);
+
 /* Node graph access for callers that walk the tree (self_play.py:229-232,499-509; diagnose_model.py:164,222-255) */
 int mz_export_tree(MzHandle* h, int32_t game, MzTreeExport* out);
 /* The inverse: seed game `game`'s tree in the pool from host arrays in the same layout (n_expansions, root_visit,

@@ -103,6 +103,12 @@ class MzReanalyseIO(C.Structure):
                 ("action_offsets", C.c_void_p), ("positions", C.c_void_p), ("values", C.c_void_p)]
 
 
+class MzReanalyseSearchIO(C.Structure):
+    _fields_ = [("games", C.c_void_p), ("legal_mask", C.c_void_p), ("to_play", C.c_void_p), ("game_id", C.c_void_p),
+                ("add_exploration_noise", C.c_int32), ("reserved", C.c_int32), ("visit_counts", C.c_void_p),
+                ("root_value", C.c_void_p)]
+
+
 class MzSelfPlayDesc(C.Structure):
     _fields_ = [("env", C.c_int32), ("max_moves", C.c_int32), ("temperature_threshold", C.c_int32),
                 ("reward_scale", C.c_int32), ("first_game_id", C.c_int64), ("game_id_stride", C.c_int64),
@@ -149,6 +155,7 @@ SYMBOLS = [
     ("mz_recurrent_inference", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(MzInferenceOut)]),
     ("mz_reanalyse_values", C.c_int, [C.c_void_p, C.POINTER(MzReanalyseIO)]),
     ("mz_debug_reanalyse_stack", C.c_int, [C.c_void_p, C.POINTER(MzReanalyseIO), C.c_int32, C.c_void_p]),
+    ("mz_reanalyse_search", C.c_int, [C.c_void_p, C.POINTER(MzReanalyseSearchIO)]),
     ("mz_export_tree", C.c_int, [C.c_void_p, C.c_int32, C.POINTER(MzTreeExport)]),
     ("mz_import_tree", C.c_int, [C.c_void_p, C.c_int32, C.POINTER(MzTreeExport)]),
     ("mz_hidden_elems", C.c_int64, [C.c_void_p]),

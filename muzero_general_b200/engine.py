@@ -434,6 +434,39 @@ class SearchEngine:
         self._check(self.lib.mz_reanalyse_values(self._h, C.byref(io)))
         return values
 
+    def reanalyse_search(self, frames, frame_offsets, actions, action_offsets, positions, legal_mask=None, to_play=None,
+                         game_id=None, add_exploration_noise=True, stacked_observations=None):
+        """The self-play search re-run at every position of a batch of games (mz_reanalyse_search): the positions are
+        reanalyse_values', ``legal_mask`` [sum positions][A] and ``to_play`` [sum positions] are theirs in game order,
+        ``game_id`` [n games] keys each game's Philox streams (the move index is the position).  Returns
+        (visit_counts int32 [sum positions][A], root_value float64 [sum positions]): numpy arrays for host frames, CUDA
+        tensors for CUDA frames, actions, legal masks and to_play."""
+        keep = []
+        io, total, device_mem = self._reanalyse_io(frames, frame_offsets, actions, action_offsets, positions,
+                                                   stacked_observations, keep)
+        if device_mem:
+            import torch
+            to_dev = lambda x, dt: x if x is None or _is_torch(x) else torch.as_tensor(numpy.asarray(x, dt), device=frames.device)
+            legal_mask, to_play = to_dev(legal_mask, numpy.uint8), to_dev(to_play, numpy.int32)
+        sio = _lib.MzReanalyseSearchIO()
+        sio.games = C.addressof(io)
+        sio.legal_mask = self._ptr(legal_mask, numpy.uint8, keep)
+        sio.to_play = self._ptr(to_play, numpy.int32, keep)
+        sio.game_id = self._ptr(None if game_id is None else numpy.asarray(game_id, dtype=numpy.int64).reshape(-1),
+                                numpy.int64, keep)
+        sio.add_exploration_noise = int(bool(add_exploration_noise))
+        if device_mem:
+            visits = torch.empty((total, self.A), dtype=torch.int32, device=frames.device)
+            root = torch.empty(total, dtype=torch.float64, device=frames.device)
+            p = lambda t: t.data_ptr() if total else None
+        else:
+            visits = numpy.empty((total, self.A), numpy.int32)
+            root = numpy.empty(total, numpy.float64)
+            p = lambda a: a.ctypes.data if total else None
+        sio.visit_counts, sio.root_value = p(visits), p(root)
+        self._check(self.lib.mz_reanalyse_search(self._h, C.byref(sio)))
+        return visits, root
+
     def debug_reanalyse_stack(self, chunk, frames, frame_offsets, actions, action_offsets, positions,
                               stacked_observations=None):
         """The stacked inputs [n_c][obs_elems] chunk ``chunk`` of reanalyse_values builds (mz_debug_reanalyse_stack)."""

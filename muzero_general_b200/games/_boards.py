@@ -159,6 +159,16 @@ class BoardGame:
     def legal_actions(self):
         return [int(a) for a in numpy.nonzero(self.env.legal_mask()[0])[0]]
 
+    @classmethod
+    def legal_masks(cls, observations):
+        """The legal mask of each raw frame [n, 3, H, W] (Reanalyse's hook), read from the stone planes: the empty
+        cells, or with gravity the columns whose top cell ``board[H - 1][c]`` is empty.  The side comes from the shape."""
+        obs = numpy.asarray(observations)
+        empty = (obs[:, 0] == 0) & (obs[:, 1] == 0)
+        if cls.VECTOR.GRAVITY:
+            return empty[:, -1, :].astype(numpy.uint8)
+        return empty.reshape(len(obs), obs.shape[2] * obs.shape[3]).astype(numpy.uint8)
+
     def reset(self):
         return self.env.reset()[0]
 

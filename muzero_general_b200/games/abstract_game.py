@@ -1,13 +1,16 @@
 """Game plug-in surface kept from the reference (``games/abstract_game.py:4-105``).
 
 Same method names, argument meaning and return conventions, so a reference ``Game`` class
-works here unchanged and vice versa.  Two OPTIONAL additions, both discovered with
+works here unchanged and vice versa.  OPTIONAL additions, all discovered with
 ``getattr`` so stock plug-ins keep working:
 
 * ``Game.vector(num_games, seed)`` - a classmethod returning a ``VectorGame`` that steps
   ``num_games`` independent copies at once (struct-of-arrays, numpy).  The batched
   self-play loop uses it when present and falls back to ``num_games`` ordinary ``Game``
   objects otherwise.
+* ``Game.legal_masks(observations)`` - uint8 ``[n, |A|]``, the legal mask of each raw frame
+  ``[n, *observation_shape]``; Reanalyse with ``config.reanalyse_search`` needs it, because a
+  ``GameHistory`` stores no legal actions.
 """
 from abc import ABC, abstractmethod
 

@@ -78,6 +78,11 @@ class Game(AbstractGame):
     def legal_actions(self):
         return list(range(4))
 
+    @staticmethod
+    def legal_masks(observations):
+        """The legal mask of each raw frame [n, *observation_shape] (Reanalyse's hook): every action, as legal_actions."""
+        return numpy.ones((len(observations), 4), numpy.uint8)
+
     def reset(self):
         return self.env.reset()[0]
 

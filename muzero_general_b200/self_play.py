@@ -365,21 +365,27 @@ class PackedGameHistory(GameHistory):
         raise AttributeError(name)
 
     def _materialise(self):
+        """Builds the lists not present yet: one set before (Reanalyse's fresh ``child_visits``) is kept."""
         g, shape, dtype, reward_type = self._packed
         T = int(g["length"])
-        obs = g["obs"].reshape((T + 1,) + shape).astype(dtype)
         d = self.__dict__
-        d["observation_history"] = list(obs)
-        d["action_history"] = [0] + list(g["action"].astype(numpy.int64))
-        d["reward_history"] = [0] + [reward_type(r) for r in g["reward"].tolist()]
-        d["to_play_history"] = [int(g["first_to_play"])] + g["to_play"].tolist()
+        if "observation_history" not in d:
+            d["observation_history"] = list(g["obs"].reshape((T + 1,) + shape).astype(dtype))
+        if "action_history" not in d:
+            d["action_history"] = [0] + list(g["action"].astype(numpy.int64))
+        if "reward_history" not in d:
+            d["reward_history"] = [0] + [reward_type(r) for r in g["reward"].tolist()]
+        if "to_play_history" not in d:
+            d["to_play_history"] = [int(g["first_to_play"])] + g["to_play"].tolist()
         # a test-mode game's opponent moves carry a NaN root value: store_search_statistics(None) (self_play.py:496-511)
         # appends None to root_values and no child_visits row
         root = g["root_value"]
         searched = ~numpy.isnan(root)
-        visits = g["visits"][searched]
-        d["child_visits"] = (visits / visits.sum(1, keepdims=True)).tolist()
-        d["root_values"] = [v if s else None for v, s in zip(root.tolist(), searched.tolist())]
+        if "child_visits" not in d:
+            visits = g["visits"][searched]
+            d["child_visits"] = (visits / visits.sum(1, keepdims=True)).tolist()
+        if "root_values" not in d:
+            d["root_values"] = [v if s else None for v, s in zip(root.tolist(), searched.tolist())]
 
     def __reduce__(self):
         self._materialise()
