@@ -35,6 +35,17 @@ struct LaneGroup {
     MZ_DEVINL static T bcast(T v, int src) { return __shfl_sync(kWarp, v, src, G); }
     // true in every lane while any group of the warp passes p (the trip-count test of a loop that contains collectives)
     MZ_DEVINL static bool warp_any(bool p) { return __any_sync(kWarp, p); }
+    // Waits until all 32 lanes of the warp are converged here (WARPSYNC.ALL).  Where ptxas cannot prove the warp converged
+    // at a collective - after a loop whose trip count depends on threadIdx, such as the persistent loop over games - it
+    // wraps the collective in a run-time divergence test (BRA.DIV) with an out-of-line WARPSYNC.COLLECTIVE / ENDCOLLECTIVE
+    // fallback, and since that fallback may rejoin diverged, every later collective gets one too.  A warp-wide reduction
+    // needs a converged warp and its WARPSYNC.ALL re-establishes the proof: placed in front of a loop whose every path
+    // ends converged, it leaves the loop's collectives without any test.  (An asm volatile, so that the unused result
+    // does not let the compiler drop it.)
+    MZ_DEVINL static void converge() {
+        unsigned r;
+        asm volatile("redux.sync.or.b32 %0, %1, 0xffffffff;" : "=r"(r) : "r"(0u));
+    }
 };
 
 MZ_DEVINL double shfl_xor_f64(unsigned mask, double v, int off, int width) {

@@ -260,6 +260,9 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
 
         // ------------------------------------------------------------------ simulations
         int max_depth = 0;
+        // every path through a simulation ends converged (the backup's REDUX waits for the warp), so with the loop entered
+        // converged ptxas proves each of its collectives and emits no divergence test (LaneGroup::converge)
+        LaneGroup<G>::converge();
         for (int sim = 0; sim < N; ++sim) {
             int rounds;
             const Leaf leaf = tree_select_lookahead<G, kMaxD, kA>(c, t, sl, sim, game_id, move, first_index, rounds);
