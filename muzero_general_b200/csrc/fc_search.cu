@@ -48,9 +48,9 @@ __host__ __device__ inline GameSmem game_smem_layout(int N, int A, int E, int ma
 // root, select, network, expand and backup phases with clock() and adds them, with the levels and selection rounds it
 // walked, to device counters that mz_fc_phase_counters reads.  It also stores the %globaltimer at which its game started
 // and finished (mz_fc_phase_spans): games that start after others have finished ran in a later pass of the persistent
-// loop.  The library built without the macro is unchanged.
+// loop, and the SM it ran on (%smid; mz_fc_phase_rows reads whole rows).  The library built without the macro is unchanged.
 enum { kPhRoot, kPhSelect, kPhNet, kPhExpand, kPhBackup, kPhLevels, kPhRounds, kPhSims, kPhSums,
-       kPhStart = kPhSums, kPhEnd, kPhCount };
+       kPhStart = kPhSums, kPhEnd, kPhSm, kPhCount };
 // The counters are per game and added to in memory as the game goes (fire-and-forget reductions to distinct addresses):
 // accumulators held in registers would push the kernel past 128 registers and change its occupancy.  The start and end
 // times sit in the same row.
@@ -71,7 +71,13 @@ struct PhaseClock {
         last = (unsigned)clock();
     }
     // an exchange, like the counters' reductions, leaves the kernel without spills where a plain store did not
-    MZ_DEVINL void finish() { if (row >= 0) atomicExch(&g_fc_phase[row][kPhEnd], global_ns()); }
+    MZ_DEVINL void finish() {
+        if (row < 0) return;
+        unsigned sm;
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+        atomicExch(&g_fc_phase[row][kPhEnd], global_ns());
+        atomicExch(&g_fc_phase[row][kPhSm], (unsigned long long)sm);
+    }
     MZ_DEVINL void mark(int p) {
         const unsigned now = (unsigned)clock();
         if (row >= 0) atomicAdd(&g_fc_phase[row][p], (unsigned long long)(now - last));
@@ -79,6 +85,10 @@ struct PhaseClock {
     }
     MZ_DEVINL void count(int p, int n) { if (row >= 0) atomicAdd(&g_fc_phase[row][p], (unsigned long long)n); }
 };
+// %globaltimer at which each CTA entered the kernel, before it stages the tables and weights (mz_fc_phase_ctas)
+constexpr int kPhMaxCtas = 1 << 14;
+__device__ unsigned long long g_fc_cta_entry[kPhMaxCtas];
+MZ_DEVINL void phase_cta_entry() { if (threadIdx.x == 0 && blockIdx.x < kPhMaxCtas) g_fc_cta_entry[blockIdx.x] = global_ns(); }
 #else
 struct PhaseClock {
     MZ_DEVINL void start(int, bool) {}
@@ -86,6 +96,7 @@ struct PhaseClock {
     MZ_DEVINL void mark(int) {}
     MZ_DEVINL void count(int, int) {}
 };
+MZ_DEVINL void phase_cta_entry() {}
 #endif
 
 // ---- the search's two network calls (fc_search_kernel and fc_debug_net_kernel run these)
@@ -162,6 +173,15 @@ MZ_DEVINL void fc_sim_inference(const FcNet& net, const float* blob, const float
     }
 }
 
+// global -> shared copies that do not pass through registers (cp.async, sm_80+); cp_async_wait_all waits for the thread's own
+MZ_DEVINL void cp_async8(void* dst, const void* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+MZ_DEVINL void cp_async16(void* dst, const void* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+MZ_DEVINL void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
 template <typename SH>
 constexpr int fixed_actions() {
     if constexpr (SH::kEnabled) return SH::A;
@@ -180,9 +200,19 @@ __global__ void __launch_bounds__(kFcMaxThreads, 2) fc_search_kernel(const __gri
     double* s_pbc = reinterpret_cast<double*>(smem);
     double* s_sqrt = s_pbc + (N + 2);
     float* s_blob = reinterpret_cast<float*>(s_sqrt + (N + 2));
-    for (int i = threadIdx.x; i < N + 2; i += blockDim.x) { s_pbc[i] = a.pbc[i]; s_sqrt[i] = a.sqrtn[i]; }
+    phase_cta_entry();
+    // Asynchronous copies (LDGSTS): every thread's share of the tables and the blob is in flight at once, so a CTA waits
+    // one global-memory latency (cold: the L2 holds nothing of this launch yet) instead of one per strided iteration.
+    // The blob is padded to a multiple of 4 floats in global memory (abi.cu) and starts 16-byte aligned in both spaces;
+    // the prefetch brings the first game's observation row in meanwhile.
+    if (!kTeacher && (threadIdx.x & (G - 1)) == 0) {
+        const int g = min((int)blockIdx.x * (int)(blockDim.x / G) + (int)threadIdx.x / G, a.n_games - 1);
+        asm volatile("prefetch.global.L1 [%0];" ::"l"(a.obs + (size_t)g * a.net.obs_elems));
+    }
+    for (int i = threadIdx.x; i < N + 2; i += blockDim.x) { cp_async8(s_pbc + i, a.pbc + i); cp_async8(s_sqrt + i, a.sqrtn + i); }
     if (!kTeacher)
-        for (int i = threadIdx.x; i < a.net.blob_floats; i += blockDim.x) s_blob[i] = a.blob[i];
+        for (int i = threadIdx.x; i < (a.net.blob_floats + 3) >> 2; i += blockDim.x) cp_async16(s_blob + 4 * i, a.blob + 4 * i);
+    cp_async_wait_all();
     __syncthreads();
 
     const int shared_bytes = ((2 * (N + 2) * 8 + (kTeacher ? 0 : a.net.blob_floats) * 4) + 15) & ~15;
@@ -632,6 +662,23 @@ extern "C" int mz_fc_phase_spans(unsigned long long* out, int n) {
         out[2 * g] = rows[(size_t)g * kPhCount + kPhStart];
         out[2 * g + 1] = rows[(size_t)g * kPhCount + kPhEnd];
     }
+    return e == cudaSuccess ? 0 : (int)e;
+}
+
+// out[g * cols + c] = column c of game g's row (cycles and counts of kPhRoot..kPhSims, then start ns, end ns, SM), games
+// g < n; cols must be the row width (kPhCount)
+extern "C" int mz_fc_phase_rows(unsigned long long* out, int n, int cols) {
+    if (!out || n < 0 || n > kPhMaxGames || cols != kPhCount) return (int)cudaErrorInvalidValue;
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpyFromSymbol(out, g_fc_phase, (size_t)n * kPhCount * 8);
+    return e == cudaSuccess ? 0 : (int)e;
+}
+
+// out[b] = %globaltimer (ns) at which CTA b < n of the last launch entered the kernel
+extern "C" int mz_fc_phase_ctas(unsigned long long* out, int n) {
+    if (!out || n < 0 || n > kPhMaxCtas) return (int)cudaErrorInvalidValue;
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpyFromSymbol(out, g_fc_cta_entry, (size_t)n * 8);
     return e == cudaSuccess ? 0 : (int)e;
 }
 #endif

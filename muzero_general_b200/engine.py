@@ -147,10 +147,11 @@ class SearchEngine:
         self.obs_elems = int(self.lib.mz_obs_elems(self._h))
         self._dio = _lib.MzDeviceSearchIO()            # one argument struct for every mz_search_device call
         self._dio_ref = C.byref(self._dio)
-        self._layouts = {}                              # n_games -> output_layout
+        self._next_out = None                           # ((n_games, device), (buffer, layout, offsets)) of the next device search
 
     # ------------------------------------------------------------------ plumbing
     def close(self):
+        self._next_out = None
         if getattr(self, "_h", None):
             self.lib.mz_destroy(self._h)
             self._h = None
@@ -339,8 +340,9 @@ class SearchEngine:
         return out
 
     def _search_device(self, n, obs, legal_mask, to_play, add_noise, noise, first_index, game_id, move_index):
-        """search() on device tensors through mz_search_device: the seven outputs are views of one fresh buffer, made
-        while the search runs."""
+        """search() on device tensors through mz_search_device: the seven outputs are views of one buffer, carved while
+        the search runs.  The buffer of the next search of as many games on the same device is allocated while this one
+        runs too; every buffer belongs to one search only, so returned arrays stay valid as long as the caller holds them."""
         import torch
         keep, io = [], self._dio
         io.n_games = n
@@ -352,17 +354,21 @@ class SearchEngine:
         io.legal_mask = self._ptr(legal_mask, numpy.uint8, keep)
         io.to_play = self._ptr(to_play, numpy.int32, keep)
         io.first_index = self._ptr(first_index, numpy.int32, keep)
-        layout = self._layouts.get(n)
-        if layout is None:
-            layout = self._layouts[n] = output_layout(n, self.A)
-        fields, nbytes = layout
-        buf = torch.empty(nbytes // 8, dtype=torch.float64, device=obs.device)
+        key = (n, obs.get_device())
+        nxt, self._next_out = self._next_out, None
+        if nxt is not None and nxt[0] == key:
+            buf, fields, offsets = nxt[1]
+        else:
+            fields, nbytes = output_layout(n, self.A)
+            offsets = tuple(f[3] for f in fields)
+            buf = torch.empty(nbytes // 8, dtype=torch.float64, device=obs.device)
         base = buf.data_ptr()
         (io.visit_counts, io.root_value, io.root_predicted_value, io.max_tree_depth, io.tie_count, io.root_priors,
-         io.value_range) = (base + f[3] for f in fields)
+         io.value_range) = (base + o for o in offsets)
         self._check(self.lib.mz_search_device(self._h, self._dio_ref))
         try:
             out = carve_outputs(buf, fields)
+            self._next_out = (key, (torch.empty_like(buf), fields, offsets))
         finally:
             self._check(self.lib.mz_search_device_wait(self._h, self._dio_ref))
         out.device_ms = io.device_ms
