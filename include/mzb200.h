@@ -759,6 +759,51 @@ int mz_selfplay_begin_host_vs(MzHandle* h, const MzSelfPlayDesc* desc, const MzH
 int mz_selfplay_host_opponent_turn(MzHandle* h, int32_t* defaults);
 int mz_selfplay_host_opponent_act(MzHandle* h, const int32_t* actions, int32_t* played);
 
+/* User environments (env = MZ_ENV_USER): the device loop for a game plug-in that brings its environment as CUDA source.
+ * The library compiles the source with NVRTC (-arch=sm_90a -std=c++17 -fmad=false, the built-in environments' flags)
+ * behind the prelude csrc/user_env.cuh, which states the contract: the source defines
+ *   __device__ void mz_env_reset(void* state, const MzEnvCtx& ctx, MzEnvRow& row);
+ *   __device__ void mz_env_step(void* state, int action, const MzEnvCtx& ctx, MzEnvRow& row);
+ * on the slot's own state_bytes of device memory; MzEnvCtx carries the handle's seed, the slot's game id, the move index
+ * and the slot, MzEnvRow the slot's observation, reward, done, legal-mask and to_play entries, and the prelude exposes
+ * philox_uniform53, the Philox draw of the built-in environments.  Each move is then the host-stepped loop's with the
+ * step on the device: search, the action sample and the search records (as mz_selfplay_host_act), the step kernel, the
+ * rest of the records, packing and stacking (as mz_selfplay_host_observe), the reset kernel on the slots whose game was
+ * packed and their next game's first rows (as mz_selfplay_host_restart); nothing crosses to the host but the counters
+ * at the end of the call.  NVRTC is loaded with dlopen("libnvrtc.so.12") on first use: without it these calls fail
+ * with MZ_EUNSUPPORTED and every other entry point works. */
+#define MZ_ENV_USER 8
+#define MZ_USER_ENV_MAX_STATE_BYTES 4096
+typedef struct MzUserEnvDesc {
+    const char* source;           /* NUL-terminated CUDA source defining mz_env_reset and mz_env_step */
+    int32_t state_bytes;          /* bytes of environment state per slot, 0 .. MZ_USER_ENV_MAX_STATE_BYTES */
+    int32_t obs_channels;         /* the observation is obs_channels x obs_h x obs_w floats (as MzHostEnvDesc) */
+    int32_t obs_h;
+    int32_t obs_w;
+} MzUserEnvDesc;
+
+/* Compiles env->source (or takes it from the handle's cache of sources compiled before), resets every slot (games
+ * first_game_id + g) and begins the loop as mz_selfplay_begin_host does, stacked_observations and device priorities
+ * included.  Refused with MZ_EINVAL: desc->env other than MZ_ENV_USER, state_bytes outside [0,
+ * MZ_USER_ENV_MAX_STATE_BYTES], a source that does not compile or lacks one of the two functions (NVRTC's log in
+ * mz_last_error), mz_selfplay_begin_host's refusals, and a reset that left a slot without a legal action or with a
+ * to_play outside the players.  MZ_EUNSUPPORTED: no NVRTC. */
+int mz_selfplay_begin_user(MzHandle* h, const MzSelfPlayDesc* desc, const MzUserEnvDesc* env);
+/* mz_selfplay_moves for a loop begun with mz_selfplay_begin_user (mz_selfplay_moves refuses those; mz_selfplay_enqueue /
+ * _wait, _drain and _peek serve both).  A finished game that does not fit into the staging area is parked as in the
+ * device loop.  MZ_EINVAL when the environment wrote a row the loop cannot play (a game in play without a legal action,
+ * a to_play outside the players): such a game was ended there, and the loop should be begun again. */
+int mz_selfplay_user_moves(MzHandle* h, int32_t n_moves, double temperature, const MzSelfPlayInject* inject,
+                           MzSelfPlayStats* stats);
+/* Debug, host only (no device needed): compiles source as mz_selfplay_begin_user does.  log (may be NULL) receives
+ * NVRTC's log, ptxas's resource report included, truncated to log_bytes - 1 bytes and NUL-terminated; info (may be
+ * NULL) receives info[9] = {registers, stack frame bytes, spill store bytes, spill load bytes} of the reset wrapper
+ * kernel, the same of the step wrapper kernel, and NVRTC's version as 1000 * major + 10 * minor (-1 for a count the log
+ * does not give).  MZ_EINVAL on a compile failure or a missing function, MZ_EUNSUPPORTED without NVRTC. */
+int mz_debug_user_env_compile(const char* source, char* log, int64_t log_bytes, int32_t* info);
+/* NVRTC compiles made for this handle's user environments so far (a begin with a cached source makes none) */
+int64_t mz_debug_user_env_compiles(const MzHandle* h);
+
 /* Debug / parity: the device opponent (MZ_OPPONENT_EXPERT or MZ_OPPONENT_RANDOM) of env (MZ_ENV_TICTACTOE,
  * MZ_ENV_CONNECT4, or MZ_ENV_GOMOKU with MZ_OPPONENT_RANDOM only, on its default 11 x 11 board: this call has no handle
  * to read another side from) on n host positions.  board is [n][H*W] of +1 / -1 / 0 (row 0 = bottom), player [n] the side to

@@ -130,6 +130,11 @@ class MzHostEnvDesc(C.Structure):
     _fields_ = [("obs_channels", C.c_int32), ("obs_h", C.c_int32), ("obs_w", C.c_int32)]
 
 
+class MzUserEnvDesc(C.Structure):
+    _fields_ = [("source", C.c_char_p), ("state_bytes", C.c_int32), ("obs_channels", C.c_int32), ("obs_h", C.c_int32),
+                ("obs_w", C.c_int32)]
+
+
 class MzSelfPlayPeek(C.Structure):
     _fields_ = [("obs", C.c_void_p), ("legal_mask", C.c_void_p), ("to_play", C.c_void_p), ("game_id", C.c_void_p),
                 ("move_index", C.c_void_p), ("last_action", C.c_void_p)]
@@ -138,6 +143,8 @@ class MzSelfPlayPeek(C.Structure):
 MZ_ENV_CARTPOLE, MZ_ENV_TICTACTOE, MZ_ENV_CONNECT4, MZ_ENV_GOMOKU, MZ_ENV_TWENTYONE, MZ_ENV_SIMPLE_GRID = 0, 1, 2, 3, 4, 5
 MZ_ENV_HOST = 6
 MZ_ENV_GRIDWORLD = 7
+MZ_ENV_USER = 8
+MZ_USER_ENV_MAX_STATE_BYTES = 4096
 MZ_OPPONENT_SELF, MZ_OPPONENT_EXPERT, MZ_OPPONENT_RANDOM = 0, 1, 2
 MZ_STAGED_HEADER_BYTES = 32
 
@@ -188,6 +195,11 @@ SYMBOLS = [
                                             C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("mz_selfplay_host_opponent_turn", C.c_int, [C.c_void_p, C.c_void_p]),
     ("mz_selfplay_host_opponent_act", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("mz_selfplay_begin_user", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayDesc), C.POINTER(MzUserEnvDesc)]),
+    ("mz_selfplay_user_moves", C.c_int, [C.c_void_p, C.c_int32, C.c_double, C.POINTER(MzSelfPlayInject),
+                                         C.POINTER(MzSelfPlayStats)]),
+    ("mz_debug_user_env_compile", C.c_int, [C.c_char_p, C.c_char_p, C.c_int64, C.POINTER(C.c_int32)]),
+    ("mz_debug_user_env_compiles", C.c_int64, [C.c_void_p]),
     ("mz_debug_opponent_action", C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p]),
     ("mz_debug_small_search_plan", C.c_int, [C.c_int32] * 10 + [C.POINTER(C.c_int64)]),

@@ -204,6 +204,7 @@ extern "C" int mz_destroy(MzHandle* h) {
     if (h->stream) cudaStreamSynchronize(h->stream);
     mz_selfplay_destroy(h);
     mz_reanalyse_destroy(h);
+    mz_user_env_destroy(h);
     NodePool& p = h->pool;
     void* ptrs[] = {p.visit, p.vsum, p.mval, p.reward, p.prior, p.expansion, p.root_prior, p.hidden, p.root_visit, p.root_vsum,
                     p.root_reward, p.range, p.n_expanded, p.ties, p.max_depth, p.legal, p.path, p.path_reward, p.leaf_depth,

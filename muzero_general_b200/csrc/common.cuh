@@ -5,6 +5,8 @@
 
 #define MZ_DEVINL __device__ __forceinline__
 
+#include "philox.cuh"
+
 namespace mz {
 
 // ------------------------------------------------------------------------------------------
@@ -116,26 +118,8 @@ MZ_DEVINL float group_sum_f32(float v) {
 }
 
 // ------------------------------------------------------------------------------------------
-// Philox4x32-10 (Salmon et al. SC'11); mirrored in oracle/philox.py.
+// Philox4x32-10 draws (philox.cuh)
 // ------------------------------------------------------------------------------------------
-constexpr uint32_t kPhiloxM0 = 0xD2511F53u, kPhiloxM1 = 0xCD9E8D57u;
-constexpr uint32_t kPhiloxW0 = 0x9E3779B9u, kPhiloxW1 = 0xBB67AE85u;
-constexpr uint32_t kTagTie = 0x7169E001u, kTagNoise = 0x7169E002u, kTagAction = 0x7169E003u;
-
-struct Philox4 { uint32_t x, y, z, w; };
-
-MZ_DEVINL Philox4 philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1) {
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t p0h = __umulhi(kPhiloxM0, c0), p0l = kPhiloxM0 * c0;
-        const uint32_t p1h = __umulhi(kPhiloxM1, c2), p1l = kPhiloxM1 * c2;
-        c0 = p1h ^ c1 ^ k0; c1 = p1l;
-        c2 = p0h ^ c3 ^ k1; c3 = p0l;
-        k0 += kPhiloxW0; k1 += kPhiloxW1;
-    }
-    return Philox4{c0, c1, c2, c3};
-}
-
 // index in [0, n) for an exact UCB tie at (game, move, sim, depth)
 MZ_DEVINL int philox_tie_index(uint64_t seed, int64_t game, int move, int sim, int depth, int n) {
     const Philox4 r = philox4x32_10((uint32_t)game, (uint32_t)move, (uint32_t)sim, (uint32_t)depth,

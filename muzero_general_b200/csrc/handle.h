@@ -12,6 +12,7 @@
 
 struct MzSelfPlay;                     // device-resident self-play state (selfplay.cu)
 struct MzReanalyse;                    // Reanalyse's staging buffers and copy stream (reanalyse.cu)
+struct MzUserEnvCache;                 // compiled user environments of mz_selfplay_begin_user (user_env.cu)
 using namespace mz;
 
 struct MzHandle {
@@ -71,6 +72,8 @@ struct MzHandle {
     std::map<std::string, std::pair<void*, size_t>> named;
     MzSelfPlay* sp = nullptr;          // mz_selfplay_begin
     MzReanalyse* ra = nullptr;         // mz_reanalyse_values, on first use
+    MzUserEnvCache* user_env = nullptr;   // mz_selfplay_begin_user's modules by source, on first use
+    int64_t user_env_compiles = 0;     // NVRTC compiles made for this handle (mz_debug_user_env_compiles)
     int pool_n = 0;                    // layout "N" of the node pool and tables: num_simulations + extra_expansions
     int imported_expansions = 0;       // expansions of the tree mz_import_tree seeded last (MZ_FLAG_CONTINUE)
     int range_fallbacks = 0;           // times the x3 range guard switched this handle to the fp32 towers (0 or 1)
@@ -109,5 +112,11 @@ int mz_network_enqueue(MzHandle* h, const mz::InferCall& c);
 int mz_network_guard(MzHandle* h, const mz::InferCall& c);
 void mz_reanalyse_destroy(MzHandle* h);
 void mz_selfplay_destroy(MzHandle* h);
+// The wrapper kernels of a user environment (user_env.cuh) compiled from `source`, from the handle's cache or by NVRTC.
+struct MzUserEnvKernels {
+    cudaKernel_t reset = nullptr, step = nullptr;
+};
+int mz_user_env_kernels(MzHandle* h, const char* source, MzUserEnvKernels* out);
+void mz_user_env_destroy(MzHandle* h);
 void mz_switch_to_strict(MzHandle* h);
 void mz_drop_graphs(MzHandle* h);             // captured graphs refer to buffers or kernels that are about to change

@@ -53,6 +53,11 @@
 // the opponent's play the opponent's move as a move of its own: opponent_turn (host_opponent_turn_kernel, the random
 // default of opponent_move's draw) -> opponent_act (host_opponent_act_kernel: the host's or the default move, recorded
 // with a NaN root and no visits) -> the host's step -> observe, which completes it as it completes MuZero's.
+//
+// User environments (MZ_ENV_USER, mz_selfplay_begin_user): the host-stepped loop's kernels with the host's step replaced
+// by the wrapper kernels of a plug-in's CUDA source (user_env.cuh, compiled by user_env.cu), which write the rows the
+// host would have uploaded.  A move is act -> mz_user_env_step -> observe -> mz_user_env_reset on the slots observe
+// packed -> restart, all on the handle's stream (user_move).
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -60,13 +65,10 @@
 #include "handle.h"
 #include "common.cuh"
 #include "stack.cuh"
+#include "user_env.cuh"
 
 namespace mz {
 
-constexpr uint32_t kTagReset = 0x7169E004u;
-constexpr uint32_t kTagOpponent = 0x7169E005u;
-constexpr uint32_t kTagCard = 0x7169E006u;
-constexpr uint32_t kTagPlace = 0x7169E007u;
 constexpr int kMaxCells = 256;             // board cells per slot (Gomoku: up to 16 x 16)
 
 struct SpDev {
@@ -110,9 +112,11 @@ struct SpDev {
     int32_t* fin;              // [B] 0 = playing, T > 0 = finished after T moves, waiting to be packed,
                                //     -1 = MZ_ENV_HOST: packed, waiting for the next game's first rows
     int32_t* last_action;      // [B]
-    int32_t* host_action;      // [B] MZ_ENV_HOST: the action of the move in flight, -1 for a slot not playing it
+    int32_t* host_action;      // [B] MZ_ENV_HOST / MZ_ENV_USER: the action of the move in flight, -1 for a slot not
+                               //     playing it
     // counters: [0] env_steps, [1] games_finished, [2] staging cursor (may run past the capacity), [3] staged games,
-    //           [4] park events of this call, [5] end of the valid staged bytes
+    //           [4] park events of this call, [5] end of the valid staged bytes, [6] illegal opponent moves
+    //           (MZ_ENV_HOST), [7] rows a user environment wrote that the loop could not play (MZ_ENV_USER)
     unsigned long long* counters;
     unsigned char* staging;    // mapped pinned host memory
     unsigned long long staging_cap;
@@ -122,13 +126,6 @@ struct SpDev {
     const double* uniform;
     double temperature;
 };
-
-MZ_DEVINL double philox_uniform53(uint64_t seed, int64_t game, int move, uint32_t c2, uint32_t tag) {
-    const Philox4 r = philox4x32_10((uint32_t)game, (uint32_t)move, c2, (uint32_t)((uint64_t)game >> 32),
-                                    (uint32_t)seed, (uint32_t)(seed >> 32) ^ tag);
-    // 53 random bits like numpy's random_sample: (a >> 5) * 2^26 + (b >> 6)
-    return ((double)(r.x >> 5) * 67108864.0 + (double)(r.y >> 6)) * (1.0 / 9007199254740992.0);
-}
 
 // ------------------------------------------------------------------------------------------
 // environments
@@ -891,6 +888,12 @@ __global__ void __launch_bounds__(kActThreads) host_opponent_act_kernel(const Sp
 
 using namespace mz;
 
+// one thread per slot (the wrappers' __launch_bounds__)
+static cudaError_t launch_user_env(cudaKernel_t k, const MzUserEnvArgs& a, cudaStream_t stream) {
+    void* args[] = {const_cast<MzUserEnvArgs*>(&a)};
+    return cudaLaunchKernel(reinterpret_cast<const void*>(k), dim3((a.B + 127) / 128), dim3(128), args, 0, stream);
+}
+
 struct MzSelfPlay {
     MzSelfPlayDesc desc{};
     SpDev dev{};
@@ -925,6 +928,10 @@ struct MzSelfPlay {
     int opp_phase = 0;
     int32_t* d_defaults = nullptr;             // [B] the turn's random defaults, -1 for a slot without an opponent move
     int32_t* d_opp_actions = nullptr;          // [B] the host's opponent moves
+    // MZ_ENV_USER: the rows and kernels of MZ_ENV_HOST, with the step and the reset on the device
+    bool user = false;
+    MzUserEnvKernels user_k{};
+    MzUserEnvArgs user_args{};                 // the step's arguments; the reset's differ in `which`
 };
 
 void mz_selfplay_destroy(MzHandle* h) {
@@ -971,7 +978,8 @@ static int check_host_rows(MzHandle* h, const char* who, const uint8_t* which, c
 }
 
 static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int32_t muzero_player, const MzHostEnvDesc* e,
-                    const float* obs, const uint8_t* legal, const int32_t* to_play, bool window);
+                    const float* obs, const uint8_t* legal, const int32_t* to_play, bool window,
+                    const MzUserEnvDesc* u = nullptr, const MzUserEnvKernels* uk = nullptr);
 
 extern "C" int mz_selfplay_begin(MzHandle* h, const MzSelfPlayDesc* d) {
     return mz_selfplay_begin_vs(h, d, MZ_OPPONENT_SELF, 0);
@@ -1009,8 +1017,10 @@ extern "C" int mz_selfplay_begin_host_vs(MzHandle* h, const MzSelfPlayDesc* d, c
 
 // window: rec_obs keeps the last stacked_observations + 1 observations of a slot's game and the staged blocks none
 // (mz_selfplay_begin_host_window); otherwise the whole game's
+// u, uk: the user environment of MZ_ENV_USER and its compiled kernels
 static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int32_t muzero_player, const MzHostEnvDesc* e,
-                    const float* obs, const uint8_t* legal, const int32_t* to_play, bool window) {
+                    const float* obs, const uint8_t* legal, const int32_t* to_play, bool window,
+                    const MzUserEnvDesc* u, const MzUserEnvKernels* uk) {
     if (!h || !d) return fail(h, MZ_EINVAL, "mz_selfplay_begin: null argument");
     if (opponent != MZ_OPPONENT_SELF && opponent != MZ_OPPONENT_EXPERT && opponent != MZ_OPPONENT_RANDOM)
         return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin_vs: unknown opponent " + std::to_string(opponent));
@@ -1069,6 +1079,14 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
             name = "the host-stepped environment"; C = e->obs_channels; ph = e->obs_h; pw = e->obs_w; A_env = A;
             break;
         }
+        case MZ_ENV_USER: {
+            if (!u || !uk) return fail(h, MZ_EINVAL, "mz_selfplay_begin: user environments (MZ_ENV_USER) start with mz_selfplay_begin_user");
+            if (opponent != MZ_OPPONENT_SELF) return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: user environments play against themselves only");
+            if (u->obs_channels < 1 || u->obs_h < 1 || u->obs_w < 1)
+                return fail(h, MZ_EINVAL, "mz_selfplay_begin_user: the observation's channels, height and width must be >= 1");
+            name = "the user environment"; C = u->obs_channels; ph = u->obs_h; pw = u->obs_w; A_env = A;
+            break;
+        }
         default: return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin: unknown environment");
     }
     // the network input: the observation and, per stacked step, an earlier observation and its action plane
@@ -1089,7 +1107,8 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
         const unsigned long long Tm = (unsigned long long)d->max_moves;
         const unsigned long long per_slot = (unsigned long long)h->obs_elems * 4 + (unsigned long long)rows * O * 4 +
                                             Tm * (8 + 4ull * A + 12) +
-                                            (d->env == MZ_ENV_HOST ? (unsigned long long)O * 4 + A + 16 : 0) + 24ull * A + 64;
+                                            (d->env == MZ_ENV_HOST || d->env == MZ_ENV_USER ? (unsigned long long)O * 4 + A + 16 : 0) +
+                                            (d->env == MZ_ENV_USER ? (unsigned long long)u->state_bytes + 16 : 0) + 24ull * A + 64;
         size_t free_bytes = 0, total_bytes = 0;
         if (cudaMemGetInfo(&free_bytes, &total_bytes) == cudaSuccess && per_slot * B > free_bytes)
             return fail(h, MZ_ENOMEM, "mz_selfplay_begin: the records of " + std::to_string(B) + " slots do not fit on the device: " +
@@ -1129,7 +1148,7 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
               sp_alloc(sp, &s.fin, B) && sp_alloc(sp, &s.last_action, B) && sp_alloc(sp, &s.counters, 8) &&
               sp_alloc(sp, &sp->d_forced, B) && sp_alloc(sp, &sp->d_uniform, B) && sp_alloc(sp, &sp->d_noise, (size_t)B * A) &&
               sp_alloc(sp, &sp->d_first, B) && sp_alloc(sp, &s.host_action, B);
-    if (ok && d->env == MZ_ENV_HOST) {
+    if (ok && (d->env == MZ_ENV_HOST || d->env == MZ_ENV_USER)) {
         float *r_obs = nullptr, *r_reward = nullptr;
         uint8_t *r_done = nullptr, *r_legal = nullptr;
         int32_t* r_to_play = nullptr;
@@ -1137,10 +1156,22 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
              sp_alloc(sp, &r_legal, (size_t)B * A) && sp_alloc(sp, &r_to_play, B) && sp_alloc(sp, &sp->d_which, B) &&
              sp_alloc(sp, &sp->d_finished, B) && sp_alloc(sp, &sp->d_defaults, B) && sp_alloc(sp, &sp->d_opp_actions, B);
         sp->rows = HostRows{r_obs, r_reward, r_done, r_legal, r_to_play};
-        sp->host = true;
+        sp->host = d->env == MZ_ENV_HOST;
         sp->opp_phase = opponent != MZ_OPPONENT_SELF;
         sp->actions.assign(B, -1);
         sp->awaiting.assign(B, 0);
+    }
+    if (ok && d->env == MZ_ENV_USER) {
+        MzUserEnvArgs& a = sp->user_args;
+        a.state_stride = ((int64_t)u->state_bytes + 15) & ~(int64_t)15;
+        ok = sp_alloc(sp, &a.state, (size_t)B * (a.state_stride > 0 ? a.state_stride : 1));
+        a.B = B; a.O = O; a.A = A; a.P = h->search.num_players; a.seed = h->search.seed;
+        a.game_id = s.game_id; a.move = s.move; a.action = s.host_action; a.which = sp->d_finished;
+        a.first_game_id = d->first_game_id; a.id_stride = s.id_stride;
+        a.obs = sp->rows.obs; a.reward = sp->rows.reward; a.done = sp->rows.done; a.legal = sp->rows.legal;
+        a.to_play = sp->rows.to_play; a.bad = s.counters + 7;
+        sp->user = true;
+        sp->user_k = *uk;
     }
     if (!ok) { mz_selfplay_destroy(h); return fail(h, MZ_ENOMEM, "mz_selfplay_begin: out of device memory"); }
     // staging (two areas of this size): by default 4x the room for every slot finishing a maximum-length game at once,
@@ -1177,10 +1208,17 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
     s.index = sp->d_index[0];
     s.staging_cap = cap;
     cudaEventCreate(&sp->e0); cudaEventCreate(&sp->e1);
-    if (sp->host) {
-        MZ_CUDA(h, cudaMemcpyAsync(sp->rows.obs, obs, (size_t)B * O * 4, cudaMemcpyHostToDevice, h->stream));
-        MZ_CUDA(h, cudaMemcpyAsync(sp->rows.legal, legal, (size_t)B * A, cudaMemcpyHostToDevice, h->stream));
-        MZ_CUDA(h, cudaMemcpyAsync(sp->rows.to_play, to_play, (size_t)B * 4, cudaMemcpyHostToDevice, h->stream));
+    if (sp->host || sp->user) {
+        if (sp->host) {
+            MZ_CUDA(h, cudaMemcpyAsync(sp->rows.obs, obs, (size_t)B * O * 4, cudaMemcpyHostToDevice, h->stream));
+            MZ_CUDA(h, cudaMemcpyAsync(sp->rows.legal, legal, (size_t)B * A, cudaMemcpyHostToDevice, h->stream));
+            MZ_CUDA(h, cudaMemcpyAsync(sp->rows.to_play, to_play, (size_t)B * 4, cudaMemcpyHostToDevice, h->stream));
+        } else {
+            MzUserEnvArgs a = sp->user_args;
+            a.which = nullptr;
+            MZ_CUDA(h, launch_user_env(sp->user_k.reset, a, h->stream));
+            h->launches += 1;
+        }
         host_start_kernel<<<B, host_slot_threads(s), 0, h->stream>>>(s, sp->rows, nullptr, d->first_game_id);
     } else {
         selfplay_reset_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(s, d->first_game_id);
@@ -1188,6 +1226,15 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
     h->launches += 1;
     MZ_CUDA(h, cudaGetLastError());
     MZ_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (sp->user) {
+        unsigned long long bad = 0;
+        MZ_CUDA(h, cudaMemcpy(&bad, s.counters + 7, 8, cudaMemcpyDeviceToHost));
+        if (bad) {
+            mz_selfplay_destroy(h);
+            return fail(h, MZ_EINVAL, "mz_selfplay_begin_user: mz_env_reset left " + std::to_string(bad) +
+                                      " slots without a legal action or with a to_play outside the players");
+        }
+    }
     return MZ_OK;
 }
 
@@ -1235,6 +1282,26 @@ static int sp_move_setup(MzHandle* h, double temperature, const MzSelfPlayInject
     return MZ_OK;
 }
 
+// One pass of a user environment's loop: act != 0 plays a move (the act kernel, then the user step on the slots that
+// played), act == 0 only packs the games parked by an earlier call; then observe packs the finished games and their
+// slots start the next game from the user reset's rows.
+static int user_pass(MzHandle* h, const SpDev& s, int act) {
+    MzSelfPlay* sp = h->sp;
+    const int B = s.B;
+    if (act) {
+        if (s.A <= 128) host_act_kernel<128><<<(B + kActThreads - 1) / kActThreads, kActThreads, 0, h->stream>>>(s);
+        else host_act_kernel<256><<<(B + kActThreads - 1) / kActThreads, kActThreads, 0, h->stream>>>(s);
+        MZ_CUDA(h, launch_user_env(sp->user_k.step, sp->user_args, h->stream));
+    } else {
+        MZ_CUDA(h, cudaMemsetAsync(s.host_action, 0xFF, (size_t)B * 4, h->stream));     // -1: no slot plays
+    }
+    host_observe_kernel<<<B, host_slot_threads(s), 0, h->stream>>>(s, sp->rows, sp->d_finished);
+    MZ_CUDA(h, launch_user_env(sp->user_k.reset, sp->user_args, h->stream));            // which = d_finished
+    host_start_kernel<<<B, host_slot_threads(s), 0, h->stream>>>(s, sp->rows, sp->d_finished, 0);
+    h->launches += act ? 5 : 3;
+    return MZ_OK;
+}
+
 static int sp_enqueue(MzHandle* h, int32_t n_moves, double temperature, const MzSelfPlayInject* inj, const char* who) {
     if (!h || !h->sp) return fail(h, MZ_ESTATE, std::string(who) + ": call mz_selfplay_begin first");
     if (!h->weights_loaded) return fail(h, MZ_ESTATE, std::string(who) + ": weights not loaded");
@@ -1263,15 +1330,25 @@ static int sp_enqueue(MzHandle* h, int32_t n_moves, double temperature, const Mz
     }
     MZ_CUDA(h, cudaEventRecord(sp->e0, h->stream));
     if (sp->h_counters[4]) {                           // games parked by the previous call first, so their slots play again
-        launch_selfplay_step(s, 0, h->stream);
-        h->launches += 1;
+        if (sp->user) {
+            rc = user_pass(h, s, 0);
+            if (rc) return rc;
+        } else {
+            launch_selfplay_step(s, 0, h->stream);
+            h->launches += 1;
+        }
     }
     MZ_CUDA(h, cudaMemsetAsync(s.counters + 4, 0, 8, h->stream));      // [4] = park events of THIS call
     for (int m = 0; m < n_moves; ++m) {
         int rc = mz_dispatch_search(h, call, false, false, 0);
         if (rc) return rc;
-        launch_selfplay_step(s, 1, h->stream);
-        h->launches += 1;
+        if (sp->user) {
+            rc = user_pass(h, s, 1);
+            if (rc) return rc;
+        } else {
+            launch_selfplay_step(s, 1, h->stream);
+            h->launches += 1;
+        }
     }
     MZ_CUDA(h, cudaGetLastError());
     MZ_CUDA(h, cudaEventRecord(sp->e1, h->stream));
@@ -1291,11 +1368,41 @@ static int sp_wait(MzHandle* h, MzSelfPlayStats* stats) {
     }
     float ms = 0.0f;
     if (cudaEventElapsedTime(&ms, sp->e0, sp->e1) == cudaSuccess && stats) stats->device_ms = ms;
+    if (sp->user) {
+        MZ_CUDA(h, cudaMemcpy(sp->h_counters + 7, sp->dev.counters + 7, 8, cudaMemcpyDeviceToHost));
+        if (sp->h_counters[7])
+            return fail(h, MZ_EINVAL, "the user environment wrote " + std::to_string(sp->h_counters[7]) +
+                                      " rows without a legal action or with a to_play outside the players (those games "
+                                      "were ended there); begin the loop again");
+    }
     return MZ_OK;
 }
 
 extern "C" int mz_selfplay_moves(MzHandle* h, int32_t n_moves, double temperature, const MzSelfPlayInject* inj, MzSelfPlayStats* stats) {
+    if (h && h->sp && h->sp->user)
+        return fail(h, MZ_ESTATE, "mz_selfplay_moves: a user environment's loop moves with mz_selfplay_user_moves");
     int rc = sp_enqueue(h, n_moves, temperature, inj, "mz_selfplay_moves");
+    if (rc) return rc;
+    return sp_wait(h, stats);
+}
+
+extern "C" int mz_selfplay_begin_user(MzHandle* h, const MzSelfPlayDesc* d, const MzUserEnvDesc* e) {
+    if (!h || !d || !e || !e->source) return fail(h, MZ_EINVAL, "mz_selfplay_begin_user: null argument");
+    if (d->env != MZ_ENV_USER) return fail(h, MZ_EINVAL, "mz_selfplay_begin_user: desc->env must be MZ_ENV_USER");
+    if (e->state_bytes < 0 || e->state_bytes > MZ_USER_ENV_MAX_STATE_BYTES)
+        return fail(h, MZ_EINVAL, "mz_selfplay_begin_user: state_bytes must lie in [0, " +
+                                  std::to_string(MZ_USER_ENV_MAX_STATE_BYTES) + "], got " + std::to_string(e->state_bytes));
+    MZ_CUDA(h, cudaSetDevice(h->device));
+    MzUserEnvKernels k;
+    const int rc = mz_user_env_kernels(h, e->source, &k);
+    if (rc) return rc;
+    return sp_begin(h, d, MZ_OPPONENT_SELF, 0, nullptr, nullptr, nullptr, nullptr, false, e, &k);
+}
+
+extern "C" int mz_selfplay_user_moves(MzHandle* h, int32_t n_moves, double temperature, const MzSelfPlayInject* inj,
+                                      MzSelfPlayStats* stats) {
+    if (!h || !h->sp || !h->sp->user) return fail(h, MZ_ESTATE, "mz_selfplay_user_moves: call mz_selfplay_begin_user first");
+    int rc = sp_enqueue(h, n_moves, temperature, inj, "mz_selfplay_user_moves");
     if (rc) return rc;
     return sp_wait(h, stats);
 }

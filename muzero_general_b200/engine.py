@@ -777,6 +777,53 @@ class HostEnvSelfPlayLoop(DeviceSelfPlayLoop):
         return buf, index, {gid: self._finished_rows.pop(gid) for gid in ids}
 
 
+class UserEnvSelfPlayLoop(DeviceSelfPlayLoop):
+    """Python face of mz_selfplay_begin_user / _user_moves: the device loop for a game whose environment is CUDA source
+    (``source`` defines ``mz_env_reset`` and ``mz_env_step`` against csrc/user_env.cuh; ``state_bytes`` per slot).  The
+    library compiles the source with NVRTC for sm_90a, once per handle and source.  ``moves``, ``enqueue`` / ``wait``,
+    ``drain`` and ``peek`` are the device loop's."""
+
+    def __init__(self, engine: SearchEngine, source: str, state_bytes: int, obs_shape, max_moves: int,
+                 temperature_threshold=None, first_game_id: int = 0, staging_bytes: int = 0, game_id_stride: int = 0,
+                 td_steps: int = 0, per_alpha: float = 1.0, discount: float = 1.0, stacked_observations: int = 0):
+        self.engine = engine
+        self.opponent, self.muzero_player = "self", 0
+        d = self._desc(_lib.MZ_ENV_USER, max_moves, temperature_threshold, 0, first_game_id, staging_bytes, game_id_stride,
+                       td_steps, per_alpha, discount, stacked_observations)
+        self._source = source.encode()
+        e = _lib.MzUserEnvDesc(self._source, int(state_bytes), *(int(x) for x in obs_shape))
+        rc = engine.lib.mz_selfplay_begin_user(engine._h, C.byref(d), C.byref(e))
+        if rc == _lib.MZ_EUNSUPPORTED:
+            raise NotImplementedError(engine.lib.mz_last_error(engine._h).decode())
+        engine._check(rc)
+        self.stats = _lib.MzSelfPlayStats()
+
+    def moves(self, n_moves: int, temperature: float, forced_action=None, uniform=None, noise=None, first_index=None):
+        eng = self.engine
+        keep = []
+        inj = self._inject(keep, forced_action, uniform, noise, first_index)
+        eng._check(eng.lib.mz_selfplay_user_moves(eng._h, int(n_moves), float(temperature),
+                                                 C.byref(inj) if inj is not None else None, C.byref(self.stats)))
+        return self.stats
+
+    @property
+    def compiles(self):
+        """NVRTC compiles made for this engine's user environments so far."""
+        return int(self.engine.lib.mz_debug_user_env_compiles(self.engine._h))
+
+
+def debug_user_env_compile(source: str, log_bytes: int = 1 << 16):
+    """Compiles a user environment's source as mz_selfplay_begin_user does, on the host (no GPU needed).  Returns
+    ``(rc, log, info)``: the library's return code, NVRTC's log (ptxas's resource report included) and a dict of the
+    wrapper kernels' ``{kernel: (registers, stack frame bytes, spill store bytes, spill load bytes)}`` plus
+    ``"nvrtc_version"``; ``mz_last_error(NULL)`` holds the reason of a failure."""
+    lib = _lib.load_library()
+    log = C.create_string_buffer(int(log_bytes))
+    info = (C.c_int32 * 9)()
+    rc = lib.mz_debug_user_env_compile(source.encode(), log, int(log_bytes), info)
+    return rc, log.value.decode(), {"reset": tuple(info[0:4]), "step": tuple(info[4:8]), "nvrtc_version": int(info[8])}
+
+
 def parse_staged_game(buf: bytes, off: int):
     """One packed block of ``mz_selfplay_drain`` -> dict of numpy views into ``buf`` (no copies)."""
     H = _lib.MZ_STAGED_HEADER_BYTES

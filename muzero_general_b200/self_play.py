@@ -27,7 +27,7 @@ from collections import deque
 import numpy
 
 from . import _lib
-from .engine import DeviceSelfPlayLoop, HostEnvSelfPlayLoop, SearchEngine, parse_staged_game
+from .engine import DeviceSelfPlayLoop, HostEnvSelfPlayLoop, SearchEngine, UserEnvSelfPlayLoop, parse_staged_game
 
 
 # ----------------------------------------------------------------------------------------
@@ -450,7 +450,7 @@ class SelfPlay:
                     trained_steps=_call(shared_storage, "get_info", "training_step"))
                 if self.num_parallel_games > 1:
                     # the lockstep batch advances between two weight refreshes; every finished game goes to the buffer
-                    if self.loop_path in ("device", "device-host-env"):
+                    if self.loop_path != "host":
                         games = self.play_moves(int(getattr(cfg, "moves_per_weight_refresh", 8)), temperature,
                                                 cfg.temperature_threshold)
                     else:
@@ -619,12 +619,24 @@ class SelfPlay:
         return (bool(getattr(self.config, "host_env_device_loop", False)) and self.rng_mode == "philox"
                 and not self._device_env_name())
 
+    def _user_env_source(self):
+        """The plug-in's environment as CUDA source (``Game.DEVICE_SOURCE``) when it plays on the device: philox draws,
+        no built-in device environment in use and ``config.device_envs`` not False; else None."""
+        source = getattr(self.Game, "DEVICE_SOURCE", None)
+        if (source is None or self.rng_mode != "philox" or self._device_env_name()
+                or not getattr(self.config, "device_envs", True)):
+            return None
+        return source
+
     @property
     def loop_path(self):
-        """"device": environments, sampling and records on the GPU (mz_selfplay_*); "device-host-env": the same with the
+        """"device": environments, sampling and records on the GPU (mz_selfplay_*); "device-user-env": the same with the
+        plug-in's ``DEVICE_SOURCE`` as the environment (mz_selfplay_begin_user); "device-host-env": the same with the
         game's own environment stepped on the host (mz_selfplay_host_*); "host": the host loop."""
         if self._device_env_name():
             return "device"
+        if self._user_env_source() is not None:
+            return "device-user-env"
         return "device-host-env" if self._host_env_device_loop() else "host"
 
     @property
@@ -643,10 +655,12 @@ class SelfPlay:
         GPU (``mz_selfplay_moves``) and only finished games cross to the host, as ``PackedGameHistory`` objects.  With
         ``rng_mode="philox"``, ``config.host_env_device_loop`` and no device environment in use, the same loop runs
         with the game's own environment stepped on the host (``DeviceHostEnvSelfPlay``).  Otherwise the host loop
-        (``BatchedSelfPlay.move``) is used."""
+        (``BatchedSelfPlay.move``) is used.  A plug-in whose ``Game`` has ``DEVICE_SOURCE`` (the CUDA source of its
+        environment, against csrc/user_env.cuh) and ``DEVICE_STATE_BYTES`` plays the device loop with that source as
+        its environment (``loop_path == "device-user-env"``), compiled at the first call."""
         if self.loop_path != "host":
             if getattr(self, "_device_loop", None) is None:
-                self._device_loop = (DeviceBatchedSelfPlay if self.loop_path == "device" else DeviceHostEnvSelfPlay)(
+                self._device_loop = (DeviceHostEnvSelfPlay if self.loop_path == "device-host-env" else DeviceBatchedSelfPlay)(
                     self, temperature_threshold)
             games = self._device_loop.moves(n_moves, temperature)
             self.played_games += len(games)
@@ -677,7 +691,9 @@ class SelfPlay:
         calls give the same games.  The device loop replaces the handle's self-play loop: with one running, call
         ``reset_stream()`` first."""
         cfg = self.config
-        if self.loop_path == "host":
+        # the routes test games have without a user environment (none plays against opponents on one)
+        path = "device" if self._device_env_name() else ("device-host-env" if self._host_env_device_loop() else "host")
+        if path == "host":
             raise NotImplementedError(
                 "test games on the device need rng_mode='philox' and a device environment (CartPole, TicTacToe, "
                 "Connect4, Gomoku, Twenty-One, Simple Grid or Gridworld with device_envs on) or "
@@ -696,7 +712,7 @@ class SelfPlay:
         B, stride, first = self.num_parallel_games, self.game_id_stride, self._next_test_game_id
         i = numpy.arange(n_games)
         wanted = first + (i // B) * stride + i % B
-        Loop = DeviceBatchedSelfPlay if self.loop_path == "device" else DeviceHostEnvSelfPlay
+        Loop = DeviceBatchedSelfPlay if path == "device" else DeviceHostEnvSelfPlay
         dev = Loop(self, cfg.temperature_threshold, opponent, muzero_player, first_game_id=first)
         games = PackedGames(dev.obs_shape, dev.obs_dtype, dev.reward_type)
         missing = n_games
@@ -796,16 +812,19 @@ class DeviceBatchedSelfPlay:
         self.reward_type = getattr(vec, "REWARD_TYPE", int) if vec is not None else float
         # test-mode games never reach a replay buffer (self_play.py:54-66): no priorities against an opponent
         priorities = opponent == "self" and getattr(cfg, "PER", False) and getattr(cfg, "device_priorities", True)
-        self.loop = DeviceSelfPlayLoop(worker.model.engine, Game.DEVICE_ENV, cfg.max_moves,
-                                       temperature_threshold=temperature_threshold,
-                                       reward_scale=getattr(vec, "REWARD_SCALE", 1),
-                                       first_game_id=worker.first_game_id if first_game_id is None else first_game_id,
-                                       game_id_stride=worker.game_id_stride,
-                                       td_steps=int(cfg.td_steps) if priorities else 0,
-                                       per_alpha=cfg.PER_alpha, discount=cfg.discount,
-                                       staging_bytes=int(getattr(cfg, "selfplay_staging_bytes", 0) or 0),
-                                       opponent=opponent, muzero_player=muzero_player,
-                                       stacked_observations=int(cfg.stacked_observations))
+        kw = dict(temperature_threshold=temperature_threshold,
+                  first_game_id=worker.first_game_id if first_game_id is None else first_game_id,
+                  game_id_stride=worker.game_id_stride, td_steps=int(cfg.td_steps) if priorities else 0,
+                  per_alpha=cfg.PER_alpha, discount=cfg.discount,
+                  staging_bytes=int(getattr(cfg, "selfplay_staging_bytes", 0) or 0),
+                  stacked_observations=int(cfg.stacked_observations))
+        if worker.loop_path == "device-user-env":
+            self.loop = UserEnvSelfPlayLoop(worker.model.engine, Game.DEVICE_SOURCE, int(Game.DEVICE_STATE_BYTES),
+                                            self.obs_shape, cfg.max_moves, **kw)
+        else:
+            self.loop = DeviceSelfPlayLoop(worker.model.engine, Game.DEVICE_ENV, cfg.max_moves,
+                                           reward_scale=getattr(vec, "REWARD_SCALE", 1), opponent=opponent,
+                                           muzero_player=muzero_player, **kw)
         self.moves_per_call = int(getattr(cfg, "selfplay_moves_per_call", 64) or 64)   # upper bound of a chunk
         self.chunk = min(4, self.moves_per_call)                                      # adapted to the staging fill below
         self.device_ms = 0.0          # device time of all mz_selfplay_moves calls so far
