@@ -11,7 +11,8 @@
 // reset starts game ctx.game_id in slot ctx.slot: it fills the slot's state and the row's observation, legal mask and
 // to_play.  step plays `action` (legal in the row's mask): it updates the state and writes the row after the move.
 // Before reset the row's legal mask is all ones and to_play 0; before step its reward and done are 0; whatever a call
-// does not write keeps those values (step: the row of the previous move).  `state` is the slot's own
+// does not write keeps those values (step: the row of the previous move).  A row that ends the game (done = 1) may have
+// no legal action; a reset's row, and a step's row of a game still in play, must have one.  `state` is the slot's own
 // MzUserEnvDesc.state_bytes bytes (16-byte aligned, zero before the slot's first reset, not cleared between games).
 // One thread runs one slot; the slots of a batch run concurrently.
 //
