@@ -655,7 +655,8 @@ typedef struct MzSelfPlayPeek {
  *   float priority[T] (zeros unless td_steps > 0); float observation[T+1][O] (index 0 = reset observation); padding to 8.
  * Loops begun with mz_selfplay_begin_host_window stage O = 0 and no observations: the caller kept them.
  * = the fields of GameHistory (self_play.py:479-511) minus the dummy first entries.
- * In test-mode games (mz_selfplay_begin_vs or mz_selfplay_begin_host_vs with an opponent) a move the opponent played has root_value NaN and all
+ * In test-mode games (mz_selfplay_begin_vs, mz_selfplay_begin_host_vs or mz_selfplay_begin_user_vs with an opponent) a move the
+ * opponent played has root_value NaN and all
  * visit counts 0 (store_search_statistics(None), self_play.py:496-511: root_values holds None there and child_visits
  * has no row); its action, reward, to_play and observation are recorded like MuZero's. */
 #define MZ_STAGED_HEADER_BYTES 32
@@ -795,12 +796,39 @@ int mz_selfplay_begin_user(MzHandle* h, const MzSelfPlayDesc* desc, const MzUser
  * a to_play outside the players): such a game was ended there, and the loop should be begun again. */
 int mz_selfplay_user_moves(MzHandle* h, int32_t n_moves, double temperature, const MzSelfPlayInject* inject,
                            MzSelfPlayStats* stats);
+/* Test-mode games of user environments: play_game(temperature, threshold, False, opponent, muzero_player) as
+ * mz_selfplay_begin_vs plays them, with the opponent's moves stepped by the source's mz_env_step.  With MZ_OPPONENT_SELF
+ * and muzero_player 0 the call IS mz_selfplay_begin_user.  EXPERT needs a source that defines the macro MZ_ENV_EXPERT
+ * and (csrc/user_env_expert.cuh)
+ *   __device__ int mz_env_expert(const void* state, const MzEnvCtx& ctx, const MzEnvRow& row, int default_action);
+ * the opponent's move in the slot's current position: row is the published row (observation, legal mask, to_play; not
+ * to be written), ctx.move the index of the move about to be played, default_action the random default of
+ * MZ_OPPONENT_RANDOM (the same Philox draw), so an expert that falls back to it falls back as the built-in experts do.
+ * Each move of mz_selfplay_user_moves / _enqueue then runs on the device with no host synchronisation: the search and
+ * MuZero's moves (slots whose to_play is not muzero_player do not move), then two opponent passes (the random default,
+ * the expert for EXPERT, recorded with root_value NaN and zero visit counts, the user step, observe, reset and
+ * restart); begin runs the two passes too, so the opponent opens the games where it moves first.  The second pass
+ * opens the games the first one ended, so games whose sides alternate are played in the same moves as by
+ * mz_selfplay_begin_vs.  A slot whose opponent moves a third time in a row, or whose side to move is MuZero's again
+ * after MuZero moved, waits for the next pass of its side; its games do not change, since every draw is keyed by game
+ * id and move.  max_moves counts both sides' moves, and so does MzSelfPlayStats.env_steps.
+ * Refused: mz_selfplay_begin_user's refusals and mz_selfplay_begin_vs's (an unknown opponent: MZ_EUNSUPPORTED;
+ * muzero_player outside {0, 1}, td_steps > 0 with an opponent: MZ_EINVAL), an opponent on a handle of one player
+ * (MZ_EINVAL), EXPERT on a source without mz_env_expert (MZ_EUNSUPPORTED); all before the running loop is dropped.
+ * An expert move out of range or not legal in the slot's mask is replaced by the default and fails the call (begin or
+ * moves) with MZ_EINVAL, as a bad row does; begin the loop again. */
+int mz_selfplay_begin_user_vs(MzHandle* h, const MzSelfPlayDesc* desc, const MzUserEnvDesc* env, int32_t opponent,
+                              int32_t muzero_player);
 /* Debug, host only (no device needed): compiles source as mz_selfplay_begin_user does.  log (may be NULL) receives
  * NVRTC's log, ptxas's resource report included, truncated to log_bytes - 1 bytes and NUL-terminated; info (may be
  * NULL) receives info[9] = {registers, stack frame bytes, spill store bytes, spill load bytes} of the reset wrapper
  * kernel, the same of the step wrapper kernel, and NVRTC's version as 1000 * major + 10 * minor (-1 for a count the log
  * does not give).  MZ_EINVAL on a compile failure or a missing function, MZ_EUNSUPPORTED without NVRTC. */
 int mz_debug_user_env_compile(const char* source, char* log, int64_t log_bytes, int32_t* info);
+/* Debug, host only: mz_debug_user_env_compile with info[14]: info[0..8] as there, info[9] = 1 when the expert wrapper
+ * was compiled (the source defines MZ_ENV_EXPERT), info[10..13] {registers, stack frame bytes, spill store bytes,
+ * spill load bytes} of it (-1 without one).  A source that defines MZ_ENV_EXPERT but not mz_env_expert: MZ_EINVAL. */
+int mz_debug_user_env_expert_compile(const char* source, char* log, int64_t log_bytes, int32_t* info);
 /* NVRTC compiles made for this handle's user environments so far (a begin with a cached source makes none) */
 int64_t mz_debug_user_env_compiles(const MzHandle* h);
 

@@ -199,6 +199,9 @@ SYMBOLS = [
     ("mz_selfplay_user_moves", C.c_int, [C.c_void_p, C.c_int32, C.c_double, C.POINTER(MzSelfPlayInject),
                                          C.POINTER(MzSelfPlayStats)]),
     ("mz_debug_user_env_compile", C.c_int, [C.c_char_p, C.c_char_p, C.c_int64, C.POINTER(C.c_int32)]),
+    ("mz_selfplay_begin_user_vs", C.c_int, [C.c_void_p, C.POINTER(MzSelfPlayDesc), C.POINTER(MzUserEnvDesc), C.c_int32,
+                                            C.c_int32]),
+    ("mz_debug_user_env_expert_compile", C.c_int, [C.c_char_p, C.c_char_p, C.c_int64, C.POINTER(C.c_int32)]),
     ("mz_debug_user_env_compiles", C.c_int64, [C.c_void_p]),
     ("mz_debug_opponent_action", C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p]),

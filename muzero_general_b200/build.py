@@ -24,10 +24,12 @@ def needs_build():
 
 
 def write_prelude(out_dir):
-    """The NVRTC prelude of user environments (csrc/user_env.cuh and the philox.cuh it includes) as C++ string
-    literals, so the library carries the headers it compiles user sources against."""
+    """The NVRTC prelude of user environments (csrc/user_env.cuh and the philox.cuh it includes) and their epilogue
+    (csrc/user_env_expert.cuh) as C++ string literals, so the library carries the headers it compiles user sources
+    against."""
     parts = []
-    for name, var in (("philox.cuh", "kPhiloxCuh"), ("user_env.cuh", "kUserEnvCuh")):
+    for name, var in (("philox.cuh", "kPhiloxCuh"), ("user_env.cuh", "kUserEnvCuh"),
+                      ("user_env_expert.cuh", "kUserEnvExpertCuh")):
         text = open(os.path.join(CSRC, name)).read()
         assert ")MZPRELUDE\"" not in text
         parts.append(f'static const char {var}[] = R"MZPRELUDE({text})MZPRELUDE";\n')

@@ -112,9 +112,10 @@ int mz_network_enqueue(MzHandle* h, const mz::InferCall& c);
 int mz_network_guard(MzHandle* h, const mz::InferCall& c);
 void mz_reanalyse_destroy(MzHandle* h);
 void mz_selfplay_destroy(MzHandle* h);
-// The wrapper kernels of a user environment (user_env.cuh) compiled from `source`, from the handle's cache or by NVRTC.
+// The wrapper kernels of a user environment (user_env.cuh) compiled from `source`, from the handle's cache or by NVRTC;
+// expert is nullptr for a source without MZ_ENV_EXPERT (user_env_expert.cuh).
 struct MzUserEnvKernels {
-    cudaKernel_t reset = nullptr, step = nullptr;
+    cudaKernel_t reset = nullptr, step = nullptr, expert = nullptr;
 };
 int mz_user_env_kernels(MzHandle* h, const char* source, MzUserEnvKernels* out);
 void mz_user_env_destroy(MzHandle* h);

@@ -57,7 +57,15 @@
 // User environments (MZ_ENV_USER, mz_selfplay_begin_user): the host-stepped loop's kernels with the host's step replaced
 // by the wrapper kernels of a plug-in's CUDA source (user_env.cuh, compiled by user_env.cu), which write the rows the
 // host would have uploaded.  A move is act -> mz_user_env_step -> observe -> mz_user_env_reset on the slots observe
-// packed -> restart, all on the handle's stream (user_move).
+// packed -> restart, all on the handle's stream (user_pass).
+// Their test-mode games (mz_selfplay_begin_user_vs): a move is that pass for MuZero (host_act_kernel skips the slots whose
+// side to move is the opponent's), then kUserOpponentPasses opponent passes: opponent_turn -> [mz_user_env_expert, the
+// source's mz_env_expert, for MZ_OPPONENT_EXPERT] -> opponent_act -> the same step, observe, reset and restart; begin
+// runs them too, so the opponent opens the games where it moves first.  The second pass plays the openings of the games
+// the first pass's moves ended, so a game whose sides alternate is played in the moves the device environments' loop
+// plays it in (that loop replies and opens in its step kernel), and finishes in the same call.  A slot whose opponent
+// moves a third time in a row idles through the next search: every draw is keyed by game id and move, so its games
+// do not change.
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -116,7 +124,8 @@ struct SpDev {
                                //     playing it
     // counters: [0] env_steps, [1] games_finished, [2] staging cursor (may run past the capacity), [3] staged games,
     //           [4] park events of this call, [5] end of the valid staged bytes, [6] illegal opponent moves
-    //           (MZ_ENV_HOST), [7] rows a user environment wrote that the loop could not play (MZ_ENV_USER)
+    //           (MZ_ENV_HOST), [7] rows a user environment wrote that the loop could not play and illegal moves of its
+    //           expert (MZ_ENV_USER)
     unsigned long long* counters;
     unsigned char* staging;    // mapped pinned host memory
     unsigned long long staging_cap;
@@ -888,9 +897,10 @@ __global__ void __launch_bounds__(kActThreads) host_opponent_act_kernel(const Sp
 
 using namespace mz;
 
-// one thread per slot (the wrappers' __launch_bounds__)
-static cudaError_t launch_user_env(cudaKernel_t k, const MzUserEnvArgs& a, cudaStream_t stream) {
-    void* args[] = {const_cast<MzUserEnvArgs*>(&a)};
+// one thread per slot (the wrappers' __launch_bounds__); the expert wrapper takes the turn's defaults and writes actions
+static cudaError_t launch_user_env(cudaKernel_t k, const MzUserEnvArgs& a, cudaStream_t stream,
+                                   const int32_t* defaults = nullptr, int32_t* actions = nullptr) {
+    void* args[] = {const_cast<MzUserEnvArgs*>(&a), &defaults, &actions};
     return cudaLaunchKernel(reinterpret_cast<const void*>(k), dim3((a.B + 127) / 128), dim3(128), args, 0, stream);
 }
 
@@ -980,6 +990,9 @@ static int check_host_rows(MzHandle* h, const char* who, const uint8_t* which, c
 static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int32_t muzero_player, const MzHostEnvDesc* e,
                     const float* obs, const uint8_t* legal, const int32_t* to_play, bool window,
                     const MzUserEnvDesc* u = nullptr, const MzUserEnvKernels* uk = nullptr);
+enum { kUserPack = 0, kUserMuZero = 1, kUserOpponent = 2 };      // the passes of user_pass
+constexpr int kUserOpponentPasses = 2;                            // opponent passes per move (and at begin)
+static int user_pass(MzHandle* h, const SpDev& s, int pass);
 
 extern "C" int mz_selfplay_begin(MzHandle* h, const MzSelfPlayDesc* d) {
     return mz_selfplay_begin_vs(h, d, MZ_OPPONENT_SELF, 0);
@@ -1029,6 +1042,12 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
                                   "of host-stepped games begin with mz_selfplay_begin_host_vs)");
     if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_HOST && h->search.num_players < 2)
         return fail(h, MZ_EINVAL, "mz_selfplay_begin_host_vs: the handle's game has one player, its opponent is \"self\"");
+    if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_USER && u && h->search.num_players < 2)
+        return fail(h, MZ_EINVAL, "mz_selfplay_begin_user_vs: the handle's game has one player, its opponent is \"self\"");
+    if (opponent == MZ_OPPONENT_EXPERT && d->env == MZ_ENV_USER && u && uk && !uk->expert)
+        return fail(h, MZ_EUNSUPPORTED, "mz_selfplay_begin_user_vs: the source has no expert opponent: define MZ_ENV_EXPERT "
+                                        "and __device__ int mz_env_expert(const void* state, const MzEnvCtx& ctx, "
+                                        "const MzEnvRow& row, int default_action)");
     if (muzero_player != 0 && muzero_player != 1)
         return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: muzero_player must be 0 or 1, got " + std::to_string(muzero_player));
     if (opponent != MZ_OPPONENT_SELF && d->env == MZ_ENV_CARTPOLE)
@@ -1081,7 +1100,6 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
         }
         case MZ_ENV_USER: {
             if (!u || !uk) return fail(h, MZ_EINVAL, "mz_selfplay_begin: user environments (MZ_ENV_USER) start with mz_selfplay_begin_user");
-            if (opponent != MZ_OPPONENT_SELF) return fail(h, MZ_EINVAL, "mz_selfplay_begin_vs: user environments play against themselves only");
             if (u->obs_channels < 1 || u->obs_h < 1 || u->obs_w < 1)
                 return fail(h, MZ_EINVAL, "mz_selfplay_begin_user: the observation's channels, height and width must be >= 1");
             name = "the user environment"; C = u->obs_channels; ph = u->obs_h; pw = u->obs_w; A_env = A;
@@ -1220,6 +1238,10 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
             h->launches += 1;
         }
         host_start_kernel<<<B, host_slot_threads(s), 0, h->stream>>>(s, sp->rows, nullptr, d->first_game_id);
+        for (int p = 0; sp->user && opponent != MZ_OPPONENT_SELF && p < kUserOpponentPasses; ++p) {
+            const int rc = user_pass(h, s, kUserOpponent);      // the opponent opens the games where it moves first
+            if (rc) { mz_selfplay_destroy(h); return rc; }
+        }
     } else {
         selfplay_reset_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(s, d->first_game_id);
     }
@@ -1231,6 +1253,10 @@ static int sp_begin(MzHandle* h, const MzSelfPlayDesc* d, int32_t opponent, int3
         MZ_CUDA(h, cudaMemcpy(&bad, s.counters + 7, 8, cudaMemcpyDeviceToHost));
         if (bad) {
             mz_selfplay_destroy(h);
+            if (opponent != MZ_OPPONENT_SELF)
+                return fail(h, MZ_EINVAL, "mz_selfplay_begin_user_vs: the user environment's reset and the opponent's "
+                                          "opening moves left " + std::to_string(bad) + " rows without a legal action or "
+                                          "with a to_play outside the players, or expert moves that are not legal");
             return fail(h, MZ_EINVAL, "mz_selfplay_begin_user: mz_env_reset left " + std::to_string(bad) +
                                       " slots without a legal action or with a to_play outside the players");
         }
@@ -1282,23 +1308,33 @@ static int sp_move_setup(MzHandle* h, double temperature, const MzSelfPlayInject
     return MZ_OK;
 }
 
-// One pass of a user environment's loop: act != 0 plays a move (the act kernel, then the user step on the slots that
-// played), act == 0 only packs the games parked by an earlier call; then observe packs the finished games and their
-// slots start the next game from the user reset's rows.
-static int user_pass(MzHandle* h, const SpDev& s, int act) {
+// One pass of a user environment's loop, then observe packs the finished games and their slots start the next game from
+// the user reset's rows.  The pass's moves: kUserMuZero plays MuZero's (the act kernel on the search just run, then the
+// user step on the slots that played), kUserOpponent the opponent's of the slots whose opponent move is due (its random
+// default, improved by the source's expert for MZ_OPPONENT_EXPERT, recorded as host_opponent_act_kernel records, then the
+// user step), kUserPack none: it only packs the games parked by an earlier call.
+static int user_pass(MzHandle* h, const SpDev& s, int pass) {
     MzSelfPlay* sp = h->sp;
-    const int B = s.B;
-    if (act) {
-        if (s.A <= 128) host_act_kernel<128><<<(B + kActThreads - 1) / kActThreads, kActThreads, 0, h->stream>>>(s);
-        else host_act_kernel<256><<<(B + kActThreads - 1) / kActThreads, kActThreads, 0, h->stream>>>(s);
+    const int B = s.B, grid = (B + kActThreads - 1) / kActThreads;
+    if (pass == kUserMuZero) {
+        if (s.A <= 128) host_act_kernel<128><<<grid, kActThreads, 0, h->stream>>>(s);
+        else host_act_kernel<256><<<grid, kActThreads, 0, h->stream>>>(s);
         MZ_CUDA(h, launch_user_env(sp->user_k.step, sp->user_args, h->stream));
+        h->launches += 2;
+    } else if (pass == kUserOpponent) {
+        const bool expert = s.opponent == MZ_OPPONENT_EXPERT;
+        host_opponent_turn_kernel<<<grid, kActThreads, 0, h->stream>>>(s, sp->d_defaults);
+        if (expert) MZ_CUDA(h, launch_user_env(sp->user_k.expert, sp->user_args, h->stream, sp->d_defaults, sp->d_opp_actions));
+        host_opponent_act_kernel<false><<<grid, kActThreads, 0, h->stream>>>(s, sp->d_defaults, expert ? sp->d_opp_actions : nullptr);
+        MZ_CUDA(h, launch_user_env(sp->user_k.step, sp->user_args, h->stream));
+        h->launches += expert ? 4 : 3;
     } else {
         MZ_CUDA(h, cudaMemsetAsync(s.host_action, 0xFF, (size_t)B * 4, h->stream));     // -1: no slot plays
     }
     host_observe_kernel<<<B, host_slot_threads(s), 0, h->stream>>>(s, sp->rows, sp->d_finished);
     MZ_CUDA(h, launch_user_env(sp->user_k.reset, sp->user_args, h->stream));            // which = d_finished
     host_start_kernel<<<B, host_slot_threads(s), 0, h->stream>>>(s, sp->rows, sp->d_finished, 0);
-    h->launches += act ? 5 : 3;
+    h->launches += 3;
     return MZ_OK;
 }
 
@@ -1331,7 +1367,7 @@ static int sp_enqueue(MzHandle* h, int32_t n_moves, double temperature, const Mz
     MZ_CUDA(h, cudaEventRecord(sp->e0, h->stream));
     if (sp->h_counters[4]) {                           // games parked by the previous call first, so their slots play again
         if (sp->user) {
-            rc = user_pass(h, s, 0);
+            rc = user_pass(h, s, kUserPack);
             if (rc) return rc;
         } else {
             launch_selfplay_step(s, 0, h->stream);
@@ -1343,7 +1379,9 @@ static int sp_enqueue(MzHandle* h, int32_t n_moves, double temperature, const Mz
         int rc = mz_dispatch_search(h, call, false, false, 0);
         if (rc) return rc;
         if (sp->user) {
-            rc = user_pass(h, s, 1);
+            rc = user_pass(h, s, kUserMuZero);
+            for (int p = 0; rc == MZ_OK && s.opponent != MZ_OPPONENT_SELF && p < kUserOpponentPasses; ++p)
+                rc = user_pass(h, s, kUserOpponent);
             if (rc) return rc;
         } else {
             launch_selfplay_step(s, 1, h->stream);
@@ -1370,6 +1408,11 @@ static int sp_wait(MzHandle* h, MzSelfPlayStats* stats) {
     if (cudaEventElapsedTime(&ms, sp->e0, sp->e1) == cudaSuccess && stats) stats->device_ms = ms;
     if (sp->user) {
         MZ_CUDA(h, cudaMemcpy(sp->h_counters + 7, sp->dev.counters + 7, 8, cudaMemcpyDeviceToHost));
+        if (sp->h_counters[7] && sp->dev.opponent == MZ_OPPONENT_EXPERT)
+            return fail(h, MZ_EINVAL, "the user environment wrote " + std::to_string(sp->h_counters[7]) +
+                                      " rows without a legal action or with a to_play outside the players (those games "
+                                      "were ended there), or its mz_env_expert returned moves out of range or not legal "
+                                      "(the random default was played instead); begin the loop again");
         if (sp->h_counters[7])
             return fail(h, MZ_EINVAL, "the user environment wrote " + std::to_string(sp->h_counters[7]) +
                                       " rows without a legal action or with a to_play outside the players (those games "
@@ -1386,17 +1429,28 @@ extern "C" int mz_selfplay_moves(MzHandle* h, int32_t n_moves, double temperatur
     return sp_wait(h, stats);
 }
 
-extern "C" int mz_selfplay_begin_user(MzHandle* h, const MzSelfPlayDesc* d, const MzUserEnvDesc* e) {
-    if (!h || !d || !e || !e->source) return fail(h, MZ_EINVAL, "mz_selfplay_begin_user: null argument");
-    if (d->env != MZ_ENV_USER) return fail(h, MZ_EINVAL, "mz_selfplay_begin_user: desc->env must be MZ_ENV_USER");
+static int begin_user(MzHandle* h, const MzSelfPlayDesc* d, const MzUserEnvDesc* e, int32_t opponent, int32_t muzero_player,
+                      const char* who) {
+    if (!h || !d || !e || !e->source) return fail(h, MZ_EINVAL, std::string(who) + ": null argument");
+    if (d->env != MZ_ENV_USER) return fail(h, MZ_EINVAL, std::string(who) + ": desc->env must be MZ_ENV_USER");
     if (e->state_bytes < 0 || e->state_bytes > MZ_USER_ENV_MAX_STATE_BYTES)
-        return fail(h, MZ_EINVAL, "mz_selfplay_begin_user: state_bytes must lie in [0, " +
+        return fail(h, MZ_EINVAL, std::string(who) + ": state_bytes must lie in [0, " +
                                   std::to_string(MZ_USER_ENV_MAX_STATE_BYTES) + "], got " + std::to_string(e->state_bytes));
     MZ_CUDA(h, cudaSetDevice(h->device));
     MzUserEnvKernels k;
     const int rc = mz_user_env_kernels(h, e->source, &k);
     if (rc) return rc;
-    return sp_begin(h, d, MZ_OPPONENT_SELF, 0, nullptr, nullptr, nullptr, nullptr, false, e, &k);
+    return sp_begin(h, d, opponent, muzero_player, nullptr, nullptr, nullptr, nullptr, false, e, &k);
+}
+
+extern "C" int mz_selfplay_begin_user(MzHandle* h, const MzSelfPlayDesc* d, const MzUserEnvDesc* e) {
+    return begin_user(h, d, e, MZ_OPPONENT_SELF, 0, "mz_selfplay_begin_user");
+}
+
+extern "C" int mz_selfplay_begin_user_vs(MzHandle* h, const MzSelfPlayDesc* d, const MzUserEnvDesc* e, int32_t opponent,
+                                         int32_t muzero_player) {
+    if (opponent == MZ_OPPONENT_SELF && muzero_player == 0) return mz_selfplay_begin_user(h, d, e);
+    return begin_user(h, d, e, opponent, muzero_player, "mz_selfplay_begin_user_vs");
 }
 
 extern "C" int mz_selfplay_user_moves(MzHandle* h, int32_t n_moves, double temperature, const MzSelfPlayInject* inj,

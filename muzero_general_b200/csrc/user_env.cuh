@@ -15,6 +15,10 @@
 // no legal action; a reset's row, and a step's row of a game still in play, must have one.  `state` is the slot's own
 // MzUserEnvDesc.state_bytes bytes (16-byte aligned, zero before the slot's first reset, not cleared between games).
 // One thread runs one slot; the slots of a batch run concurrently.
+// For test-mode games against the EXPERT opponent a source also defines the macro MZ_ENV_EXPERT and
+//   __device__ int mz_env_expert(const void* state, const MzEnvCtx& ctx, const MzEnvRow& row, int default_action);
+// (user_env_expert.cuh, compiled after the source): the opponent's move in the slot's position, from the published row
+// (not to be written), with ctx.move the move about to be played and default_action the library's random default.
 //
 // Random draws: philox_uniform53(ctx.seed, ctx.game_id, k, c2, tag) is the draw of the built-in environments (CartPole's
 // reset: k = 0, c2 = component, kTagReset; Twenty-One: k = draw index, c2 = 0, kTagCard; Gridworld: k = draw index,

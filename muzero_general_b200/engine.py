@@ -781,18 +781,29 @@ class UserEnvSelfPlayLoop(DeviceSelfPlayLoop):
     """Python face of mz_selfplay_begin_user / _user_moves: the device loop for a game whose environment is CUDA source
     (``source`` defines ``mz_env_reset`` and ``mz_env_step`` against csrc/user_env.cuh; ``state_bytes`` per slot).  The
     library compiles the source with NVRTC for sm_90a, once per handle and source.  ``moves``, ``enqueue`` / ``wait``,
-    ``drain`` and ``peek`` are the device loop's."""
+    ``drain`` and ``peek`` are the device loop's.
+
+    ``opponent`` "expert" or "random" plays test-mode games (mz_selfplay_begin_user_vs): every move is MuZero's pass,
+    then two passes of the opponent's moves, stepped by the same source; "expert" needs a source that defines
+    ``MZ_ENV_EXPERT`` and ``mz_env_expert`` (csrc/user_env_expert.cuh), else NotImplementedError."""
 
     def __init__(self, engine: SearchEngine, source: str, state_bytes: int, obs_shape, max_moves: int,
                  temperature_threshold=None, first_game_id: int = 0, staging_bytes: int = 0, game_id_stride: int = 0,
-                 td_steps: int = 0, per_alpha: float = 1.0, discount: float = 1.0, stacked_observations: int = 0):
+                 td_steps: int = 0, per_alpha: float = 1.0, discount: float = 1.0, stacked_observations: int = 0,
+                 opponent: str = "self", muzero_player: int = 0):
+        if opponent not in self.OPPONENTS:
+            raise NotImplementedError(f"no device opponent {opponent!r} (expected one of {sorted(self.OPPONENTS)})")
         self.engine = engine
-        self.opponent, self.muzero_player = "self", 0
+        self.opponent, self.muzero_player = opponent, int(muzero_player)
         d = self._desc(_lib.MZ_ENV_USER, max_moves, temperature_threshold, 0, first_game_id, staging_bytes, game_id_stride,
                        td_steps, per_alpha, discount, stacked_observations)
         self._source = source.encode()
         e = _lib.MzUserEnvDesc(self._source, int(state_bytes), *(int(x) for x in obs_shape))
-        rc = engine.lib.mz_selfplay_begin_user(engine._h, C.byref(d), C.byref(e))
+        if opponent == "self" and self.muzero_player == 0:
+            rc = engine.lib.mz_selfplay_begin_user(engine._h, C.byref(d), C.byref(e))
+        else:
+            rc = engine.lib.mz_selfplay_begin_user_vs(engine._h, C.byref(d), C.byref(e), self.OPPONENTS[opponent],
+                                                      self.muzero_player)
         if rc == _lib.MZ_EUNSUPPORTED:
             raise NotImplementedError(engine.lib.mz_last_error(engine._h).decode())
         engine._check(rc)
@@ -822,6 +833,18 @@ def debug_user_env_compile(source: str, log_bytes: int = 1 << 16):
     info = (C.c_int32 * 9)()
     rc = lib.mz_debug_user_env_compile(source.encode(), log, int(log_bytes), info)
     return rc, log.value.decode(), {"reset": tuple(info[0:4]), "step": tuple(info[4:8]), "nvrtc_version": int(info[8])}
+
+
+def debug_user_env_expert_compile(source: str, log_bytes: int = 1 << 16):
+    """``debug_user_env_compile`` with the expert wrapper (mz_debug_user_env_expert_compile): the info dict has
+    ``"expert"`` (True when the source defines MZ_ENV_EXPERT and the wrapper was compiled) and ``"expert_kernel"``, its
+    (registers, stack frame bytes, spill store bytes, spill load bytes), -1s without one."""
+    lib = _lib.load_library()
+    log = C.create_string_buffer(int(log_bytes))
+    info = (C.c_int32 * 14)()
+    rc = lib.mz_debug_user_env_expert_compile(source.encode(), log, int(log_bytes), info)
+    return rc, log.value.decode(), {"reset": tuple(info[0:4]), "step": tuple(info[4:8]), "nvrtc_version": int(info[8]),
+                                    "expert": bool(info[9]), "expert_kernel": tuple(info[10:14])}
 
 
 def parse_staged_game(buf: bytes, off: int):

@@ -678,7 +678,10 @@ class SelfPlay:
         ``play_game(temperature, config.temperature_threshold, False, opponent, muzero_player)`` with the opponent
         ("expert", "random" or "self") moving on the GPU - or, for a game whose environment the host steps
         (``loop_path == "device-host-env"``), the opponent's moves stepped on the host like MuZero's, the "expert" from
-        the vector game's ``expert_actions`` or the plug-in's ``expert_agent``.  ``opponent`` and ``muzero_player``
+        the vector game's ``expert_actions`` or the plug-in's ``expert_agent``.  A plug-in whose environment is CUDA
+        source (``loop_path == "device-user-env"``) plays them on the device with that source stepping both sides, the
+        "expert" being the source's ``mz_env_expert``; against the "expert" a source without one takes the routes
+        above (the host-stepped loop with ``config.host_env_device_loop``).  ``opponent`` and ``muzero_player``
         default to the config's, like the test worker ("self" for one-player games).  Returns ``(PackedGames, summary)``: the games have the
         reference's test-mode shape (``root_values`` is None at opponent moves, ``child_visits`` has rows for MuZero's
         moves only), and ``summary`` holds the means over the games of what the test worker reports
@@ -691,9 +694,15 @@ class SelfPlay:
         calls give the same games.  The device loop replaces the handle's self-play loop: with one running, call
         ``reset_stream()`` first."""
         cfg = self.config
-        # the routes test games have without a user environment (none plays against opponents on one)
+        if opponent is None:
+            opponent = "self" if len(cfg.players) == 1 else cfg.opponent
+        if muzero_player is None:
+            muzero_player = cfg.muzero_player
         path = "device" if self._device_env_name() else ("device-host-env" if self._host_env_device_loop() else "host")
-        if path == "host":
+        # a user environment plays every opponent the device loop has; whether its source has an expert, only the
+        # library knows (mz_selfplay_begin_user_vs answers MZ_EUNSUPPORTED)
+        user = self.loop_path == "device-user-env" and opponent in DeviceSelfPlayLoop.OPPONENTS
+        if path == "host" and not user:
             raise NotImplementedError(
                 "test games on the device need rng_mode='philox' and a device environment (CartPole, TicTacToe, "
                 "Connect4, Gomoku, Twenty-One, Simple Grid or Gridworld with device_envs on) or "
@@ -705,15 +714,19 @@ class SelfPlay:
         n_games = int(n_games)
         if n_games < 1:
             raise ValueError("n_games must be >= 1")
-        if opponent is None:
-            opponent = "self" if len(cfg.players) == 1 else cfg.opponent
-        if muzero_player is None:
-            muzero_player = cfg.muzero_player
         B, stride, first = self.num_parallel_games, self.game_id_stride, self._next_test_game_id
         i = numpy.arange(n_games)
         wanted = first + (i // B) * stride + i % B
-        Loop = DeviceBatchedSelfPlay if path == "device" else DeviceHostEnvSelfPlay
-        dev = Loop(self, cfg.temperature_threshold, opponent, muzero_player, first_game_id=first)
+        dev = None
+        if user:
+            try:
+                dev = DeviceBatchedSelfPlay(self, cfg.temperature_threshold, opponent, muzero_player, first_game_id=first)
+            except NotImplementedError:
+                if opponent != "expert" or path == "host":
+                    raise
+        if dev is None:
+            Loop = DeviceBatchedSelfPlay if path == "device" else DeviceHostEnvSelfPlay
+            dev = Loop(self, cfg.temperature_threshold, opponent, muzero_player, first_game_id=first)
         games = PackedGames(dev.obs_shape, dev.obs_dtype, dev.reward_type)
         missing = n_games
         while missing:
@@ -820,7 +833,8 @@ class DeviceBatchedSelfPlay:
                   stacked_observations=int(cfg.stacked_observations))
         if worker.loop_path == "device-user-env":
             self.loop = UserEnvSelfPlayLoop(worker.model.engine, Game.DEVICE_SOURCE, int(Game.DEVICE_STATE_BYTES),
-                                            self.obs_shape, cfg.max_moves, **kw)
+                                            self.obs_shape, cfg.max_moves, opponent=opponent,
+                                            muzero_player=muzero_player, **kw)
         else:
             self.loop = DeviceSelfPlayLoop(worker.model.engine, Game.DEVICE_ENV, cfg.max_moves,
                                            reward_scale=getattr(vec, "REWARD_SCALE", 1), opponent=opponent,
