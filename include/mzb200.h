@@ -97,7 +97,8 @@ typedef struct MzTrace {
     int32_t max_depth;            /* D: entries kept per path */
     int32_t reserved;
     int32_t* depth;               /* [n, N]      number of select_child calls of simulation i */
-    uint8_t* actions;             /* [n, N, D]   actions chosen root->leaf */
+    uint8_t* actions;             /* [n, N, D]   actions chosen root->leaf; 0 past the path's depth (host buffers; a
+                                                  device buffer keeps what it held there) */
     float* value;                 /* [n, N]      scalarised value of the expanded leaf */
     float* reward;                /* [n, N]      scalarised reward of the expanded leaf */
     float* priors;                /* [n, N, A]   fp32 softmax priors of the expanded leaf */
@@ -351,10 +352,11 @@ int mz_debug_fc_search_plan(int32_t N, int32_t A, int32_t E, int32_t maxw, int32
                             int32_t regs, int32_t threads, int64_t* plan);
 
 /* Debug / tests (host only, no device needed): launch plan of the CUDA-core conv3x3 kernel (csrc/resnet.cu) for n boards of
- * cin x H x W -> cout channels at stride 1 or 2.  Returns 1 and fills plan[11] = {P (pixels per thread), stride,
+ * cin x H x W -> cout channels at stride 1 or 2.  Returns 1 and fills plan[12] = {P (pixels per thread), stride,
  * MAX_ITEMS (accumulator tiles per thread), row bands, rows per band, boards per CTA, cin chunk, grid x, grid y (cout
- * tiles of <= 64 channels), grid z, shared-memory bytes}, or 0 with the reason in mz_last_error(NULL) when the shape
- * cannot be launched.  mz_create refuses a net with such a conv. */
+ * tiles), grid z, shared-memory bytes, cout tile (64, or fewer channels when one output row of 64 exceeds a CTA's
+ * items)}, or 0 with the reason in mz_last_error(NULL) when the shape cannot be launched.  mz_create refuses a net with
+ * such a conv. */
 int mz_debug_conv3x3_plan(int32_t n, int32_t cin, int32_t cout, int32_t H, int32_t W, int32_t stride, int64_t* plan);
 
 /* Debug / parity: one conv3x3 (cin -> cout, stride 1 or 2, pad 1; models.py:206-209) with optional bias, residual and
@@ -556,6 +558,18 @@ int mz_debug_cnn_stem_plan(int32_t n, int32_t in, int32_t C, int32_t H, int32_t 
  * plan refuses. */
 int mz_debug_cnn_stem(int device, int32_t n, int32_t in, int32_t C, int32_t H, int32_t W, const float* x, const float* w1,
                       const float* b1, const float* w2, const float* b2, float* out, int64_t* plan);
+
+/* Debug / parity: the DownSample stem (downsample = 1, models.py:233-275) alone on host NCHW fp32 data, through the
+ * network's weight packer and launcher: x [n][in][H][W]; w the 18 convs' [cout][cin][3][3] weights one after another
+ * in execution order (conv1 in -> C/2 at stride 2; resblocks1.0.conv1, .conv2, resblocks1.1.conv1, .conv2 at C/2;
+ * conv2 C/2 -> C at stride 2; resblocks2.0 to .2 and resblocks3.0 to .2, conv1 then conv2 each, at C), BatchNorm
+ * folded in; bias their [cout] biases in the same order, conv1's and conv2's zero (the reference's convs have none).
+ * out [n][C][ceil(H / 16)][ceil(W / 16)].  stages (or NULL) gets, one after another, the outputs of conv1 and of
+ * resblocks1 ([n][C/2][H1][W1] each, H1 = ceil(H / 2)), of conv2 and of resblocks2 ([n][C][H2][W2], H2 = ceil(H1 / 2)),
+ * of the first pool and of resblocks3 ([n][C][H3][W3], H3 = ceil(H2 / 2)).  Every device buffer but the input starts
+ * as NaN.  C must be a positive multiple of 8; MZ_EUNSUPPORTED when a conv's launch plan is refused. */
+int mz_debug_downsample(int device, int32_t n, int32_t in, int32_t C, int32_t H, int32_t W, const float* x, const float* w,
+                        const float* bias, float* out, float* stages);
 
 /* Arithmetic the handle's search path computes in, e.g. "f32 nets + f64 tree statistics" (bench.py's dtype). */
 const char* mz_numerics(const MzHandle* h);

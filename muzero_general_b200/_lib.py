@@ -235,6 +235,7 @@ SYMBOLS = [
      + [C.c_void_p] * 3 + [C.c_int32, C.c_int32] + [C.c_void_p] * 9 + [C.POINTER(C.c_int64)]),
     ("mz_debug_cnn_stem_plan", C.c_int, [C.c_int32] * 6 + [C.POINTER(C.c_int64)]),
     ("mz_debug_cnn_stem", C.c_int, [C.c_int] + [C.c_int32] * 5 + [C.c_void_p] * 6 + [C.POINTER(C.c_int64)]),
+    ("mz_debug_downsample", C.c_int, [C.c_int] + [C.c_int32] * 5 + [C.c_void_p] * 5),
 ]
 
 _lib = None

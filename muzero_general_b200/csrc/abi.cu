@@ -626,6 +626,9 @@ static int use_device(MzHandle* h) {
 static int enqueue_search(MzHandle* h, const SearchCall& call, bool teacher, bool trace, int flags, size_t out_bytes,
                           const std::vector<DebugOut>& dbg_outs) {
     int rc;
+    // each debug output is copied back whole, and the search leaves some entries unwritten (trace actions past a leaf's
+    // depth): those read 0, not whatever the device buffer held before (an earlier search, another allocation)
+    for (const DebugOut& d : dbg_outs) MZ_CUDA(h, cudaMemsetAsync(d.dev, 0, d.bytes, h->stream));
     MZ_CUDA(h, cudaEventRecord(h->ev0, h->stream));
     if ((rc = mz_dispatch_search(h, call, teacher, trace, flags))) return rc;
     h->host_ns[1] = mz_host_ns();
@@ -1172,6 +1175,19 @@ extern "C" int mz_debug_cnn_stem(int device, int32_t n, int32_t in, int32_t C, i
     std::string e;
     int rc = cnn_stem_debug(n, in, C, H, W, x, w1, b1, w2, b2, out, plan, prop.multiProcessorCount, &e);
     if (rc) return fail(nullptr, rc, "mz_debug_cnn_stem: " + e);
+    return MZ_OK;
+}
+
+// debug: the DownSample stem alone (host NCHW in / out)
+extern "C" int mz_debug_downsample(int device, int32_t n, int32_t in, int32_t C, int32_t H, int32_t W, const float* x,
+                                   const float* w, const float* bias, float* out, float* stages) {
+    if (!x || !w || !bias || !out) return fail(nullptr, MZ_EINVAL, "mz_debug_downsample: bad argument");
+    if (cudaSetDevice(device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_downsample: no such device");
+    cudaDeviceProp prop;
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MZ_ECUDA, "mz_debug_downsample: device query failed");
+    std::string e;
+    int rc = resnet_debug_downsample(n, in, C, H, W, x, w, bias, out, stages, prop.multiProcessorCount, &e);
+    if (rc) return fail(nullptr, rc, "mz_debug_downsample: " + e);
     return MZ_OK;
 }
 

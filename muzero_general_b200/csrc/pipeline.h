@@ -98,6 +98,8 @@ int resnet_load_weights(ResNetDevice* r, const MzTensor* tensors, int n, std::st
 int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, int64_t* launches, std::string* err);
 int resnet_debug_conv(int n, int cin, int cout, int H, int W, int stride, const float* x, const float* w_oihw, const float* bias,
                       const float* residual, int relu, int use_tc, float* out, int sm_count, std::string* err);
+int resnet_debug_downsample(int n, int in, int C, int H, int W, const float* x, const float* w, const float* bias, float* out,
+                            float* stages, int sm_count, std::string* err);
 bool resnet_conv_plan(int n, int cin, int cout, int H, int W, int stride, int64_t* plan, std::string* err);   // host only
 const char* resnet_numerics(const ResNetDevice* r);                  // arithmetic of the residual towers (bench.py dtype)
 int resnet_take_saturations(ResNetDevice* r, cudaStream_t stream);   // x3 range guard (synchronises)

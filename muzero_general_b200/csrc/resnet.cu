@@ -18,6 +18,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <map>
 #include <string>
 #include <vector>
@@ -59,6 +60,7 @@ struct ConvArgs {
     int pool_stride;
     int n, Cin, Cout, Hin, Win, Ho, Wo, stride, relu, A;
     int boards_per_cta, cin_chunk;
+    int cout_tile;            // output channels per CTA (blockIdx.y picks the tile): 64, or fewer when one row of 64 is too many items
     int band_rows;            // output rows per CTA (blockIdx.z picks the band); = Ho unless the image is too large for one CTA
     int out_p64c4;            // kLayoutF16 / kLayoutSplit: write the tensor-core board layout (P64S) instead of NCHW
 };
@@ -73,9 +75,9 @@ __global__ void __launch_bounds__(256) conv3x3_kernel(const __grid_constant__ Co
     const int y_in0 = r0 * STRIDE - 1;
     const int Hp = (a.band_rows - 1) * STRIDE + 3, Wp = a.Win + 2;   // staged (padded) plane of the band
     const int plane = Hp * Wp;
-    // cout tiles of at most 64 channels; the last one holds the remaining Cout - cout0 (a multiple of 4)
-    const int cout0 = blockIdx.y * 64;
-    const int ct = min(a.Cout - cout0, 64);                     // cout tile of this CTA
+    // cout tiles of cout_tile (<= 64) channels; the last one holds the remaining Cout - cout0 (a multiple of 4)
+    const int cout0 = blockIdx.y * a.cout_tile;
+    const int ct = min(a.Cout - cout0, a.cout_tile);            // cout tile of this CTA
     const int cgs = ct / 4;
     const int segs = a.Wo / P;
     const int items_per_board = cgs * nbr * segs;
@@ -412,7 +414,8 @@ struct ConvPlan {
     int P, stride, max_items;      // template arguments: pixels per thread, stride, accumulator tiles per thread (1 or 4)
     int bands, band_rows;          // output rows split into bands of band_rows rows (the last one may be shorter)
     int boards, cin_chunk;         // boards per CTA (the last CTA may hold fewer), input channels staged at a time
-    dim3 grid;                     // (board groups, cout tiles of <= 64 channels, bands)
+    int cout_tile;                 // output channels per CTA (the last tile may hold fewer): 64 unless a row of 64 does not fit
+    dim3 grid;                     // (board groups, cout tiles, bands)
     size_t smem;                   // dynamic shared memory bytes
 };
 constexpr int kConvThreads = 256;
@@ -426,8 +429,13 @@ static bool conv3x3_plan(int n, int cin, int cout, int Hin, int Win, int stride,
     p->stride = stride;
     p->P = 1;
     for (int cand : {8, 7, 6, 4, 3, 2}) if (Wo % cand == 0) { p->P = cand; break; }
-    const int ct = cout < 64 ? cout : 64;          // the widest cout tile sizes the items and the weight slice
     const int threads = kConvThreads;
+    int ct = cout < 64 ? cout : 64;                // the widest cout tile sizes the items and the weight slice
+    // One output row of a 64-channel tile may exceed the item budget on its own (P = 1 on a board more than 64 wide, e.g.
+    // DownSample's first convs at 128 channels on a 129-wide frame): halve the tile until a row fits.  Every shape whose
+    // row fits keeps the 64-channel tile and the plan it always had.
+    while (ct > 4 && (ct / 4) * (Wo / p->P) > threads * 4) ct = (ct / 2 + 3) / 4 * 4;
+    p->cout_tile = ct;
     // large images (e.g. 128 output channels at 48 x 48, games/atari.py): split the output rows into bands, one CTA each
     int bands = 1;
     while (bands < Ho && (ct / 4) * ((Ho + bands - 1) / bands) * (Wo / p->P) > threads * 4) ++bands;
@@ -448,7 +456,29 @@ static bool conv3x3_plan(int n, int cin, int cout, int Hin, int Win, int stride,
     p->boards = boards; p->cin_chunk = chunk;
     p->max_items = items_per_board * boards > threads ? 4 : 1;
     p->smem = ((size_t)chunk * 9 * ct + (size_t)boards * chunk * plane) * 4;
-    p->grid = dim3((n + boards - 1) / boards, (cout + 63) / 64, p->bands);
+    p->grid = dim3((n + boards - 1) / boards, (cout + ct - 1) / ct, p->bands);
+    return true;
+}
+
+// The distinct conv shapes of a net's stage, named for the refusal message
+struct ConvShape { const char* stage; int cin, cout, H, W, stride; };
+static std::vector<ConvShape> downsample_shapes(int obs_c, int C, int H, int W) {
+    const int h1 = conv_out(H, 2), w1 = conv_out(W, 2), h2 = conv_out(h1, 2), w2 = conv_out(w1, 2);
+    return {{"DownSample conv1", obs_c, C / 2, H, W, 2}, {"DownSample resblocks1", C / 2, C / 2, h1, w1, 1},
+            {"DownSample conv2", C / 2, C, h1, w1, 2}, {"DownSample resblocks2", C, C, h2, w2, 1},
+            {"DownSample resblocks3", C, C, conv_out(h2, 2), conv_out(w2, 2), 1}};
+}
+// false with the first refused shape's reason and stage in *err
+static bool plan_shapes(int n, const std::vector<ConvShape>& shapes, std::string* err) {
+    for (const ConvShape& s : shapes) {
+        ConvPlan p;
+        std::string why;
+        if (!conv3x3_plan(n, s.cin, s.cout, s.H, s.W, s.stride, &p, &why)) {
+            *err = why + " (" + s.stage + ": " + std::to_string(s.cin) + " -> " + std::to_string(s.cout) + " channels, stride " +
+                   std::to_string(s.stride) + ", " + std::to_string(s.H) + " x " + std::to_string(s.W) + " input)";
+            return false;
+        }
+    }
     return true;
 }
 
@@ -598,29 +628,18 @@ ResNetDevice* resnet_create(const MzNetDesc& net, int max_batch, int sm_count, s
     // every other tower), so a shape the planner refuses fails here, not part-way through a search.  A plan that exists
     // for max_batch boards exists for any smaller batch (fewer boards per CTA only shrink the tile).
     {
-        struct Shape { int cin, cout, H, W, stride; };
         const int C = net.channels, h = r->hh, w = r->hw;
-        std::vector<Shape> shapes;
+        std::vector<ConvShape> shapes;
         if (net.downsample == 1) {
-            const int h1 = conv_out(H, 2), w1 = conv_out(W, 2), h2 = conv_out(h1, 2), w2 = conv_out(w1, 2);
-            shapes = {{net.obs_c, C / 2, H, W, 2}, {C / 2, C / 2, h1, w1, 1}, {C / 2, C, h1, w1, 2}, {C, C, h2, w2, 1},
-                      {C, C, conv_out(h2, 2), conv_out(w2, 2), 1}};
+            shapes = downsample_shapes(net.obs_c, C, H, W);
         } else if (net.downsample == 2) {
             // the stem was planned above; the representation trunk is blocks only
         } else {
-            shapes = {{net.obs_c, C, H, W, 1}};
+            shapes = {{"representation stem", net.obs_c, C, H, W, 1}};
         }
-        shapes.push_back({C + 1, C, h, w, 1});                     // dynamics stem (action plane)
-        if (net.blocks > 0) shapes.push_back({C, C, h, w, 1});
-        for (const Shape& s : shapes) {
-            ConvPlan p;
-            std::string why;
-            if (!conv3x3_plan(max_batch, s.cin, s.cout, s.H, s.W, s.stride, &p, &why)) {
-                *err = why + " (" + std::to_string(s.cin) + " -> " + std::to_string(s.cout) + " channels, stride " +
-                       std::to_string(s.stride) + ", " + std::to_string(s.H) + " x " + std::to_string(s.W) + " input)";
-                delete r; return nullptr;
-            }
-        }
+        shapes.push_back({"dynamics stem", C + 1, C, h, w, 1});                     // (action plane)
+        if (net.blocks > 0) shapes.push_back({"residual blocks", C, C, h, w, 1});
+        if (!plan_shapes(max_batch, shapes, err)) { delete r; return nullptr; }
     }
     // the route is known here, so the hidden-state pool and the workspaces are sized for it
     r->route = choose_route(net, r->hh, r->hw, max_batch, sm_count, &r->note);
@@ -845,6 +864,28 @@ bool pack_resblock(Loader& L, const std::string& p, int ch, std::vector<float>& 
            pack_conv(L, p + ".conv2", p + ".bn2", ch, ch, 1, blob, layers, tc);
 }
 
+// DownSample's 18 convs under the prefix dp, in the order Runner::downsample runs them: conv1, resblocks1 x2, conv2,
+// resblocks2 x3, resblocks3 x3.  Without `bn` (mz_debug_downsample) a block's conv takes the bias "<conv>.bias" instead
+// of a BatchNorm.
+bool pack_downsample(Loader& L, const std::string& dp, int obs_c, int C, bool bn, std::vector<float>& blob,
+                     std::vector<ConvLayer>& layers) {
+    auto conv = [&](const std::string& c, const std::string& norm, int ch) {
+        if (bn) return pack_conv(L, c, norm, ch, ch, 1, blob, layers);
+        const MzTensor* b = L.get(c + ".bias", ch);
+        if (!b || !pack_conv(L, c, "", ch, ch, 1, blob, layers)) return false;
+        layers.back().b_off = (long)blob.size();
+        blob.insert(blob.end(), b->data, b->data + ch);                  // (ch % 4 == 0: stays aligned)
+        return true;
+    };
+    auto block = [&](const std::string& p, int ch) { return conv(p + ".conv1", p + ".bn1", ch) && conv(p + ".conv2", p + ".bn2", ch); };
+    bool ok = pack_conv(L, dp + ".conv1", "", obs_c, C / 2, 2, blob, layers);
+    for (int i = 0; ok && i < 2; ++i) ok = block(dp + ".resblocks1." + std::to_string(i), C / 2);
+    ok = ok && pack_conv(L, dp + ".conv2", "", C / 2, C, 2, blob, layers);
+    for (int i = 0; ok && i < 3; ++i) ok = block(dp + ".resblocks2." + std::to_string(i), C);
+    for (int i = 0; ok && i < 3; ++i) ok = block(dp + ".resblocks3." + std::to_string(i), C);
+    return ok;
+}
+
 bool pack_head(Loader& L, const std::string& conv, const std::string& fc, int C, int rc, int HW, const int32_t* hidden,
                int n_hidden, int n_out, std::vector<float>& blob, HeadDesc& d) {
     const MzTensor* w = L.get(conv + ".weight", (int64_t)rc * C);
@@ -888,12 +929,7 @@ int resnet_load_weights(ResNetDevice* r, const MzTensor* tensors, int n, std::st
         ok = w1 && b1 && w2 && b2;
         if (ok) r->cnn = cnn_stem_pack(w1->data, b1->data, w2->data, b2->data, nd.obs_c, mid, C, k, conv);
     } else if (nd.downsample) {
-        const std::string dp = rp + ".downsample_net";
-        ok = ok && pack_conv(L, dp + ".conv1", "", nd.obs_c, C / 2, 2, conv, r->rep_down);
-        for (int i = 0; ok && i < 2; ++i) ok = pack_resblock(L, dp + ".resblocks1." + std::to_string(i), C / 2, conv, r->rep_down);
-        ok = ok && pack_conv(L, dp + ".conv2", "", C / 2, C, 2, conv, r->rep_down);
-        for (int i = 0; ok && i < 3; ++i) ok = pack_resblock(L, dp + ".resblocks2." + std::to_string(i), C, conv, r->rep_down);
-        for (int i = 0; ok && i < 3; ++i) ok = pack_resblock(L, dp + ".resblocks3." + std::to_string(i), C, conv, r->rep_down);
+        ok = pack_downsample(L, rp + ".downsample_net", nd.obs_c, C, true, conv, r->rep_down);
     } else {
         ok = ok && pack_conv(L, rp + ".conv", rp + ".bn", nd.obs_c, C, 1, conv, r->rep_trunk);
     }
@@ -1105,7 +1141,7 @@ struct Runner {
         ConvPlan plan;
         if (!conv3x3_plan(n, l.cin, l.cout, Hin, Win, l.stride, &plan, err)) return false;
         const int P = plan.P, threads = kConvThreads;
-        a.band_rows = plan.band_rows; a.boards_per_cta = plan.boards; a.cin_chunk = plan.cin_chunk;
+        a.band_rows = plan.band_rows; a.boards_per_cta = plan.boards; a.cin_chunk = plan.cin_chunk; a.cout_tile = plan.cout_tile;
         const size_t smem = plan.smem;
         const dim3 grid = plan.grid;
         const bool multi = plan.max_items == 4;
@@ -1264,6 +1300,41 @@ struct Runner {
             if (!conv(layers[first + 2 * b], *cur, *tmp, nullptr, true, H, W)) return false;
             if (!conv(layers[first + 2 * b + 1], *tmp, *spare, *cur, true, H, W)) return false;
             float* t = *cur; *cur = *spare; *spare = t;
+        }
+        return true;
+    }
+
+    // DownSample (models.py:233-275) of the observations `in`, r->rep_down's 24 convs and two pools: conv1 at stride 2
+    // (no ReLU), resblocks1 x2 at C/2 channels, conv2 at stride 2, resblocks2 x3, pool, resblocks3 x3, pool.  The
+    // workspaces rotate; the result is left in *cur.  With ds_stages set (mz_debug_downsample), the outputs of conv1,
+    // resblocks1, conv2, resblocks2, the first pool and resblocks3 are copied there.
+    float* const* ds_stages = nullptr;
+    bool downsample(const float* in, float** cur, float** tmp, float** spare) {
+        const std::vector<ConvLayer>& d = r->rep_down;
+        const int C = r->C;
+        int H = r->net.obs_h, W = r->net.obs_w, stage = 0;
+        auto keep = [&](int channels) {
+            if (!ds_stages) return true;
+            cudaError_t e = cudaMemcpyAsync(ds_stages[stage++], *cur, (size_t)n * channels * H * W * 4, cudaMemcpyDeviceToDevice, stream);
+            return e == cudaSuccess || fail("downsample stage copy", e);
+        };
+        if (!conv(d[0], in, *cur, nullptr, false, H, W)) return false;
+        H = conv_out(H, 2); W = conv_out(W, 2);
+        if (!keep(C / 2) || !blocks(d, 1, 2, cur, tmp, spare, H, W) || !keep(C / 2)) return false;
+        if (!conv(d[5], *cur, *tmp, nullptr, false, H, W)) return false;
+        std::swap(*cur, *tmp);
+        H = conv_out(H, 2); W = conv_out(W, 2);
+        if (!keep(C) || !blocks(d, 6, 3, cur, tmp, spare, H, W) || !keep(C)) return false;
+        for (int pool = 0; pool < 2; ++pool) {
+            const int Ho = conv_out(H, 2), Wo = conv_out(W, 2);
+            const size_t total = (size_t)n * C * Ho * Wo;
+            avgpool3x3s2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(*cur, *tmp, n * C, H, W, Ho, Wo);
+            cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess) return fail("avgpool3x3s2 launch", e);
+            *launches += 1;
+            std::swap(*cur, *tmp);
+            H = Ho; W = Wo;
+            if (pool == 0 && (!keep(C) || !blocks(d, 12, 3, cur, tmp, spare, H, W) || !keep(C))) return false;
         }
         return true;
     }
@@ -1520,14 +1591,14 @@ void resnet_use_strict(ResNetDevice* r) {
     r->route = TowerRoute::CudaCore;                 // dense NCHW states: smaller than the board layout, the pool fits
 }
 
-// Launch plan of conv3x3_kernel for a shape (host only, behind mz_debug_conv3x3_plan): plan[11] = {P, stride, MAX_ITEMS,
-// bands, band_rows, boards per CTA, cin chunk, grid x, grid y, grid z, shared-memory bytes}.
+// Launch plan of conv3x3_kernel for a shape (host only, behind mz_debug_conv3x3_plan): plan[12] = {P, stride, MAX_ITEMS,
+// bands, band_rows, boards per CTA, cin chunk, grid x, grid y, grid z, shared-memory bytes, cout tile}.
 bool resnet_conv_plan(int n, int cin, int cout, int H, int W, int stride, int64_t* plan, std::string* err) {
     ConvPlan p;
     if (!conv3x3_plan(n, cin, cout, H, W, stride, &p, err)) return false;
-    const int64_t out[11] = {p.P, p.stride, p.max_items, p.bands, p.band_rows, p.boards, p.cin_chunk,
-                             p.grid.x, p.grid.y, p.grid.z, (int64_t)p.smem};
-    for (int i = 0; i < 11; ++i) plan[i] = out[i];
+    const int64_t out[12] = {p.P, p.stride, p.max_items, p.bands, p.band_rows, p.boards, p.cin_chunk,
+                             p.grid.x, p.grid.y, p.grid.z, (int64_t)p.smem, p.cout_tile};
+    for (int i = 0; i < 12; ++i) plan[i] = out[i];
     return true;
 }
 
@@ -1626,6 +1697,82 @@ int resnet_debug_conv(int n, int cin, int cout, int H, int W, int stride, const 
         cudaEventDestroy(e0); cudaEventDestroy(e1);
     }
     if (good) cudaMemcpy(out, d_out, dense * 4, cudaMemcpyDeviceToHost);
+    r.d_conv = nullptr;
+    cleanup();
+    return good ? MZ_OK : MZ_ECUDA;
+}
+
+// Stand-alone DownSample stem on host NCHW data, behind mz_debug_downsample: the network's packer (pack_downsample) and
+// Runner::downsample.  w holds the 18 convs' [cout][cin][3][3] weights in execution order (conv1; resblocks1.0.conv1,
+// .conv2, resblocks1.1.conv1, .conv2; conv2; resblocks2.0 ... 2; resblocks3.0 ... 2), bias their [cout] biases in the
+// same order; conv1's and conv2's must be zero (the reference's have none).  Every device buffer but the input starts
+// as NaN bytes (0xFF), so a stage that reads a plane nobody wrote produces NaN.
+int resnet_debug_downsample(int n, int in, int C, int H, int W, const float* x, const float* w, const float* bias, float* out,
+                            float* stages, int sm_count, std::string* err) {
+    if (n < 1 || in < 1 || H < 1 || W < 1 || C < 8 || C % 8) { *err = "bad shape (C a positive multiple of 8)"; return MZ_EINVAL; }
+    if (!plan_shapes(n, downsample_shapes(in, C, H, W), err)) return MZ_EUNSUPPORTED;
+    // the state_dict of the stem under the prefix "d", one bias per conv
+    std::vector<std::string> names;
+    std::vector<int> cins, couts;
+    auto add = [&](const std::string& s, int ci, int co) { names.push_back(s); cins.push_back(ci); couts.push_back(co); };
+    add("d.conv1", in, C / 2);
+    for (int i = 0; i < 2; ++i)
+        for (int k = 1; k <= 2; ++k) add("d.resblocks1." + std::to_string(i) + ".conv" + std::to_string(k), C / 2, C / 2);
+    add("d.conv2", C / 2, C);
+    for (const std::string s : {"d.resblocks2.", "d.resblocks3."})
+        for (int i = 0; i < 3; ++i)
+            for (int k = 1; k <= 2; ++k) add(s + std::to_string(i) + ".conv" + std::to_string(k), C, C);
+    const size_t n_convs = names.size();
+    std::vector<std::string> keys;
+    keys.reserve(2 * n_convs);                          // (c_str() of each key must stay put)
+    std::vector<MzTensor> tensors;
+    size_t w_off = 0, b_off = 0;
+    for (size_t i = 0; i < n_convs; ++i) {
+        if ((i == 0 || i == 5) && std::any_of(bias + b_off, bias + b_off + couts[i], [](float b) { return b != 0.0f; })) {
+            *err = "conv1 and conv2 have no bias"; return MZ_EINVAL;
+        }
+        keys.push_back(names[i] + ".weight");
+        tensors.push_back(MzTensor{keys.back().c_str(), w + w_off, (int64_t)couts[i] * cins[i] * 9});
+        keys.push_back(names[i] + ".bias");
+        tensors.push_back(MzTensor{keys.back().c_str(), bias + b_off, (int64_t)couts[i]});
+        w_off += (size_t)couts[i] * cins[i] * 9;
+        b_off += couts[i];
+    }
+    ResNetDevice r{};
+    r.net.kind = MZ_NET_RESNET; r.net.channels = C; r.net.obs_c = in; r.net.obs_h = H; r.net.obs_w = W;
+    r.net.action_space = 1; r.net.downsample = 1;
+    r.max_batch = n; r.sm_count = sm_count; r.C = C; r.hh = (H + 15) / 16; r.hw = (W + 15) / 16;
+    std::vector<float> blob;
+    Loader L{tensors.data(), (int)tensors.size(), err};
+    if (!pack_downsample(L, "d", in, C, false, blob, r.rep_down) || !L.ok) return MZ_EINVAL;
+
+    const int h1 = conv_out(H, 2), w1 = conv_out(W, 2), h2 = conv_out(h1, 2), w2 = conv_out(w1, 2);
+    const size_t half = (size_t)n * (C / 2) * h1 * w1, full = (size_t)n * C * h2 * w2;
+    const size_t pooled = (size_t)n * C * conv_out(h2, 2) * conv_out(w2, 2), dense = (size_t)n * C * r.hh * r.hw;
+    const size_t stage_elems[6] = {half, half, full, full, pooled, pooled};
+    float *d_blob = nullptr, *d_x = nullptr, *d_stage[6] = {};
+    auto cleanup = [&]() {
+        for (float* p : {d_blob, d_x, r.ws[0], r.ws[1], r.ws[2]}) if (p) cudaFree(p);
+        for (float* p : d_stage) if (p) cudaFree(p);
+    };
+    auto alloc = [](float** p, size_t floats) { return cudaMalloc(p, floats * 4 + 64) == cudaSuccess && cudaMemset(*p, 0xFF, floats * 4 + 64) == cudaSuccess; };
+    bool ok = alloc(&d_blob, blob.size()) && alloc(&d_x, (size_t)n * in * H * W);
+    for (int i = 0; ok && i < 3; ++i) ok = alloc(&r.ws[i], std::max(half, full));
+    for (int i = 0; ok && stages && i < 6; ++i) ok = alloc(&d_stage[i], stage_elems[i]);
+    if (!ok) { cleanup(); *err = "allocation failed"; return MZ_ENOMEM; }
+    cudaMemcpy(d_blob, blob.data(), blob.size() * 4, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_x, x, (size_t)n * in * H * W * 4, cudaMemcpyHostToDevice);
+    r.d_conv = d_blob;
+    int64_t launches = 0;
+    Runner R{&r, nullptr, &launches, err, n};
+    if (stages) R.ds_stages = d_stage;
+    float *cur = r.ws[0], *tmp = r.ws[1], *spare = r.ws[2];
+    bool good = R.downsample(d_x, &cur, &tmp, &spare);
+    cudaError_t e = cudaDeviceSynchronize();
+    if (good && e == cudaSuccess) e = cudaMemcpy(out, cur, dense * 4, cudaMemcpyDeviceToHost);
+    for (int i = 0; good && stages && i < 6 && e == cudaSuccess; stages += stage_elems[i], ++i)
+        e = cudaMemcpy(stages, d_stage[i], stage_elems[i] * 4, cudaMemcpyDeviceToHost);
+    if (good && e != cudaSuccess) { good = false; *err = std::string("debug downsample: ") + cudaGetErrorString(e); }
     r.d_conv = nullptr;
     cleanup();
     return good ? MZ_OK : MZ_ECUDA;
@@ -2125,24 +2272,7 @@ int resnet_inference(ResNetDevice* r, const InferCall& c, cudaStream_t stream, i
             if (!R.cnn_stem(c.in, tmp, cur)) return MZ_ECUDA;
             x = R.site_tower(R.representation_site(cur), kAll, &cur, &tmp, &spare);
         } else if (nd.downsample) {
-            int H = nd.obs_h, W = nd.obs_w;
-            const auto& d = r->rep_down;
-            if (!R.conv(d[0], c.in, cur, nullptr, false, H, W)) return MZ_ECUDA;
-            H = conv_out(H, 2); W = conv_out(W, 2);
-            if (!R.blocks(d, 1, 2, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
-            if (!R.conv(d[5], cur, tmp, nullptr, false, H, W)) return MZ_ECUDA;
-            { float* t = cur; cur = tmp; tmp = t; }
-            H = conv_out(H, 2); W = conv_out(W, 2);
-            if (!R.blocks(d, 6, 3, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
-            for (int pool = 0; pool < 2; ++pool) {
-                const int Ho = conv_out(H, 2), Wo = conv_out(W, 2);
-                const size_t total = (size_t)n * C * Ho * Wo;
-                avgpool3x3s2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(cur, tmp, n * C, H, W, Ho, Wo);
-                *launches += 1;
-                { float* t = cur; cur = tmp; tmp = t; }
-                H = Ho; W = Wo;
-                if (pool == 0 && !R.blocks(d, 12, 3, &cur, &tmp, &spare, H, W)) return MZ_ECUDA;
-            }
+            if (!R.downsample(c.in, &cur, &tmp, &spare)) return MZ_ECUDA;
             // the stems stay on the CUDA cores; the trunk's blocks take the wide launch on the Wide256 route (the only
             // wide route that accepts a downsampled net)
             x = R.site_tower(R.representation_site(cur), kAll, &cur, &tmp, &spare);

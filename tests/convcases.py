@@ -4,7 +4,8 @@ planner conv3x3_plan, reached through mz_debug_conv3x3 / mz_debug_conv3x3_plan).
 The planner picks P (pixels per thread) from the output width (the first of 8, 7, 6, 4, 3, 2 that divides Wo, else 1),
 MAX_ITEMS (accumulator tiles per thread: 4 when a CTA holds more than 256 items of 4 channels x P pixels), row bands
 for large images, boards per CTA for small ones, a cin chunk when the staged planes do not fit in shared memory, and
-cout tiles of at most 64 channels (the last one narrower when 64 does not divide Cout).  The cases were taken from the
+cout tiles of 64 channels (the last one narrower when 64 does not divide Cout), halved down to 4 channels while one
+output row of a tile is more than the 4 x 256 items a CTA holds.  The cases were taken from the
 planner, not guessed; tests/test_conv_plan_cpu.py asserts what they reach:
 
   * all 28 instantiations: P in {1, 2, 3, 4, 6, 7, 8} x stride {1, 2} x MAX_ITEMS {1, 4}
@@ -12,7 +13,8 @@ planner, not guessed; tests/test_conv_plan_cpu.py asserts what they reach:
   * several boards per CTA with a partial last CTA; batches of 1, exactly the boards per CTA, one more, and 300
   * a cin chunk smaller than Cin that does not divide it: games/atari.py's 131 -> 128 stride-2 stem at 96 x 96
   * Cout 4, 12, 48, 64, 68, 96, 128, 160 and 256; Cin != Cout, Cin 3, 33 and 131
-  * boards of 1 x 1, 1 x W and H x 1, prime widths (5, 13, 43, 67)
+  * boards of 1 x 1, 1 x W and H x 1, prime widths (5, 13, 43, 67, 131, 521)
+  * cout tiles of 32, 16 and 4 channels on rows too wide for 64 (ct32_*, ct16_*, ct4_*), a narrower last tile behind them
   * one shape the planner refuses (REFUSED)
 """
 from __future__ import annotations
@@ -68,13 +70,18 @@ CASES = [
     ConvCase("s2_p6_m4", 2, 32, 64, 12, 35, 2),
     ConvCase("s2_p7_m4", 2, 16, 160, 12, 41, 2),
     ConvCase("s2_p8_m4_atari_stem", 1, 131, 128, 96, 96, 2),
+    # cout tiles narrower than 64: P = 1 and one output row of a 64-channel tile is more than 1024 items
+    ConvCase("ct32_s1_6x67", 4, 64, 64, 6, 67),                 # 16 x 67 items; 32 channels: 8 x 67
+    ConvCase("ct32_s2_ds129", 3, 16, 128, 7, 129, 2),           # DownSample conv1 of a 256-channel net, 129-wide frame
+    ConvCase("ct16_s1_3x131", 2, 8, 68, 3, 131),                # 16-channel tiles, the fifth one of 4 channels
+    ConvCase("ct4_s1_2x521", 1, 4, 12, 2, 521),                 # three 4-channel tiles
 ]
 
 BY_NAME = {c.name: c for c in CASES}
 
-# a 64-channel board 67 wide: 67 is prime, so P = 1, and one output row alone is 16 x 67 = 1072 items, beyond the
-# 4 x 256 a CTA holds
-REFUSED = ConvCase("refused_6x67", 4, 64, 64, 6, 67)
+# a board 1031 wide: 1031 is prime, so P = 1, and one output row alone is 1031 items even in a 4-channel cout tile,
+# beyond the 4 x 256 a CTA holds
+REFUSED = ConvCase("refused_1x1031", 2, 4, 8, 1, 1031)
 REFUSED_REASON = "image too large for the item budget"
 
 

@@ -29,7 +29,12 @@ Routes (``ROUTES``) and the cases that take them:
   heads_wide      heads_kernel<128> (C*HW > 1024) on the CUDA-core route: hw_c128_6x7
   heads_big       generic heads route (weights beyond shared memory) on the CUDA-core route: hb_c32_6x7
   downsample      DownSample stem: ds_20x24 (3 x 20 x 24 frames -> 2 x 2 hidden, 16 channels), ds_c96_20x24 (96
-                  channels: the stride-2 48 -> 96 conv and the 96-channel blocks have a 32-channel last cout tile)
+                  channels: the stride-2 48 -> 96 conv and the 96-channel blocks have a 32-channel last cout tile),
+                  ds_33x17 (every halving of the frame odd), ds_c8_1x1 (C / 2 = 4 channels on a 1 x 1
+                  frame), ds_breakout_96x96 (games/breakout.py's net), ds_atari_96x96 (games/atari.py's 131 planes, 256
+                  channels and support 300 with the generic heads, one block per tower so the fp64 oracle stays short;
+                  batches of 1 to 3) and ds_atari_96x96_wide (the same under MZ_TC_WIDE=3: the towers on the 256-channel
+                  x3 tensor-core route, the stem on the CUDA cores)
 
 Edge weights (``edge_weights``), applied to the representation and dynamics towers:
 
@@ -64,6 +69,7 @@ class NetCase:
     over: dict = field(default_factory=dict)
     weights: str = "synthetic"          # synthetic | const | tiny | wide | sat | large | tiny_bn | overflow
     env: dict = field(default_factory=dict)
+    batches: tuple = ()                 # the inference sweep's batch sizes, when not the route's default
 
     @property
     def tensor_cores(self):
@@ -139,6 +145,13 @@ CASES = [
                                                        channels=16, blocks=1, downsample="resnet", **_HEADS16)),
     NetCase("ds_c96_20x24", "connect4", "downsample", dict(observation_shape=(3, 20, 24), action_space=list(range(4)),
                                                            channels=96, blocks=1, downsample="resnet", **_HEADS16)),
+    NetCase("ds_33x17", "connect4", "downsample", dict(observation_shape=(3, 33, 17), action_space=list(range(4)),
+                                                       channels=16, blocks=1, downsample="resnet", **_HEADS16)),
+    NetCase("ds_c8_1x1", "connect4", "downsample", dict(observation_shape=(3, 1, 1), action_space=list(range(4)),
+                                                        channels=8, blocks=1, downsample="resnet", **_HEADS16)),
+    NetCase("ds_breakout_96x96", "breakout", "downsample"),
+    NetCase("ds_atari_96x96", "atari", "downsample", dict(blocks=1), batches=(1, 2, 3)),
+    NetCase("ds_atari_96x96_wide", "atari", "downsample", dict(blocks=1), env=dict(MZ_TC_WIDE="3"), batches=(1, 2, 3)),
 ]
 
 BY_NAME = {c.name: c for c in CASES}
@@ -147,7 +160,8 @@ BY_NAME = {c.name: c for c in CASES}
 # fp16; the 6-block tensor-core case, whose gathered dynamics tower is split across launches, with two partitions; the
 # nets kept off the tensor cores by their heads, in fp16 and x3) and every FC route
 SEARCH_CASES = ["pl_9x9_c32", "pl_c96_6x7", "st_c32_6x7", "ss_5x6_a4", "ss_7x3_a12", "tc_6x7", "tc_6x7_b6", "tc_6x7_s300",
-                "tc_6x7_bigheads", "fc_cartpole", "fc_cartpole_s20", "fc_e5_a3", "fc_a40"]
+                "tc_6x7_bigheads", "fc_cartpole", "fc_cartpole_s20", "fc_e5_a3", "fc_a40", "ds_breakout_96x96",
+                "ds_atari_96x96", "ds_atari_96x96_wide"]
 
 
 def make_config(case: NetCase):

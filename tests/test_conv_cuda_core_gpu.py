@@ -89,7 +89,7 @@ def test_cuda_core_conv_against_fp64(name, epilogue):
     print(f"[conv3x3] {name} {epilogue}: worst err / bound {worst:.2e}")
 
 
-def test_refused_shape_is_refused_before_any_launch():
+def test_row_no_cout_tile_holds_is_refused_before_any_launch():
     from muzero_general_b200 import _lib
     from muzero_general_b200.engine import debug_conv3x3
     c = REFUSED
@@ -98,18 +98,21 @@ def test_refused_shape_is_refused_before_any_launch():
         debug_conv3x3(x, w, b, r, True, stride=c.stride)
 
 
-def test_create_refuses_a_net_with_a_conv_the_planner_refuses():
-    """A 64-channel net on a 6 x 67 board: its stem's launch plan is refused, so mz_create fails and names the reason
-    (rather than the first search failing part-way).  The same net one column narrower is created."""
+def test_create_refuses_a_net_whose_row_no_cout_tile_holds():
+    """An 8-channel net on a 1 x 1031 board: its stem's launch plan is refused, so mz_create fails and names the reason
+    and the stage (rather than the first search failing part-way).  The same net one column narrower is created, and
+    so is the 64-channel net on a 6 x 67 board that was refused before the cout tiles could be narrower than 64."""
     from muzero_general_b200 import _lib
     from muzero_general_b200.engine import SearchEngine
     from muzero_general_b200.games import load_game_module
     cfg = load_game_module("connect4").MuZeroConfig()
-    cfg.observation_shape, cfg.action_space, cfg.channels, cfg.blocks = (3, 6, 67), list(range(4)), 64, 1
+    cfg.observation_shape, cfg.action_space, cfg.channels, cfg.blocks = (3, 1, 1031), list(range(4)), 8, 1
     with pytest.raises(_lib.MzError, match=REFUSED_REASON) as e:
         SearchEngine(cfg, max_games=4, num_simulations=2)
-    assert "3 -> 64 channels" in str(e.value) and "6 x 67" in str(e.value)
-    cfg.observation_shape = (3, 6, 66)
+    assert "representation stem: 3 -> 8 channels" in str(e.value) and "1 x 1031" in str(e.value)
+    cfg.observation_shape = (3, 1, 1030)
+    SearchEngine(cfg, max_games=4, num_simulations=2).close()
+    cfg.observation_shape, cfg.channels = (3, 6, 67), 64
     SearchEngine(cfg, max_games=4, num_simulations=2).close()
 
 

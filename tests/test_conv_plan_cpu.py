@@ -1,14 +1,14 @@
 """Host-side launch planner of the CUDA-core conv3x3 kernel (csrc/resnet.cu::conv3x3_plan, through
 mz_debug_conv3x3_plan): the case table of tests/convcases.py reaches every feature it claims, the planner refuses the
 shape it cannot launch and says why, and the plans of the bundled games' layers are the ones the launcher used before
-the cout tiles were allowed a narrower last tile."""
+the cout tiles were allowed a narrower last tile, or narrower tiles on rows too wide for 64 channels."""
 import ctypes
 
 import pytest
 
 from convcases import BY_NAME, CASES, REFUSED, REFUSED_REASON, net_conv_shapes
 
-FIELDS = ("P", "stride", "max_items", "bands", "band_rows", "boards", "cin_chunk", "gx", "gy", "gz", "smem")
+FIELDS = ("P", "stride", "max_items", "bands", "band_rows", "boards", "cin_chunk", "gx", "gy", "gz", "smem", "cout_tile")
 
 
 @pytest.fixture(scope="module")
@@ -30,7 +30,9 @@ def _case_plan(lib, c):
 
 def _earlier_plan(n, cin, cout, H, W, stride):
     """The launcher's arithmetic before this planner existed, restated, with its grid.y = cout // 64 (which dropped the
-    last cout % 64 channels).  Only shapes with cout <= 64 or a multiple of 64 are compared with it."""
+    last cout % 64 channels) and its one cout tile width, min(cout, 64); None where one output row of that tile was
+    more than a CTA's 1024 items (the shape was refused).  Only shapes with cout <= 64 or a multiple of 64 are compared
+    with it."""
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
     P = next((c for c in (8, 7, 6, 4, 3, 2) if Wo % c == 0), 1)
     ct = min(cout, 64)
@@ -41,14 +43,15 @@ def _earlier_plan(n, cin, cout, H, W, stride):
     bands = -(-Ho // band_rows)
     items = (ct // 4) * band_rows * (Wo // P)
     boards = min(256 // items if items < 256 else 1, 32, n)
-    assert items * boards <= 1024
+    if items * boards > 1024:
+        return None
     plane = ((band_rows - 1) * stride + 3) * (W + 2)
     chunk = cin
     while chunk > 1 and chunk * 9 * ct + boards * chunk * plane > 200 * 1024 // 4:
         chunk = (chunk + 1) // 2
     return dict(P=P, stride=stride, max_items=4 if items * boards > 256 else 1, bands=bands, band_rows=band_rows,
                 boards=boards, cin_chunk=chunk, gx=-(-n // boards), gy=cout // ct, gz=bands,
-                smem=(chunk * 9 * ct + boards * chunk * plane) * 4)
+                smem=(chunk * 9 * ct + boards * chunk * plane) * 4, cout_tile=ct)
 
 
 def test_case_table_reaches_every_planner_feature(lib):
@@ -60,8 +63,15 @@ def test_case_table_reaches_every_planner_feature(lib):
     assert inst == want, sorted(want - inst)
     for c in CASES:
         p, (Ho, Wo) = plans[c.name], c.out_hw
-        assert (p["stride"], p["gx"], p["gy"], p["gz"]) == (c.stride, -(-c.n // p["boards"]), -(-c.cout // 64), p["bands"])
+        assert (p["stride"], p["gx"], p["gy"], p["gz"]) == (c.stride, -(-c.n // p["boards"]), -(-c.cout // p["cout_tile"]),
+                                                             p["bands"])
         assert p["bands"] == -(-Ho // p["band_rows"]) and p["cin_chunk"] <= c.cin and p["smem"] <= 200 * 1024
+        # a tile narrower than min(cout, 64) only where one output row of the wider tile exceeds the 1024 items, and
+        # then the widest multiple-of-4 halving that fits
+        ct = min(c.cout, 64)
+        while ct > 4 and ct // 4 * (Wo // p["P"]) > 1024:
+            ct = (ct // 2 + 3) // 4 * 4
+        assert p["cout_tile"] == ct and p["cout_tile"] // 4 * p["band_rows"] * (Wo // p["P"]) * p["boards"] <= 1024, c.name
     # several bands with a shorter last band; one band per output row of a tall image
     assert any(p["bands"] > 1 and BY_NAME[k].out_hw[0] % p["band_rows"] for k, p in plans.items())
     assert any(p["bands"] == BY_NAME[k].out_hw[0] > 1 for k, p in plans.items())
@@ -85,16 +95,24 @@ def test_case_table_reaches_every_planner_feature(lib):
     shapes = {(c.H, c.W) for c in CASES}
     assert (1, 1) in shapes and any(h == 1 < w for h, w in shapes) and any(w == 1 < h for h, w in shapes)
     assert {5, 13, 43, 67} <= {w for _, w in shapes}
+    # cout tiles of 32, 16 and 4 channels, each behind a last tile of fewer channels or a full one
+    tiles = {p["cout_tile"] for p in plans.values()}
+    assert {4, 16, 32, 64} <= tiles, tiles
+    assert any(p["cout_tile"] < 64 and BY_NAME[k].cout % p["cout_tile"] for k, p in plans.items())
+    assert any(p["cout_tile"] < 64 and p["stride"] == 2 for p in plans.values())
 
 
-def test_refused_shape_is_refused_with_its_reason(lib):
+def test_row_no_cout_tile_holds_is_refused_with_its_reason(lib):
     c = REFUSED
     assert _case_plan(lib, c) is None
     assert REFUSED_REASON in lib.mz_last_error(None).decode()
-    # the same board one column narrower (66 = 6 x 11: P = 6) launches
-    assert _plan(lib, c.n, c.cin, c.cout, c.H, c.W - 1, c.stride) is not None
-    # and so does a 32-channel board of the same width: one row is 8 x 67 = 536 items, a band per row
-    assert _plan(lib, c.n, 32, 32, c.H, c.W, c.stride)["band_rows"] == 1
+    # the same board one column narrower (1030 = 2 x 515: P = 2) launches, in 4-channel tiles
+    assert _plan(lib, c.n, c.cin, c.cout, c.H, c.W - 1, c.stride)["cout_tile"] == 4
+    # the 64-channel board 67 wide that a 64-channel tile cannot hold (one row is 16 x 67 = 1072 items) launches in
+    # 32-channel tiles, a band per row; the planner refused it before the tiles could be narrower
+    p = _plan(lib, 4, 64, 64, 6, 67, 1)
+    assert (p["cout_tile"], p["gy"], p["band_rows"]) == (32, 2, 1)
+    assert _earlier_plan(4, 64, 64, 6, 67, 1) is None
 
 
 @pytest.mark.parametrize("args,reason", [((1, 4, 6, 3, 3, 1), "multiple of 4"), ((1, 4, 0, 3, 3, 1), "multiple of 4"),
@@ -127,7 +145,9 @@ def test_bundled_games_and_earlier_shapes_keep_their_launch_plans(lib):
             assert _plan(lib, n, cin, cout, H, W, stride) == _earlier_plan(n, cin, cout, H, W, stride), (game, cin, cout, H, W)
     for c in CASES:
         p, old = _case_plan(lib, c), _earlier_plan(c.n, c.cin, c.cout, c.H, c.W, c.stride)
-        if c.cout <= 64 or c.cout % 64 == 0:
+        if old is None:
+            assert p["cout_tile"] < min(c.cout, 64), c.name         # refused before: launches in narrower tiles now
+        elif c.cout <= 64 or c.cout % 64 == 0:
             assert p == old, c.name
         else:
             assert p == dict(old, gy=old["gy"] + 1), c.name

@@ -81,3 +81,21 @@ def test_planned_cta_size_is_bit_identical_to_64_threads(G, weights, monkeypatch
     # G = 16: 64-thread CTAs for the small batches, larger ones for the rest.  G = 32: registers hold every CTA size to
     # 16 games per SM, so the plan keeps 64 threads throughout.
     assert 64 in blocks and (len(blocks) > 1) == (G == 16)
+
+
+def test_trace_actions_are_zero_past_each_leaf(monkeypatch, game_configs):
+    """A traced search's actions past each simulation's depth read 0, also where the handle's device trace buffer still
+    holds an earlier search's paths: the second search keeps 13 actions per path instead of 51, so it reuses the
+    buffer with every path at another offset (and the buffer is copied back whole)."""
+    from muzero_general_b200.netspec import netspec_from_config
+    cfg = game_configs["cartpole"]
+    spec = netspec_from_config(cfg)
+    n = 256
+    eng = _engine(monkeypatch, cfg, spec, "synthetic", None, n)
+    runs = [eng.search(trace=True, trace_depth=D, **_inputs(spec, cfg, n, seed)) for seed, D in ((1, N_SIM + 1), (2, 13))]
+    eng.close()
+    assert runs[0].trace["actions"].any()
+    for out in runs:
+        depth, actions = out.trace["depth"], out.trace["actions"]
+        past = numpy.arange(actions.shape[2])[None, None, :] >= depth[:, :, None]
+        assert past.any() and not actions[past].any(), int(numpy.count_nonzero(actions[past]))

@@ -76,7 +76,7 @@ def test_case_table_covers_every_route_with_shapes_that_select_it():
         if c.route == "heads_wide":
             assert spec.channels * H * W > 1024
         if c.route == "downsample":
-            assert spec.downsample and (H, W) == (2, 2)
+            assert spec.downsample and (H, W) == tuple(-(-x // 16) for x in spec.obs_shape[1:])
     assert any(case_spec(c).blocks == 0 and c.route == "tc" for c in CASES)
     # tensor-core towers: one 8-layer launch (4 blocks) and towers split across launches (the dynamics tower from 4
     # blocks on, every tower from 5), the split in-search dynamics tower inside a partitioned search too

@@ -110,11 +110,11 @@ def test_atari_keeps_its_cuda_core_plans():
         plan, why = debug_small_tower_plan(128, cin, 256, 6, 6, 16, stem, 132)
         assert plan is None and "layers" in why
     lib = _lib.load_library()
-    out = (C.c_int64 * 11)()
+    out = (C.c_int64 * 12)()
     for cin, chunk, smem in ((256, 64, 180224), (257, 65, 183040)):
         for n, grid in ((2, 1), (128, 64)):
             assert lib.mz_debug_conv3x3_plan(n, cin, 256, 6, 6, 1, out)
-            assert list(out) == [6, 1, 1, 1, 6, 2, chunk, grid, 4, 1, smem]
+            assert list(out) == [6, 1, 1, 1, 6, 2, chunk, grid, 4, 1, smem, 64]
 
 
 # ---------------------------------------------------------------------------------------------- reference fixtures

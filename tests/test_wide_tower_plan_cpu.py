@@ -85,8 +85,8 @@ def test_unset_routes_are_unchanged():
         plan, why = debug_small_tower_plan(128, cin, 128, 11, 11, blocks, stem, 132)
         assert plan is None and why
     lib = _lib.load_library()
-    out = (C.c_int64 * 11)()
+    out = (C.c_int64 * 12)()
     for cin in (3, 128, 129):
         assert lib.mz_debug_conv3x3_plan(128, cin, 128, 11, 11, 1, out)
         # P = 1, stride 1, 4 items, 3 bands of 4 rows, one board per CTA, grid (128 boards, 2 cout tiles, 3 bands)
-        assert list(out)[:6] == [1, 1, 4, 3, 4, 1] and list(out)[7:10] == [128, 2, 3]
+        assert list(out)[:6] == [1, 1, 4, 3, 4, 1] and list(out)[7:10] == [128, 2, 3] and out[11] == 64
